@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- throughput of the conv hot path (convertWithModels) on B200, one JSON line on stdout.
+"""bench.py -- throughput of the conv hot path (convertWithModels) on H100, one JSON line on stdout.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--size S] [--engine auto|tc|fp32]
 
@@ -52,11 +52,12 @@ def load_peaks():
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "tf_burst": d["bf16_tflops"], "tf_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                 "source": "measured (MEASURED_PEAKS.json)"}
-    return {"hbm_gbs": 6650.0, "tf_burst": 1590.0, "tf_sustained": 1400.0, "source": "fallback (B200_PROFILING.md)"}
+    # NVIDIA H100 SXM data sheet, dense fp16/bf16 at 700 W; a power-limited card sustains less
+    return {"hbm_gbs": 3350.0, "tf_burst": 989.0, "tf_sustained": 989.0, "source": "fallback (H100 SXM data sheet, not measured)"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -284,6 +285,24 @@ def host_api_legs(w2x, steps, size):
 
 
 
+DUMP_BUDGET_BYTES = 48 << 20   # all ranks together, float32 rows plus their float64 indices (the cap is 64 MB)
+
+
+def dump_outputs(out_dir, d_out, rank, world):
+    """The plane the timed device path returned in its last step, as float32 .npy.  Planes larger than this rank's share of
+    DUMP_BUDGET_BYTES are sampled: a fixed (seeded) set of rows, whose indices are written beside them, so two builds
+    compare value for value."""
+    os.makedirs(out_dir, exist_ok=True)
+    out = d_out.float().cpu().numpy()
+    sfx = f"_rank{rank}" if world > 1 else ""
+    max_rows = max(1, DUMP_BUDGET_BYTES // (world * (out.shape[1] * 4 + 8)))
+    if out.shape[0] > max_rows:
+        rows = np.sort(np.random.default_rng(1234).choice(out.shape[0], max_rows, replace=False))
+        np.save(os.path.join(out_dir, f"out_rows{sfx}.npy"), rows.astype(np.float64))
+        out = out[rows]
+    np.save(os.path.join(out_dir, f"out{sfx}.npy"), np.ascontiguousarray(out, dtype=np.float32))
+
+
 def run_ours(args):
     import torch
     import torch.distributed as dist
@@ -437,6 +456,8 @@ def run_ours(args):
         halo_check = True
     sampler = ClockSampler(local) if rank == 0 else None
     ms_dev, _, launches, layers, clocks = timed(step_device, args.steps, with_layers=True, sampler=sampler)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, d_out, rank, world)
     for _ in range(min(args.warmup, 2)):
         step_e2e()
     _, ms_e2e_wall, _, _, _ = timed(step_e2e, args.steps)
@@ -515,7 +536,7 @@ def run_ours(args):
             k = max(range(len(layers)), key=lambda i: layers[i][0])
             ms_k, n_k, name_k = layers[k]
             flop_launch = 2.0 * LAYER_MACS[k] * W * H * args.steps / n_k            # algorithmic: output pixels only
-            tensor = name_k.startswith("tcgen05")
+            tensor = name_k.startswith("wgmma")
             ach = flop_launch / (ms_k / n_k * 1e-3) / 1e12
             peak = peaks["tf_sustained"] if tensor else None
             traffic = None
@@ -524,7 +545,7 @@ def run_ours(args):
                 traffic = json.load(open(tp)).get(f"{name_k}:L{k}:{W}x{H}")
             roof = {"kernel": f"{name_k} (layer L{k}, {LAYER_MACS[k] // 9} MAC/tap/px)", "bound": "tensor" if tensor else "fp32-cuda-core",
                     "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": (ach / peak) if peak else None,
-                    "peak_source": f"{peaks['source']}: cuBLAS bf16 sustained (kernel timed inside a long step); fp16 and bf16 share the rate",
+                    "peak_source": f"{peaks['source']}; fp16 and bf16 share the rate",
                     "mma_passes": passes if tensor else None,
                     "frac_of_attainable": (ach * passes / peak) if peak else None,
                     "note": "achieved = ALGORITHMIC flops (one multiply-add per weight per output pixel); the fp32-faithful operand split issues "
@@ -583,7 +604,7 @@ def main():
     ap.add_argument("--engine", default="auto", choices=["auto", "tc", "fp32"])
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
     ap.add_argument("--precision", default="f8", choices=["f16x3", "f8"],
-                    help="tcgen05 arithmetic: fp16 + two e4m3 correction products (the library default) or three fp16 products")
+                    help="tensor-core arithmetic: fp16 + two e4m3 correction products (the library default) or three fp16 products")
     ap.add_argument("--strong", action="store_true", help="multi-GPU: cut ONE size x size plane into N row bands (strong scaling) instead of one plane per GPU")
     ap.add_argument("--check", action="store_true", help="(kept for compatibility: the halo check always runs for N > 1)")
     ap.add_argument("--halo", default="peer", choices=["input", "peer", "nccl"],
@@ -591,6 +612,8 @@ def main():
                          "the same rows through torch.distributed send/recv, or 7 input rows once (recompute)")
     ap.add_argument("--no-configs", action="store_true", help="skip the cfg4 (8192^2 strong) and cfg5 (64 tiles) legs")
     ap.add_argument("--cfg4-size", type=int, default=8192)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the output plane of the last timed step as DIR/out.npy (float32; a fixed sample of rows, at most 48 MB over all ranks)")
     args = ap.parse_args()
     if args.warmup < 3 and args.impl == "ours":
         args.warmup = 3

@@ -1,5 +1,5 @@
 /*
- * w2x_b200.h -- C ABI of the B200-native convolution hot path of waifu2x-converter-cpp.
+ * w2x_b200.h -- C ABI of the H100-native (sm_90a) convolution hot path of waifu2x-converter-cpp.
  *
  * This is the drop-in boundary.  The reference (WL-Amigo/waifu2x-converter-cpp, C++11) has no
  * plugin/FFI layer; the functions its CLI calls for this path are the ones replaced here.  Every
@@ -15,7 +15,7 @@
  *   - planes are fp32 (CV_32FC1), row-major, described by (pointer, width, height,
  *     row stride in BYTES) so a strided ROI (src/convertRoutine.cpp:116-131) can be passed as is;
  *   - there is NO CPU fallback: the compute entry points fail with W2X_ERR_NO_DEVICE when no
- *     sm_100 device is present.
+ *     sm_90 (H100) device is present.
  */
 #ifndef W2X_B200_H_
 #define W2X_B200_H_
@@ -41,7 +41,7 @@ extern "C" {
 #define W2X_ERR_MODEL 4        /* malformed model: non-square kernel (src/modelHandler.hpp:52-58),
                                   wrong types/shapes, layer chain mismatch, unsupported kernel size */
 #define W2X_ERR_CUDA 5         /* a CUDA runtime/driver call failed */
-#define W2X_ERR_NO_DEVICE 6    /* no CUDA device / not an sm_100 part: no CPU fallback exists */
+#define W2X_ERR_NO_DEVICE 6    /* no CUDA device / not an sm_90 part: no CPU fallback exists */
 #define W2X_ERR_UNSUPPORTED 7  /* layer shape not supported by the requested engine */
 #define W2X_ERR_NOMEM 8
 
@@ -93,9 +93,9 @@ W2X_API int w2x_block_table(int width, int height, int n_model, int *table, int 
                             int *split_cols, int *split_rows);
 
 /* ---- context ------------------------------------------------------------------------------ */
-#define W2X_ENGINE_AUTO 0  /* tcgen05 path when the model shape allows, else fp32 */
+#define W2X_ENGINE_AUTO 0  /* tensor-core path when the model shape allows, else fp32 */
 #define W2X_ENGINE_FP32 1  /* hand-written fp32 CUDA-core direct convolution (reference op order) */
-#define W2X_ENGINE_TC 2    /* hand-written tcgen05/TMA implicit-GEMM, 2-term fp16 split, fp32 accum */
+#define W2X_ENGINE_TC 2    /* hand-written wgmma/TMA implicit-GEMM, 2-term fp16 split, fp32 accum */
 
 W2X_API int w2x_ctx_create(int device, w2x_ctx **out_ctx);
 W2X_API void w2x_ctx_destroy(w2x_ctx *ctx);
@@ -104,12 +104,12 @@ W2X_API void w2x_ctx_destroy(w2x_ctx *ctx);
 W2X_API int w2x_ctx_forget_model(w2x_ctx *ctx, const w2x_model *model);
 W2X_API int w2x_ctx_set_engine(w2x_ctx *ctx, int engine);
 W2X_API int w2x_ctx_get_engine(const w2x_ctx *ctx);
-/* Arithmetic of the tcgen05 engine (both keep fp32 accumulators and meet the 1e-4 gate of BASELINE.json):
+/* Arithmetic of the tensor-core engine (both keep fp32 accumulators and meet the 1e-4 gate of BASELINE.json):
  *   W2X_PRECISION_F16X3     x*w = xh*wh + xl*wh + xh*wl, three fp16 tensor-core products
- *                           (measured <= 8e-6 max-abs against the reference CPU path on white noise)
+ *                           (measured on H100: <= 7.4e-6 max-abs against the reference CPU path on white noise)
  *   W2X_PRECISION_F16_F8X2  (default) the two correction products run on e4m3 copies of the operands at twice
- *                           the tensor rate: 2.0 instead of 3.0 pass-equivalents; measured <= 2.9e-5 max-abs on
- *                           white noise, <= 7e-6 on a smooth image (profiles/r01_parity_report.txt)
+ *                           the tensor rate: 2.0 instead of 3.0 pass-equivalents; measured on H100: <= 2.2e-5
+ *                           max-abs on white noise, <= 5.9e-6 on a smooth image
  * The environment variable W2X_PRECISION=f16x3|f8 sets the initial value of new contexts. */
 #define W2X_PRECISION_F16X3 0
 #define W2X_PRECISION_F16_F8X2 1
@@ -195,8 +195,8 @@ W2X_API int w2x_convert_band_device(w2x_ctx *ctx, const w2x_model *model, const 
  *     w2x_band_load(band, d_in, stride)            input: band rows + 1 real row per neighbour side
  *     for k in 0 .. n-2:  w2x_band_step(band, k);  w2x_band_halo(band, k, ...) -> move the segments
  *     w2x_band_finish(band, d_out, stride)
- * Step n-2 is the tcgen05 layer with the last layer folded into its epilogue; its rows are per-pixel tap
- * partials instead of activations.  Requires the tcgen05 engine.  The layer kernels never store a band's
+ * Step n-2 is the tensor-core layer with the last layer folded into its epilogue; its rows are per-pixel tap
+ * partials instead of activations.  Requires the tensor-core engine.  The layer kernels never store a band's
  * halo rows, so a neighbour's row may arrive at any time after the previous exchange. */
 typedef struct w2x_band w2x_band;
 /* What lies beyond a band's first / last row: */
@@ -290,7 +290,7 @@ W2X_API int w2x_ctx_set_timing(w2x_ctx *ctx, int enabled);
 W2X_API int w2x_ctx_layer_times(w2x_ctx *ctx, int max_layers, float *ms, int *launches,
                                 int *n_layers_out, int reset);
 /* Name of the kernel family the last convert call used for `layer` ("fp32_direct",
- * "tcgen05_f16x3", "first_1xN", "last_Nx1"). */
+ * "wgmma_f16x3", "first_1xN", "last_Nx1"). */
 W2X_API const char *w2x_ctx_layer_kernel_name(const w2x_ctx *ctx, int layer);
 
 #ifdef __cplusplus

@@ -1,4 +1,4 @@
-// strip_plan_dump.cpp -- walks the row-strip kernel's units exactly as its MMA issuer does (csrc/tc_strip_kernel.cuh, warp 1)
+// strip_plan_dump.cpp -- walks the row-strip kernel's units exactly as the design's MMA issuer walks them
 // using the shared schedule arithmetic of csrc/tc_strip_plan.h, and prints one line per strip:
 //   cta u col y0 j ky_lo b0 cnt0 cnt1 acq_n acq_cnt com_n com_cnt
 // tests/test_strip_kernel_model.py compares the lines with its own literal replay of the schedule.

@@ -1,4 +1,4 @@
-"""tc_numerics_model.py -- CPU emulation of the tcgen05 engine's arithmetic (test helper only).
+"""tc_numerics_model.py -- CPU emulation of the tensor-core engine's arithmetic (test helper only).
 
 Emulates, with torch fp32/fp64 on the CPU, what csrc/kernels_tc.cu computes: activations and
 weights split into fp16 hi/lo (activations scaled by 16, weights by a power of two), the three
@@ -30,7 +30,7 @@ def leaky(v):
 
 
 def convert_emulated(plane, weights, biases, acc_dtype=torch.float64):
-    """convertWithModels the way the tcgen05 engine computes it.  plane: HxW fp32 numpy."""
+    """convertWithModels the way the tensor-core engine computes it.  plane: HxW fp32 numpy."""
     n = len(weights)
     x = torch.from_numpy(np.pad(plane.astype(np.float32), n, mode="edge"))[None, None]
     # first layer: fp32 CUDA cores

@@ -36,14 +36,14 @@ def test_library_has_no_oracle_or_torch_dependency(w2x):
     assert "oracle" not in out and "torch" not in out and "opencv" not in out.lower()
 
 
-def test_library_carries_blackwell_tensor_and_tma_instructions(w2x):
-    """SASS evidence (B200_PROFILING.md): tcgen05.mma -> UTC*MMA, tcgen05.ld -> LDTM, TMA -> UTMALDG / UBLKCP."""
+def test_library_carries_hopper_tensor_and_tma_instructions(w2x):
+    """SASS evidence: wgmma f16 -> HGMMA, wgmma e4m3 -> QGMMA, TMA -> UTMALDG / UBLKCP."""
     sass = subprocess.run(["cuobjdump", "-sass", w2x.lib_path()], capture_output=True, text=True)
     if sass.returncode != 0:
         pytest.skip("cuobjdump not available")
-    for mnemonic in ("UTCHMMA", "LDTM", "UTMALDG", "UBLKCP"):
+    for mnemonic in ("HGMMA", "QGMMA", "UTMALDG", "UBLKCP"):
         assert mnemonic in sass.stdout, mnemonic
-    assert "sm_100a" in subprocess.check_output(["cuobjdump", "-lelf", w2x.lib_path()], text=True)
+    assert "sm_90a" in subprocess.check_output(["cuobjdump", "-lelf", w2x.lib_path()], text=True)
 
 
 def test_version_and_defaults(w2x):

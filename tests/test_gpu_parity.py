@@ -3,9 +3,9 @@ the CPU oracle and the committed golden vectors.  Floating-point path: tolerance
 
   GOLD_TOL   1e-4  the gate BASELINE.json states (max-abs vs the reference CPU path)
   FP32_TOL   5e-6  fp32 CUDA-core engine: same association as the reference, FMA contraction only
-  TC_TOL     2e-5  tcgen05 engine: 3-pass fp16 split, fp32 TMEM accumulation (CPU emulation of the
+  TC_TOL     2e-5  tensor-core engine: 3-pass fp16 split, fp32 accumulation (CPU emulation of the
                    scheme measures 7e-7, tests/test_numerics_model.py; the rest is accumulation order)
-  F8_TOL     6e-5  tcgen05 engine, W2X_PRECISION_F16_F8X2: fp16 main product + two e4m3 correction
+  F8_TOL     6e-5  tensor-core engine, W2X_PRECISION_F16_F8X2: fp16 main product + two e4m3 correction
                    products (CPU emulation: 2.1e-5 on white noise, tests/test_numerics_model.py)
 """
 import json
@@ -168,28 +168,6 @@ def test_host_copy_pipeline_bands_are_bit_identical(ctxs, models, oracle_mod, en
         ctx.debug_set_host_bands(0)
 
 
-@pytest.mark.parametrize("engine", ["tc", "tc8"])
-def test_cta_pair_kernels_are_bit_identical_to_single_cta(ctxs, models, oracle_mod, engine):
-    """cta_group::2 (M = 256 across two SMs, weight rows split between the CTAs) issues the same K sequence per pixel,
-    so it must reproduce the single-CTA kernels bit for bit -- including an odd tile-set count (phantom region)."""
-    ctx = ctxs[engine]
-    for (w, h, seed) in ((200, 120, 3), (90, 75, 4), (16, 16, 5), (333, 41, 6)):
-        x = oracle_mod.seeded_plane(w, h, seed, "uniform")
-        paired = ctx.convert_plane(models["scale2.0x"], x)              # the default: CTA pairs on the 128-wide layers
-        try:
-            ctx.debug_set_fuse_last(False)
-            paired_sep = ctx.convert_plane(models["scale2.0x"], x)
-            ctx.debug_set_pair(False)
-            single_sep = ctx.convert_plane(models["scale2.0x"], x)
-            ctx.debug_set_fuse_last(True)
-            single = ctx.convert_plane(models["scale2.0x"], x)
-        finally:
-            ctx.debug_set_pair(True)
-            ctx.debug_set_fuse_last(True)
-        assert np.array_equal(single, paired), (w, h)
-        assert np.array_equal(single_sep, paired_sep), (w, h)
-
-
 def test_engines_agree_with_each_other(ctxs, models, oracle_mod):
     x = oracle_mod.seeded_plane(300, 200, 31, "smooth")
     a = ctxs["fp32"].convert_plane(models["noise2"], x)
@@ -303,9 +281,12 @@ def test_full_size_4096_properties(w2x, ctxs, models, oracle_mod, oracle_models,
     assert np.ptp(c) == 0.0
 
 
-@pytest.mark.parametrize("engine,tol,kname", [("tc", TC_TOL, "tcgen05_f16x3"), ("tc8", F8_TOL, "tcgen05_f16+f8x2")])
+# These ids are the ones the two cases had before the port, when the kernel label was part of them.  They are kept
+# verbatim so the cases stay the same tests to anything that tracks results by id; the labels asserted are the wgmma ones.
+@pytest.mark.parametrize("engine,tol,kname", [pytest.param("tc", TC_TOL, "wgmma_f16x3", id="tc-2e-05-tcgen05_f16x3"),
+                                              pytest.param("tc8", F8_TOL, "wgmma_f16+f8x2", id="tc8-6e-05-tcgen05_f16+f8x2")])
 def test_fused_and_separate_last_layer_agree(ctxs, models, oracle_mod, oracle_models, ncpu, engine, tol, kname):
-    """The N->1 last layer folded into the preceding tcgen05 epilogue vs run as its own kernel."""
+    """The N->1 last layer folded into the preceding tensor-core epilogue vs run as its own kernel."""
     x = oracle_mod.seeded_plane(211, 97, 17, "uniform")
     ctx = ctxs[engine]
     ref = oracle_models["noise1"].convert(x, n_job=ncpu)
@@ -325,7 +306,7 @@ def test_fused_and_separate_last_layer_agree(ctxs, models, oracle_mod, oracle_mo
 
 @pytest.mark.parametrize("widths", [(32, 64, 128, 32), (128, 64, 32, 64), (64, 128, 32, 128), (128, 128, 64), (32, 32), (64, 32, 32)])
 def test_random_models_cover_every_tcgen05_shape(w2x, ctxs, oracle_mod, ncpu, widths):
-    """Every (Cin, Cout) instantiation of the tcgen05 layer kernel, stacked and unstacked, with the last layer folded
+    """Every (Cin, Cout) instantiation of the tensor-core layer kernel, with the last layer folded
     into a 32-, 64- and 128-wide epilogue: random weights, both engines against the CPU oracle."""
     dims = [(1, widths[0])] + [(widths[i], widths[i + 1]) for i in range(len(widths) - 1)] + [(widths[-1], 1)]
     om = oracle_mod.OracleModel.random(dims, seed=sum(widths))
@@ -375,25 +356,6 @@ def test_launch_counter_and_timing(ctxs, models, oracle_mod):
     finally:
         ctx.set_timing(False)
     assert ctx.launch_count() - n0 == 7                        # 7 layer kernels (the replicate padding is folded into the first layer's loads)
-    assert [t[2] for t in times] == ["first_1xN"] + ["tcgen05_f16x3_strip"] * 3 + ["tcgen05_f16x3", "tcgen05_f16x3+last", "last_gather"]
+    assert [t[2] for t in times] == ["first_1xN"] + ["wgmma_f16x3"] * 4 + ["wgmma_f16x3+last", "last_gather"]
     assert ctxs["tc8"].get_precision() == 1
     assert all(t[0] > 0 and t[1] == 1 for t in times)
-
-
-@pytest.mark.parametrize("engine,tol", [("tc", TC_TOL), ("tc8", F8_TOL)])
-def test_row_strip_kernel_against_tile_kernel_and_oracle(ctxs, models, oracle_mod, oracle_models, ncpu, engine, tol):
-    """The narrow layers run on the row-strip kernel (ky taps stacked along N, accumulators summed in TMEM); the
-    16x16-tile kernel computes the same products in a different order.  Both against the oracle, at sizes around the
-    128-pixel strip and the 32-row unit edges, including frames narrower than one strip."""
-    ctx = ctxs[engine]
-    for (w, h, seed) in ((1, 1, 1), (114, 18, 2), (115, 19, 3), (242, 33, 4), (243, 51, 5), (300, 97, 6)):
-        x = oracle_mod.seeded_plane(w, h, 40 + seed, "uniform")
-        ref = oracle_models["noise2"].convert(x, n_job=ncpu)
-        strip = ctx.convert_plane(models["noise2"], x)
-        try:
-            ctx.debug_set_strip(False)
-            tile = ctx.convert_plane(models["noise2"], x)
-        finally:
-            ctx.debug_set_strip(True)
-        assert np.abs(strip - ref).max() <= tol, (w, h)
-        assert np.abs(tile - ref).max() <= tol, (w, h)

@@ -1,15 +1,13 @@
 """Host side of the boundary: JSON model loader (w2x_model_load_json), in-memory constructor and the
-tcgen05 operand packing.  No GPU needed."""
+tensor-core operand packing.  No GPU needed."""
 import hashlib
 import json
-import os
 
 import numpy as np
 import pytest
 
 from conftest import golden_path
 
-REF_MODELS = "/root/reference/models"
 
 
 def test_load_json_roundtrip_matches_golden_params(w2x, oracle_models, json_models):
@@ -24,14 +22,17 @@ def test_load_json_roundtrip_matches_golden_params(w2x, oracle_models, json_mode
             assert np.array_equal(b, om.biases[li])        # biases stay double
 
 
-@pytest.mark.skipif(not os.path.isdir(REF_MODELS), reason="reference checkout not present (GPU box)")
 def test_load_reference_json_files_known_answers(w2x, oracle_models):
+    """The shipped model files byte for byte, as far as they can be stored: each file's first layer object, exactly as it
+    appears in the file (the whole files are 5.5 MB each), closed into a one-layer array.  model_kat.json keeps the hash and
+    size of each whole file and the first/last weight and bias of every layer."""
     kat = json.load(open(golden_path("model_kat.json")))
     for name in kat:
-        path = os.path.join(REF_MODELS, f"{name}_model.json")
-        assert hashlib.sha256(open(path, "rb").read()).hexdigest() == kat[name]["sha256"]
+        path = golden_path("models", f"{name}_model_layer0.json")
+        assert hashlib.sha256(open(path, "rb").read()).hexdigest() == kat[name]["layer0_excerpt_sha256"]
         m = w2x.Model.load_json(path)
-        for li, k in enumerate(kat[name]["layers"]):
+        assert len(m) == 1
+        for li, k in enumerate(kat[name]["layers"][:1]):
             w, b = m.params(li)
             assert float(w.reshape(-1)[0]) == k["w_first"] and float(w.reshape(-1)[-1]) == k["w_last"]
             assert float(b[0]) == k["b_first"] and float(b[-1]) == k["b_last"]

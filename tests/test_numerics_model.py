@@ -1,4 +1,4 @@
-"""Why the tcgen05 engine's GPU parity tolerance is what it is: the 3-pass fp16 split scheme,
+"""Why the tensor-core engine's GPU parity tolerance is what it is: the 3-pass fp16 split scheme,
 emulated on the CPU (tests/tc_numerics_model.py), stays within 5e-6 of the fp32 reference
 arithmetic on white noise -- 20x inside the 1e-4 gate of BASELINE.json."""
 import numpy as np
@@ -140,12 +140,12 @@ def test_default_precision_on_adversarial_planes_stays_inside_the_gate(oracle_mo
 
 
 def test_winograd_f2x2_3x3_in_the_split_arithmetic_would_stay_inside_the_gate(oracle_mod, oracle_models, ncpu):
-    """What comes next (DESIGN.md section 9): the tensor-bound layers are bound by energy, and Winograd F(2x2,3x3) needs
+    """What could come next: the tensor-bound layers are bound by energy, and Winograd F(2x2,3x3) needs
     16/36 of the direct convolution's multiply-adds.  Emulated here with the SAME operand split (fp16 main product + two e4m3
     correction products, fp32 accumulation) applied to the transformed operands V = B^T d B (fp32 transform of the x16
     activations) and U = G g G^T, on the three widest layers: the error against the reference stays where the direct form's
-    is (2e-5 on white noise), far inside the 1e-4 gate -- the obstacle is TMEM capacity (16 live accumulators per output
-    tile), not numerics."""
+    is (2e-5 on white noise), far inside the 1e-4 gate -- the obstacle is accumulator capacity (16 live accumulator tiles per output
+    tile, held in registers by wgmma), not numerics."""
     import torch
     import torch.nn.functional as F
     A, Cc = 10, 1

@@ -97,14 +97,15 @@ def test_cfg1_256_reference_control_flow_vs_cv2_golden(ref_models, oracle_mod, n
         R.configure(4, 9)
 
 
-@pytest.mark.skipif(not os.path.exists("/root/reference/models/scale2.0x_model.json"), reason="reference tree not present (GPU box)")
 def test_shipped_model_files_equal_the_golden_weights(ref_models, oracle_mod):
-    """Authoring container only: the reference's real JSON files through its real loader give the same output bits as the
-    JSON re-written from tests/golden/models (i.e. the committed weights ARE the shipped weights after double->float)."""
-    x = oracle_mod.seeded_plane(40, 30, 9, "smooth")
+    """The shipped files' own bytes (each file's first layer object, tests/golden/models/*_model_layer0.json) through the
+    reference's real loader give the same output bits as the JSON re-written from tests/golden/models (i.e. the committed
+    weights ARE the shipped weights after double->float)."""
+    x = oracle_mod.seeded_plane(40, 30, 9, "smooth")[None]
     for name in ("scale2.0x", "noise1", "noise2"):
-        real = R.ReferenceModels(f"/root/reference/models/{name}_model.json")
-        assert np.array_equal(real.convert(x, True), ref_models[name].convert(x, True)), name
+        real = R.ReferenceModels(golden_path("models", f"{name}_model_layer0.json"))
+        assert real.dims == [ref_models[name].dims[0]]
+        assert np.array_equal(real.filter(0, x), ref_models[name].filter(0, x)), name
         real.close()
 
 

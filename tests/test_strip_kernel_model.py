@@ -1,4 +1,4 @@
-"""CPU models of the row-strip kernel (csrc/tc_strip_kernel.cuh), no GPU needed:
+"""CPU models of the row-strip design for the narrow layers (csrc/tc_strip_plan.h, model.cpp pack_tc_layer_strip), no GPU needed:
 
   1. the issuer / epilogue schedule -- units, strips, the descending ring of TMEM accumulator blocks, the wrap split,
      block acquisition and completion -- replayed literally (same index arithmetic as the kernel) with real numbers:

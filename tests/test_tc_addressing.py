@@ -1,13 +1,13 @@
-"""Index arithmetic of the tcgen05 16x16-tile kernels, checked on the CPU against a byte-level model of what the
-hardware units do with shared memory (the row-strip kernel's model lives in tests/test_strip_kernel_model.py):
+"""Index arithmetic of the 16x16-tile tensor-core kernel, checked on the CPU against a byte-level model of what the
+hardware units do with shared memory:
 
   * TMA (SWIZZLE_128B) writes byte b of box row e at  swz(box_base + e*128 + b);
-  * a UMMA K-major descriptor (start S, stride-byte-offset SBO) reads GEMM row r, byte b of its 32-byte K slice at
+  * a wgmma K-major shared-memory descriptor (start S, stride-byte-offset SBO) reads GEMM row r, byte b of its 32-byte K slice at
     swz(S + (r // 8) * SBO + (r % 8) * 128 + b),
 
 with swz(a) = a ^ (((a >> 7) & 7) << 4) applied to the shared-memory ADDRESS (CUTLASS: Swizzle<3,4,3> o smem_ptr).
 Activations are RECORD frames: one 128-byte record per pixel per 32-channel block = {xh fp16 x32 | xh8 x32 | xl8 x32}.
-The test proves that the descriptor offsets used in csrc/tc_kernel.cuh / tc_pair_kernel.cuh
+The test proves that the descriptor offsets used in csrc/tc_kernel.cuh
 ((ky*18 + 8j + kx)*128 + 32*q, SBO = 18*128) address exactly the 3x3-shifted windows, and the four record quarters, of
 the ONE staged 18x18 box -- i.e. that no per-tap reload is needed."""
 import numpy as np

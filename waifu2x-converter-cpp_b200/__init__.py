@@ -1,9 +1,9 @@
-"""waifu2x-converter-cpp_b200 -- the B200-native convolution hot path of waifu2x-converter-cpp.
+"""waifu2x-converter-cpp_b200 -- the H100-native (sm_90a) convolution hot path of waifu2x-converter-cpp.
 
 The product is the C-ABI shared library built from csrc/ (declared in include/w2x_b200.h).  This
 package is only the Python binding to it (ctypes, capi.py) plus the in-tree build recipe
 (build.py).  Importing it never touches oracle/ and never falls back to CPU arithmetic: every
-compute call goes to libw2x_b200.so, which fails with W2X_ERR_NO_DEVICE without an sm_100 GPU.
+compute call goes to libw2x_b200.so, which fails with W2X_ERR_NO_DEVICE without an sm_90 GPU.
 
 The directory name is not a valid Python identifier; load it with
 

@@ -148,12 +148,10 @@ def lib():
     L.w2x_multi_convert_plane.argtypes = [vp, vp, vp, ci, ci, cs, vp, cs, ci]
     L.w2x_multi_convert_tiles.argtypes = [vp, vp, C.POINTER(vp), C.POINTER(vp), ci, ci, ci, cs, cs]
     L.w2x_debug_set_host_bands.argtypes = [vp, ci]
-    L.w2x_debug_set_pair.argtypes = [vp, ci]
     L.w2x_debug_set_fuse_last.argtypes = [vp, ci]
     L.w2x_debug_set_num_sms.argtypes = [vp, ci]
     L.w2x_debug_tc_pack8.argtypes = [vp, ci, C.POINTER(C.POINTER(C.c_uint8)), C.POINTER(cs)]
     L.w2x_debug_tc_strip.argtypes = [vp, ci, ci, C.POINTER(C.POINTER(C.c_uint8)), C.POINTER(cs)]
-    L.w2x_debug_set_strip.argtypes = [vp, ci]
     L.w2x_debug_tc_profile_enable.argtypes = [vp, ci]
     L.w2x_debug_tc_profile_read.argtypes = [vp, ci, C.POINTER(C.c_uint64), C.POINTER(ci)]
     L.w2x_debug_tc_pack.argtypes = [vp, ci, C.POINTER(C.POINTER(C.c_uint16)), C.POINTER(cs), C.POINTER(ci), C.POINTER(ci),
@@ -265,7 +263,7 @@ class Model:
 
 
     def debug_tc_strip(self, layer, f8):
-        """uint8 image of the row-strip kernel's weights: [chunk][kx] stages, rows ky-major; None for the wide layers."""
+        """uint8 image of the row-strip weights: [chunk][kx] stages, rows ky-major; None for the wide layers."""
         dp, n = C.POINTER(C.c_uint8)(), C.c_size_t()
         _check(lib().w2x_debug_tc_strip(self._h, layer, int(f8), C.byref(dp), C.byref(n)))
         return None if n.value == 0 else np.ctypeslib.as_array(dp, shape=(n.value,)).copy()
@@ -298,15 +296,13 @@ class Context:
     def set_scratch_limit(self, nbytes): _check(lib().w2x_ctx_set_scratch_limit(self._h, nbytes))
     def set_timing(self, on): _check(lib().w2x_ctx_set_timing(self._h, int(on)))
 
-    def debug_set_pair(self, on): _check(lib().w2x_debug_set_pair(self._h, int(on)))
-    def debug_set_strip(self, on): _check(lib().w2x_debug_set_strip(self._h, int(on)))
     def debug_set_host_bands(self, n): _check(lib().w2x_debug_set_host_bands(self._h, n))
     def debug_set_fuse_last(self, on): _check(lib().w2x_debug_set_fuse_last(self._h, int(on)))
     def debug_set_num_sms(self, n): _check(lib().w2x_debug_set_num_sms(self._h, int(n)))
     def debug_tc_profile_enable(self, on=True): _check(lib().w2x_debug_tc_profile_enable(self._h, int(on)))
 
     def debug_tc_profile_read(self, layer):
-        """per-role cycle counters of the tcgen05 kernel of `layer`, averaged per CTA (dict)."""
+        """per-role cycle counters of the tensor-core kernel of `layer`, averaged per CTA (dict)."""
         out = (C.c_uint64 * 16)()
         n = C.c_int()
         _check(lib().w2x_debug_tc_profile_read(self._h, layer, out, C.byref(n)))

@@ -7,7 +7,7 @@
 // and the operation order it sees inside its reference block, so the result is bit-identical);
 // W2X_WALK_BLOCKS walks the reference's blocks literally.
 //
-// There is no CPU fallback anywhere in this file: without an sm_100 device every compute entry
+// There is no CPU fallback anywhere in this file: without an sm_90 device every compute entry
 // point fails with W2X_ERR_NO_DEVICE.
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -55,8 +55,6 @@ int get_dev_model(w2x_ctx *ctx, const w2x_model *m, DevModel **out) {
     dm.b.assign(n, nullptr);
     dm.pack.assign(n, nullptr);
     dm.pack8.assign(n, nullptr);
-    dm.strip.assign(n, nullptr);
-    dm.strip8.assign(n, nullptr);
     dm.out_scale.assign(n, 1.f);
     for (size_t i = 0; i < n; i++) {
         const Layer &L = m->layers[i];
@@ -75,12 +73,6 @@ int get_dev_model(w2x_ctx *ctx, const w2x_model *m, DevModel **out) {
             dm.out_scale[i] = 1.0f / (P.wscale * tc::ACT_SCALE);
             CU_CHECK(cudaMalloc(&dm.pack8[i], P.bytes8.size()));
             CU_CHECK(cudaMemcpyAsync(dm.pack8[i], P.bytes8.data(), P.bytes8.size(), cudaMemcpyHostToDevice, ctx->stream));
-            if (!P.strip.empty()) {
-                CU_CHECK(cudaMalloc(&dm.strip[i], P.strip.size()));
-                CU_CHECK(cudaMemcpyAsync(dm.strip[i], P.strip.data(), P.strip.size(), cudaMemcpyHostToDevice, ctx->stream));
-                CU_CHECK(cudaMalloc(&dm.strip8[i], P.strip8.size()));
-                CU_CHECK(cudaMemcpyAsync(dm.strip8[i], P.strip8.data(), P.strip8.size(), cudaMemcpyHostToDevice, ctx->stream));
-            }
         }
     }
     if (m->tc_eligible) {
@@ -149,7 +141,7 @@ int pick_engine(w2x_ctx *ctx, const w2x_model *m) {
     int e = ctx->engine;
     if (e == W2X_ENGINE_AUTO) e = m->tc_eligible ? W2X_ENGINE_TC : W2X_ENGINE_FP32;
     if (e == W2X_ENGINE_TC && !m->tc_eligible) {
-        fail(W2X_ERR_UNSUPPORTED, "tcgen05 engine needs a 1->{32,64,128}...->1 layer chain");
+        fail(W2X_ERR_UNSUPPORTED, "tensor-core engine needs a 1->{32,64,128}...->1 layer chain");
         return -1;
     }
     return e;
@@ -162,35 +154,21 @@ int ensure_tc(w2x_ctx *ctx) {
     return W2X_OK;
 }
 
-// Does layer li run on the row-strip kernel?  A property of the layer's shape and position only, never of the frame size,
-// so every tiling of a plane picks the same kernels.
-bool layer_is_strip(const w2x_ctx *ctx, const w2x_model *m, const DevModel *dm, int li) {
-    const int n = (int)m->layers.size();
-    if (li < 1 || li > n - 2 || !ctx->strip) return false;
-    const Layer &L = m->layers[(size_t)li];
-    const bool fused = ctx->fuse_last && n >= 3 && !dm->last_w_t.empty() && li == n - 2;
-    return !fused && tc::strip_supported(L.n_in, L.n_out) && dm->strip[(size_t)li] != nullptr;
-}
-
-// One tcgen05 layer `li` on frames of pw x ph: in -> out (or, fused with the last layer, -> per-pixel tap partials in `out`).
+// One tensor-core layer `li` on frames of pw x ph: in -> out (or, fused with the last layer, -> per-pixel tap partials in `out`).
 int launch_layer_tc(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int li, const __half *in, __half *out, int pw, int ph,
                     bool fused, bool profile, int out_y0, int out_rows) {
     if (out_rows < 0) { out_y0 = 0; out_rows = ph; }
     const Layer &L = m->layers[(size_t)li];
     const int f8 = ctx->precision == W2X_PRECISION_F16_F8X2 ? 1 : 0;
-    const bool strip = !fused && layer_is_strip(ctx, m, dm, li);
     {
         LayerTimer t(ctx, li);
         CU_CHECK(tc::launch_tc_layer(in, f8 ? (const void *)dm->pack8[(size_t)li] : (const void *)dm->pack[(size_t)li],
-                                     strip ? (f8 ? (const void *)dm->strip8[(size_t)li] : (const void *)dm->strip[(size_t)li]) : nullptr,
                                      dm->b_host[(size_t)li].data(), out, L.n_in, L.n_out, pw, ph, dm->out_scale[(size_t)li], f8,
                                      ctx->num_sms, ctx->stream,
                                      profile && ctx->prof_buf ? ctx->prof_buf + (size_t)li * tc::PROF_MAX_CTAS * tc::PROF_WORDS : nullptr,
-                                     fused ? dm->last_w_t.data() : nullptr, fused ? reinterpret_cast<float *>(out) : nullptr, ctx->pair,
-                                     out_y0, out_rows));
+                                     fused ? dm->last_w_t.data() : nullptr, fused ? reinterpret_cast<float *>(out) : nullptr, out_y0, out_rows));
     }
-    note_kernel(ctx, li, f8 ? (fused ? "tcgen05_f16+f8x2+last" : strip ? "tcgen05_f16+f8x2_strip" : "tcgen05_f16+f8x2")
-                            : (fused ? "tcgen05_f16x3+last" : strip ? "tcgen05_f16x3_strip" : "tcgen05_f16x3"));
+    note_kernel(ctx, li, f8 ? (fused ? "wgmma_f16+f8x2+last" : "wgmma_f16+f8x2") : (fused ? "wgmma_f16x3+last" : "wgmma_f16x3"));
     ctx->launches++;
     return W2X_OK;
 }
@@ -198,10 +176,10 @@ int launch_layer_tc(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int li, cons
 // ---- convertWithModelsBasic on an already padded ROI ------------------------------------------
 // src: pw x ph fp32 region (row stride src_stride floats) that already contains the n-pixel ring.
 // dst: receives the (pw-2n) x (ph-2n) interior.
-// n_tiles > 1 (tcgen05 engine with the fused last layer only): src holds n_tiles padded planes of pw x ph stacked vertically; the
+// n_tiles > 1 (tensor-core engine with the fused last layer only): src holds n_tiles padded planes of pw x ph stacked vertically; the
 // layers run ONCE on the (n_tiles * ph)-row frame -- the seams pollute only the rings that are cropped anyway -- and tile t's
 // interior goes to dst + t * (ph - 2n) * dst_stride.
-// direct (tcgen05 engine, one plane): the first layer reads the UNPADDED plane it describes and folds the replicate padding into
+// direct (tensor-core engine, one plane): the first layer reads the UNPADDED plane it describes and folds the replicate padding into
 // its loads; src / src_stride are then unused.
 int run_basic(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int engine, const float *src, long src_stride, int pw,
               int ph, float *dst, long dst_stride, int n_tiles = 1, const tc::FirstSource *direct = nullptr) {
@@ -236,7 +214,7 @@ int run_basic(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int engine, const 
         ctx->launches++;
         return W2X_OK;
     }
-    // ---- tcgen05 engine ----
+    // ---- tensor-core engine ----
     const int f8 = ctx->precision == W2X_PRECISION_F16_F8X2 ? 1 : 0;
     int rc = ensure_tc(ctx);
     if (rc) return rc;
@@ -286,7 +264,7 @@ int run_basic(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int engine, const 
 
 // Whole plane (or row band) already available as a padded plane: cut it into horizontal bands that
 // respect the scratch limit, each band re-reads n rows of context above and below.
-// direct_in != nullptr (tcgen05 engine): no padded plane exists; the first layer reads d_in (rows_above / rows_below real rows
+// direct_in != nullptr (tensor-core engine): no padded plane exists; the first layer reads d_in (rows_above / rows_below real rows
 // beyond the plane) with the padding folded into its loads.
 int run_padded_plane(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int engine, const float *padp, int w, int h,
                      float *dst, long dst_stride, const float *direct_in = nullptr, long in_stride = 0, int rows_above = 0, int rows_below = 0) {
@@ -394,8 +372,8 @@ int w2x_ctx_create(int device, w2x_ctx **out_ctx) {
     if (device < 0 || device >= count) return fail(W2X_ERR_ARG, "w2x_ctx_create: device %d out of range [0,%d)", device, count);
     cudaDeviceProp prop;
     CU_CHECK(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10)
-        return fail(W2X_ERR_NO_DEVICE, "device %d (%s) is sm_%d%d; this build carries sm_100a code only", device,
+    if (prop.major != 9 || prop.minor != 0)
+        return fail(W2X_ERR_NO_DEVICE, "device %d (%s) is sm_%d%d; this build carries sm_90a code only", device,
                     prop.name, prop.major, prop.minor);
     auto ctx = std::make_unique<w2x_ctx>();
     ctx->device = device;
@@ -424,8 +402,6 @@ static void free_dev_model(DevModel &dm) {
     for (auto p : dm.b) cudaFree(p);
     for (auto p : dm.pack) cudaFree(p);
     for (auto p : dm.pack8) cudaFree(p);
-    for (auto p : dm.strip) cudaFree(p);
-    for (auto p : dm.strip8) cudaFree(p);
 }
 
 // Drops the context's device copies of a model (weights, packed operands); call it before w2x_model_free in a long-lived
@@ -514,7 +490,7 @@ int w2x_ctx_set_scratch_limit(w2x_ctx *ctx, size_t bytes) {
     return W2X_OK;
 }
 
-// Probe hooks (not part of the stable ABI): per-role wait/work cycle counters of the tcgen05 layer kernels.
+// Probe hooks (not part of the stable ABI): per-role wait/work cycle counters of the tensor-core layer kernels.
 W2X_API int w2x_debug_tc_profile_enable(w2x_ctx *ctx, int on) {
     if (check_ctx(ctx)) return W2X_ERR_ARG;
     DeviceGuard g(ctx->device);
@@ -548,21 +524,7 @@ W2X_API int w2x_debug_tc_profile_read(w2x_ctx *ctx, int layer, unsigned long lon
     return W2X_OK;
 }
 
-// Probe switch (not part of the stable ABI): 1 = CTA-pair (cta_group::2) kernels for the 128-wide layers.
-W2X_API int w2x_debug_set_pair(w2x_ctx *ctx, int on) {
-    if (check_ctx(ctx)) return W2X_ERR_ARG;
-    ctx->pair = on != 0;
-    return W2X_OK;
-}
-
-// Probe switch (not part of the stable ABI): 1 = row-strip kernel for the narrow layers (default), 0 = the 16x16-tile kernel.
-W2X_API int w2x_debug_set_strip(w2x_ctx *ctx, int on) {
-    if (check_ctx(ctx)) return W2X_ERR_ARG;
-    ctx->strip = on != 0;
-    return W2X_OK;
-}
-
-// Probe switch (not part of the stable ABI): number of SMs the persistent tcgen05 kernels of this context occupy (0 = all).
+// Probe switch (not part of the stable ABI): number of SMs the persistent tensor-core kernels of this context occupy (0 = all).
 W2X_API int w2x_debug_set_num_sms(w2x_ctx *ctx, int n) {
     if (check_ctx(ctx)) return W2X_ERR_ARG;
     cudaDeviceProp prop;
@@ -578,7 +540,7 @@ W2X_API int w2x_debug_set_host_bands(w2x_ctx *ctx, int bands) {
     return W2X_OK;
 }
 
-// Probe switch (not part of the stable ABI): 1 = fold the last layer into the preceding tcgen05 layer (default), 0 = separate kernel.
+// Probe switch (not part of the stable ABI): 1 = fold the last layer into the preceding tensor-core layer (default), 0 = separate kernel.
 W2X_API int w2x_debug_set_fuse_last(w2x_ctx *ctx, int on) {
     if (check_ctx(ctx)) return W2X_ERR_ARG;
     ctx->fuse_last = on != 0;
@@ -681,11 +643,11 @@ int w2x_filter_layer_device(w2x_ctx *ctx, const w2x_model *model, int layer, con
     int engine = ctx->engine == W2X_ENGINE_AUTO ? W2X_ENGINE_FP32 : ctx->engine;
     if (engine == W2X_ENGINE_TC) {
         if (!tc::layer_supported(L.n_in, L.n_out))
-            return fail(W2X_ERR_UNSUPPORTED, "tcgen05 engine does not support a %d->%d layer", L.n_in, L.n_out);
+            return fail(W2X_ERR_UNSUPPORTED, "tensor-core engine does not support a %d->%d layer", L.n_in, L.n_out);
         rc = ensure_tc(ctx);
         if (rc) return rc;
         // Model::filter semantics (same size, BORDER_REPLICATE): stage a frame with a replicated ring
-        // of one pixel, run the same-size tcgen05 layer on it, return the interior.
+        // of one pixel, run the same-size tensor-core layer on it, return the interior.
         const int pw = width + 2, ph = height + 2;
         rc = ensure(&ctx->buf[0], &ctx->buf_bytes[0], tc::act_bytes(L.n_in, pw, ph));
         if (rc) return rc;

@@ -75,7 +75,7 @@ int w2x_band_create(w2x_ctx *ctx, const w2x_model *model, int width, int band_ro
     if (!model || !out_band || width < 1 || band_rows < 1) return fail(W2X_ERR_ARG, "w2x_band_create: bad argument");
     *out_band = nullptr;
     if (!model->tc_eligible || ctx->engine == W2X_ENGINE_FP32)
-        return fail(W2X_ERR_UNSUPPORTED, "w2x_band_create: the per-layer halo mode needs the tcgen05 engine and a 1->{32,64,128}..->1 model");
+        return fail(W2X_ERR_UNSUPPORTED, "w2x_band_create: the per-layer halo mode needs the tensor-core engine and a 1->{32,64,128}..->1 model");
     DeviceGuard g(ctx->device);
     int rc = ensure_tc(ctx);
     if (rc) return rc;

@@ -24,10 +24,9 @@ namespace eng {
 struct DevModel {                       // device-resident copy of one model
     std::vector<float *> w;             // per layer [Cout][Cin][9] fp32
     std::vector<float *> b;             // per layer [Cout] fp32  ((float)bias, src/modelHandler.cpp:147)
-    std::vector<std::vector<float>> b_host;   // the same on the host (the tcgen05 kernels take them as kernel parameters)
-    std::vector<uint16_t *> pack;       // per layer tcgen05 operand image (nullptr if not eligible)
+    std::vector<std::vector<float>> b_host;   // the same on the host (the tensor-core kernels take them as kernel parameters)
+    std::vector<uint16_t *> pack;       // per layer tensor-core operand image (nullptr if not eligible)
     std::vector<uint8_t *> pack8;       // same for the "f8" flavour (fp16 main product + e4m3 corrections)
-    std::vector<uint8_t *> strip, strip8;   // row-strip kernel images of the narrow layers (nullptr otherwise), both flavours
     std::vector<float> out_scale;       // 1 / (wscale * ACT_SCALE)
     std::vector<float> last_w_t;        // HOST: last layer's weights transposed to [9][Cin] (fused last layer, passed as kernel parameters)
 };
@@ -43,10 +42,8 @@ struct w2x_ctx {
     int cc_major = 0, cc_minor = 0;
     int engine = W2X_ENGINE_AUTO;
     int walk = W2X_WALK_FUSED;
-    bool fuse_last = true;             // fold the N->1 last layer into the preceding tcgen05 layer's epilogue
+    bool fuse_last = true;             // fold the N->1 last layer into the preceding tensor-core layer's epilogue
     int precision = W2X_PRECISION_F16_F8X2;   // default; W2X_PRECISION=f16x3 in the environment or w2x_ctx_set_precision() selects the 3 x fp16 scheme
-    int strip = 1;                     // 1 = run the narrow layers (Cin, Cout <= 64) on the row-strip kernel; w2x_debug_set_strip(0) = 16x16-tile kernel
-    int pair = 1;                      // 1 = run the 128-wide layers on CTA pairs (cta_group::2); w2x_debug_set_pair(0) = single-CTA kernels
     cudaStream_t own_stream = nullptr;
     cudaStream_t stream = nullptr;
     size_t scratch_limit = (size_t)16 << 30;
@@ -133,8 +130,7 @@ int ensure_tc(w2x_ctx *ctx);
 int check_ctx(w2x_ctx *ctx);
 int pick_engine(w2x_ctx *ctx, const w2x_model *m);
 void emit_reference_progress(w2x_ctx *ctx, int w, int h, int n_layers, bool split);   // the reference's stdout lines of one convertWithModels call
-bool layer_is_strip(const w2x_ctx *ctx, const w2x_model *m, const DevModel *dm, int li);   // does layer li run on the row-strip kernel?
-// One tcgen05 layer `li` on frames of pw x ph: in -> out (or, fused with the last layer, -> per-pixel tap partials in `out`).
+// One tensor-core layer `li` on frames of pw x ph: in -> out (or, fused with the last layer, -> per-pixel tap partials in `out`).
 // Only frame rows [out_y0, out_y0 + out_rows) are stored (out_rows < 0: the whole frame).
 int launch_layer_tc(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int li, const __half *in, __half *out, int pw, int ph,
                     bool fused, bool profile, int out_y0 = 0, int out_rows = -1);

@@ -61,24 +61,20 @@ struct FirstSource {
 };
 cudaError_t launch_first(const FirstSource &src, int pw, int ph, const float *wgt /*[C][9]*/, const float *bias, int cout, __half *out,
                          cudaStream_t s, int f8 = 0, int out_y0 = 0, int out_rows = -1);
-// tcgen05 layer: in/out NHWC frames (pw x ph); the tensor maps are built inside.
+// Tensor-core (wgmma) layer: in/out NHWC frames (pw x ph); the tensor maps are built inside.
 // `bias` is a HOST pointer to the layer's (float)bias values (they travel as kernel parameters).
-// f8 = 0: "f16x3" frames [hi][lo], wpack = TcPack::bytes, wstrip = TcPack::strip;
-// f8 = 1: frames [xh][xh8][xl8], wpack = TcPack::bytes8, wstrip = TcPack::strip8.
-// wstrip (device copy of the row-strip image, nullptr if the layer has none) selects the row-strip kernel for the
-// narrow layers (Cin, Cout <= 64, not fused); the choice depends on the layer shape only, never on the frame size.
-cudaError_t launch_tc_layer(const __half *in, const void *wpack, const void *wstrip, const float *bias, __half *out,
+// f8 = 0: "f16x3" frames [hi][lo], wpack = TcPack::bytes;  f8 = 1: frames [xh][xh8][xl8], wpack = TcPack::bytes8.
+cudaError_t launch_tc_layer(const __half *in, const void *wpack, const float *bias, __half *out,
                             int cin, int cout, int pw, int ph, float out_scale, int f8, int num_sms,
                             cudaStream_t s, unsigned long long *prof = nullptr, const float *last_w = nullptr,
-                            float *partial = nullptr, int pair = 0, int out_y0 = 0, int out_rows = -1);
+                            float *partial = nullptr, int out_y0 = 0, int out_rows = -1);
 // Frames: every activation between layers is a RECORD frame [Hp][Wp][C/32][128 B] -- one 128-byte record per pixel per
 // 32-channel block = {xh fp16 x32 | xh8 e4m3 x32 | xl8 e4m3 x32} (f8) or {hi fp16 x32 | lo fp16 x32} (f16x3): 4 bytes per
 // element, one TMA box row per record (SWIZZLE_128B).
 // out_y0 / out_rows (both launchers): only frame rows [out_y0, out_y0 + out_rows) are stored (-1 = the whole frame); a
 // row-band session keeps its halo rows out of the window because its neighbours write them.
-bool strip_supported(int cin, int cout);
 // Fused last layer: launch_tc_layer(..., last_w = HOST pointer to [9][cout] fp32 tap-major, partial = [ph][pw][12] fp32) makes the
-// tcgen05 layer emit per-pixel tap partials instead of activations; launch_last_gather sums the 3x3
+// tensor-core layer emit per-pixel tap partials instead of activations; launch_last_gather sums the 3x3
 // neighbourhood of partials, adds the bias, applies the leaky-ReLU and writes the cropped fp32 plane.
 cudaError_t launch_last_gather(const float *partial, int pw, int ph, float bias, int crop, float *dst,
                                long dst_stride_floats, cudaStream_t s);

@@ -1,15 +1,15 @@
-// kernels_tc.cu -- the tcgen05 engine (W2X_ENGINE_TC): sm_100a only.
+// kernels_tc.cu -- the tensor-core engine (W2X_ENGINE_TC): sm_90a (Hopper wgmma + TMA).
 //
 // What it computes (reference src/modelHandler.cpp:134-152 for all output planes of a layer at
 // once): out[o](y,x) = leaky( sum_i sum_{ky,kx} W[o][i][ky][kx] * in[i](y+ky-1, x+kx-1) + bias[o] ).
 //
-// How: implicit GEMM, D[pixel][o] += A[pixel][(tap,i)] * B[(tap,i)][o], on the 5th-generation
-// tensor cores (tcgen05.mma, fp32 accumulators in TMEM).  fp32 fidelity comes from a 2-term split of
+// How: implicit GEMM, D[pixel][o] += A[pixel][(tap,i)] * B[(tap,i)][o], on the Hopper tensor cores
+// (wgmma.mma_async, fp32 accumulators in registers).  fp32 fidelity comes from a 2-term split of
 // both operands (x = xh + xl, w = wh + wl, h = the fp16 rounding) and three accumulated products
 // xh*wh + xl*wh + xh*wl (the dropped xl*wl term is ~2^-22 relative); SURVEY.md section 7 shows a
 // single fp16/tf32 pass misses the 1e-4 gate by 10x.  Two arithmetic modes (template flag F8):
-//   f16x3      all three products as kind::f16 MMAs on fp16 hi/lo planes
-//   f16+f8x2   xh*wh as kind::f16; the two correction products as kind::f8f6f4 MMAs on e4m3 copies of the
+//   f16x3      all three products as f16 wgmmas on fp16 hi/lo planes
+//   f16+f8x2   xh*wh as f16; the two correction products as e4m3 wgmmas on e4m3 copies of the
 //              operands (K = 32 per instruction, twice the rate) -- the default, 2.0 instead of 3.0 passes
 //
 // Data layout in HBM: every activation is an NHWC "frame" of 4 bytes per element holding value*ACT_SCALE,
@@ -19,17 +19,15 @@
 // same argument that makes the reference's per-layer BORDER_REPLICATE harmless (SURVEY.md section 8a).
 //
 // Per CTA (persistent, 1 per SM, 12 warps):
-//   warp 0      A producer   one TMA box {KC ch, 18, 18} per (tile-set, channel chunk, plane): the
-//                            16x16 output region plus a 1-pixel ring, staged ONCE and addressed nine
-//                            times (the 3x3 taps are UMMA-descriptor start-address offsets into it)
-//   warps 1, 7  MMA issuers  one per M-tile (8 wide x 16 tall pixels): tcgen05.mma, M=128 (M=256 across a CTA
-//                            pair for the 128-wide layers), N=Cout, K=16 (fp16) / 32 (e4m3) per instruction;
-//                            operands provably warp-uniform, so the MMAs issue back to back from uniform registers
-//   warp 2      B producer   pre-swizzled 32-channel weight stages: a cp.async.bulk ring, or resident for the
-//                            narrow layers; owns TMEM
-//   warps 3-6, 8-11 epilogue one set per M-tile: tcgen05.ld -> scale, +bias, leaky-ReLU -> either the frame's
-//                            planes, staged in the TMA swizzle pattern and TMA-stored, or (FUSE) the last
-//                            layer's nine tap partials; overlaps the next tile-set (TMEM double buffer)
+//   warp 0      A producer   one TMA box {KC ch, 18, 18} per (tile-set, channel chunk): the 16x16 output
+//                            region plus a 1-pixel ring, staged ONCE and addressed nine times (the 3x3 taps
+//                            are wgmma-descriptor start-address offsets into it)
+//   warp 1      B producer   pre-swizzled (32-channel, tap) weight stages: a cp.async.bulk ring, or resident
+//                            for the narrow layers
+//   warps 4-11  consumers    two warpgroups, one per M-tile (8 wide x 16 tall pixels = two m64 wgmmas), N = Cout,
+//                            K = 16 (fp16) / 32 (e4m3) per instruction; each drains its own accumulators: scale,
+//                            +bias, leaky-ReLU -> either the frame's records, staged in the TMA swizzle pattern and
+//                            TMA-stored, or (FUSE) the last layer's nine tap partials
 //
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -46,12 +44,9 @@ namespace w2x {
 namespace tc {
 
 #include "tc_ptx.cuh"
+#include "tc_wgmma.cuh"
 #include "tc_config.cuh"
-#include "tc_issue.cuh"
-#include "tc_epilogue.cuh"
 #include "tc_kernel.cuh"
-#include "tc_pair_kernel.cuh"
-#include "tc_strip_kernel.cuh"
 #include "tc_edge_kernels.cuh"
 
 // ================================================================================================
@@ -87,32 +82,11 @@ size_t layer_smem_bytes(int cin, int cout) {
     return 0;
 }
 
-template <int CIN, bool FUSE, bool F8>
-static cudaError_t set_attr_pair() {
-    return cudaFuncSetAttribute(tc_conv3x3_pair_kernel<CIN, 128, FUSE, F8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                PairCfg<CIN, 128, FUSE, F8>::SMEM_BYTES);
-}
-#define W2X_PAIR_CINS(X) X(32) X(64) X(128)
-
 cudaError_t init_kernels() {
     cudaError_t e;
-#define X(ci)                                                            \
-    if ((e = set_attr_pair<ci, false, false>()) != cudaSuccess) return e; \
-    if ((e = set_attr_pair<ci, true, false>()) != cudaSuccess) return e;  \
-    if ((e = set_attr_pair<ci, false, true>()) != cudaSuccess) return e;  \
-    if ((e = set_attr_pair<ci, true, true>()) != cudaSuccess) return e;
-    W2X_PAIR_CINS(X)
-#undef X
 #define X(ci, co) \
     if ((e = set_attr<ci, co>()) != cudaSuccess) return e;
     W2X_TC_SHAPES(X)
-#undef X
-#define X(ci, co)                                                                                                                          \
-    if ((e = cudaFuncSetAttribute(tc_conv3x3_strip_kernel<ci, co, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,                    \
-                                  StripCfg<ci, co, false>::SMEM_BYTES)) != cudaSuccess) return e;                                           \
-    if ((e = cudaFuncSetAttribute(tc_conv3x3_strip_kernel<ci, co, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,                     \
-                                  StripCfg<ci, co, true>::SMEM_BYTES)) != cudaSuccess) return e;
-    X(32, 32) X(32, 64) X(64, 32) X(64, 64)
 #undef X
     return cudaSuccess;
 }
@@ -130,87 +104,12 @@ static cudaError_t launch_one(const CUtensorMap *tmap, const CUtensorMap *omap, 
     return p.partial ? launch_k<CIN, COUT, true, false>(tmap, omap, p, grid, s) : launch_k<CIN, COUT, false, false>(tmap, omap, p, grid, s);
 }
 
-static int make_weight_stream_map(CUtensorMap *map, const void *base, size_t bytes);
 static int make_rec_map(CUtensorMap *map, const void *base, int C, int Wp, int Hp, int box_w, int box_h, int y0, int rows);
 
-template <int CIN, bool FUSE, bool F8>
-static cudaError_t launch_pair_k(const CUtensorMap *tmap, const CUtensorMap *tmapw, const CUtensorMap *omap, const TcParams &p, int grid, cudaStream_t s) {
-    tc_conv3x3_pair_kernel<CIN, 128, FUSE, F8><<<grid, NUM_THREADS, PairCfg<CIN, 128, FUSE, F8>::SMEM_BYTES, s>>>(*tmap, *tmapw, *omap, p);
-    return cudaGetLastError();
-}
-
-template <int CIN>
-static cudaError_t launch_pair(const CUtensorMap *tmap, const CUtensorMap *omap, const TcParams &p, int num_sms, bool f8, cudaStream_t s) {
-    using C0 = Cfg<CIN, 128, false, false>;
-    const size_t bytes = (size_t)C0::NCHUNK * 9 * 2 * C0::B_BLOCK;   // both flavours stream the same number of bytes per tile-set
-    CUtensorMap tmapw;
-    if (make_weight_stream_map(&tmapw, p.wpack, bytes)) return cudaErrorInvalidValue;
-    const int n_pair_sets = (p.n_tilesets + 1) / 2;
-    int grid = 2 * (n_pair_sets < num_sms / 2 ? n_pair_sets : num_sms / 2);
-    if (f8) return p.partial ? launch_pair_k<CIN, true, true>(tmap, &tmapw, omap, p, grid, s) : launch_pair_k<CIN, false, true>(tmap, &tmapw, omap, p, grid, s);
-    return p.partial ? launch_pair_k<CIN, true, false>(tmap, &tmapw, omap, p, grid, s) : launch_pair_k<CIN, false, false>(tmap, &tmapw, omap, p, grid, s);
-}
-
-// ---- row-strip kernel (narrow layers) ----
-bool strip_supported(int cin, int cout) { return (cin == 32 || cin == 64) && (cout == 32 || cout == 64); }
-
-static int strip_seg_rows() {   // rows per work unit (tuning knob: W2X_STRIP_ROWS)
-    static const int v = [] {
-        const char *e = std::getenv("W2X_STRIP_ROWS");
-        const int n = e ? std::atoi(e) : 0;
-        return n >= 2 && n <= 4096 ? n : 32;
-    }();
-    return v;
-}
-
-template <int CIN, int COUT, bool F8>
-static cudaError_t launch_strip_k(const CUtensorMap *maps, const StripParams &p, int num_sms, cudaStream_t s) {
-    using C = StripCfg<CIN, COUT, F8>;
-    const int grid = p.n_units < num_sms ? p.n_units : num_sms;
-    tc_conv3x3_strip_kernel<CIN, COUT, F8><<<grid, C::THREADS, C::SMEM_BYTES, s>>>(maps[0], maps[1], p);
-    return cudaGetLastError();
-}
-
-#define W2X_STRIP_SHAPES(X) X(32, 32) X(32, 64) X(64, 32) X(64, 64)
-
-static cudaError_t launch_strip(const __half *in, const void *wstrip, const float *bias, __half *out, int cin, int cout, int pw, int ph,
-                                float out_scale, int f8, int num_sms, cudaStream_t s, unsigned long long *prof, int out_y0, int out_rows) {
-    StripParams p;
-    p.wpack = reinterpret_cast<const uint8_t *>(wstrip);
-    for (int i = 0; i < cout; i++) p.bias[i] = bias[i] * ACT_SCALE;
-    p.Wp = pw;
-    p.Hp = ph;
-    p.out_y0 = out_y0;
-    p.out_rows = out_rows;
-    p.seg_rows = strip_seg_rows();
-    p.ncols = (pw + STRIP_W - 1) / STRIP_W;
-    p.n_units = p.ncols * ((ph + p.seg_rows - 1) / p.seg_rows);
-    p.out_scale = out_scale * ACT_SCALE;
-    p.prof = prof;
-    p.out_win = reinterpret_cast<uint8_t *>(out) + (size_t)out_y0 * pw * cout * 4;
-#ifdef W2X_EPI_EXPERIMENTS
-    static const int dbg_strip = std::getenv("W2X_DEBUG_STRIP") ? std::atoi(std::getenv("W2X_DEBUG_STRIP")) : 0;
-    p.dbg = dbg_strip;
-#else
-    p.dbg = 0;
-#endif
-    CUtensorMap maps[2];   // in | out
-    if (make_rec_map(&maps[0], in, cin, pw, ph, STRIP_BOXW, 1, 0, ph)) return cudaErrorInvalidValue;
-    if (make_rec_map(&maps[1], out, cout, pw, ph, 32, 1, out_y0, out_rows)) return cudaErrorInvalidValue;
-#define X(ci, co)                                                                                       \
-    if (cin == ci && cout == co)                                                                        \
-        return f8 ? launch_strip_k<ci, co, true>(maps, p, num_sms, s) : launch_strip_k<ci, co, false>(maps, p, num_sms, s);
-    W2X_STRIP_SHAPES(X)
-#undef X
-    return cudaErrorInvalidValue;
-}
-
-cudaError_t launch_tc_layer(const __half *in, const void *wpack, const void *wstrip, const float *bias, __half *out, int cin,
+cudaError_t launch_tc_layer(const __half *in, const void *wpack, const float *bias, __half *out, int cin,
                             int cout, int pw, int ph, float out_scale, int f8, int num_sms, cudaStream_t s,
-                            unsigned long long *prof, const float *last_w, float *partial, int pair, int out_y0, int out_rows) {
+                            unsigned long long *prof, const float *last_w, float *partial, int out_y0, int out_rows) {
     if (out_rows < 0) { out_y0 = 0; out_rows = ph; }
-    if (wstrip && !partial && strip_supported(cin, cout))
-        return launch_strip(in, wstrip, bias, out, cin, cout, pw, ph, out_scale, f8, num_sms, s, prof, out_y0, out_rows);
     CUtensorMap tmap_in;
     if (make_rec_map(&tmap_in, in, cin, pw, ph, HALO, HALO, 0, ph)) return cudaErrorInvalidValue;
     TcParams p;
@@ -218,7 +117,6 @@ cudaError_t launch_tc_layer(const __half *in, const void *wpack, const void *wst
     // ACT_SCALE (a power of two) is folded into the epilogue's affine step: leaky(16 v) = 16 leaky(v) exactly, so the
     // kernel produces the frame's x16 values without a separate multiply; the fused last layer gets weights / 16.
     for (int i = 0; i < cout; i++) p.bias[i] = bias[i] * ACT_SCALE;      // HOST pointer
-    p.out = out;
     p.Wp = pw;
     p.Hp = ph;
     p.out_y0 = out_y0;
@@ -227,27 +125,15 @@ cudaError_t launch_tc_layer(const __half *in, const void *wpack, const void *wst
     p.n_tilesets = p.tiles_x * ((out_rows + REGION - 1) / REGION);   // tile-sets tile the store window (TMA store coordinates stay non-negative)
     p.out_scale = out_scale * ACT_SCALE;
     p.prof = prof;
-#ifdef W2X_EPI_EXPERIMENTS   // timing experiments only (results are wrong): build with -DW2X_EPI_EXPERIMENTS, then W2X_DEBUG_EPI=1|2
-    static const int dbg_epi = std::getenv("W2X_DEBUG_EPI") ? std::atoi(std::getenv("W2X_DEBUG_EPI")) : 0;
-    p.dbg = dbg_epi;
-#else
-    p.dbg = 0;
-#endif
     p.partial = partial;
     if (partial) {
         if (!last_w) return cudaErrorInvalidValue;
         for (int i = 0; i < 9 * cout; i++) p.last_w[i] = last_w[i] * (1.0f / ACT_SCALE);      // HOST pointer: [9][cout]
     }
-    // the epilogue's TMA stores: 8x4-pixel boxes of records of this layer's output frame (fused layers store no frame)
+    // the epilogue's TMA stores: one 8x16-pixel box of records (an M-tile) per 32-channel block (fused layers store no frame)
     CUtensorMap omap;
     if (partial) omap = tmap_in;
-    else if (make_rec_map(&omap, out, cout, pw, ph, 8, 4, out_y0, out_rows)) return cudaErrorInvalidValue;
-    if (pair && cout == 128 && num_sms >= 2) {
-#define X(ci) \
-    if (cin == ci) return launch_pair<ci>(&tmap_in, &omap, p, num_sms, f8 != 0, s);
-        W2X_PAIR_CINS(X)
-#undef X
-    }
+    else if (make_rec_map(&omap, out, cout, pw, ph, 8, 16, out_y0, out_rows)) return cudaErrorInvalidValue;
 #define X(ci, co) \
     if (cin == ci && cout == co) return launch_one<ci, co>(&tmap_in, &omap, p, num_sms, f8 != 0, s);
     W2X_TC_SHAPES(X)
@@ -348,23 +234,7 @@ static PFN_encodeTiled get_encode() {
     return fn;
 }
 
-// The packed weight stream as rows of 1 KB (256 x 32-bit words), box = 2 rows (2 KB), no swizzle: the CTA-pair kernel's
-// B loads.  (Long rows matter: the TMA unit issues one request per box row, and 64-byte rows made the weight ring
-// request-bound.)
-static int make_weight_stream_map(CUtensorMap *map, const void *base, size_t bytes) {
-    PFN_encodeTiled enc = get_encode();
-    if (!enc || bytes % 2048) return -1;
-    cuuint64_t dims[2] = {256, (cuuint64_t)(bytes / 1024)};
-    cuuint64_t strides[1] = {1024};
-    cuuint32_t box[2] = {256, 2};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_INT32, 2, const_cast<void *>(base), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    return r == CUDA_SUCCESS ? 0 : (int)r;
-}
-
-// RECORD frame [Hp][Wp][C/32][128 B] (tc_epilogue.cuh) as a byte tensor {128, C/32, Wp, rows}, box {128, 1, box_w, box_h},
+// RECORD frame [Hp][Wp][C/32][128 B] (kernels.h) as a byte tensor {128, C/32, Wp, rows}, box {128, 1, box_w, box_h},
 // SWIZZLE_128B; only frame rows [y0, y0 + rows) are part of the map (row coordinate 0 = frame row y0).
 static int make_rec_map(CUtensorMap *map, const void *base, int C, int Wp, int Hp, int box_w, int box_h, int y0, int rows) {
     PFN_encodeTiled enc = get_encode();

@@ -342,7 +342,7 @@ int parse_model_json(const char *path, w2x_model **out) {
     return W2X_OK;
 }
 
-// ---- tcgen05 operand packing ------------------------------------------------------------------
+// ---- tensor-core operand packing ------------------------------------------------------------------
 // Shared-memory image of one B block: n_out rows (one per output plane) of 32 fp16 values, K-major.
 // Byte address of element (n, k) before swizzling: n*64 + 2k; the 16-byte unit index is then XORed
 // with address bits [7,9) -- CUTLASS Swizzle<2,4,3>, the SWIZZLE_64B pattern of TMA / UMMA descriptors.
@@ -416,7 +416,8 @@ static void pack_tc_layer_f8(const Layer &L, TcPack &P) {
             }
 }
 
-// Operand images of the row-strip kernel (csrc/tc_strip_kernel.cuh; narrow layers, Cin and Cout <= 64): per
+// Operand images of the row-strip design (narrow layers, Cin and Cout <= 64; no kernel of this build reads them, the
+// 16x16-tile kernel runs every layer; tests/test_strip_kernel_model.py checks them against the weights): per
 // (32-channel chunk c, tap column kx) ONE stage whose rows are ky-major, row = ky * n_out + n, so that an N = 3*n_out MMA
 // multiplies one staged input row by the three taps W(ky = 0..2, kx) at once:
 //   strip   (f16x3): [wh: 3*n_out rows x 64 B, SWIZZLE_64B][wl: same]
@@ -462,7 +463,7 @@ int finalize_model(w2x_model *m) {
             return fail(W2X_ERR_MODEL, "Error : model layer %zu : nInputPlane %d does not match previous nOutputPlane %d",
                         i, L.n_in, m->layers[i - 1].n_out);
     }
-    // tcgen05 eligibility: 1 -> C1 -> ... -> Cn -> 1 with every inner width in {32, 64, 128}
+    // tensor-core eligibility: 1 -> C1 -> ... -> Cn -> 1 with every inner width in {32, 64, 128}
     auto okc = [](int c) { return c == 32 || c == 64 || c == 128; };
     size_t n = m->layers.size();
     bool ok = n >= 3 && m->layers.front().n_in == 1 && m->layers.back().n_out == 1 &&
@@ -475,7 +476,6 @@ int finalize_model(w2x_model *m) {
         if (okc(L.n_in) && okc(L.n_out)) {
             pack_tc_layer(L, m->tc[i]);
             pack_tc_layer_f8(L, m->tc[i]);
-            pack_tc_layer_strip(L, m->tc[i]);
         }
     }
     m->uid = g_uid.fetch_add(1);
@@ -552,7 +552,7 @@ int w2x_model_layer_params(const w2x_model *model, int layer, const float **weig
     return W2X_OK;
 }
 
-// Probe hook (not part of the stable ABI): the tcgen05 operand image of one layer, for the packing tests.
+// Probe hook (not part of the stable ABI): the tensor-core operand image of one layer, for the packing tests.
 W2X_API int w2x_debug_tc_pack(const w2x_model *model, int layer, const uint16_t **data, size_t *n_elems, int *kc,
                               int *n_chunk, float *wscale, int *kblocks) {
     if (!model || layer < 0 || layer >= (int)model->tc.size())
@@ -567,11 +567,14 @@ W2X_API int w2x_debug_tc_pack(const w2x_model *model, int layer, const uint16_t 
     return W2X_OK;
 }
 
-// f8 = 0: TcPack::strip ([wh | wl]), f8 = 1: TcPack::strip8 ([wh | wh8 | wl8]); empty for layers the row-strip kernel does not run.
+// f8 = 0: TcPack::strip ([wh | wl]), f8 = 1: TcPack::strip8 ([wh | wh8 | wl8]); empty for layers outside the row-strip design.
 W2X_API int w2x_debug_tc_strip(const w2x_model *model, int layer, int f8, const uint8_t **data, size_t *n_bytes) {
     if (!model || layer < 0 || layer >= (int)model->tc.size())
         return w2x::fail(W2X_ERR_ARG, "w2x_debug_tc_strip: bad model or layer index");
-    const std::vector<uint8_t> &v = f8 ? model->tc[(size_t)layer].strip8 : model->tc[(size_t)layer].strip;
+    // packed on the first request: no kernel reads these images, so loading a model does not build them
+    w2x::TcPack &P = const_cast<w2x::TcPack &>(model->tc[(size_t)layer]);
+    if (P.strip.empty() && !P.bytes.empty()) pack_tc_layer_strip(model->layers[(size_t)layer], P);
+    const std::vector<uint8_t> &v = f8 ? P.strip8 : P.strip;
     if (data) *data = v.data();
     if (n_bytes) *n_bytes = v.size();
     return W2X_OK;

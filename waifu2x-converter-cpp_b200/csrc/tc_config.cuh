@@ -1,6 +1,6 @@
-// tc_config.cuh -- per-layer compile-time configuration (shared-memory map, stages, TMEM columns), kernel parameters, profile record
-// Part of the tcgen05 engine's single translation unit: included by kernels_tc.cu inside namespace w2x::tc, in this order:
-//   tc_ptx.cuh, tc_config.cuh, tc_issue.cuh, tc_epilogue.cuh, tc_kernel.cuh, tc_pair_kernel.cuh, tc_strip_kernel.cuh, tc_edge_kernels.cuh
+// tc_config.cuh -- per-layer compile-time configuration (shared-memory map, stages), kernel parameters, profile record
+// Part of the tensor-core engine's single translation unit: included by kernels_tc.cu inside namespace w2x::tc, in this order:
+//   tc_ptx.cuh, tc_wgmma.cuh, tc_config.cuh, tc_kernel.cuh, tc_edge_kernels.cuh
 // (pure code organisation: the generated SASS is the same as with one file).
 
 // ================================================================================================
@@ -11,9 +11,9 @@
 // region of ONE 32-channel block: 324 rows of 128 B, SWIZZLE_128B; the fp16 K steps / xh8 / xl8 (or lo) slices of a pixel
 // are the 32-byte quarters of its row (+0, +2, +4, +6 sixteen-byte units in the descriptor start address).
 //
-// F8 = false: three kind::f16 products xh*wh + xl*wh + xh*wl ("f16x3").
-// F8 = true : xh*wh in kind::f16, the two correction products in kind::f8f6f4 on e4m3 copies
-//             xl8*wh8 + xh8*wl8 (K = 32 per MMA at twice the rate: 2.0 instead of 3.0 pass-equivalents).
+// F8 = false: three f16 products xh*wh + xl*wh + xh*wl ("f16x3").
+// F8 = true : xh*wh in f16, the two correction products in e4m3 on e4m3 copies
+//             xl8*wh8 + xh8*wl8 (K = 32 per wgmma at twice the rate: 2.0 instead of 3.0 pass-equivalents).
 constexpr int F8_A = 10, F8_C = 1;   // xl8 = e4m3((x16 - xh) * 2^F8_A), xh8 = e4m3(xh * 2^-F8_C); must match w2x_internal.h
 
 template <int CIN, int COUT, bool FUSE = false, bool F8 = false>
@@ -22,66 +22,49 @@ struct Cfg {
     static constexpr int KC = 32;                       // channels per activation chunk
     static constexpr int NCHUNK = CIN / KC;
     static constexpr int ROWB = 128;                    // bytes per pixel per chunk (one record = the swizzle span)
-    static constexpr uint32_t A_LAYOUT = 2u;            // SWIZZLE_128B
     static constexpr int A_TX = HALO * HALO * ROWB;     // bytes the TMA load of one slot delivers
     static constexpr int A_SLOT = (A_TX + 1023) / 1024 * 1024;
     static constexpr int A_SLOTS = 2;
-    // ---- B operand (weights): stages of 32 input channels (two K=16 steps), SWIZZLE_64B rows of 64 B ----
-    static constexpr int KB = 32;
-    static constexpr int KBLOCKS = 1;                   // weight stages per (chunk, tap, part)
-    static constexpr int B_ROWB = KB * 2;
-    static constexpr uint32_t B_LAYOUT = 4u;
-    // Cout <= 64: hi and lo weights form ONE stage of 2*Cout rows, so xh*[wh;wl] is a single N = 2*Cout MMA
-    // (accumulators D1 | D2 side by side, summed in the epilogue) -- two MMAs per K step instead of three.
-    static constexpr bool STACK = COUT <= 64 && !F8;
-    static constexpr int B_BLOCK = COUT * B_ROWB;                            // one (chunk, tap, hi|lo) block
-    // F8: per 32-channel block ONE stage [wh fp16 (Cout x 64 B) | wh8 | wl8 (e4m3, Cout x 32 B each)]: four MMAs per
-    // issuer per barrier round trip.
-    static constexpr bool MERGE = F8;
-    static constexpr int B_STAGE = (STACK || MERGE) ? 2 * B_BLOCK : B_BLOCK;
-    static constexpr int STAGES_PER_TILESET = NCHUNK * 9 * ((STACK || MERGE) ? 1 : 2);
-    // ---- accumulators ----
-    static constexpr int TILE_COLS = STACK ? 2 * COUT : COUT;                // TMEM columns per M-tile
-    static constexpr int ACC_COLS = 4 * TILE_COLS;                           // 2 sets x 2 M-tiles
-    static constexpr int TMEM_COLS = ACC_COLS <= 32 ? 32 : ACC_COLS <= 64 ? 64 : ACC_COLS <= 128 ? 128 : ACC_COLS <= 256 ? 256 : 512;
-    // ---- shared memory map: [A slots][B stages][barriers (1 KB)][store staging] ----
+    // ---- B operand (weights): one stage per (32-channel block, tap), rows of 64 B (fp16, SWIZZLE_64B) ----
+    //   f16x3: [wh (Cout rows) | wl (Cout rows)]        F8: [wh (Cout rows of 64 B) | wh8 | wl8 (Cout rows of 32 B, SWIZZLE_32B)]
+    static constexpr int B_ROWB = KC * 2;
+    static constexpr int B_BLOCK = COUT * B_ROWB;
+    static constexpr int B_STAGE = 2 * B_BLOCK;
+    static constexpr int STAGES_PER_TILESET = NCHUNK * 9;
+    // ---- shared memory map: [A slots][B stages][store staging][barriers (1 KB)][bias | last-layer weights] ----
     static constexpr int BAR_BYTES = 1024;
-    static constexpr int W6_BYTES = 0;                                       // (the fused last layer's weights travel as kernel parameters)
-    static constexpr int STG_WARP = 4096;                                    // one record tile: 32 px x 128 B
-    static constexpr int STG_BYTES = FUSE ? 0 : 8 * STG_WARP;               // epilogue store staging per epilogue warp
+    static constexpr int PRM_BYTES = 4 * COUT * (FUSE ? 10 : 1);             // the epilogue indexes them per lane: shared, not parameter space
+    static constexpr int STG_WG = 128 * 128;                                 // one 32-channel record block of an M-tile (128 px)
+    static constexpr int STG_BYTES = FUSE ? 0 : 2 * STG_WG;
     static constexpr int SMEM_MAX = 227 * 1024;
-    static constexpr int NB_FIT = (SMEM_MAX - 1024 - BAR_BYTES - W6_BYTES - STG_BYTES - A_SLOTS * A_SLOT) / B_STAGE;
+    static constexpr int NB_FIT = (SMEM_MAX - 1024 - BAR_BYTES - PRM_BYTES - STG_BYTES - A_SLOTS * A_SLOT) / B_STAGE;
     // Narrow layers: ALL weight stages of a tile-set fit -> loaded once per CTA and kept (no ring traffic, no stage barriers
-    // after the first tile-set; the TMA unit is left to the activation boxes and the epilogue's stores).
+    // after the first tile-set).
     static constexpr bool RESIDENT = STAGES_PER_TILESET <= NB_FIT && STAGES_PER_TILESET <= 24;
     static constexpr int NB = RESIDENT ? STAGES_PER_TILESET : (NB_FIT > 8 ? 8 : NB_FIT);
-    static constexpr int SMEM_BYTES = 1024 + A_SLOTS * A_SLOT + NB * B_STAGE + BAR_BYTES + W6_BYTES + STG_BYTES;
+    static constexpr int SMEM_BYTES = 1024 + A_SLOTS * A_SLOT + NB * B_STAGE + STG_BYTES + BAR_BYTES + PRM_BYTES;
     static_assert(NB >= 3, "need at least three weight stages");
-    static_assert((8 + 2 * NB) * 8 + 4 <= 512 && COUT * 4 <= 512, "barrier/bias area overflow");
-    static_assert(ACC_COLS <= 512, "accumulators exceed TMEM");
+    static_assert((4 + 2 * NB) * 8 <= BAR_BYTES, "barrier area overflow");
+    static_assert(SMEM_BYTES <= SMEM_MAX, "shared memory");
     static_assert(B_STAGE % 1024 == 0 && A_SLOT % 1024 == 0, "swizzle pattern alignment");
-    static_assert(CIN % KC == 0 && COUT % 16 == 0 && COUT <= 128, "shape");
+    static_assert(CIN % KC == 0 && COUT % 32 == 0 && COUT <= 128, "shape");
 };
 
-// warps: 0 A producer | 1, 7 MMA issuers (M-tile 0, 1) | 2 B producer + TMEM owner | 3-6 epilogue of M-tile 0 | 8-11 epilogue of M-tile 1
+// warps: 0 A producer | 1 B producer | 2, 3 idle | 4-7 consumer warpgroup of M-tile 0 | 8-11 consumer warpgroup of M-tile 1
 constexpr int NUM_THREADS = 12 * 32;
 
 struct TcParams {
-    const uint16_t *wpack;   // [chunk][tap][kblock][hi|lo][COUT rows x 64 B], pre-swizzled (see model.cpp)
-    float bias[128];         // [COUT] (float)bias, by value (constant bank, see last_w)
-    __half *out;             // [2][Hp][Wp][COUT]
+    const uint16_t *wpack;   // [chunk][tap] stages (see Cfg::B_STAGE), pre-swizzled (see model.cpp)
+    float bias[128];         // [COUT] (float)bias * ACT_SCALE, by value
     int Wp, Hp;
     int out_y0, out_rows;    // only frame rows [out_y0, out_y0 + out_rows) are stored (row-band sessions keep the halo rows their neighbours write)
     int tiles_x, n_tilesets;
     float out_scale;         // 1 / wscale  (accumulator -> ACT_SCALE * conv)
     unsigned long long *prof;   // optional [gridDim.x][16] cycle counters (see PROF_* below), nullptr = off
-    int dbg;                    // always 0 in product builds; -DW2X_EPI_EXPERIMENTS + W2X_DEBUG_EPI: 1 = no global stores, 2 = no staging either (timing only, results WRONG)
     // fused last layer (FUSE kernels only): this layer's activations never reach HBM; instead each pixel's
     // nine tap partials P[t] = sum_c act[c] * w_last[c][t] are written ([Hp][Wp][12] fp32, 3 pad words).
     float *partial;             // nullptr = not fused
-    float last_w[9 * 128];      // [9][COUT] tap-major, by value: the epilogue's FFMAs read them straight from the constant
-                                // bank (kernel parameters), which keeps 288 broadcast LDS.128 per pixel off the shared-memory
-                                // pipe the tensor core's operand fetches saturate
+    float last_w[9 * 128];      // [9][COUT] tap-major, by value
 };
 
 // per-CTA profile record (cycles, accumulated over launches)
@@ -97,18 +80,3 @@ __device__ __forceinline__ void mbar_wait_prof(uint32_t bar, uint32_t parity, bo
         mbar_wait(bar, parity);
     }
 }
-
-template <int CIN, int COUT, bool FUSE, bool F8>
-struct PairCfg : Cfg<CIN, COUT, FUSE, F8> {
-    using Base = Cfg<CIN, COUT, FUSE, F8>;
-    static_assert(COUT == 128, "the CTA-pair kernel is built for the 128-wide layers");
-    static constexpr int A_SLOTS = FUSE ? 3 : 2;                          // (a fused layer has no store staging: room for a third box)
-    static constexpr int B_HALF = Base::B_BLOCK;                         // bytes of one weight stage held by ONE CTA: its 64 rows of BOTH blocks
-                                                                         // of a 32-channel step ([hi | lo] or [wh | wh8 | wl8])
-    static constexpr int NBP_FIT = (Base::SMEM_MAX - 1024 - Base::BAR_BYTES - Base::W6_BYTES - Base::STG_BYTES - A_SLOTS * Base::A_SLOT) / B_HALF;
-    static constexpr int NBP = NBP_FIT > 12 ? 12 : NBP_FIT;
-    static constexpr int SMEM_BYTES = 1024 + A_SLOTS * Base::A_SLOT + NBP * B_HALF + Base::BAR_BYTES + Base::W6_BYTES + Base::STG_BYTES;
-    static_assert((2 * A_SLOTS + 4 + 2 * NBP) * 8 + 4 <= 512, "barrier area overflow");
-    static_assert(B_HALF % 2048 == 0, "weight halves are moved as 2 KB TMA boxes");
-    static_assert(NBP >= 6, "weight ring too shallow");
-};

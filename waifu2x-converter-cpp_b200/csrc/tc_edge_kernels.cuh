@@ -1,17 +1,17 @@
 // tc_edge_kernels.cuh -- CUDA-core kernels at the edges of the stack: first layer, last layer, fused-last gather, layout converters
-// Part of the tcgen05 engine's single translation unit: included by kernels_tc.cu inside namespace w2x::tc, in this order:
-//   tc_ptx.cuh, tc_config.cuh, tc_issue.cuh, tc_epilogue.cuh, tc_kernel.cuh, tc_pair_kernel.cuh, tc_strip_kernel.cuh, tc_edge_kernels.cuh
+// Part of the tensor-core engine's single translation unit: included by kernels_tc.cu inside namespace w2x::tc, in this order:
+//   tc_ptx.cuh, tc_wgmma.cuh, tc_config.cuh, tc_kernel.cuh, tc_edge_kernels.cuh
 // (pure code organisation: the generated SASS is the same as with one file).
 
 // ================================================================================================
 // First layer (Cin = 1), last layer (Cout = 1), layout converters -- CUDA-core, HBM-bound
 // ================================================================================================
-// First layer: Model::filterWorker with nInputPlanes = 1 on the replicate-padded plane; writes the RECORD frame the tcgen05
+// First layer: Model::filterWorker with nInputPlanes = 1 on the replicate-padded plane; writes the RECORD frame the tensor-core
 // layers consume.  One thread per pixel, 32 x 8 pixels per block.
 //   * the plane is NOT padded beforehand: `in` is the caller's plane (w x h, possibly a row band with real rows above / below)
 //     and frame pixel (fy, fx) reads in[clamp(fy - pad_y), clamp(fx - pad_x)] -- cv::copyMakeBorder(BORDER_REPLICATE)
 //     (src/convertRoutine.cpp:35,96) folded into the loads;
-//   * two output channels per instruction: packed fp32 (FFMA2, sm_100) with the weight PAIRS straight from the constant bank
+//   * two output channels per step (channel pairs) with the weight PAIRS straight from the constant bank
 //     (kernel parameters -> uniform registers) and the pixel broadcast to both halves; every lane's arithmetic is the
 //     reference's: per tap an fma chain, + (float)bias, leaky = max(v, 0.1f v) (= min(v,0)*0.1f + max(v,0) bit for bit).
 //     ACT_SCALE (16, a power of two) is folded into the weights and biases on the host: exact;
@@ -24,22 +24,10 @@ struct FirstParams {
 };
 constexpr int FIRST_TILE_BYTES = 32 * 1024;   // [256 px][128 B]
 
-__device__ __forceinline__ float2 f32x2_fma(float2 a, float2 b, float2 c) {
-    unsigned long long ra = *reinterpret_cast<unsigned long long *>(&a), rb = *reinterpret_cast<unsigned long long *>(&b),
-                       rc = *reinterpret_cast<unsigned long long *>(&c), r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(ra), "l"(rb), "l"(rc));
-    return *reinterpret_cast<float2 *>(&r);
-}
-__device__ __forceinline__ float2 f32x2_mul(float2 a, float2 b) {
-    unsigned long long ra = *reinterpret_cast<unsigned long long *>(&a), rb = *reinterpret_cast<unsigned long long *>(&b), r;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(ra), "l"(rb));
-    return *reinterpret_cast<float2 *>(&r);
-}
-__device__ __forceinline__ float2 f32x2_add(float2 a, float2 b) {
-    unsigned long long ra = *reinterpret_cast<unsigned long long *>(&a), rb = *reinterpret_cast<unsigned long long *>(&b), r;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(ra), "l"(rb));
-    return *reinterpret_cast<float2 *>(&r);
-}
+// channel pairs: two independent round-to-nearest fp32 operations (what a packed f32x2 instruction computes per half)
+__device__ __forceinline__ float2 f32x2_fma(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 f32x2_mul(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 f32x2_add(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 
 // in: plane of w x h (row stride in_stride), readable at rows [-rows_above, h + rows_below); frame = (w + 2 pad_x) x (h + pad_top + pad_bottom)
 struct FirstSrc {

@@ -1,47 +1,145 @@
-// tc_kernel.cuh -- tc_conv3x3_kernel: the single-CTA layer kernel (warp roles, pipelines)
-// Part of the tcgen05 engine's single translation unit: included by kernels_tc.cu inside namespace w2x::tc, in this order:
-//   tc_ptx.cuh, tc_config.cuh, tc_issue.cuh, tc_epilogue.cuh, tc_kernel.cuh, tc_pair_kernel.cuh, tc_strip_kernel.cuh, tc_edge_kernels.cuh
+// tc_kernel.cuh -- tc_conv3x3_kernel: the layer kernel (warp roles, pipelines, epilogue)
+// Part of the tensor-core engine's single translation unit: included by kernels_tc.cu inside namespace w2x::tc, in this order:
+//   tc_ptx.cuh, tc_wgmma.cuh, tc_config.cuh, tc_kernel.cuh, tc_edge_kernels.cuh
 // (pure code organisation: the generated SASS is the same as with one file).
+
+// Bias, scale and leaky-ReLU of one accumulator value: = ACT_SCALE * leaky(conv + bias)
+__device__ __forceinline__ float activate(float acc, float scale, float bias) {
+    const float v = fmaf(acc, scale, bias);
+    return fmaxf(v, 0.1f * v);                                           // leaky 0.1: min(v,0)*0.1 + max(v,0)
+}
+
+// One consumer warpgroup's M-tile (8 wide x 16 tall pixels = two m64 halves) of a tile-set: accumulators -> scale, bias,
+// leaky-ReLU -> records of each 32-channel block written into the warpgroup's staging tile in the TMA SWIZZLE_128B pattern
+// (staging row = pixel = y * 8 + x, conflict-free: the eight rows a warp writes at once fall into eight different 16-byte
+// units) and sent as ONE 8x16-pixel TMA store box; the frame edge is clipped by the TMA unit.
+template <int COUT, bool F8>
+__device__ __forceinline__ void epilogue_store(const TcParams &p, const float *bias, const CUtensorMap *tmap_out, const float (&acc)[2][COUT / 2],
+                                               uint32_t stg, int wg, int wq, int lane, int gx0, int gy0) {
+    const int q = lane & 3, r_lo = wq * 16 + (lane >> 2);
+#pragma unroll
+    for (int cb = 0; cb < COUT / 32; cb++) {
+        if (wq == 0) {                    // the lanes of warp 0 wait for their own store of the previous block to have left
+            bulk_wait_read();
+            __syncwarp();
+        }
+        named_sync(1 + wg, 128);
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+#pragma unroll
+            for (int e = 0; e < 2; e++) {
+                const uint32_t row = (uint32_t)(64 * h + r_lo + 8 * e), sw = row & 7u, rowaddr = stg + row * 128u;
+#pragma unroll
+                for (int j = 0; j < 4; j++) {
+                    const int jj = cb * 4 + j, ch = 8 * jj + 2 * q;
+                    const float v0 = activate(acc[h][4 * jj + 2 * e], p.out_scale, bias[ch]);
+                    const float v1 = activate(acc[h][4 * jj + 2 * e + 1], p.out_scale, bias[ch + 1]);
+                    const __half2 hh = __floats2half2_rn(v0, v1);
+                    const float2 hf = __half22float2(hh);
+                    asm volatile("st.shared.b32 [%0], %1;" ::"r"(rowaddr + (((uint32_t)j ^ sw) << 4) + 4u * q), "r"(*reinterpret_cast<const uint32_t *>(&hh)) : "memory");
+                    if constexpr (F8) {
+                        constexpr float kDown = 1.0f / (float)(1 << F8_C), kUp = (float)(1 << F8_A);
+                        const __half2 hd = __hmul2(hh, __float2half2_rn(kDown));
+                        const uint16_t h8 = __nv_cvt_halfraw2_to_fp8x2(static_cast<__half2_raw>(hd), __NV_SATFINITE, __NV_E4M3);
+                        const uint16_t l8 = __nv_cvt_float2_to_fp8x2(make_float2((v0 - hf.x) * kUp, (v1 - hf.y) * kUp), __NV_SATFINITE, __NV_E4M3);
+                        const uint32_t in_unit = 8u * (uint32_t)(j & 1) + 2u * q;
+                        asm volatile("st.shared.b16 [%0], %1;" ::"r"(rowaddr + (((uint32_t)(4 + (j >> 1)) ^ sw) << 4) + in_unit), "h"(h8) : "memory");
+                        asm volatile("st.shared.b16 [%0], %1;" ::"r"(rowaddr + (((uint32_t)(6 + (j >> 1)) ^ sw) << 4) + in_unit), "h"(l8) : "memory");
+                    } else {
+                        const __half2 lo = __floats2half2_rn(v0 - hf.x, v1 - hf.y);
+                        asm volatile("st.shared.b32 [%0], %1;" ::"r"(rowaddr + (((uint32_t)(4 + j) ^ sw) << 4) + 4u * q), "r"(*reinterpret_cast<const uint32_t *>(&lo)) : "memory");
+                    }
+                }
+            }
+        }
+        fence_proxy_async();
+        named_sync(1 + wg, 128);
+        if (wq == 0) {
+            tma_store_4d(tmap_out, stg, 0, cb, gx0, gy0);
+            bulk_commit();
+        }
+    }
+}
+
+// The last layer folded in: per pixel the nine tap dot products over this layer's activated channels.  The four lanes of
+// a quad hold the pixel's channels (8j + 2q, +1); their partial sums meet through two shuffles.
+template <int COUT>
+__device__ __forceinline__ void epilogue_fuse(const TcParams &p, const float *bias, const float *last_w, const float (&acc)[2][COUT / 2], int wq, int lane,
+                                              int fx0, int fy0) {
+    const int q = lane & 3, r_lo = wq * 16 + (lane >> 2);
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+#pragma unroll
+        for (int e = 0; e < 2; e++) {
+            float pt[9];
+#pragma unroll
+            for (int t = 0; t < 9; t++) pt[t] = 0.f;
+#pragma unroll
+            for (int jj = 0; jj < COUT / 8; jj++) {
+#pragma unroll
+                for (int k = 0; k < 2; k++) {
+                    const int ch = 8 * jj + 2 * q + k;
+                    const float a = activate(acc[h][4 * jj + 2 * e + k], p.out_scale, bias[ch]);
+#pragma unroll
+                    for (int t = 0; t < 9; t++) pt[t] = fmaf(a, last_w[t * COUT + ch], pt[t]);
+                }
+            }
+#pragma unroll
+            for (int t = 0; t < 9; t++) {
+                pt[t] += __shfl_xor_sync(0xffffffffu, pt[t], 1);
+                pt[t] += __shfl_xor_sync(0xffffffffu, pt[t], 2);
+            }
+            const int row = 64 * h + r_lo + 8 * e;
+            const int fx = fx0 + (row & 7), fy = fy0 + (row >> 3);
+            if (q == 0 && fy < p.Hp && fx < p.Wp && fy >= p.out_y0 && fy < p.out_y0 + p.out_rows) {
+                float4 *dst = reinterpret_cast<float4 *>(p.partial + ((size_t)fy * p.Wp + fx) * 12);
+                dst[0] = make_float4(pt[0], pt[1], pt[2], pt[3]);
+                dst[1] = make_float4(pt[4], pt[5], pt[6], pt[7]);
+                dst[2] = make_float4(pt[8], 0.f, 0.f, 0.f);
+            }
+        }
+    }
+}
 
 // ================================================================================================
 // The layer kernel
 // ================================================================================================
+// Persistent, one CTA per SM, tile-sets of 16x16 output pixels round-robin over the CTAs.  Each consumer warpgroup owns an
+// 8-wide x 16-tall M-tile (two m64 wgmma halves: halo rows 0..7 and 8..15), N = Cout; the 3x3 taps are descriptor start
+// offsets into the staged 18x18 box.  Per tap one wgmma group is committed and the one before it waited for, so a weight
+// stage (and, after the ninth tap, an activation slot) is handed back while the next group runs (F8: every group of a tap has
+// completed when its e4m3 corrections are added in; the other warpgroup keeps the tensor core busy meanwhile).
 template <int CIN, int COUT, bool FUSE, bool F8>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-tc_conv3x3_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ CUtensorMap tmap_out, const TcParams p) {
+tc_conv3x3_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ TcParams p) {
     using C = Cfg<CIN, COUT, FUSE, F8>;
     extern __shared__ uint8_t smem_raw[];
     // 1024-byte alignment: the SWIZZLE_128B pattern repeats every 1024 B
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     const uint32_t a_base = smem_base;
     const uint32_t b_base = a_base + C::A_SLOTS * C::A_SLOT;
-    const uint32_t bar_base = b_base + C::NB * C::B_STAGE;
+    const uint32_t stg_base = b_base + C::NB * C::B_STAGE;
+    const uint32_t bar_base = stg_base + C::STG_BYTES;
+    float *prm = reinterpret_cast<float *>(smem_raw + (bar_base + C::BAR_BYTES - smem_u32(smem_raw)));   // [bias (COUT)][last_w (9 x COUT)]
     // barrier map (8 bytes each)
-    auto a_full = [&](int i) { return bar_base + 8u * (uint32_t)i; };
-    auto a_empty = [&](int i) { return bar_base + 8u * (uint32_t)(2 + i); };
-    auto acc_full = [&](int i) { return bar_base + 8u * (uint32_t)(4 + i); };
-    auto acc_empty = [&](int i) { return bar_base + 8u * (uint32_t)(6 + i); };
-    auto b_full = [&](int i) { return bar_base + 8u * (uint32_t)(8 + i); };
-    auto b_empty = [&](int i) { return bar_base + 8u * (uint32_t)(8 + C::NB + i); };
-    const uint32_t tmem_slot = bar_base + 8u * (uint32_t)(8 + 2 * C::NB);   // 4 bytes: TMEM base address
-    uint32_t *tmem_slot_ptr = reinterpret_cast<uint32_t *>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
+    auto a_full = [&](uint32_t i) { return bar_base + 8u * i; };
+    auto a_empty = [&](uint32_t i) { return bar_base + 8u * (2u + i); };
+    auto b_full = [&](uint32_t i) { return bar_base + 8u * (4u + i); };
+    auto b_empty = [&](uint32_t i) { return bar_base + 8u * (4u + C::NB + i); };
+    constexpr uint32_t CONSUMER_WARPS = 8;
 
-    // warp index through a shuffle: ptxas then knows it is warp-uniform, and with it the role branch, the M-tile index and
-    // every descriptor derived from them (uniform registers feed tcgen05.mma directly, no per-MMA R2UR waterfall)
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
     const bool prof_on = p.prof != nullptr;
     unsigned long long *prof = prof_on ? p.prof + (size_t)blockIdx.x * PROF_N : nullptr;
 
     if (threadIdx.x == 0) {
-        for (int i = 0; i < 2; i++) {
+        for (uint32_t i = 0; i < 2; i++) {
             mbar_init(a_full(i), 1);
-            mbar_init(a_empty(i), 2);     // one tcgen05.commit per MMA issuer
-            mbar_init(acc_full(i), 2);
-            mbar_init(acc_empty(i), 8);   // one arrive per epilogue warp
+            mbar_init(a_empty(i), CONSUMER_WARPS);   // lane 0 of every consumer warp, after its wgmma wait
         }
-        for (int i = 0; i < C::NB; i++) {
+        for (uint32_t i = 0; i < (uint32_t)C::NB; i++) {
             mbar_init(b_full(i), 1);
-            mbar_init(b_empty(i), 2);
+            mbar_init(b_empty(i), CONSUMER_WARPS);
         }
         fence_barrier_init();
         fence_proxy_async();
@@ -50,179 +148,147 @@ tc_conv3x3_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_cons
         prefetch_tmap(&tmap_in);
         if constexpr (!FUSE) prefetch_tmap(&tmap_out);
     }
-    if (warp == 2) {
-        tmem_alloc(tmem_slot, C::TMEM_COLS);
-        tmem_relinquish();
-    }
-    tc_fence_before();
+    for (int i = threadIdx.x; i < COUT; i += NUM_THREADS) prm[i] = p.bias[i];
+    if constexpr (FUSE)
+        for (int i = threadIdx.x; i < 9 * COUT; i += NUM_THREADS) prm[COUT + i] = p.last_w[i];
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot_ptr, 0);   // uniform for the compiler as well
 
     if (warp == 0) {
         // ===================== A producer: one halo'd box of records per (tile-set, 32-channel block) ==============
         // (whole warp walks the loop; the arrive and the TMA instructions elect one lane)
-        {
-            uint32_t it = 0;
-            unsigned long long w_a = 0;
-            for (int ts = blockIdx.x; ts < p.n_tilesets; ts += gridDim.x) {
-                const int ty = ts / p.tiles_x, tx = ts - ty * p.tiles_x;
-                const int x0 = tx * REGION - 1, y0 = p.out_y0 + ty * REGION - 1;   // box origin incl. ring (may be -1); tile-sets tile the store window
-                for (int c = 0; c < C::NCHUNK; c++, it++) {
-                    const uint32_t slot = it & 1u, round = it >> 1;
-                    mbar_wait_prof(a_empty(slot), (round & 1u) ^ 1u, prof_on, w_a);
-                    mbar_arrive_expect_tx(a_full(slot), (uint32_t)C::A_TX);
-                    tma_load_4d(a_base + slot * C::A_SLOT, &tmap_in, a_full(slot), 0, c, x0, y0);
-                }
+        uint32_t it = 0;
+        unsigned long long w_a = 0;
+        for (int ts = blockIdx.x; ts < p.n_tilesets; ts += gridDim.x) {
+            const int ty = ts / p.tiles_x, tx = ts - ty * p.tiles_x;
+            const int x0 = tx * REGION - 1, y0 = p.out_y0 + ty * REGION - 1;   // box origin incl. ring (may be -1); tile-sets tile the store window
+            for (int c = 0; c < C::NCHUNK; c++, it++) {
+                const uint32_t slot = it & 1u, round = it >> 1;
+                mbar_wait_prof(a_empty(slot), (round & 1u) ^ 1u, prof_on, w_a);
+                mbar_arrive_expect_tx(a_full(slot), (uint32_t)C::A_TX);
+                tma_load_4d(a_base + slot * C::A_SLOT, &tmap_in, a_full(slot), 0, c, x0, y0);
             }
-            if (prof_on && lane == 0) prof[PROF_APROD_WAIT] += w_a;
         }
-    } else if (warp == 2) {
+        if (prof_on && lane == 0) prof[PROF_APROD_WAIT] += w_a;
+    } else if (warp == 1) {
         // ===================== B producer: stream the packed weights in consumption order ============
-        {
-            uint32_t stage = 0, phase = 0;
-            unsigned long long w_b = 0;
-            for (int ts = blockIdx.x; ts < p.n_tilesets; ts += gridDim.x) {
-                const uint8_t *src = reinterpret_cast<const uint8_t *>(p.wpack);
-                if (C::RESIDENT && ts != (int)blockIdx.x) break;           // resident weights: one pass fills every stage for good
-                for (int blk = 0; blk < C::STAGES_PER_TILESET; blk++) {
-                    if constexpr (!C::RESIDENT) mbar_wait_prof(b_empty(stage), phase ^ 1u, prof_on, w_b);
-                    mbar_arrive_expect_tx(b_full(stage), C::B_STAGE);
-                    bulk_load(b_base + stage * C::B_STAGE, src + (size_t)blk * C::B_STAGE, C::B_STAGE, b_full(stage));
-                    if (++stage == (uint32_t)C::NB) { stage = 0; phase ^= 1u; }
-                }
+        uint32_t stage = 0, phase = 0;
+        unsigned long long w_b = 0;
+        const uint8_t *src = reinterpret_cast<const uint8_t *>(p.wpack);
+        for (int ts = blockIdx.x; ts < p.n_tilesets; ts += gridDim.x) {
+            if (C::RESIDENT && ts != (int)blockIdx.x) break;           // resident weights: one pass fills every stage for good
+            for (int blk = 0; blk < C::STAGES_PER_TILESET; blk++) {
+                if constexpr (!C::RESIDENT) mbar_wait_prof(b_empty(stage), phase ^ 1u, prof_on, w_b);
+                mbar_arrive_expect_tx(b_full(stage), C::B_STAGE);
+                bulk_load(b_base + stage * C::B_STAGE, src + (size_t)blk * C::B_STAGE, C::B_STAGE, b_full(stage));
+                if (++stage == (uint32_t)C::NB) { stage = 0; phase ^= 1u; }
             }
-            if (prof_on && lane == 0) prof[PROF_BPROD_WAIT] += w_b;
         }
-    } else if (warp == 1 || warp == 7) {
-        // ===================== MMA issuers (warp 1: M-tile 0, warp 7: M-tile 1) ========================
-        // The whole warp walks the loop converged; each MMA / commit elects one lane inside its asm block.
-        const uint32_t leader = lane == 0 ? 1u : 0u;
-        const uint32_t jt = warp == 1 ? 0u : 1u;
-        constexpr uint32_t idesc_c = make_idesc(128, COUT);          // N = Cout
-        constexpr uint32_t idesc_2c = make_idesc(128, 2 * COUT);     // N = 2*Cout (stacked [wh;wl]); only used when STACK
-        constexpr uint32_t A_SBO = HALO * C::ROWB;                   // next output row = next halo row
-        constexpr uint32_t B_SBO = 8 * C::B_ROWB;                    // dense rows
-        constexpr uint32_t A_HI32 = (uint32_t)(make_desc_const(A_SBO, C::A_LAYOUT) >> 32);
-        constexpr uint32_t B_HI32 = (uint32_t)(make_desc_const(B_SBO, C::B_LAYOUT) >> 32);
-        constexpr uint32_t LO_FIXED = 1u << 16;                      // LBO field = 1
-        // e4m3 weight blocks: 32-byte rows (SWIZZLE_32B); the e4m3 activation slices are quarters of the same 128-byte records
-        constexpr uint32_t B8_HI32 = (uint32_t)(make_desc_const(8 * 32, 6u) >> 32);
-        auto desc = [](uint32_t hi32, uint32_t lo32) { return ((uint64_t)hi32 << 32) | (uint64_t)lo32; };
+        if (prof_on && lane == 0) prof[PROF_BPROD_WAIT] += w_b;
+    } else if (warp >= 4) {
+        // ===================== consumers: warpgroup wg = M-tile wg (pixels x in [8 wg, 8 wg + 8) of the tile-set) ===========
+        const int wg = (warp - 4) >> 2, wq = warp & 3;
+        constexpr uint32_t ROWB = C::ROWB;
+        constexpr uint32_t A_HI = desc_hi(HALO * ROWB, SW128);      // next 8-pixel group = next halo row
+        constexpr uint32_t B_HI = desc_hi(8 * 64, SW64);             // fp16 weight rows of 64 B
+        constexpr uint32_t HALF = 8 * HALO * ROWB;                   // second m64 half: eight halo rows down
+        float acc[2][COUT / 2];
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+#pragma unroll
+            for (int i = 0; i < COUT / 2; i++) acc[h][i] = 0.f;
         uint32_t a_it = 0, stage = 0, phase = 0, n = 0;
-        uint32_t b_ready = 0;                         // result of the early probe of b_full(stage)
-        unsigned long long w_acc = 0, w_af = 0, w_bf = 0;
+        unsigned long long w_af = 0, w_bf = 0;
         const long long t_begin = clock64();
-        // wait for the current weight stage (usually already known to be full), then probe the NEXT one
-        auto acquire_b = [&](uint32_t &b0_out) {
-            if constexpr (C::RESIDENT) {
-                if (n == 0) {                             // the stages arrive once, during the first tile-set
-                    mbar_wait_prof(b_full(stage), 0u, prof_on, w_bf);
-                    tc_fence_after();
-                }
-                b0_out = (((b_base + stage * C::B_STAGE) >> 4) & 0x3FFFu) | LO_FIXED;
-            } else {
-                if (!b_ready) mbar_wait_prof(b_full(stage), phase, prof_on, w_bf);
-                tc_fence_after();
-                b0_out = (((b_base + stage * C::B_STAGE) >> 4) & 0x3FFFu) | LO_FIXED;
-                uint32_t ns = stage + 1, np = phase;
-                if (ns == (uint32_t)C::NB) { ns = 0; np ^= 1u; }
-                b_ready = mbar_test(b_full(ns), np);      // consumed at the next acquire_b
-            }
-        };
-        auto release_b = [&]() {
-            if constexpr (!C::RESIDENT) umma_commit_one(b_empty(stage));
-            if (++stage == (uint32_t)C::NB) { stage = 0; phase ^= 1u; }
-        };
         for (int ts = blockIdx.x; ts < p.n_tilesets; ts += gridDim.x, n++) {
-            const uint32_t set = n & 1u;
-            mbar_wait_prof(acc_empty(set), ((n >> 1) & 1u) ^ 1u, prof_on, w_acc);
-            tc_fence_after();
-            const uint32_t dj = tmem_base + (set * 2u + jt) * C::TILE_COLS;   // this issuer's accumulator columns
+            const int ty = ts / p.tiles_x, tx = ts - ty * p.tiles_x;
+            int pend_b = -1, pend_a = -1;                            // stage / slot read by the group in flight
             for (int c = 0; c < C::NCHUNK; c++, a_it++) {
                 const uint32_t slot = a_it & 1u;
                 mbar_wait_prof(a_full(slot), (a_it >> 1) & 1u, prof_on, w_af);
-                tc_fence_after();
-                // descriptor low word (address >> 4) of this issuer's window into the staged records; a record's quarters:
-                // +0 / +2 the fp16 K steps, +4 xh8 (f16x3: lo step 0), +6 xl8 (f16x3: lo step 1)   [16-byte units]
-                const uint32_t ah0 = ((((a_base + slot * C::A_SLOT) >> 4) & 0x3FFFu) | LO_FIXED) + jt * (8u * C::ROWB >> 4);
-                uint32_t tap_off = 0;                 // ((ky*HALO + kx) * ROWB) >> 4
+                const uint32_t a0 = a_base + slot * C::A_SLOT + (uint32_t)wg * 8u * ROWB;
+#pragma unroll 1
                 for (int t = 0; t < 9; t++) {
+                    const uint32_t tap = (uint32_t)((t / 3) * HALO + t % 3) * ROWB;
+                    if (!C::RESIDENT) mbar_wait_prof(b_full(stage), phase, prof_on, w_bf);
+                    else if (n == 0) mbar_wait_prof(b_full(stage), 0u, prof_on, w_bf);   // the stages arrive once, during the first tile-set
+                    const uint32_t b = b_base + stage * C::B_STAGE;
                     const uint32_t first = (c | t) != 0 ? 1u : 0u;
-                    {
-                        const uint32_t ah = ah0 + tap_off, al = ah + 4u;
-                        const uint32_t acc0 = first;
-                        uint32_t b0;
-                        if constexpr (C::MERGE) {
-                            // one stage = [wh fp16 | wh8 | wl8]: main product (two K=16 steps) + both e4m3 corrections (K=32 each)
-                            acquire_b(b0);
-                            issue_tap_f8<false>(dj, ah, b0, COUT, A_HI32, B_HI32, B8_HI32, idesc_c, acc0);
-                            release_b();
-                        } else if constexpr (C::STACK) {
-                            // one stage = [wh ; wl]: xh*[wh;wl] (N = 2*Cout, D1|D2) then xl*wh (N = Cout, D1)
-                            acquire_b(b0);
-                            umma_f16(dj, desc(A_HI32, ah), desc(B_HI32, b0), idesc_2c, acc0);
-                            umma_f16(dj, desc(A_HI32, ah + 2u), desc(B_HI32, b0 + 2u), idesc_2c, 1u);
-                            umma_f16(dj, desc(A_HI32, al), desc(B_HI32, b0), idesc_c, 1u);
-                            umma_f16(dj, desc(A_HI32, al + 2u), desc(B_HI32, b0 + 2u), idesc_c, 1u);
-                            release_b();
-                        } else {
-                            // ---- hi weights: xh*wh and xl*wh ----
-                            acquire_b(b0);
-                            umma_f16(dj, desc(A_HI32, ah), desc(B_HI32, b0), idesc_c, acc0);
-                            umma_f16(dj, desc(A_HI32, ah + 2u), desc(B_HI32, b0 + 2u), idesc_c, 1u);
-                            umma_f16(dj, desc(A_HI32, al), desc(B_HI32, b0), idesc_c, 1u);
-                            umma_f16(dj, desc(A_HI32, al + 2u), desc(B_HI32, b0 + 2u), idesc_c, 1u);
-                            release_b();
-                            // ---- lo weights: xh*wl ----
-                            acquire_b(b0);
-                            umma_f16(dj, desc(A_HI32, ah), desc(B_HI32, b0), idesc_c, 1u);
-                            umma_f16(dj, desc(A_HI32, ah + 2u), desc(B_HI32, b0 + 2u), idesc_c, 1u);
-                            release_b();
+                    acc_fence(acc[0]);
+                    acc_fence(acc[1]);
+                    wgmma_fence();
+#pragma unroll
+                    for (int h = 0; h < 2; h++) {
+                        const uint32_t ah = a0 + (uint32_t)h * HALF + tap;
+                        // a record's quarters: +0 / +32 the fp16 K steps, +64 xh8 (f16x3: lo step 0), +96 xl8 (f16x3: lo step 1)
+                        Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah), make_desc(B_HI, b), first);
+                        Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah + 32u), make_desc(B_HI, b + 32u), 1u);
+                        if constexpr (!F8) {
+                            Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah + 64u), make_desc(B_HI, b), 1u);                // xl * wh
+                            Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah + 96u), make_desc(B_HI, b + 32u), 1u);
+                            Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah), make_desc(B_HI, b + COUT * 64u), 1u);         // xh * wl
+                            Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah + 32u), make_desc(B_HI, b + COUT * 64u + 32u), 1u);
                         }
                     }
-                    // next tap: kx+1, or the next halo row
-                    tap_off += tap_step<C::ROWB>(t);
+                    if constexpr (F8) {
+                        // Hopper's e4m3 wgmma accumulates in reduced precision, which would also round the fp32 sums it adds to: the
+                        // two corrections of a tap go into a fresh accumulator of NS columns (scale_d = 0) and reach the fp32 sums
+                        // through ordinary adds once that group has completed.
+                        constexpr int NS = COUT < 64 ? COUT : 64;
+                        constexpr uint32_t B8_HI = desc_hi(8 * 32, SW32);    // e4m3 weight rows of 32 B
+                        wgmma_commit();
+#pragma unroll
+                        for (int h = 0; h < 2; h++) {
+                            const uint32_t ah = a0 + (uint32_t)h * HALF + tap;
+#pragma unroll
+                            for (int s = 0; s < COUT / NS; s++) {
+                                float corr[NS / 2];
+                                wgmma_fence();
+                                Wgmma<NS>::e4m3(corr, make_desc(A_HI, ah + 96u), make_desc(B8_HI, b + COUT * 64u + s * NS * 32u), 0u);   // xl8 * wh8
+                                Wgmma<NS>::e4m3(corr, make_desc(A_HI, ah + 64u), make_desc(B8_HI, b + COUT * 96u + s * NS * 32u), 1u);   // xh8 * wl8
+                                wgmma_commit();
+                                wgmma_wait<0>();                             // (also completes the f16 group before acc is touched)
+                                acc_fence(corr);
+                                acc_fence(acc[h]);
+#pragma unroll
+                                for (int i = 0; i < NS / 2; i++) acc[h][s * (NS / 2) + i] += corr[i];
+                            }
+                        }
+                    }
+                    if constexpr (!F8) {
+                        wgmma_commit();
+                        wgmma_wait<1>();                             // the previous group is done: its stage / slot may be refilled
+                    }
+                    acc_fence(acc[0]);
+                    acc_fence(acc[1]);
+                    if (lane == 0) {
+                        if (!C::RESIDENT && pend_b >= 0) mbar_arrive(b_empty((uint32_t)pend_b));
+                        if (pend_a >= 0) mbar_arrive(a_empty((uint32_t)pend_a));
+                    }
+                    pend_b = (int)stage;
+                    pend_a = t == 8 ? (int)slot : -1;
+                    if (++stage == (uint32_t)C::NB) { stage = 0; phase ^= 1u; }
                 }
-                umma_commit_one(a_empty(slot));   // the staged boxes may be overwritten once these MMAs retire
             }
-            umma_commit_one(acc_full(set));       // this issuer's accumulators of the tile-set are final
+            wgmma_wait<0>();
+            acc_fence(acc[0]);
+            acc_fence(acc[1]);
+            if (lane == 0) {
+                if (!C::RESIDENT) mbar_arrive(b_empty((uint32_t)pend_b));
+                mbar_arrive(a_empty((uint32_t)pend_a));
+            }
+            if constexpr (FUSE)
+                epilogue_fuse<COUT>(p, prm, prm + COUT, acc, wq, lane, tx * REGION + 8 * wg, p.out_y0 + ty * REGION);
+            else
+                epilogue_store<COUT, F8>(p, prm, &tmap_out, acc, stg_base + (uint32_t)wg * C::STG_WG, wg, wq, lane, tx * REGION + 8 * wg, ty * REGION);
         }
-        if (prof_on && leader && jt == 0) {
+        if constexpr (!FUSE) {
+            if (wq == 0) bulk_wait_all();    // this warpgroup's TMA stores are complete before the CTA may exit
+        }
+        if (prof_on && wg == 0 && wq == 0 && lane == 0) {
             prof[PROF_TOTAL] += (unsigned long long)(clock64() - t_begin);
-            prof[PROF_MMA_WAIT_ACC] += w_acc;
             prof[PROF_MMA_WAIT_A] += w_af;
             prof[PROF_MMA_WAIT_B] += w_bf;
             prof[PROF_TILESETS] += n;
         }
-    } else {
-        // ===================== epilogue: warps 3..6 drain M-tile 0, warps 8..11 drain M-tile 1 ==========
-        const uint32_t q = (uint32_t)warp & 3u;          // TMEM lane quarter this warp may access
-        const int j = warp >= 8 ? 1 : 0;                 // M-tile
-        const uint32_t row = q * 32u + (uint32_t)lane;   // GEMM row = pixel inside the 8x16 M-tile
-        const int oy = (int)(row >> 3), ox = (int)(row & 7u);
-        const uint32_t stg = bar_base + C::BAR_BYTES + C::W6_BYTES + (uint32_t)(j * 4 + (int)q) * (uint32_t)C::STG_WARP;   // this warp's staging tile
-        uint32_t n = 0;
-        unsigned long long w_e = 0, work_e = 0;
-        for (int ts = blockIdx.x; ts < p.n_tilesets; ts += gridDim.x, n++) {
-            const uint32_t set = n & 1u;
-            const int ty = ts / p.tiles_x, tx = ts - ty * p.tiles_x;
-            mbar_wait_prof(acc_full(set), (n >> 1) & 1u, prof_on, w_e);
-            const long long t_work = prof_on ? clock64() : 0;
-            tc_fence_after();
-            const uint32_t tcol = tmem_base + ((q * 32u) << 16) + (set * 2u + (uint32_t)j) * C::TILE_COLS;
-            tile_epilogue<COUT, FUSE, F8, C::STACK>(p, &tmap_out, tcol, stg, lane, tx * REGION + 8 * j, ty * REGION + 4 * (int)q,
-                                                    tx * REGION + 8 * j + ox, p.out_y0 + ty * REGION + oy, [&] { mbar_arrive(acc_empty(set)); });
-            if (prof_on) work_e += (unsigned long long)(clock64() - t_work);
-        }
-        if constexpr (!FUSE) bulk_wait_all();    // this warp's TMA stores are complete before the CTA may exit
-        if (prof_on && warp == 3 && lane == 0) {
-            prof[PROF_EPI_WAIT] += w_e;
-            prof[PROF_EPI_WORK] += work_e;
-        }
     }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) tmem_dealloc(tmem_base, C::TMEM_COLS);
 }

@@ -1,6 +1,6 @@
-// tc_ptx.cuh -- inline-PTX wrappers: mbarrier, TMA (loads, stores, cta_group::2), tcgen05 (alloc, mma, commit, ld), UMMA descriptors
-// Part of the tcgen05 engine's single translation unit: included by kernels_tc.cu inside namespace w2x::tc, in this order:
-//   tc_ptx.cuh, tc_config.cuh, tc_issue.cuh, tc_epilogue.cuh, tc_kernel.cuh, tc_pair_kernel.cuh, tc_strip_kernel.cuh, tc_edge_kernels.cuh
+// tc_ptx.cuh -- inline-PTX wrappers: mbarrier, TMA (tiled loads and stores, bulk copies), wgmma shared-memory descriptors
+// Part of the tensor-core engine's single translation unit: included by kernels_tc.cu inside namespace w2x::tc, in this order:
+//   tc_ptx.cuh, tc_wgmma.cuh, tc_config.cuh, tc_kernel.cuh, tc_edge_kernels.cuh
 // (pure code organisation: the generated SASS is the same as with one file).
 
 // ================================================================================================
@@ -12,7 +12,7 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
 }
 // Producer-side helpers are called by a whole converged warp; ONE elected lane executes the instruction (elect.sync inside
-// the asm block).  For the TMA / tcgen05 instructions this is what lets ptxas keep their operands in uniform registers.
+// the asm block).  For the TMA instructions this is what lets ptxas keep their operands in uniform registers.
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
     asm volatile("{\n\t.reg .pred q;\n\telect.sync _|q, 0xffffffff;\n\t@q mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n\t}" ::"r"(bar), "r"(bytes) : "memory");
 }
@@ -41,25 +41,10 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         }
     }
 }
-// Non-blocking probe of a phase: issued EARLY (before the MMAs of the current stage) so that the ~100-cycle
-// mbarrier round trip of the next stage's wait overlaps with issue work instead of draining the tensor queue.
-__device__ __forceinline__ uint32_t mbar_test(uint32_t bar, uint32_t parity) {
-    uint32_t done;
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t"
-        "}"
-        : "=r"(done)
-        : "r"(bar), "r"(parity)
-        : "memory");
-    return done;
-}
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// named barrier of `count` threads (the two consumer warpgroups synchronise separately: ids 1 and 2)
+__device__ __forceinline__ void named_sync(uint32_t id, uint32_t count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 
 // TMA: 4-D tiled load global -> shared, completion on an mbarrier
 __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap *map, uint32_t bar, int c0, int c1, int c2,
@@ -94,78 +79,6 @@ __device__ __forceinline__ void prefetch_tmap(const CUtensorMap *map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
 
-// tcgen05
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t addr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(ncols) : "memory");
-}
-// The issuing WARP walks the MMA loop converged; each tcgen05.mma / commit is predicated by an elect.sync inside its asm
-// block.  Together with a shuffle-derived (provably uniform) warp index and TMEM base this lets ptxas keep every
-// descriptor in uniform registers and emit back-to-back UTC*MMA -- a lane predicate or a thread-derived operand
-// costs an ELECT / R2UR / BRA.U.ANY waterfall of ~20 dependent instructions per MMA (measured ~140 cycles per MMA per
-// issuer: that, not the tensor pipe, was what bounded the narrow layers).
-#define W2X_UMMA_VARIANT(NAME, OPCODE)                                                                        \
-    __device__ __forceinline__ void NAME(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,      \
-                                         uint32_t accum) {                                                     \
-        asm volatile("{\n\t.reg .pred p, q;\n\tsetp.ne.b32 p, %4, 0;\n\telect.sync _|q, 0xffffffff;\n\t@q " OPCODE \
-                     " [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),                                                \
-                     "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)                                            \
-                     : "memory");                                                                              \
-    }
-W2X_UMMA_VARIANT(umma_f16, "tcgen05.mma.cta_group::1.kind::f16")
-W2X_UMMA_VARIANT(umma_f8, "tcgen05.mma.cta_group::1.kind::f8f6f4")   // e4m3 x e4m3 -> f32, K = 32 per instruction, twice the f16 rate
-#undef W2X_UMMA_VARIANT
-__device__ __forceinline__ void umma_commit_one(uint32_t bar) {   // whole (converged) warp calls, one elected lane commits
-    asm volatile("{\n\t.reg .pred q;\n\telect.sync _|q, 0xffffffff;\n\t@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}" ::"r"(bar) : "memory");
-}
-
-// arrive on an mbarrier once every previously issued tcgen05.mma of this thread has completed
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// 32 lanes x 32 columns of fp32: thread i of the warp receives TMEM lane (base_lane + i), 32 consecutive columns
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// wait::ld that also names the destination registers of the load it waits for, so the compiler cannot move their first
-// use above the wait when another tcgen05.ld has already been issued in between (software-pipelined epilogue)
-__device__ __forceinline__ void tmem_ld_wait_dep(uint32_t (&r)[32]) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "+r"(r[8]),
-                   "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]), "+r"(r[16]),
-                   "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]), "+r"(r[22]), "+r"(r[23]), "+r"(r[24]),
-                   "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]), "+r"(r[30]), "+r"(r[31])
-                 :
-                 : "memory");
-}
-
-// 32 lanes x 32 columns of zeros into TMEM (the strip kernel hands accumulator blocks back zeroed, so every MMA accumulates)
-__device__ __forceinline__ void tmem_st32_zero(uint32_t taddr) {
-    const uint32_t z = 0u;
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, "
-        "%1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1};"
-        ::"r"(taddr), "r"(z)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
 __device__ __forceinline__ void sts128(uint32_t addr, uint4 v) {
     asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
 }
@@ -178,81 +91,19 @@ __device__ __forceinline__ uint4 lds128(uint32_t addr) {
 // ================================================================================================
 // Descriptors
 // ================================================================================================
-// Shared-memory matrix descriptor (K-major, swizzled).  Field layout as in CUTLASS
-// cute/arch/mma_sm100_desc.hpp (UMMA::SmemDescriptor): start address >>4 in [0,14), leading byte
-// offset >>4 in [16,30), stride byte offset >>4 in [32,46), version=1 in [46,48), base_offset in
-// [49,52), layout type in [61,64) (2 = SWIZZLE_128B, 4 = SWIZZLE_64B).
-// Canonical K-major layout, 16-byte units: ((8, n), 2) : ((ROWB/16, SBO), 1) -- eight rows ROWB
-// bytes apart form a group, groups are SBO bytes apart, the swizzle XOR is a function of the
-// shared-memory ADDRESS bits (Swizzle<B,4,3> o smem_ptr), which is what lets a descriptor start
-// anywhere inside a TMA-written box.
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t sbo_bytes, uint32_t layout_type, uint32_t base_off) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr >> 4) & 0x3FFFu);
-    d |= (uint64_t)1u << 16;                               // LBO: unused for swizzled K-major; CUTLASS writes 1
-    d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    d |= (uint64_t)1u << 46;                               // descriptor version (Blackwell)
-    d |= (uint64_t)(base_off & 7u) << 49;
-    d |= (uint64_t)(layout_type & 7u) << 61;
-    return d;
-}
+// wgmma shared-memory matrix descriptor (K-major, swizzled), PTX ISA "Matrix Descriptor Format": start address >>4 in
+// [0,14), leading byte offset >>4 in [16,30) (unused for swizzled K-major; written as 1), stride byte offset >>4 in [32,46),
+// base offset in [49,52) (0: every swizzle pattern here starts 1024-byte aligned), layout type in [62,64)
+// (1 = SWIZZLE_128B, 2 = SWIZZLE_64B, 3 = SWIZZLE_32B).
+// Canonical K-major layout, 16-byte units: ((8, n), 2) : ((ROWB/16, SBO), 1) -- eight rows ROWB bytes apart form a group,
+// groups are SBO bytes apart, the swizzle XOR is a function of the shared-memory ADDRESS bits, which is what lets a
+// descriptor start at any row inside a TMA-written box (the 3x3 taps are start-address offsets).
+enum : uint32_t { SW128 = 1u, SW64 = 2u, SW32 = 3u };
 
-// Everything of a descriptor except the start address (compile-time part).
-__host__ __device__ constexpr uint64_t make_desc_const(uint32_t sbo_bytes, uint32_t layout_type) {
-    return ((uint64_t)1u << 16) | ((uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32) | ((uint64_t)1u << 46) |
-           ((uint64_t)(layout_type & 7u) << 61);
+// Everything of a descriptor except the start address: the high word.
+__host__ __device__ constexpr uint32_t desc_hi(uint32_t sbo_bytes, uint32_t layout_type) {
+    return ((sbo_bytes >> 4) & 0x3FFFu) | (layout_type << 30);
 }
-
-// Instruction descriptor (UMMA::InstrDescriptor): c_format F32 (1) at [4,6), a/b format F16 (0) at
-// [7,10)/[10,13), a/b major K (0) at 15/16, N>>3 at [17,23), M>>4 at [24,29).
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N) {
-    return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-// ---- cluster / cta_group::2 forms used by the CTA-pair kernel ----
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ uint32_t mapa_rank(uint32_t saddr, uint32_t rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(saddr), "r"(rank));
-    return r;
-}
-__device__ __forceinline__ void tma_load_4d_2cta(uint32_t dst, const CUtensorMap *map, uint32_t bar_cluster, int c0, int c1, int c2, int c3) {
-    asm volatile(
-        "{\n\t.reg .pred q;\n\telect.sync _|q, 0xffffffff;\n\t@q cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];\n\t}"
-        ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar_cluster), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_2cta(uint32_t dst, const CUtensorMap *map, uint32_t bar_cluster, int c0, int c1) {
-    asm volatile(
-        "{\n\t.reg .pred q;\n\telect.sync _|q, 0xffffffff;\n\t@q cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];\n\t}"
-        ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar_cluster), "r"(c0), "r"(c1)
-        : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar_cluster) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(bar_cluster) : "memory");
-}
-#define W2X_UMMA2_VARIANT(NAME, OPCODE)                                                                       \
-    __device__ __forceinline__ void NAME(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,      \
-                                         uint32_t accum) {                                                     \
-        asm volatile("{\n\t.reg .pred p, q;\n\tsetp.ne.b32 p, %4, 0;\n\telect.sync _|q, 0xffffffff;\n\t@q " OPCODE \
-                     " [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),                                                \
-                     "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)                                            \
-                     : "memory");                                                                              \
-    }
-W2X_UMMA2_VARIANT(umma2_f16, "tcgen05.mma.cta_group::2.kind::f16")
-W2X_UMMA2_VARIANT(umma2_f8, "tcgen05.mma.cta_group::2.kind::f8f6f4")
-#undef W2X_UMMA2_VARIANT
-__device__ __forceinline__ void umma2_commit_one(uint32_t bar) {   // arrives on `bar` in BOTH CTAs of the pair; one elected lane commits
-    asm volatile(
-        "{\n\t.reg .pred q;\n\telect.sync _|q, 0xffffffff;\n\t"
-        "@q tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n\t}" ::"r"(bar),
-        "h"((uint16_t)3)
-        : "memory");
+__device__ __forceinline__ uint64_t make_desc(uint32_t hi32, uint32_t saddr) {
+    return ((uint64_t)hi32 << 32) | (uint64_t)(((saddr >> 4) & 0x3FFFu) | (1u << 16));
 }

@@ -1,6 +1,6 @@
-// tc_strip_plan.h -- the row-strip kernel's schedule as plain integer arithmetic, shared by the kernel's MMA issuer
-// (tc_strip_kernel.cuh) and a CPU test that replays it against the reference model (tests/test_strip_kernel_model.py,
-// tests/cpp/strip_plan_dump.cpp).  No CUDA types: compiles with g++ as is.
+// tc_strip_plan.h -- the row-strip design's schedule (narrow layers, ky taps stacked along N, a ring of accumulator blocks)
+// as plain integer arithmetic, checked by a CPU test that replays it against the reference model
+// (tests/test_strip_kernel_model.py, tests/cpp/strip_plan_dump.cpp).  No kernel of this build includes it.  No CUDA types: compiles with g++ as is.
 //
 // A unit is `rows` output rows [y0, y0 + rows) of one 128-pixel column.  Its strips are the input rows r = y0 - 1 + j,
 // j = j_first .. j_last (j_first = 1 at the frame's top edge, j_last = rows at its bottom edge, else 0 .. rows + 1).

@@ -22,7 +22,7 @@ struct Layer {
     std::vector<double> b;   // [n_out]
 };
 
-// Packed operands of one layer for the tcgen05 path (built once per model, host side):
+// Packed operands of one layer for the tensor-core path (built once per model, host side):
 //   bytes = [activation chunk c][tap t][32-channel block kb][part hi|lo][n_out rows x 64 bytes], every
 //   block an exact shared memory image: K-major rows of 32 fp16 channels, 16-byte units XOR-swizzled
 //   (SWIZZLE_64B).  hi = fp16(w * wscale), lo = fp16(w * wscale - hi).
@@ -34,7 +34,7 @@ struct TcPack {
     //   [wh fp16: n_out rows x 64 B, SWIZZLE_64B][wh8 = e4m3(wh * 2^-F8_A): n_out rows x 32 B, SWIZZLE_32B]
     //   [wl8 = e4m3((w*wscale - wh) * 2^F8_C): n_out rows x 32 B, SWIZZLE_32B]
     std::vector<uint8_t> bytes8;
-    // Row-strip kernel images (Cin, Cout <= 64 only, else empty): [chunk][kx] stages with ky-major rows, see model.cpp
+    // Row-strip design images, built only on request by w2x_debug_tc_strip (Cin, Cout <= 64 only, else empty): [chunk][kx] stages with ky-major rows, see model.cpp
     // pack_tc_layer_strip.  strip = f16x3 flavour [wh | wl], strip8 = f8 flavour [wh | wh8 | wl8].
     std::vector<uint8_t> strip, strip8;
 };
@@ -47,7 +47,7 @@ constexpr int F8_A = 10, F8_C = 1;
 
 struct w2x_model {
     std::vector<w2x::Layer> layers;
-    std::vector<w2x::TcPack> tc;   // per layer; empty pack when the layer is not tcgen05-eligible
+    std::vector<w2x::TcPack> tc;   // per layer; empty pack when the layer is not tensor-core-eligible
     bool tc_eligible = false;      // 1->32 ... ->1 chain with every inner layer in {32,64,128}
     uint64_t uid = 0;              // identity for per-context device caches
 };
@@ -55,7 +55,7 @@ struct w2x_model {
 namespace w2x {
 // model.cpp
 int parse_model_json(const char *path, w2x_model **out);
-int finalize_model(w2x_model *m);   // validation + tcgen05 packing
+int finalize_model(w2x_model *m);   // validation + tensor-core packing
 uint16_t f32_to_f16_rn(float f);    // round-to-nearest-even, subnormals kept
 float f16_to_f32(uint16_t h);
 uint8_t f32_to_e4m3_rn(float f);    // OCP e4m3 (max 448, no inf), round-to-nearest-even, saturating (cvt.rn.satfinite.e4m3x2.f32)
