@@ -62,40 +62,55 @@ __device__ __forceinline__ void epilogue_store(const TcParams &p, const float *b
 }
 
 // The last layer folded in: per pixel the nine tap dot products over this layer's activated channels.  The four lanes of
-// a quad hold the pixel's channels (8j + 2q, +1); their partial sums meet through two shuffles.
+// a quad hold the pixel's channels (8j + 2q, +1); their partial sums meet through two shuffles.  The thread's four pixels
+// (h, e) are summed side by side, so each channel pair's nine weight pairs are loaded once (a weight set per pixel would
+// not fit in registers next to the accumulators); per pixel the sums still run over the channels in ascending order.
 template <int COUT>
 __device__ __forceinline__ void epilogue_fuse(const TcParams &p, const float *bias, const float *last_w, const float (&acc)[2][COUT / 2], int wq, int lane,
                                               int fx0, int fy0) {
     const int q = lane & 3, r_lo = wq * 16 + (lane >> 2);
+    float pt[2][2][9];
+#pragma unroll
+    for (int h = 0; h < 2; h++)
+#pragma unroll
+        for (int e = 0; e < 2; e++)
+#pragma unroll
+            for (int t = 0; t < 9; t++) pt[h][e][t] = 0.f;
+#pragma unroll
+    for (int jj = 0; jj < COUT / 8; jj++) {
+        const int ch = 8 * jj + 2 * q;
+        const float2 b2 = *reinterpret_cast<const float2 *>(bias + ch);
+        float2 w[9];
+#pragma unroll
+        for (int t = 0; t < 9; t++) w[t] = *reinterpret_cast<const float2 *>(last_w + t * COUT + ch);
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+#pragma unroll
+            for (int e = 0; e < 2; e++) {
+                const float a0 = activate(acc[h][4 * jj + 2 * e], p.out_scale, b2.x);
+                const float a1 = activate(acc[h][4 * jj + 2 * e + 1], p.out_scale, b2.y);
+#pragma unroll
+                for (int t = 0; t < 9; t++) pt[h][e][t] = fmaf(a1, w[t].y, fmaf(a0, w[t].x, pt[h][e][t]));
+            }
+        }
+    }
 #pragma unroll
     for (int h = 0; h < 2; h++) {
 #pragma unroll
         for (int e = 0; e < 2; e++) {
-            float pt[9];
-#pragma unroll
-            for (int t = 0; t < 9; t++) pt[t] = 0.f;
-#pragma unroll
-            for (int jj = 0; jj < COUT / 8; jj++) {
-#pragma unroll
-                for (int k = 0; k < 2; k++) {
-                    const int ch = 8 * jj + 2 * q + k;
-                    const float a = activate(acc[h][4 * jj + 2 * e + k], p.out_scale, bias[ch]);
-#pragma unroll
-                    for (int t = 0; t < 9; t++) pt[t] = fmaf(a, last_w[t * COUT + ch], pt[t]);
-                }
-            }
+            float (&pe)[9] = pt[h][e];
 #pragma unroll
             for (int t = 0; t < 9; t++) {
-                pt[t] += __shfl_xor_sync(0xffffffffu, pt[t], 1);
-                pt[t] += __shfl_xor_sync(0xffffffffu, pt[t], 2);
+                pe[t] += __shfl_xor_sync(0xffffffffu, pe[t], 1);
+                pe[t] += __shfl_xor_sync(0xffffffffu, pe[t], 2);
             }
             const int row = 64 * h + r_lo + 8 * e;
             const int fx = fx0 + (row & 7), fy = fy0 + (row >> 3);
             if (q == 0 && fy < p.Hp && fx < p.Wp && fy >= p.out_y0 && fy < p.out_y0 + p.out_rows) {
                 float4 *dst = reinterpret_cast<float4 *>(p.partial + ((size_t)fy * p.Wp + fx) * 12);
-                dst[0] = make_float4(pt[0], pt[1], pt[2], pt[3]);
-                dst[1] = make_float4(pt[4], pt[5], pt[6], pt[7]);
-                dst[2] = make_float4(pt[8], 0.f, 0.f, 0.f);
+                dst[0] = make_float4(pe[0], pe[1], pe[2], pe[3]);
+                dst[1] = make_float4(pe[4], pe[5], pe[6], pe[7]);
+                dst[2] = make_float4(pe[8], 0.f, 0.f, 0.f);
             }
         }
     }
@@ -106,9 +121,20 @@ __device__ __forceinline__ void epilogue_fuse(const TcParams &p, const float *bi
 // ================================================================================================
 // Persistent, one CTA per SM, tile-sets of 16x16 output pixels round-robin over the CTAs.  Each consumer warpgroup owns an
 // 8-wide x 16-tall M-tile (two m64 wgmma halves: halo rows 0..7 and 8..15), N = Cout; the 3x3 taps are descriptor start
-// offsets into the staged 18x18 box.  Per tap one wgmma group is committed and the one before it waited for, so a weight
-// stage (and, after the ninth tap, an activation slot) is handed back while the next group runs (F8: every group of a tap has
-// completed when its e4m3 corrections are added in; the other warpgroup keeps the tensor core busy meanwhile).
+// offsets into the staged 18x18 box.  Every commit is followed by a wait for the group before it, so one group is always in
+// flight while the warpgroup works on the previous one's results.  f16x3: one group per tap.  F8: one group per (half h,
+// 64-column slice s) of a tap, [h's f16 product if s == 0 | the slice's two e4m3 corrections into a fresh buffer]; the
+// buffers alternate between two register sets, and a group's buffer is added to acc[h] once the NEXT group has been issued
+// (that group never writes acc[h]: it is a correction-only group or the other half's).  Per accumulator element the order
+// stays f16 product of tap t, correction of tap t, f16 product of tap t + 1.  A weight stage is handed back once every group
+// reading it has completed: after the first wait of the next tap (F8: tap 8's stage and the activation slot after the wait
+// for all groups that ends each 32-channel chunk).
+//
+// Register budget: 384 threads at one CTA per SM get 168 registers each.  The producer warpgroup (warps 0-3) drops to
+// PRODUCER_REGS, and the consumer warpgroups take the rest: the accumulators alone are COUT fp32 registers per thread.
+constexpr uint32_t PRODUCER_REGS = 40, CONSUMER_REGS = 232;
+static_assert(128 * PRODUCER_REGS + 256 * CONSUMER_REGS == NUM_THREADS * 168, "register hand-off must balance");
+
 template <int CIN, int COUT, bool FUSE, bool F8>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 tc_conv3x3_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ TcParams p) {
@@ -153,128 +179,157 @@ tc_conv3x3_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_cons
         for (int i = threadIdx.x; i < 9 * COUT; i += NUM_THREADS) prm[COUT + i] = p.last_w[i];
     __syncthreads();
 
-    if (warp == 0) {
-        // ===================== A producer: one halo'd box of records per (tile-set, 32-channel block) ==============
-        // (whole warp walks the loop; the arrive and the TMA instructions elect one lane)
-        uint32_t it = 0;
-        unsigned long long w_a = 0;
-        for (int ts = blockIdx.x; ts < p.n_tilesets; ts += gridDim.x) {
-            const int ty = ts / p.tiles_x, tx = ts - ty * p.tiles_x;
-            const int x0 = tx * REGION - 1, y0 = p.out_y0 + ty * REGION - 1;   // box origin incl. ring (may be -1); tile-sets tile the store window
-            for (int c = 0; c < C::NCHUNK; c++, it++) {
-                const uint32_t slot = it & 1u, round = it >> 1;
-                mbar_wait_prof(a_empty(slot), (round & 1u) ^ 1u, prof_on, w_a);
-                mbar_arrive_expect_tx(a_full(slot), (uint32_t)C::A_TX);
-                tma_load_4d(a_base + slot * C::A_SLOT, &tmap_in, a_full(slot), 0, c, x0, y0);
+    if (warp < 4) {
+        setmaxnreg_dec<PRODUCER_REGS>();   // all four warps, idle warps 2 and 3 included: the instruction is warpgroup-wide
+        if (warp == 0) {
+            // ===================== A producer: one halo'd box of records per (tile-set, 32-channel block) ==============
+            // (whole warp walks the loop; the arrive and the TMA instructions elect one lane)
+            uint32_t it = 0;
+            unsigned long long w_a = 0;
+            for (int ts = blockIdx.x; ts < p.n_tilesets; ts += gridDim.x) {
+                const int ty = ts / p.tiles_x, tx = ts - ty * p.tiles_x;
+                const int x0 = tx * REGION - 1, y0 = p.out_y0 + ty * REGION - 1;   // box origin incl. ring (may be -1); tile-sets tile the store window
+                for (int c = 0; c < C::NCHUNK; c++, it++) {
+                    const uint32_t slot = it & 1u, round = it >> 1;
+                    mbar_wait_prof(a_empty(slot), (round & 1u) ^ 1u, prof_on, w_a);
+                    mbar_arrive_expect_tx(a_full(slot), (uint32_t)C::A_TX);
+                    tma_load_4d(a_base + slot * C::A_SLOT, &tmap_in, a_full(slot), 0, c, x0, y0);
+                }
             }
-        }
-        if (prof_on && lane == 0) prof[PROF_APROD_WAIT] += w_a;
-    } else if (warp == 1) {
-        // ===================== B producer: stream the packed weights in consumption order ============
-        uint32_t stage = 0, phase = 0;
-        unsigned long long w_b = 0;
-        const uint8_t *src = reinterpret_cast<const uint8_t *>(p.wpack);
-        for (int ts = blockIdx.x; ts < p.n_tilesets; ts += gridDim.x) {
-            if (C::RESIDENT && ts != (int)blockIdx.x) break;           // resident weights: one pass fills every stage for good
-            for (int blk = 0; blk < C::STAGES_PER_TILESET; blk++) {
-                if constexpr (!C::RESIDENT) mbar_wait_prof(b_empty(stage), phase ^ 1u, prof_on, w_b);
-                mbar_arrive_expect_tx(b_full(stage), C::B_STAGE);
-                bulk_load(b_base + stage * C::B_STAGE, src + (size_t)blk * C::B_STAGE, C::B_STAGE, b_full(stage));
-                if (++stage == (uint32_t)C::NB) { stage = 0; phase ^= 1u; }
+            if (prof_on && lane == 0) prof[PROF_APROD_WAIT] += w_a;
+        } else if (warp == 1) {
+            // ===================== B producer: stream the packed weights in consumption order ============
+            uint32_t stage = 0, phase = 0;
+            unsigned long long w_b = 0;
+            const uint8_t *src = reinterpret_cast<const uint8_t *>(p.wpack);
+            for (int ts = blockIdx.x; ts < p.n_tilesets; ts += gridDim.x) {
+                if (C::RESIDENT && ts != (int)blockIdx.x) break;           // resident weights: one pass fills every stage for good
+                for (int blk = 0; blk < C::STAGES_PER_TILESET; blk++) {
+                    if constexpr (!C::RESIDENT) mbar_wait_prof(b_empty(stage), phase ^ 1u, prof_on, w_b);
+                    mbar_arrive_expect_tx(b_full(stage), C::B_STAGE);
+                    bulk_load(b_base + stage * C::B_STAGE, src + (size_t)blk * C::B_STAGE, C::B_STAGE, b_full(stage));
+                    if (++stage == (uint32_t)C::NB) { stage = 0; phase ^= 1u; }
+                }
             }
+            if (prof_on && lane == 0) prof[PROF_BPROD_WAIT] += w_b;
         }
-        if (prof_on && lane == 0) prof[PROF_BPROD_WAIT] += w_b;
-    } else if (warp >= 4) {
+    } else {
+        setmaxnreg_inc<CONSUMER_REGS>();
         // ===================== consumers: warpgroup wg = M-tile wg (pixels x in [8 wg, 8 wg + 8) of the tile-set) ===========
         const int wg = (warp - 4) >> 2, wq = warp & 3;
         constexpr uint32_t ROWB = C::ROWB;
         constexpr uint32_t A_HI = desc_hi(HALO * ROWB, SW128);      // next 8-pixel group = next halo row
         constexpr uint32_t B_HI = desc_hi(8 * 64, SW64);             // fp16 weight rows of 64 B
         constexpr uint32_t HALF = 8 * HALO * ROWB;                   // second m64 half: eight halo rows down
+        // F8: e4m3 corrections of NS columns per wgmma, S slices per half, 2 S groups per tap; group g = h S + s uses buffer g & 1
+        constexpr int NS = COUT < 64 ? COUT : 64, S = COUT / NS, LAST = 2 * S - 1;
+        constexpr uint32_t B8_HI = desc_hi(8 * 32, SW32);            // e4m3 weight rows of 32 B
         float acc[2][COUT / 2];
+        float corr[F8 ? 2 : 1][NS / 2];
 #pragma unroll
         for (int h = 0; h < 2; h++)
 #pragma unroll
             for (int i = 0; i < COUT / 2; i++) acc[h][i] = 0.f;
+        // Adds the correction of the tap's group gq (completed) to the columns of its slice.
+        auto add_corr = [&](int gq) {
+            const int h = gq / S, s = gq % S;
+            acc_fence(corr[gq & 1]);
+            acc_fence(acc[h]);
+#pragma unroll
+            for (int i = 0; i < NS / 2; i++) acc[h][s * (NS / 2) + i] += corr[gq & 1][i];
+            acc_fence(acc[h]);
+        };
         uint32_t a_it = 0, stage = 0, phase = 0, n = 0;
         unsigned long long w_af = 0, w_bf = 0;
         const long long t_begin = clock64();
         for (int ts = blockIdx.x; ts < p.n_tilesets; ts += gridDim.x, n++) {
             const int ty = ts / p.tiles_x, tx = ts - ty * p.tiles_x;
-            int pend_b = -1, pend_a = -1;                            // stage / slot read by the group in flight
+            int pend_b = -1, pend_a = -1;                            // stage / slot read by the groups of the previous tap
+            auto release = [&] {                                     // ... which have all completed
+                if (lane == 0) {
+                    if (!C::RESIDENT && pend_b >= 0) mbar_arrive(b_empty((uint32_t)pend_b));
+                    if (pend_a >= 0) mbar_arrive(a_empty((uint32_t)pend_a));
+                }
+            };
             for (int c = 0; c < C::NCHUNK; c++, a_it++) {
                 const uint32_t slot = a_it & 1u;
                 mbar_wait_prof(a_full(slot), (a_it >> 1) & 1u, prof_on, w_af);
                 const uint32_t a0 = a_base + slot * C::A_SLOT + (uint32_t)wg * 8u * ROWB;
-#pragma unroll 1
+                // F8: the taps are unrolled and the chunk ends with an empty pipe.  A group still in flight across a loop's back
+                // edge while its registers are read after the next wait makes ptxas serialise every wgmma of the loop.
+#pragma unroll(F8 ? 9 : 1)
                 for (int t = 0; t < 9; t++) {
                     const uint32_t tap = (uint32_t)((t / 3) * HALO + t % 3) * ROWB;
                     if (!C::RESIDENT) mbar_wait_prof(b_full(stage), phase, prof_on, w_bf);
                     else if (n == 0) mbar_wait_prof(b_full(stage), 0u, prof_on, w_bf);   // the stages arrive once, during the first tile-set
                     const uint32_t b = b_base + stage * C::B_STAGE;
                     const uint32_t first = (c | t) != 0 ? 1u : 0u;
-                    acc_fence(acc[0]);
-                    acc_fence(acc[1]);
-                    wgmma_fence();
+                    // a record's quarters: +0 / +32 the fp16 K steps, +64 xh8 (f16x3: lo step 0), +96 xl8 (f16x3: lo step 1)
+                    if constexpr (!F8) {
+                        acc_fence(acc[0]);
+                        acc_fence(acc[1]);
+                        wgmma_fence();
 #pragma unroll
-                    for (int h = 0; h < 2; h++) {
-                        const uint32_t ah = a0 + (uint32_t)h * HALF + tap;
-                        // a record's quarters: +0 / +32 the fp16 K steps, +64 xh8 (f16x3: lo step 0), +96 xl8 (f16x3: lo step 1)
-                        Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah), make_desc(B_HI, b), first);
-                        Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah + 32u), make_desc(B_HI, b + 32u), 1u);
-                        if constexpr (!F8) {
+                        for (int h = 0; h < 2; h++) {
+                            const uint32_t ah = a0 + (uint32_t)h * HALF + tap;
+                            Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah), make_desc(B_HI, b), first);                   // xh * wh
+                            Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah + 32u), make_desc(B_HI, b + 32u), 1u);
                             Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah + 64u), make_desc(B_HI, b), 1u);                // xl * wh
                             Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah + 96u), make_desc(B_HI, b + 32u), 1u);
                             Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah), make_desc(B_HI, b + COUT * 64u), 1u);         // xh * wl
                             Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah + 32u), make_desc(B_HI, b + COUT * 64u + 32u), 1u);
                         }
-                    }
-                    if constexpr (F8) {
-                        // Hopper's e4m3 wgmma accumulates in reduced precision, which would also round the fp32 sums it adds to: the
-                        // two corrections of a tap go into a fresh accumulator of NS columns (scale_d = 0) and reach the fp32 sums
-                        // through ordinary adds once that group has completed.
-                        constexpr int NS = COUT < 64 ? COUT : 64;
-                        constexpr uint32_t B8_HI = desc_hi(8 * 32, SW32);    // e4m3 weight rows of 32 B
                         wgmma_commit();
+                        wgmma_wait<1>();                             // the previous group is done: its stage / slot may be refilled
+                        acc_fence(acc[0]);
+                        acc_fence(acc[1]);
+                        release();
+                    } else {
+                        // Hopper's e4m3 wgmma accumulates in reduced precision, which would also round the fp32 sums it adds to: each
+                        // slice's two corrections go into a fresh buffer (scale_d = 0) and reach the fp32 sums through ordinary adds.
 #pragma unroll
                         for (int h = 0; h < 2; h++) {
                             const uint32_t ah = a0 + (uint32_t)h * HALF + tap;
 #pragma unroll
-                            for (int s = 0; s < COUT / NS; s++) {
-                                float corr[NS / 2];
+                            for (int s = 0; s < S; s++) {
+                                const int g = h * S + s;
+                                if (s == 0) acc_fence(acc[h]);
+                                acc_fence(corr[g & 1]);
                                 wgmma_fence();
-                                Wgmma<NS>::e4m3(corr, make_desc(A_HI, ah + 96u), make_desc(B8_HI, b + COUT * 64u + s * NS * 32u), 0u);   // xl8 * wh8
-                                Wgmma<NS>::e4m3(corr, make_desc(A_HI, ah + 64u), make_desc(B8_HI, b + COUT * 96u + s * NS * 32u), 1u);   // xh8 * wl8
+                                if (s == 0) {
+                                    Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah), make_desc(B_HI, b), first);           // xh * wh
+                                    Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah + 32u), make_desc(B_HI, b + 32u), 1u);
+                                }
+                                Wgmma<NS>::e4m3(corr[g & 1], make_desc(A_HI, ah + 96u), make_desc(B8_HI, b + COUT * 64u + s * NS * 32u), 0u);   // xl8 * wh8
+                                Wgmma<NS>::e4m3(corr[g & 1], make_desc(A_HI, ah + 64u), make_desc(B8_HI, b + COUT * 96u + s * NS * 32u), 1u);   // xh8 * wl8
                                 wgmma_commit();
-                                wgmma_wait<0>();                             // (also completes the f16 group before acc is touched)
-                                acc_fence(corr);
-                                acc_fence(acc[h]);
-#pragma unroll
-                                for (int i = 0; i < NS / 2; i++) acc[h][s * (NS / 2) + i] += corr[i];
+                                wgmma_wait<1>();                             // every group but this one has completed
+                                if (g > 0) {
+                                    add_corr(g - 1);
+                                } else if (t > 0) {                          // the previous tap's last group
+                                    add_corr(LAST);
+                                    release();
+                                }
                             }
                         }
-                    }
-                    if constexpr (!F8) {
-                        wgmma_commit();
-                        wgmma_wait<1>();                             // the previous group is done: its stage / slot may be refilled
-                    }
-                    acc_fence(acc[0]);
-                    acc_fence(acc[1]);
-                    if (lane == 0) {
-                        if (!C::RESIDENT && pend_b >= 0) mbar_arrive(b_empty((uint32_t)pend_b));
-                        if (pend_a >= 0) mbar_arrive(a_empty((uint32_t)pend_a));
                     }
                     pend_b = (int)stage;
                     pend_a = t == 8 ? (int)slot : -1;
                     if (++stage == (uint32_t)C::NB) { stage = 0; phase ^= 1u; }
                 }
+                if constexpr (F8) {
+                    wgmma_wait<0>();
+                    acc_fence(acc[0]);
+                    acc_fence(acc[1]);
+                    add_corr(LAST);
+                    release();
+                }
             }
-            wgmma_wait<0>();
-            acc_fence(acc[0]);
-            acc_fence(acc[1]);
-            if (lane == 0) {
-                if (!C::RESIDENT) mbar_arrive(b_empty((uint32_t)pend_b));
-                mbar_arrive(a_empty((uint32_t)pend_a));
+            if constexpr (!F8) {
+                wgmma_wait<0>();
+                acc_fence(acc[0]);
+                acc_fence(acc[1]);
+                release();
             }
             if constexpr (FUSE)
                 epilogue_fuse<COUT>(p, prm, prm + COUT, acc, wq, lane, tx * REGION + 8 * wg, p.out_y0 + ty * REGION);

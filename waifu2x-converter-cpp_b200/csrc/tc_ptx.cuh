@@ -19,27 +19,27 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t byt
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
-// Spin on try_wait; a protocol bug must not hang the GPU, so give up (trap -> launch error) after ~4 s.
+// Spin on try_wait; a protocol bug must not hang the GPU, so give up (trap -> launch error) after ~4 s.  The whole loop is
+// one asm block: a __trap() in the C++ control flow makes ptxas serialise the wgmmas that are in flight across the wait.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-    uint32_t done = 0;
-    long long t0 = 0;
-    for (uint32_t spins = 0;; spins++) {
-        asm volatile(
-            "{\n\t"
-            ".reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t"
-            "}"
-            : "=r"(done)
-            : "r"(bar), "r"(parity)
-            : "memory");
-        if (done) return;
-        if ((spins & 1023u) == 1023u) {
-            long long now = clock64();
-            if (t0 == 0) t0 = now;
-            else if (now - t0 > 8000000000LL) __trap();
-        }
-    }
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        ".reg .u64 t0, t1;\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
+        "@p bra DONE;\n\t"
+        "mov.u64 t0, %%clock64;\n"
+        "WAIT:\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
+        "@p bra DONE;\n\t"
+        "mov.u64 t1, %%clock64;\n\t"
+        "sub.u64 t1, t1, t0;\n\t"
+        "setp.lt.u64 p, t1, 8000000000;\n\t"
+        "@p bra WAIT;\n\t"
+        "trap;\n"
+        "DONE:\n\t"
+        "}" ::"r"(bar), "r"(parity)
+        : "memory");
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
@@ -78,6 +78,13 @@ __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wa
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap *map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
+
+// Per-thread register limit of the executing warpgroup (all four warps execute it, converged): .dec hands registers back
+// to the CTA's pool, .inc waits until the pool holds enough and takes them.
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 __device__ __forceinline__ void sts128(uint32_t addr, uint4 v) {
     asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
