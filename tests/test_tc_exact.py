@@ -34,64 +34,15 @@ import torch
 import torch.nn.functional as F
 
 import tc_numerics_model as T
+from exact_arith import (F8_A, F8_C, F32, e4m3, emulate_first_layer, emulate_last_fused, emulate_last_separate,
+                         f16, fma32, mul32, readback, tc_activation)
 
 SHAPES = [(32, 32), (32, 64), (32, 128), (64, 32), (64, 64), (64, 128), (128, 32), (128, 64), (128, 128)]
 PRECISIONS = ["f16x3", "f16+f8x2"]
-F8_A, F8_C = 10, 1                 # xl8 = e4m3(xl * 2^F8_A), xh8 = e4m3(xh * 2^-F8_C)   (csrc/tc_config.cuh)
 Q = 2.0 ** -4
 SUM_MAX_Q = 2 ** 22                # (b); the cases below reach 2^21.3 (128 input channels)
 GROUP_MAX_Q = 64                   # (c); the cases below reach 45
 LATTICE_WSCALE = 2.0 ** 10
-F32 = np.float32
-
-
-# ---------------------------------------------------------------------------------------------------------------------
-# float32 / fp16 / e4m3 arithmetic, rounded the way the kernels round
-# ---------------------------------------------------------------------------------------------------------------------
-def f16(x):
-    """round to fp16 (nearest, ties to even) and back to float32"""
-    return np.asarray(x, F32).astype(np.float16).astype(F32)
-
-
-def e4m3(x):
-    """nearest e4m3fn value (ties to even, saturating at +-448: cvt.rn.satfinite.e4m3), as float64"""
-    x = np.asarray(x, np.float64)
-    a = np.abs(x)
-    _, e = np.frexp(np.maximum(a, 2.0 ** -6))            # a = m 2^e, m in [0.5, 1): the binade's quantum is 2^(e - 4)
-    quantum = np.ldexp(1.0, e - 4)
-    return np.copysign(np.minimum(np.rint(a / quantum) * quantum, 448.0), x)
-
-
-def fma32(a, b, c):
-    """correctly rounded float32 fmaf(a, b, c): the float64 product is exact, the float64 sum is rounded to odd (TwoSum
-    gives its error), and a round-to-odd value with 29 spare bits rounds to the same float32 as the exact sum"""
-    a, b, c = (np.asarray(t, F32).astype(np.float64) for t in (a, b, c))
-    p = a * b
-    s = p + c
-    bb = s - p
-    err = (p - (s - bb)) + (c - bb)
-    s = np.ascontiguousarray(s)
-    even = (s.view(np.int64) & 1) == 0
-    s = np.where((err != 0) & even, np.nextafter(s, np.where(err > 0, np.inf, -np.inf)), s)
-    return s.astype(F32)
-
-
-def add32(a, b):
-    return (np.asarray(a, F32) + np.asarray(b, F32)).astype(F32)
-
-
-def mul32(a, b):
-    return (np.asarray(a, F32) * np.asarray(b, F32)).astype(F32)
-
-
-def leaky_tc(v):
-    """the tensor-core epilogue's and the first layer's leaky-ReLU: fmaxf(v, 0.1f * v)"""
-    return np.maximum(v, mul32(v, F32(0.1)))
-
-
-def leaky_last(r):
-    """last_layer_kernel / last_gather_kernel: fminf(r, 0) * 0.1f + fmaxf(r, 0)"""
-    return add32(mul32(np.minimum(r, F32(0)), F32(0.1)), np.maximum(r, F32(0)))
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -170,21 +121,10 @@ def accumulate(pairs, exact=True):
     return acc.numpy().astype(F32)
 
 
-def tc_activation(acc32, ws, bias):
-    """epilogue: v = leaky(fmaf(acc, 1 / wscale, 16 bias)) -- activations * 16 (ACT_SCALE folded in on the host)"""
-    b16 = mul32(np.asarray(bias, np.float64).astype(F32), F32(16))
-    return leaky_tc(fma32(acc32, F32(1.0 / ws), b16[:, None, None]))
 
 
-def record_lo(v, f8):
-    """what the frame's record keeps besides fp16(v), read back as float32: fp16(v - hi) or e4m3((v - hi) 2^10) 2^-10"""
-    d = np.asarray(v, F32) - f16(v)                                   # exact
-    return (e4m3(d.astype(np.float64) * 2.0 ** F8_A) * 2.0 ** -F8_A).astype(F32) if f8 else f16(d)
 
 
-def readback(v, f8):
-    """nhwc_to_planar: (hi + lo) / 16"""
-    return mul32(add32(f16(v), record_lo(v, f8)), F32(1.0 / 16))
 
 
 def emulate_filter_layer(planes, w, b, f8, exact=True):
@@ -194,20 +134,6 @@ def emulate_filter_layer(planes, w, b, f8, exact=True):
     return readback(tc_activation(accumulate(pairs, exact), ws, b), f8)
 
 
-def emulate_first_layer(frame, w0, b0):
-    """first_layer_kernel on a frame (the replicate-padded plane), replicate ring again at the frame edge: per channel
-    t = (16 w[0]) v[0], then fmaf over taps 1..8, + 16 b, leaky"""
-    p = np.pad(frame, 1, mode="edge")
-    h, wd = frame.shape
-    w16 = mul32(w0[:, 0], F32(16))                                    # [C, 3, 3]
-    b16 = mul32(np.asarray(b0, np.float64).astype(F32), F32(16))[:, None, None]
-    taps = [(ky, kx) for ky in range(3) for kx in range(3)]
-    t = None
-    for ky, kx in taps:
-        v = p[None, ky:ky + h, kx:kx + wd]
-        wk = w16[:, ky, kx][:, None, None]
-        t = mul32(wk, v) if t is None else fma32(wk, v, t)
-    return leaky_tc(add32(t, b16))
 
 
 def emulate_model(plane, model, f8, fused):
@@ -215,41 +141,11 @@ def emulate_model(plane, model, f8, fused):
     (w0, b0), (w1, b1), (w2, b2) = model
     n = 3
     frame = np.pad(plane, n, mode="edge")
-    ph, pw = frame.shape
     x16 = emulate_first_layer(frame, w0, b0)
     pairs, ws = operands(x16, w1, f8)
     zpad = [(np.pad(a, ((0, 0), (1, 1), (1, 1))), b) for a, b in pairs]     # the TMA loads zero-fill outside the frame
     a1 = tc_activation(accumulate(zpad), ws, b1)                      # [C2, ph, pw], activations * 16
-    c2 = a1.shape[0]
-    bias = F32(b2[0])
-    oy, ox = slice(n, ph - n), slice(n, pw - n)
-    if fused:
-        # epilogue_fuse: lane q of a quad sums channels 8 jj + 2q, +1 (jj ascending) with weights / 16, then two shuffles
-        lw = mul32(w2[0], F32(1.0 / 16)).reshape(c2, 9)
-        part = np.zeros((4, 9, ph, pw), F32)
-        for jj in range(c2 // 8):
-            ch = 8 * jj + 2 * np.arange(4)
-            part = fma32(a1[ch][:, None], lw[ch][:, :, None, None], part)
-            part = fma32(a1[ch + 1][:, None], lw[ch + 1][:, :, None, None], part)
-        P = add32(add32(part[0], part[1]), add32(part[2], part[3]))   # [9, ph, pw]
-        # last_gather_kernel: taps in row-major order
-        acc = np.zeros((ph - 2 * n, pw - 2 * n), F32)
-        for t in range(9):
-            ky, kx = divmod(t, 3)
-            acc = add32(acc, P[t, n - 1 + ky:ph - n - 1 + ky, n - 1 + kx:pw - n - 1 + kx])
-        return leaky_last(add32(acc, bias))
-    # last_layer_kernel: the record read back as (hi + lo) / 16; per group of 8 channels eight partial sums over the taps
-    a = mul32(add32(f16(a1), record_lo(a1, f8)), F32(1.0 / 16))
-    acc = np.zeros((ph - 2 * n, pw - 2 * n), F32)
-    for c8 in range(c2 // 8):
-        cs = slice(8 * c8, 8 * c8 + 8)
-        t = np.zeros((8,) + acc.shape, F32)
-        for ky in range(3):
-            for kx in range(3):
-                t = fma32(w2[0, cs, ky, kx][:, None, None], a[cs, n - 1 + ky:ph - n - 1 + ky, n - 1 + kx:pw - n - 1 + kx], t)
-        for e in range(8):
-            acc = add32(acc, t[e])
-    return leaky_last(add32(acc, bias))
+    return emulate_last_fused(a1, w2, b2, n) if fused else emulate_last_separate(a1, w2, b2, n, f8)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
