@@ -111,9 +111,16 @@ W2X_API int w2x_ctx_get_engine(const w2x_ctx *ctx);
  *   W2X_PRECISION_F16_F8X2  (default) the two correction products run on e4m3 copies of the operands at twice
  *                           the tensor rate: 2.0 instead of 3.0 pass-equivalents; measured on H100: <= 2.2e-5
  *                           max-abs on white noise, <= 5.9e-6 on a smooth image; 357 Mpix/s on the same pass and card
- * The environment variable W2X_PRECISION=f16x3|f8 sets the initial value of new contexts. */
+ *   W2X_PRECISION_F16       one fp16 product per MAC (xh*wh) with fp32 accumulation: a different accuracy contract,
+ *                           NOT held to the 1e-4 gate; 8-bit outputs (rint(255 y)) stay within 1 LSB of the
+ *                           reference's.  Measured on H100 (tools/precision_bench.py): 9.0e-4 max-abs against the
+ *                           fp32 engine on sampled rows of a 4096x4096 white-noise scale2.0x pass (2.1 % of the 8-bit
+ *                           values change, by 1); 566 Mpix/s on that pass against the default's 309 in the same run,
+ *                           H100 80GB HBM3 at a 400 W power limit
+ * The environment variable W2X_PRECISION=f16x3|f8|f16 sets the initial value of new contexts. */
 #define W2X_PRECISION_F16X3 0
 #define W2X_PRECISION_F16_F8X2 1
+#define W2X_PRECISION_F16 2
 W2X_API int w2x_ctx_set_precision(w2x_ctx *ctx, int precision);
 W2X_API int w2x_ctx_get_precision(const w2x_ctx *ctx);
 /* Run on a caller-owned CUDA stream (cudaStream_t passed as void*); NULL = the ctx's own stream. */
@@ -291,7 +298,8 @@ W2X_API int w2x_ctx_set_timing(w2x_ctx *ctx, int enabled);
 W2X_API int w2x_ctx_layer_times(w2x_ctx *ctx, int max_layers, float *ms, int *launches,
                                 int *n_layers_out, int reset);
 /* Name of the kernel family the last convert call used for `layer` ("fp32_direct",
- * "wgmma_f16x3", "first_1xN", "last_Nx1"). */
+ * "wgmma_f16x3", "wgmma_f16+f8x2", "wgmma_f16", each with "+last" when the last layer is folded in, "first_1xN",
+ * "last_Nx1", "last_gather"). */
 W2X_API const char *w2x_ctx_layer_kernel_name(const w2x_ctx *ctx, int layer);
 
 #ifdef __cplusplus

@@ -16,7 +16,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB_PATH = os.path.join(_HERE, "libw2x_b200.so")
 
 ENGINE_AUTO, ENGINE_FP32, ENGINE_TC = 0, 1, 2
-PRECISION_F16X3, PRECISION_F16_F8X2 = 0, 1
+PRECISION_F16X3, PRECISION_F16_F8X2, PRECISION_F16 = 0, 1, 2
 WALK_FUSED, WALK_BLOCKS = 0, 1
 
 STATUS = {0: "W2X_OK", 1: "W2X_ERR_ARG", 2: "W2X_ERR_IO", 3: "W2X_ERR_PARSE", 4: "W2X_ERR_MODEL",

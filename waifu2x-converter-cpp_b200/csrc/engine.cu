@@ -163,12 +163,13 @@ int launch_layer_tc(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int li, cons
     {
         LayerTimer t(ctx, li);
         CU_CHECK(tc::launch_tc_layer(in, f8 ? (const void *)dm->pack8[(size_t)li] : (const void *)dm->pack[(size_t)li],
-                                     dm->b_host[(size_t)li].data(), out, L.n_in, L.n_out, pw, ph, dm->out_scale[(size_t)li], f8,
+                                     dm->b_host[(size_t)li].data(), out, L.n_in, L.n_out, pw, ph, dm->out_scale[(size_t)li], ctx->precision,
                                      ctx->num_sms, ctx->stream,
                                      profile && ctx->prof_buf ? ctx->prof_buf + (size_t)li * tc::PROF_MAX_CTAS * tc::PROF_WORDS : nullptr,
                                      fused ? dm->last_w_t.data() : nullptr, fused ? reinterpret_cast<float *>(out) : nullptr, out_y0, out_rows));
     }
-    note_kernel(ctx, li, f8 ? (fused ? "wgmma_f16+f8x2+last" : "wgmma_f16+f8x2") : (fused ? "wgmma_f16x3+last" : "wgmma_f16x3"));
+    static const char *const names[3][2] = {{"wgmma_f16x3", "wgmma_f16x3+last"}, {"wgmma_f16+f8x2", "wgmma_f16+f8x2+last"}, {"wgmma_f16", "wgmma_f16+last"}};
+    note_kernel(ctx, li, names[ctx->precision][fused ? 1 : 0]);
     ctx->launches++;
     return W2X_OK;
 }
@@ -386,6 +387,7 @@ int w2x_ctx_create(int device, w2x_ctx **out_ctx) {
     if (const char *pe = std::getenv("W2X_PRECISION")) {
         if (!std::strcmp(pe, "f16x3")) ctx->precision = W2X_PRECISION_F16X3;
         else if (!std::strcmp(pe, "f16+f8x2") || !std::strcmp(pe, "f8")) ctx->precision = W2X_PRECISION_F16_F8X2;
+        else if (!std::strcmp(pe, "f16")) ctx->precision = W2X_PRECISION_F16;
     }
     CU_CHECK(cudaStreamCreateWithFlags(&ctx->copy_in, cudaStreamNonBlocking));
     CU_CHECK(cudaStreamCreateWithFlags(&ctx->copy_out, cudaStreamNonBlocking));
@@ -451,7 +453,7 @@ int w2x_ctx_get_engine(const w2x_ctx *ctx) { return ctx ? ctx->engine : -1; }
 
 int w2x_ctx_set_precision(w2x_ctx *ctx, int precision) {
     if (check_ctx(ctx)) return W2X_ERR_ARG;
-    if (precision != W2X_PRECISION_F16X3 && precision != W2X_PRECISION_F16_F8X2) return fail(W2X_ERR_ARG, "unknown precision mode %d", precision);
+    if (precision != W2X_PRECISION_F16X3 && precision != W2X_PRECISION_F16_F8X2 && precision != W2X_PRECISION_F16) return fail(W2X_ERR_ARG, "unknown precision mode %d", precision);
     ctx->precision = precision;
     return W2X_OK;
 }

@@ -43,7 +43,7 @@ struct w2x_ctx {
     int engine = W2X_ENGINE_AUTO;
     int walk = W2X_WALK_FUSED;
     bool fuse_last = true;             // fold the N->1 last layer into the preceding tensor-core layer's epilogue
-    int precision = W2X_PRECISION_F16_F8X2;   // default; W2X_PRECISION=f16x3 in the environment or w2x_ctx_set_precision() selects the 3 x fp16 scheme
+    int precision = W2X_PRECISION_F16_F8X2;   // default; W2X_PRECISION=f16x3|f16 in the environment or w2x_ctx_set_precision() selects another scheme
     cudaStream_t own_stream = nullptr;
     cudaStream_t stream = nullptr;
     size_t scratch_limit = (size_t)16 << 30;

@@ -63,9 +63,10 @@ cudaError_t launch_first(const FirstSource &src, int pw, int ph, const float *wg
                          cudaStream_t s, int f8 = 0, int out_y0 = 0, int out_rows = -1);
 // Tensor-core (wgmma) layer: in/out NHWC frames (pw x ph); the tensor maps are built inside.
 // `bias` is a HOST pointer to the layer's (float)bias values (they travel as kernel parameters).
-// f8 = 0: "f16x3" frames [hi][lo], wpack = TcPack::bytes;  f8 = 1: frames [xh][xh8][xl8], wpack = TcPack::bytes8.
+// mode = W2X_PRECISION_*: F16X3 (0) and F16 (2): "f16x3" frames [hi][lo], wpack = TcPack::bytes (F16 reads only its wh
+// halves);  F16_F8X2 (1): frames [xh][xh8][xl8], wpack = TcPack::bytes8.
 cudaError_t launch_tc_layer(const __half *in, const void *wpack, const float *bias, __half *out,
-                            int cin, int cout, int pw, int ph, float out_scale, int f8, int num_sms,
+                            int cin, int cout, int pw, int ph, float out_scale, int mode, int num_sms,
                             cudaStream_t s, unsigned long long *prof = nullptr, const float *last_w = nullptr,
                             float *partial = nullptr, int out_y0 = 0, int out_rows = -1);
 // Frames: every activation between layers is a RECORD frame [Hp][Wp][C/32][128 B] -- one 128-byte record per pixel per

@@ -7,10 +7,12 @@
 // (wgmma.mma_async, fp32 accumulators in registers).  fp32 fidelity comes from a 2-term split of
 // both operands (x = xh + xl, w = wh + wl, h = the fp16 rounding) and three accumulated products
 // xh*wh + xl*wh + xh*wl (the dropped xl*wl term is ~2^-22 relative); SURVEY.md section 7 shows a
-// single fp16/tf32 pass misses the 1e-4 gate by 10x.  Two arithmetic modes (template flag F8):
+// single fp16/tf32 pass misses the 1e-4 gate by 10x.  Three arithmetic modes (template flag F8, TcParams::xh_only):
 //   f16x3      all three products as f16 wgmmas on fp16 hi/lo planes
 //   f16+f8x2   xh*wh as f16; the two correction products as e4m3 wgmmas on e4m3 copies of the
 //              operands (K = 32 per instruction, twice the rate) -- the default, 2.0 instead of 3.0 passes
+//   f16        xh*wh alone, by the f16x3 kernels on the f16x3 frames and weights: 1.0 pass, not
+//              fp32-faithful (8-bit outputs within 1 LSB); chosen by the caller, never by default
 //
 // Data layout in HBM: every activation is an NHWC "frame" of 4 bytes per element holding value*ACT_SCALE,
 // [hi fp16][lo fp16] or [xh fp16][xh8 e4m3][xl8 e4m3] planes of [Hp][Wp][C]; all layers of one pass share
@@ -37,8 +39,10 @@
 #include <cstdint>
 #include <cstdlib>
 #include <cstdio>
+#include <type_traits>
 
 #include "kernels.h"
+#include "w2x_b200.h"
 
 namespace w2x {
 namespace tc {
@@ -107,7 +111,7 @@ static cudaError_t launch_one(const CUtensorMap *tmap, const CUtensorMap *omap, 
 static int make_rec_map(CUtensorMap *map, const void *base, int C, int Wp, int Hp, int box_w, int box_h, int y0, int rows);
 
 cudaError_t launch_tc_layer(const __half *in, const void *wpack, const float *bias, __half *out, int cin,
-                            int cout, int pw, int ph, float out_scale, int f8, int num_sms, cudaStream_t s,
+                            int cout, int pw, int ph, float out_scale, int mode, int num_sms, cudaStream_t s,
                             unsigned long long *prof, const float *last_w, float *partial, int out_y0, int out_rows) {
     if (out_rows < 0) { out_y0 = 0; out_rows = ph; }
     CUtensorMap tmap_in;
@@ -124,6 +128,7 @@ cudaError_t launch_tc_layer(const __half *in, const void *wpack, const float *bi
     p.tiles_x = (pw + REGION - 1) / REGION;
     p.n_tilesets = p.tiles_x * ((out_rows + REGION - 1) / REGION);   // tile-sets tile the store window (TMA store coordinates stay non-negative)
     p.out_scale = out_scale * ACT_SCALE;
+    p.xh_only = mode == W2X_PRECISION_F16 ? 1 : 0;
     p.prof = prof;
     p.partial = partial;
     if (partial) {
@@ -135,7 +140,7 @@ cudaError_t launch_tc_layer(const __half *in, const void *wpack, const float *bi
     if (partial) omap = tmap_in;
     else if (make_rec_map(&omap, out, cout, pw, ph, 8, 16, out_y0, out_rows)) return cudaErrorInvalidValue;
 #define X(ci, co) \
-    if (cin == ci && cout == co) return launch_one<ci, co>(&tmap_in, &omap, p, num_sms, f8 != 0, s);
+    if (cin == ci && cout == co) return launch_one<ci, co>(&tmap_in, &omap, p, num_sms, mode == W2X_PRECISION_F16_F8X2, s);
     W2X_TC_SHAPES(X)
 #undef X
     return cudaErrorInvalidValue;

@@ -14,6 +14,9 @@
 // F8 = false: three f16 products xh*wh + xl*wh + xh*wl ("f16x3").
 // F8 = true : xh*wh in f16, the two correction products in e4m3 on e4m3 copies
 //             xl8*wh8 + xh8*wl8 (K = 32 per wgmma at twice the rate: 2.0 instead of 3.0 pass-equivalents).
+// F8 = false with TcParams::xh_only ("f16", W2X_PRECISION_F16): xh*wh alone (1.0 pass-equivalent, not fp32-faithful) on the
+//             same f16x3 records and weight image, of which only the wh half of each stage is loaded.  A runtime flag, not
+//             a template parameter: the f16x3 kernels run it, choosing the loop once per tile-set.
 constexpr int F8_A = 10, F8_C = 1;   // xl8 = e4m3((x16 - xh) * 2^F8_A), xh8 = e4m3(xh * 2^-F8_C); must match w2x_internal.h
 
 template <int CIN, int COUT, bool FUSE = false, bool F8 = false>
@@ -65,6 +68,7 @@ struct TcParams {
     // nine tap partials P[t] = sum_c act[c] * w_last[c][t] are written ([Hp][Wp][12] fp32, 3 pad words).
     float *partial;             // nullptr = not fused
     float last_w[9 * 128];      // [9][COUT] tap-major, by value
+    int xh_only;                // F8 = false kernels: 1 = the xh*wh product alone (W2X_PRECISION_F16), 0 = f16x3
 };
 
 // per-CTA profile record (cycles, accumulated over launches)

@@ -122,7 +122,8 @@ __device__ __forceinline__ void epilogue_fuse(const TcParams &p, const float *bi
 // Persistent, one CTA per SM, tile-sets of 16x16 output pixels round-robin over the CTAs.  Each consumer warpgroup owns an
 // 8-wide x 16-tall M-tile (two m64 wgmma halves: halo rows 0..7 and 8..15), N = Cout; the 3x3 taps are descriptor start
 // offsets into the staged 18x18 box.  Every commit is followed by a wait for the group before it, so one group is always in
-// flight while the warpgroup works on the previous one's results.  f16x3: one group per tap.  F8: one group per (half h,
+// flight while the warpgroup works on the previous one's results.  f16x3 (and xh_only, with the xh * wh K steps alone): one
+// group per tap.  F8: one group per (half h,
 // 64-column slice s) of a tap, [h's f16 product if s == 0 | the slice's two e4m3 corrections into a fresh buffer]; the
 // buffers alternate between two register sets, and a group's buffer is added to acc[h] once the NEXT group has been issued
 // (that group never writes acc[h]: it is a correction-only group or the other half's).  Per accumulator element the order
@@ -202,12 +203,13 @@ tc_conv3x3_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_cons
             uint32_t stage = 0, phase = 0;
             unsigned long long w_b = 0;
             const uint8_t *src = reinterpret_cast<const uint8_t *>(p.wpack);
+            const uint32_t b_bytes = !F8 && p.xh_only ? (uint32_t)C::B_BLOCK : (uint32_t)C::B_STAGE;   // xh_only: the wh half of each stage
             for (int ts = blockIdx.x; ts < p.n_tilesets; ts += gridDim.x) {
                 if (C::RESIDENT && ts != (int)blockIdx.x) break;           // resident weights: one pass fills every stage for good
                 for (int blk = 0; blk < C::STAGES_PER_TILESET; blk++) {
                     if constexpr (!C::RESIDENT) mbar_wait_prof(b_empty(stage), phase ^ 1u, prof_on, w_b);
-                    mbar_arrive_expect_tx(b_full(stage), C::B_STAGE);
-                    bulk_load(b_base + stage * C::B_STAGE, src + (size_t)blk * C::B_STAGE, C::B_STAGE, b_full(stage));
+                    mbar_arrive_expect_tx(b_full(stage), b_bytes);
+                    bulk_load(b_base + stage * C::B_STAGE, src + (size_t)blk * C::B_STAGE, b_bytes, b_full(stage));
                     if (++stage == (uint32_t)C::NB) { stage = 0; phase ^= 1u; }
                 }
             }
@@ -251,42 +253,23 @@ tc_conv3x3_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_cons
                     if (pend_a >= 0) mbar_arrive(a_empty((uint32_t)pend_a));
                 }
             };
-            for (int c = 0; c < C::NCHUNK; c++, a_it++) {
-                const uint32_t slot = a_it & 1u;
-                mbar_wait_prof(a_full(slot), (a_it >> 1) & 1u, prof_on, w_af);
-                const uint32_t a0 = a_base + slot * C::A_SLOT + (uint32_t)wg * 8u * ROWB;
-                // F8: the taps are unrolled and the chunk ends with an empty pipe.  A group still in flight across a loop's back
-                // edge while its registers are read after the next wait makes ptxas serialise every wgmma of the loop.
-#pragma unroll(F8 ? 9 : 1)
-                for (int t = 0; t < 9; t++) {
-                    const uint32_t tap = (uint32_t)((t / 3) * HALO + t % 3) * ROWB;
-                    if (!C::RESIDENT) mbar_wait_prof(b_full(stage), phase, prof_on, w_bf);
-                    else if (n == 0) mbar_wait_prof(b_full(stage), 0u, prof_on, w_bf);   // the stages arrive once, during the first tile-set
-                    const uint32_t b = b_base + stage * C::B_STAGE;
-                    const uint32_t first = (c | t) != 0 ? 1u : 0u;
-                    // a record's quarters: +0 / +32 the fp16 K steps, +64 xh8 (f16x3: lo step 0), +96 xl8 (f16x3: lo step 1)
-                    if constexpr (!F8) {
-                        acc_fence(acc[0]);
-                        acc_fence(acc[1]);
-                        wgmma_fence();
-#pragma unroll
-                        for (int h = 0; h < 2; h++) {
-                            const uint32_t ah = a0 + (uint32_t)h * HALF + tap;
-                            Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah), make_desc(B_HI, b), first);                   // xh * wh
-                            Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah + 32u), make_desc(B_HI, b + 32u), 1u);
-                            Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah + 64u), make_desc(B_HI, b), 1u);                // xl * wh
-                            Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah + 96u), make_desc(B_HI, b + 32u), 1u);
-                            Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah), make_desc(B_HI, b + COUT * 64u), 1u);         // xh * wl
-                            Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah + 32u), make_desc(B_HI, b + COUT * 64u + 32u), 1u);
-                        }
-                        wgmma_commit();
-                        wgmma_wait<1>();                             // the previous group is done: its stage / slot may be refilled
-                        acc_fence(acc[0]);
-                        acc_fence(acc[1]);
-                        release();
-                    } else {
-                        // Hopper's e4m3 wgmma accumulates in reduced precision, which would also round the fp32 sums it adds to: each
-                        // slice's two corrections go into a fresh buffer (scale_d = 0) and reach the fp32 sums through ordinary adds.
+            if constexpr (F8) {
+                for (int c = 0; c < C::NCHUNK; c++, a_it++) {
+                    const uint32_t slot = a_it & 1u;
+                    mbar_wait_prof(a_full(slot), (a_it >> 1) & 1u, prof_on, w_af);
+                    const uint32_t a0 = a_base + slot * C::A_SLOT + (uint32_t)wg * 8u * ROWB;
+                    // The taps are unrolled and the chunk ends with an empty pipe.  A group still in flight across a loop's back
+                    // edge while its registers are read after the next wait makes ptxas serialise every wgmma of the loop.
+#pragma unroll 9
+                    for (int t = 0; t < 9; t++) {
+                        const uint32_t tap = (uint32_t)((t / 3) * HALO + t % 3) * ROWB;
+                        if (!C::RESIDENT) mbar_wait_prof(b_full(stage), phase, prof_on, w_bf);
+                        else if (n == 0) mbar_wait_prof(b_full(stage), 0u, prof_on, w_bf);   // the stages arrive once, during the first tile-set
+                        const uint32_t b = b_base + stage * C::B_STAGE;
+                        const uint32_t first = (c | t) != 0 ? 1u : 0u;
+                        // a record's quarters: +0 / +32 the fp16 K steps, +64 xh8, +96 xl8.  Hopper's e4m3 wgmma accumulates in
+                        // reduced precision, which would also round the fp32 sums it adds to: each slice's two corrections go into a
+                        // fresh buffer (scale_d = 0) and reach the fp32 sums through ordinary adds.
 #pragma unroll
                         for (int h = 0; h < 2; h++) {
                             const uint32_t ah = a0 + (uint32_t)h * HALF + tap;
@@ -312,20 +295,61 @@ tc_conv3x3_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_cons
                                 }
                             }
                         }
+                        pend_b = (int)stage;
+                        pend_a = t == 8 ? (int)slot : -1;
+                        if (++stage == (uint32_t)C::NB) { stage = 0; phase ^= 1u; }
                     }
-                    pend_b = (int)stage;
-                    pend_a = t == 8 ? (int)slot : -1;
-                    if (++stage == (uint32_t)C::NB) { stage = 0; phase ^= 1u; }
-                }
-                if constexpr (F8) {
                     wgmma_wait<0>();
                     acc_fence(acc[0]);
                     acc_fence(acc[1]);
                     add_corr(LAST);
                     release();
                 }
-            }
-            if constexpr (!F8) {
+            } else {
+                // f16x3, or with p.xh_only the xh * wh K steps alone: the loop is chosen once per tile-set, where no wgmma group
+                // is in flight, so each of the two is straight-line wgmma code.
+                auto chunks = [&](auto xh_only_tag) {
+                    constexpr bool XH_ONLY = decltype(xh_only_tag)::value;
+                    for (int c = 0; c < C::NCHUNK; c++, a_it++) {
+                        const uint32_t slot = a_it & 1u;
+                        mbar_wait_prof(a_full(slot), (a_it >> 1) & 1u, prof_on, w_af);
+                        const uint32_t a0 = a_base + slot * C::A_SLOT + (uint32_t)wg * 8u * ROWB;
+#pragma unroll 1
+                        for (int t = 0; t < 9; t++) {
+                            const uint32_t tap = (uint32_t)((t / 3) * HALO + t % 3) * ROWB;
+                            if (!C::RESIDENT) mbar_wait_prof(b_full(stage), phase, prof_on, w_bf);
+                            else if (n == 0) mbar_wait_prof(b_full(stage), 0u, prof_on, w_bf);   // the stages arrive once, during the first tile-set
+                            const uint32_t b = b_base + stage * C::B_STAGE;
+                            const uint32_t first = (c | t) != 0 ? 1u : 0u;
+                            // a record's quarters: +0 / +32 the fp16 K steps of hi, +64 / +96 those of lo
+                            acc_fence(acc[0]);
+                            acc_fence(acc[1]);
+                            wgmma_fence();
+#pragma unroll
+                            for (int h = 0; h < 2; h++) {
+                                const uint32_t ah = a0 + (uint32_t)h * HALF + tap;
+                                Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah), make_desc(B_HI, b), first);                   // xh * wh
+                                Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah + 32u), make_desc(B_HI, b + 32u), 1u);
+                                if constexpr (!XH_ONLY) {
+                                    Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah + 64u), make_desc(B_HI, b), 1u);            // xl * wh
+                                    Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah + 96u), make_desc(B_HI, b + 32u), 1u);
+                                    Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah), make_desc(B_HI, b + COUT * 64u), 1u);     // xh * wl
+                                    Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah + 32u), make_desc(B_HI, b + COUT * 64u + 32u), 1u);
+                                }
+                            }
+                            wgmma_commit();
+                            wgmma_wait<1>();                             // the previous group is done: its stage / slot may be refilled
+                            acc_fence(acc[0]);
+                            acc_fence(acc[1]);
+                            release();
+                            pend_b = (int)stage;
+                            pend_a = t == 8 ? (int)slot : -1;
+                            if (++stage == (uint32_t)C::NB) { stage = 0; phase ^= 1u; }
+                        }
+                    }
+                };
+                if (p.xh_only) chunks(std::true_type{});
+                else chunks(std::false_type{});
                 wgmma_wait<0>();
                 acc_fence(acc[0]);
                 acc_fence(acc[1]);
