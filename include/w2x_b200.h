@@ -268,6 +268,25 @@ W2X_API int w2x_convert_tiles_async(w2x_ctx *ctx, const w2x_model *model, const 
 W2X_API int w2x_convert_tiles_device(w2x_ctx *ctx, const w2x_model *model, const float *d_in, float *d_out,
                                      int n_tiles, int width, int height);
 
+/* ---- independent planes of any sizes in one pass ------------------------------------------------ */
+/* For collections of small images of different sizes (sprite and icon sets, dataset crops, thumbnails), which one
+ * w2x_convert_plane call each would run on a fraction of the GPU.  The reference converts such a collection a plane at a time
+ * (convertWithModels per image, src/main.cpp:96,148), and its own block loop converts blocks of up to four shapes one after
+ * another (src/convertRoutine.cpp:114-165).
+ * n_planes independent planes of any sizes, each converted exactly like w2x_convert_plane(block_splitting = 0) would convert it
+ * -- bit-identical -- but packed side by side into as few frames as the scratch limit allows, so that every layer is one launch
+ * per frame.  A plane whose padded rectangle fits no frame is converted alone.  Only the tensor-core engine with the fused last
+ * layer packs; every other case converts plane by plane.  Every plane is checked before anything is queued: NULL pointers,
+ * sizes < 1 and row strides that are not multiples of 4 or shorter than a row give W2X_ERR_ARG naming the plane index.
+ * The progress lines are the ones the single-plane calls would log, plane by plane in order.
+ * HOST buffers, synchronous; uploads, layers and downloads of successive frames overlap. */
+W2X_API int w2x_convert_planes(w2x_ctx *ctx, const w2x_model *model, int n_planes, const float *const *in, const int *widths,
+                               const int *heights, const size_t *in_strides, float *const *out, const size_t *out_strides);
+/* Same on DEVICE planes (the pointer, size and stride arrays themselves are host arrays), asynchronous on the context's stream. */
+W2X_API int w2x_convert_planes_device(w2x_ctx *ctx, const w2x_model *model, int n_planes, const float *const *d_in,
+                                      const int *widths, const int *heights, const size_t *in_strides, float *const *d_out,
+                                      const size_t *out_strides);
+
 /* ---- one process, N GPUs ---------------------------------------------------------------------- */
 /* The sibling of the reference's -j (src/main.cpp:58-60, modelUtility::setNumberOfJobs): N contexts driven by
  * one host thread.  w2x_multi_convert_plane = w2x_convert_plane with the plane cut into N row bands and the

@@ -39,6 +39,7 @@ ABI_SYMBOLS = (
     "w2x_multi_set_precision", "w2x_multi_set_log", "w2x_multi_convert_plane", "w2x_multi_convert_tiles",
     "w2x_host_alloc", "w2x_host_free", "w2x_ctx_forget_model", "w2x_slab_create", "w2x_slab_destroy", "w2x_slab_export",
     "w2x_slab_connect", "w2x_slab_connect_local", "w2x_slab_convert", "w2x_slab_convert_async", "w2x_slab_synchronize",
+    "w2x_convert_planes", "w2x_convert_planes_device",
 )
 BAND_BLOB_BYTES = 320
 
@@ -137,6 +138,10 @@ def lib():
     L.w2x_convert_tiles.argtypes = [vp, vp, C.POINTER(vp), C.POINTER(vp), ci, ci, ci, cs, cs]
     L.w2x_convert_tiles_async.argtypes = [vp, vp, C.POINTER(vp), C.POINTER(vp), ci, ci, ci, cs, cs]
     L.w2x_convert_tiles_device.argtypes = [vp, vp, vp, vp, ci, ci, ci]
+    pi, ps = C.POINTER(ci), C.POINTER(cs)
+    L.w2x_convert_planes.argtypes = [vp, vp, ci, C.POINTER(vp), pi, pi, ps, C.POINTER(vp), ps]
+    L.w2x_convert_planes_device.argtypes = [vp, vp, ci, C.POINTER(vp), pi, pi, ps, C.POINTER(vp), ps]
+    L.w2x_debug_plan_planes.argtypes = [ci, pi, pi, ci, ci, cs, pi, pi, pi, pi, ci]
     L.w2x_multi_create.argtypes = [C.POINTER(ci), ci, C.POINTER(vp)]
     L.w2x_multi_destroy.argtypes = [vp]
     L.w2x_multi_destroy.restype = None
@@ -196,6 +201,38 @@ def block_table(w, h, n_model=7):
     tab = np.zeros((n, 8), np.int32)
     lib().w2x_block_table(w, h, n_model, tab.ctypes.data_as(C.POINTER(C.c_int)), n, None, None)
     return tab, sc.value, sr.value
+
+
+def debug_plan_planes(widths, heights, n_layers=7, max_channels=128, scratch_limit=16 << 30):
+    """The frame plan of w2x_convert_planes for these plane sizes (no device needed) -> (frame [n], x0 [n], y0 [n], frames [F][2]):
+    per plane its frame (-1 = converted alone) and its padded rectangle's top-left corner; per frame (width, height)."""
+    n = len(widths)
+    w = np.ascontiguousarray(widths, np.int32)
+    h = np.ascontiguousarray(heights, np.int32)
+    frame, x0, y0 = (np.zeros(n, np.int32) for _ in range(3))
+    pi = C.POINTER(C.c_int)
+    args = [w.ctypes.data_as(pi), h.ctypes.data_as(pi), n_layers, max_channels, scratch_limit,
+            frame.ctypes.data_as(pi), x0.ctypes.data_as(pi), y0.ctypes.data_as(pi)]
+    nf = lib().w2x_debug_plan_planes(n, *args, None, 0)
+    if nf < 0:
+        raise W2xError(-nf, lib().w2x_last_error().decode())
+    dims = np.zeros((max(nf, 1), 2), np.int32)
+    lib().w2x_debug_plan_planes(n, *args, dims.ctypes.data_as(pi), nf)
+    return frame, x0, y0, dims[:nf]
+
+
+def _plane_arrays(planes, fix):
+    """2-D float32 views -> (arrays, ctypes pointer / width / height / stride arrays); fix() may copy a view the C ABI cannot take."""
+    xs = [fix(p) for p in planes]
+    for x in xs:
+        if x.ndim != 2 or x.dtype != np.float32:
+            raise ValueError("every plane must be a 2-D float32 array")
+    n = len(xs)
+    ptr = (C.c_void_p * n)(*[x.ctypes.data for x in xs])
+    ws = (C.c_int * n)(*[x.shape[1] for x in xs])
+    hs = (C.c_int * n)(*[x.shape[0] for x in xs])
+    st = (C.c_size_t * n)(*[x.strides[0] for x in xs])
+    return xs, ptr, ws, hs, st
 
 
 # ---- Model --------------------------------------------------------------------------------------
@@ -371,6 +408,33 @@ class Context:
 
     def convert_tiles_device(self, model: Model, d_in, d_out, n, w, h):
         _check(lib().w2x_convert_tiles_device(self._h, model._h, C.c_void_p(d_in), C.c_void_p(d_out), n, w, h))
+
+    # n independent planes of any sizes, packed into as few frames as the scratch limit allows (w2x_convert_planes)
+    def convert_planes(self, model: Model, planes, out=None):
+        """planes: 2-D float32 arrays (row-strided views are passed as they are) -> list of outputs; `out` may be a list of
+        2-D float32 arrays of the same shapes (strided views included), written in place."""
+        def fix(p):
+            x = np.asarray(p, np.float32)
+            if x.ndim == 2 and (x.strides[1] != 4 or x.strides[0] % 4 or x.strides[0] < x.shape[1] * 4):
+                x = np.ascontiguousarray(x)
+            return x
+        xs, ip, ws, hs, ist = _plane_arrays(planes, fix)
+        if out is None:
+            out = [np.empty(x.shape, np.float32) for x in xs]
+        if len(out) != len(xs) or any(o.shape != x.shape for o, x in zip(out, xs)):
+            raise ValueError("out must hold one array per plane, of the plane's shape")
+        if any(o.strides[1] != 4 or o.strides[0] % 4 for o in out):
+            raise ValueError("out arrays need unit column stride and row strides that are multiples of 4 bytes")
+        _, op, _, _, ost = _plane_arrays(out, lambda o: o)
+        _check(lib().w2x_convert_planes(self._h, model._h, len(xs), ip, ws, hs, ist, op, ost))
+        return out
+
+    def convert_planes_device(self, model: Model, d_in, widths, heights, in_strides, d_out, out_strides):
+        """Device pointers (ints) and host lists of sizes / row strides in bytes; asynchronous on the context's stream."""
+        n = len(d_in)
+        _check(lib().w2x_convert_planes_device(self._h, model._h, n, (C.c_void_p * n)(*d_in), (C.c_int * n)(*widths),
+                                               (C.c_int * n)(*heights), (C.c_size_t * n)(*in_strides),
+                                               (C.c_void_p * n)(*d_out), (C.c_size_t * n)(*out_strides)))
 
     # w2xc::Model::filter on host planes [n_in][h][w] -> [n_out][h][w]
     def filter_layer(self, model: Model, layer, in_planes):

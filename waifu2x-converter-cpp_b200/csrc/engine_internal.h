@@ -67,6 +67,10 @@ struct w2x_ctx {
     cudaStream_t copy_in = nullptr, copy_out = nullptr;   // host<->device copies of w2x_convert_plane overlap the compute stream
     cudaEvent_t ev_in[8] = {}, ev_done[8] = {};
     int host_bands = 0;                                   // 0 = automatic (up to 4 bands of >= 512 rows), 1 = no pipelining
+    void *plan_buf = nullptr;                             // device tables of the packed frames (w2x_convert_planes, w2x_convert_tiles)
+    size_t plan_bytes = 0;
+    cudaEvent_t plan_ev = nullptr;                        // recorded after the last kernel that reads plan_buf
+    bool plan_ev_live = false;
     unsigned long long *prof_buf = nullptr;   // [16 layers][PROF_MAX_CTAS][PROF_WORDS], debug profile
 };
 

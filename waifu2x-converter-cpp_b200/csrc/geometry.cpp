@@ -5,6 +5,7 @@
 // block_table reproduces the loop bounds of convertWithModelsBlockSplit
 // (src/convertRoutine.cpp:100-131 for the input ROI, :143-155 for the output ROI), including the
 // float ceil of :100-105 and the use of blockSize.height for the output column offset at :153-154.
+#include <algorithm>
 #include <cmath>
 
 #include "w2x_internal.h"
@@ -42,6 +43,59 @@ int block_table(int w, int h, int bw, int bh, int n_model, int *table, int capac
         }
     }
     return idx;
+}
+
+// Shelf packing: rectangles sorted by height (tallest first) fill a shelf left to right; the next one that does not fit opens a
+// shelf below, as tall as that rectangle; a shelf that would pass the frame's last row opens a new frame.
+int plan_planes(int n, const int *widths, const int *heights, int n_layers, int max_channels, size_t scratch_limit, int *frame,
+                int *x0, int *y0, std::vector<int> *fw, std::vector<int> *fh) {
+    constexpr long MAX_ROWS = 8L * 65535;   // the first layer, the pack and the per-frame gathers run 8-row blocks, grid.y <= 65535
+    const long px_limit = (long)std::min<size_t>(scratch_limit / ((size_t)max_channels * 4), (size_t)1 << 40);
+    fw->clear();
+    fh->clear();
+    std::vector<int> order;
+    long area = 0, wmax = 0;
+    for (int i = 0; i < n; i++) {
+        frame[i] = -1;
+        x0[i] = y0[i] = 0;
+        const long pw = (long)widths[i] + 2 * n_layers, ph = (long)heights[i] + 2 * n_layers;
+        if (pw * ph > px_limit || ph > MAX_ROWS) continue;
+        order.push_back(i);
+        area += pw * ph;
+        wmax = std::max(wmax, pw);
+    }
+    if (order.empty()) return 0;
+    // Frame width: the side of a square that holds every rectangle (or one full frame), rounded up to the layer kernels' 16-pixel
+    // tile-set, and never narrower than the widest rectangle.  Shelf packing wastes the end of each shelf (less than one
+    // rectangle per shelf, small when the frame is wide) and the rest of the last shelf (less than one shelf per frame, small
+    // when the frame is tall); a square keeps both small at once.
+    const long side = (long)std::ceil(std::sqrt((double)std::min(area, px_limit)));
+    const long W = std::max(wmax, (side + 15) / 16 * 16);
+    const long rows = std::min(MAX_ROWS, px_limit / W);
+    auto pw_of = [&](int i) { return (long)widths[i] + 2 * n_layers; };
+    auto ph_of = [&](int i) { return (long)heights[i] + 2 * n_layers; };
+    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return ph_of(a) != ph_of(b) ? ph_of(a) > ph_of(b) : pw_of(a) > pw_of(b); });
+    long x = 0, y = 0, shelf_h = 0;
+    for (int i : order) {
+        const long pw = pw_of(i), ph = ph_of(i);
+        if (ph > rows) continue;                          // taller than a frame of this width may be: converted alone
+        if (fw->empty() || x + pw > W) {                  // a new shelf ...
+            y += shelf_h;
+            x = 0;
+            shelf_h = ph;
+            if (fw->empty() || y + ph > rows) {           // ... in a new frame
+                fw->push_back((int)W);
+                fh->push_back(0);
+                y = 0;
+            }
+        }
+        frame[i] = (int)fw->size() - 1;
+        x0[i] = (int)x;
+        y0[i] = (int)y;
+        x += pw;
+        fh->back() = (int)(y + shelf_h);
+    }
+    return (int)fw->size();
 }
 
 }  // namespace w2x
@@ -86,6 +140,25 @@ int w2x_block_table(int width, int height, int n_model, int *table, int capacity
         return -W2X_ERR_ARG;
     }
     return n;
+}
+
+// Probe hook (not part of the stable ABI, needs no device): the frame plan w2x_convert_planes makes for these plane sizes with a
+// model of n_layers layers at most max_channels wide and the given scratch limit.  Per plane: frame index (-1 = converted alone)
+// and the padded rectangle's top-left corner; frame_dims gets (width, height) of the first `capacity` frames.  Returns the
+// frame count, or -W2X_ERR_ARG.
+W2X_API int w2x_debug_plan_planes(int n_planes, const int *widths, const int *heights, int n_layers, int max_channels,
+                                  size_t scratch_limit, int *frame, int *x0, int *y0, int *frame_dims, int capacity) {
+    if (n_planes < 1 || !widths || !heights || !frame || !x0 || !y0 || n_layers < 1 || max_channels < 1 || !scratch_limit)
+        return -w2x::fail(W2X_ERR_ARG, "w2x_debug_plan_planes: bad argument");
+    for (int i = 0; i < n_planes; i++)
+        if (widths[i] < 1 || heights[i] < 1) return -w2x::fail(W2X_ERR_ARG, "w2x_debug_plan_planes: plane %d has no pixels", i);
+    std::vector<int> fw, fh;
+    const int nf = w2x::plan_planes(n_planes, widths, heights, n_layers, max_channels, scratch_limit, frame, x0, y0, &fw, &fh);
+    for (int f = 0; f < nf && f < capacity && frame_dims; f++) {
+        frame_dims[2 * f] = fw[(size_t)f];
+        frame_dims[2 * f + 1] = fh[(size_t)f];
+    }
+    return nf;
 }
 
 }  // extern "C"

@@ -83,6 +83,23 @@ cudaError_t launch_last_gather(const float *partial, int pw, int ph, float bias,
 cudaError_t launch_last_gather_xy(const float *partial, int pw, int ph, float bias, int crop_x, int crop_top,
                                   int crop_bottom, float *dst, long dst_stride_floats, cudaStream_t s);
 inline size_t partial_bytes(int Wp, int Hp) { return (size_t)Hp * Wp * 12 * sizeof(float); }
+// Packed frames: independent planes side by side in one frame, each inside its own padded rectangle of (w + 2 pad) x (h + 2 pad)
+// pixels (pad = the model's layer count).  A DEVICE table of PlaneRect lists them by shelf: ascending y0, then ascending x0;
+// rectangles sharing a y0 form a shelf, shelf_y0[s] is its row and rect[shelf_first[s] .. shelf_first[s + 1]) its rectangles.
+struct PlaneRect {
+    const float *src;    // the plane, row stride src_stride floats (pack)
+    float *dst;          // its interior output, row stride dst_stride floats (gather)
+    long src_stride, dst_stride;
+    int w, h;            // plane size
+    int x0, y0;          // top-left corner of its padded rectangle in the frame
+    int blk0;            // first gather block: plane i owns blocks [blk0_i, blk0_i + ceil(w/32) * ceil(h/8))
+};
+// The frame's padded fp32 image (fw x fh, dense): replicate-padded planes inside the rectangles, 0 elsewhere.  One launch.
+cudaError_t launch_pack_planes(const PlaneRect *rect, const int *shelf_y0, const int *shelf_first, int n_shelf, int pad, int fw,
+                               int fh, float *frame, cudaStream_t s);
+// The fused last layer's output for every plane of the frame, from its tap partials ([fh][fw][12]).  One launch of n_blocks.
+cudaError_t launch_gather_planes(const float *partial, int fw, const PlaneRect *rect, int n_rect, int n_blocks, float bias, int pad,
+                                 cudaStream_t s);
 constexpr int PROF_WORDS = 16;      // per-CTA profile record (see tc_config.cuh PROF_*)
 constexpr int PROF_MAX_CTAS = 256;
 // Last layer (Cout = 1): NHWC hi/lo frame -> fp32 plane, interior only: out(y,x) for

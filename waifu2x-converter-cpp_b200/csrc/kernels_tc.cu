@@ -210,6 +210,22 @@ cudaError_t launch_last_gather_xy(const float *partial, int pw, int ph, float bi
     return cudaGetLastError();
 }
 
+cudaError_t launch_pack_planes(const PlaneRect *rect, const int *shelf_y0, const int *shelf_first, int n_shelf, int pad, int fw,
+                               int fh, float *frame, cudaStream_t s) {
+    if (n_shelf < 1 || fw < 1 || fh < 1) return cudaErrorInvalidValue;
+    dim3 grid((fw + 31) / 32, (fh + 7) / 8);
+    if (grid.y > 65535) return cudaErrorInvalidConfiguration;
+    pack_planes_kernel<<<grid, 256, 0, s>>>(rect, shelf_y0, shelf_first, n_shelf, pad, fw, fh, frame);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_gather_planes(const float *partial, int fw, const PlaneRect *rect, int n_rect, int n_blocks, float bias, int pad,
+                                 cudaStream_t s) {
+    if (n_rect < 1 || n_blocks < 1 || pad < 1) return cudaErrorInvalidValue;
+    gather_planes_kernel<<<n_blocks, 256, 0, s>>>(partial, fw, rect, n_rect, bias, pad);
+    return cudaGetLastError();
+}
+
 cudaError_t launch_planar_to_nhwc(const float *in, int C, int w, int h, __half *out, cudaStream_t s, int f8) {
     long total = (long)(w + 2) * (h + 2) * C;
     planar_to_nhwc_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(in, C, w, h, out, f8);

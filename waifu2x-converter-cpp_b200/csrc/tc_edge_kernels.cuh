@@ -169,13 +169,9 @@ last_layer_kernel(const __half *__restrict__ in, int pw, int ph, const float *__
     dst[(long)(y - crop) * dst_stride + (x - crop)] = fminf(r, 0.f) * 0.1f + fmaxf(r, 0.f);
 }
 
-// Second half of the fused last layer: out(y,x) = leaky(bias + sum_t P[(y+ky-1, x+kx-1)][t]), taps in
-// row-major order, for the interior [crop, ph-crop) x [crop, pw-crop).
-__global__ void __launch_bounds__(256)
-last_gather_kernel(const float *__restrict__ partial, int pw, int ph, float bias, int crop_x, int crop_top,
-                   int crop_bottom, float *__restrict__ dst, long dst_stride) {
-    const int x = crop_x + blockIdx.x * 32 + (threadIdx.x & 31), y = crop_top + blockIdx.y * 8 + (threadIdx.x >> 5);
-    if (x >= pw - crop_x || y >= ph - crop_bottom) return;
+// Second half of the fused last layer at frame pixel (y, x): leaky(bias + sum_t P[(y+ky-1, x+kx-1)][t]), taps in row-major
+// order.  The one definition of this arithmetic: last_gather_kernel and gather_planes_kernel both call it.
+__device__ __forceinline__ float last_gather_px(const float *__restrict__ partial, int pw, int x, int y, float bias) {
     float acc = 0.f;
 #pragma unroll
     for (int ky = 0; ky < 3; ky++)
@@ -183,7 +179,69 @@ last_gather_kernel(const float *__restrict__ partial, int pw, int ph, float bias
         for (int kx = 0; kx < 3; kx++)
             acc += __ldg(partial + ((size_t)(y + ky - 1) * pw + (x + kx - 1)) * 12 + ky * 3 + kx);
     const float r = acc + bias;
-    dst[(long)(y - crop_top) * dst_stride + (x - crop_x)] = fminf(r, 0.f) * 0.1f + fmaxf(r, 0.f);
+    return fminf(r, 0.f) * 0.1f + fmaxf(r, 0.f);
+}
+
+// The fused last layer's output for the interior [crop_top, ph-crop_bottom) x [crop_x, pw-crop_x) of one frame.
+__global__ void __launch_bounds__(256)
+last_gather_kernel(const float *__restrict__ partial, int pw, int ph, float bias, int crop_x, int crop_top,
+                   int crop_bottom, float *__restrict__ dst, long dst_stride) {
+    const int x = crop_x + blockIdx.x * 32 + (threadIdx.x & 31), y = crop_top + blockIdx.y * 8 + (threadIdx.x >> 5);
+    if (x >= pw - crop_x || y >= ph - crop_bottom) return;
+    dst[(long)(y - crop_top) * dst_stride + (x - crop_x)] = last_gather_px(partial, pw, x, y, bias);
+}
+
+// ---- packed frames: independent planes of any sizes side by side in one frame (w2x_convert_planes, w2x_convert_tiles) ----
+// Each plane owns the padded rectangle (w + 2 pad) x (h + 2 pad) at (x0, y0).  An interior pixel's receptive field has radius
+// pad = the layer count, so it never leaves its own rectangle: every plane's interior sees exactly the operands, in the same
+// order, as a pass on the plane alone.  The table lists the rectangles by shelf: ascending y0, then ascending x0; rectangles
+// with one y0 form a shelf, no rectangle reaches below the next shelf's y0 or right of its successor's x0.
+
+// Frame pixel (y, x) of the padded fp32 image: cv::copyMakeBorder(plane, pad, BORDER_REPLICATE) (src/convertRoutine.cpp:35)
+// inside a rectangle, 0 everywhere else.  One thread per frame pixel, 32 x 8 per block.
+__global__ void __launch_bounds__(256)
+pack_planes_kernel(const PlaneRect *__restrict__ rect, const int *__restrict__ shelf_y0, const int *__restrict__ shelf_first,
+                   int n_shelf, int pad, int fw, int fh, float *__restrict__ frame) {
+    const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = blockIdx.y * 8 + (threadIdx.x >> 5);
+    if (x >= fw || y >= fh) return;
+    int s = 0, s1 = n_shelf - 1;                 // the last shelf starting at or above row y
+    while (s < s1) {
+        const int mid = (s + s1 + 1) >> 1;
+        if (__ldg(shelf_y0 + mid) <= y) s = mid;
+        else s1 = mid - 1;
+    }
+    int r = __ldg(shelf_first + s), r1 = __ldg(shelf_first + s + 1) - 1;   // the shelf's last rectangle starting at or left of x
+    while (r < r1) {
+        const int mid = (r + r1 + 1) >> 1;
+        if (rect[mid].x0 <= x) r = mid;
+        else r1 = mid - 1;
+    }
+    const PlaneRect &R = rect[r];
+    const int px = x - R.x0, py = y - R.y0;
+    float v = 0.f;
+    if (px >= 0 && py >= 0 && px < R.w + 2 * pad && py < R.h + 2 * pad) {
+        const int sx = min(max(px - pad, 0), R.w - 1), sy = min(max(py - pad, 0), R.h - 1);
+        v = __ldg(R.src + (long)sy * R.src_stride + sx);
+    }
+    frame[(size_t)y * fw + x] = v;
+}
+
+// Every plane's interior from the fused last layer's tap partials of the packed frame (fw wide), at the plane's own output
+// pointer and stride.  Plane i owns blocks [blk0_i, blk0_{i+1}): a 32 x 8 grid over its w x h interior.
+__global__ void __launch_bounds__(256)
+gather_planes_kernel(const float *__restrict__ partial, int fw, const PlaneRect *__restrict__ rect, int n_rect, float bias, int crop) {
+    const int b = (int)blockIdx.x;
+    int r = 0, r1 = n_rect - 1;                  // the plane owning block b
+    while (r < r1) {
+        const int mid = (r + r1 + 1) >> 1;
+        if (rect[mid].blk0 <= b) r = mid;
+        else r1 = mid - 1;
+    }
+    const PlaneRect &R = rect[r];
+    const int lb = b - R.blk0, bx = (R.w + 31) / 32;
+    const int x = (lb % bx) * 32 + (threadIdx.x & 31), y = (lb / bx) * 8 + (threadIdx.x >> 5);
+    if (x >= R.w || y >= R.h) return;
+    R.dst[(long)y * R.dst_stride + x] = last_gather_px(partial, fw, R.x0 + crop + x, R.y0 + crop + y, bias);
 }
 
 __global__ void planar_to_nhwc_kernel(const float *__restrict__ in, int C, int w, int h, __half *__restrict__ out, int f8) {

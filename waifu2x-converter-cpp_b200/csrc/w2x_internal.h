@@ -64,4 +64,10 @@ uint8_t f32_to_e4m3_rn(float f);    // OCP e4m3 (max 448, no inf), round-to-near
 struct Config { int n_job = 4, block_w = 512, block_h = 512; };
 Config &config();
 int block_table(int w, int h, int bw, int bh, int n_model, int *table, int capacity, int *sc, int *sr);
+// Places the padded rectangles (w + 2 n_layers) x (h + 2 n_layers) of n independent planes side by side into frames of at most
+// scratch_limit / (max_channels * 4) pixels and 524 280 rows.  frame[i] = the plane's frame, or -1 when its rectangle fits no
+// frame (the caller converts it alone); (x0[i], y0[i]) = the rectangle's top-left corner.  Returns the frame count; fw / fh
+// receive the frame sizes.
+int plan_planes(int n, const int *widths, const int *heights, int n_layers, int max_channels, size_t scratch_limit, int *frame,
+                int *x0, int *y0, std::vector<int> *fw, std::vector<int> *fh);
 }  // namespace w2x
