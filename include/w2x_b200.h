@@ -212,6 +212,8 @@ typedef struct w2x_band w2x_band;
 #define W2X_EDGE_NEIGHBOUR 1   /* another GPU's band: one halo row, exchanged after every layer */
 #define W2X_EDGE_OVERLAP 2     /* n_layers real input rows supplied with the band and recomputed (no exchange): the seam
                                   between two sub-bands of ONE GPU (w2x_slab_*), input read through w2x_band_load_rows */
+/* A band's frame is band_rows plus 1 row per W2X_EDGE_NEIGHBOUR side and n_layers rows per other side; a frame of more than
+ * 8 * 65535 = 524280 rows is refused with W2X_ERR_ARG before anything is allocated. */
 W2X_API int w2x_band_create(w2x_ctx *ctx, const w2x_model *model, int width, int band_rows,
                             int up_edge, int down_edge, w2x_band **out_band);
 W2X_API void w2x_band_destroy(w2x_band *band);
@@ -237,7 +239,8 @@ W2X_API int w2x_band_run(w2x_band *band, const float *d_in_own_rows, size_t in_s
  * rows come out.  The slab is cut into sub-bands so that uploads, layers and downloads overlap; seams inside the slab are
  * W2X_EDGE_OVERLAP (recomputed, local data), its outer edges exchange a halo row per layer with the neighbour slab.
  * order: 0 = walk the sub-bands top -> bottom, 1 = bottom -> top; neighbouring slabs must alternate (rank parity) so that
- * both sides of a boundary are in flight at the same time.  n_sub = 0: automatic.  Blobs are 2 * W2X_BAND_BLOB_BYTES. */
+ * both sides of a boundary are in flight at the same time.  n_sub = 0: automatic.  Blobs are 2 * W2X_BAND_BLOB_BYTES.
+ * n_sub is raised, past any number asked for, until every sub-band's frame has at most 524280 rows. */
 typedef struct w2x_slab w2x_slab;
 W2X_API int w2x_slab_create(w2x_ctx *ctx, const w2x_model *model, int width, int rows, int has_up_neighbour,
                             int has_down_neighbour, int order, int n_sub, w2x_slab **out_slab);

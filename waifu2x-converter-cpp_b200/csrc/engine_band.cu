@@ -76,6 +76,14 @@ int w2x_band_create(w2x_ctx *ctx, const w2x_model *model, int width, int band_ro
     *out_band = nullptr;
     if (!model->tc_eligible || ctx->engine == W2X_ENGINE_FP32)
         return fail(W2X_ERR_UNSUPPORTED, "w2x_band_create: the per-layer halo mode needs the tensor-core engine and a 1->{32,64,128}..->1 model");
+    if (has_up < 0 || has_up > 2 || has_down < 0 || has_down > 2) return fail(W2X_ERR_ARG, "w2x_band_create: edge kind must be 0 (image border), 1 (neighbour GPU) or 2 (overlap rows)");
+    // Refused here, before anything is allocated or queued: a band whose layers failed mid-pass would leave its neighbours'
+    // exchange kernels waiting for rows that never come.
+    const int n = (int)model->layers.size();
+    const long frame_rows = (long)band_rows + (has_up == W2X_EDGE_NEIGHBOUR ? 1 : n) + (has_down == W2X_EDGE_NEIGHBOUR ? 1 : n);
+    if (frame_rows > MAX_FRAME_ROWS)
+        return fail(W2X_ERR_ARG, "w2x_band_create: the band's frame has %ld rows (%d owned + halo / border rows), more than the %ld a frame may have",
+                    frame_rows, band_rows, MAX_FRAME_ROWS);
     DeviceGuard g(ctx->device);
     int rc = ensure_tc(ctx);
     if (rc) return rc;
@@ -87,7 +95,6 @@ int w2x_band_create(w2x_ctx *ctx, const w2x_model *model, int width, int band_ro
     b->n = (int)model->layers.size();
     b->width = width;
     b->rows = band_rows;
-    if (has_up < 0 || has_up > 2 || has_down < 0 || has_down > 2) return fail(W2X_ERR_ARG, "w2x_band_create: edge kind must be 0 (image border), 1 (neighbour GPU) or 2 (overlap rows)");
     b->up = has_up == W2X_EDGE_NEIGHBOUR;
     b->down = has_down == W2X_EDGE_NEIGHBOUR;
     b->ov_up = has_up == W2X_EDGE_OVERLAP;
@@ -419,6 +426,9 @@ int w2x_slab_create(w2x_ctx *ctx, const w2x_model *model, int width, int rows, i
     const int n = (int)model->layers.size();
     if (n_sub <= 0) n_sub = std::min(4, rows / 512);            // like w2x_convert_plane's copy pipeline
     n_sub = std::max(1, std::min(n_sub, std::min(8, rows / (4 * n))));
+    // ... and as many as it takes for every sub-band's frame (its rows + at most n above and below) to stay within MAX_FRAME_ROWS
+    const long sub_max = MAX_FRAME_ROWS - 2 * n;
+    n_sub = std::max(n_sub, (int)((rows + sub_max - 1) / sub_max));
     auto s = std::unique_ptr<w2x_slab, void (*)(w2x_slab *)>(new w2x_slab(), w2x_slab_destroy);
     s->ctx = ctx;
     s->model = model;

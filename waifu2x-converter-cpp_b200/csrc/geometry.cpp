@@ -49,7 +49,6 @@ int block_table(int w, int h, int bw, int bh, int n_model, int *table, int capac
 // shelf below, as tall as that rectangle; a shelf that would pass the frame's last row opens a new frame.
 int plan_planes(int n, const int *widths, const int *heights, int n_layers, int max_channels, size_t scratch_limit, int *frame,
                 int *x0, int *y0, std::vector<int> *fw, std::vector<int> *fh) {
-    constexpr long MAX_ROWS = 8L * 65535;   // the first layer, the pack and the per-frame gathers run 8-row blocks, grid.y <= 65535
     const long px_limit = (long)std::min<size_t>(scratch_limit / ((size_t)max_channels * 4), (size_t)1 << 40);
     fw->clear();
     fh->clear();
@@ -59,7 +58,7 @@ int plan_planes(int n, const int *widths, const int *heights, int n_layers, int 
         frame[i] = -1;
         x0[i] = y0[i] = 0;
         const long pw = (long)widths[i] + 2 * n_layers, ph = (long)heights[i] + 2 * n_layers;
-        if (pw * ph > px_limit || ph > MAX_ROWS) continue;
+        if (pw * ph > px_limit || ph > MAX_FRAME_ROWS) continue;
         order.push_back(i);
         area += pw * ph;
         wmax = std::max(wmax, pw);
@@ -71,7 +70,7 @@ int plan_planes(int n, const int *widths, const int *heights, int n_layers, int 
     // when the frame is tall); a square keeps both small at once.
     const long side = (long)std::ceil(std::sqrt((double)std::min(area, px_limit)));
     const long W = std::max(wmax, (side + 15) / 16 * 16);
-    const long rows = std::min(MAX_ROWS, px_limit / W);
+    const long rows = std::min(MAX_FRAME_ROWS, px_limit / W);
     auto pw_of = [&](int i) { return (long)widths[i] + 2 * n_layers; };
     auto ph_of = [&](int i) { return (long)heights[i] + 2 * n_layers; };
     std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return ph_of(a) != ph_of(b) ? ph_of(a) > ph_of(b) : pw_of(a) > pw_of(b); });

@@ -18,6 +18,11 @@
 
 namespace w2x {
 
+// Every kernel here tiles its plane in row blocks on grid.y, which is at most 65535: a launch covers min(row blocks, 65535) of
+// them and each block also takes the row blocks gridDim.y, 2 gridDim.y, ... further down, so a plane of any height runs.
+constexpr unsigned MAX_GRID_Y = 65535;
+__device__ __forceinline__ int row_blocks(int rows, unsigned block_rows) { return (int)((rows + block_rows - 1) / block_rows); }
+
 // ---- cv::copyMakeBorder(BORDER_REPLICATE) (src/convertRoutine.cpp:35,96) ----------------------
 // rows_above/rows_below > 0 mean real neighbour rows exist there (row-band mode): the source
 // pointer addresses band row 0 and may be read at rows [-rows_above, h + rows_below).
@@ -25,30 +30,37 @@ __global__ void pad_replicate_kernel(const float *__restrict__ in, int w, int h,
                                      int pad_x, int pad_top, int pad_bottom, int rows_above, int rows_below,
                                      float *__restrict__ out, int skip_top, int skip_bottom) {
     const int W = w + 2 * pad_x, H = h + pad_top + pad_bottom;
-    int x = blockIdx.x * blockDim.x + threadIdx.x;
-    int y = blockIdx.y * blockDim.y + threadIdx.y;
-    if (x >= W || y >= H - skip_bottom || y < skip_top) return;
-    int sx = min(max(x - pad_x, 0), w - 1);
-    int sy = min(max(y - pad_top, -rows_above), h - 1 + rows_below);
-    out[(long)y * W + x] = in[(long)sy * in_stride + sx];
+    const int x = blockIdx.x * blockDim.x + threadIdx.x;
+    if (x >= W) return;
+    const int sx = min(max(x - pad_x, 0), w - 1);
+    for (int by = blockIdx.y; by < row_blocks(H, blockDim.y); by += gridDim.y) {
+        const int y = by * blockDim.y + threadIdx.y;
+        if (y >= H - skip_bottom || y < skip_top) continue;
+        const int sy = min(max(y - pad_top, -rows_above), h - 1 + rows_below);
+        out[(long)y * W + x] = in[(long)sy * in_stride + sx];
+    }
 }
 
 // crop [pad, pad+h) x [pad, pad+w) of a dense (h+2pad) x (w+2pad) plane (src/convertRoutine.cpp:40-46)
 __global__ void crop_kernel(const float *__restrict__ in, int w, int h, int pad,
                             float *__restrict__ out, long out_stride) {
-    int x = blockIdx.x * blockDim.x + threadIdx.x;
-    int y = blockIdx.y * blockDim.y + threadIdx.y;
-    if (x >= w || y >= h) return;
-    out[(long)y * out_stride + x] = in[(long)(y + pad) * (w + 2 * pad) + x + pad];
+    const int x = blockIdx.x * blockDim.x + threadIdx.x;
+    if (x >= w) return;
+    for (int by = blockIdx.y; by < row_blocks(h, blockDim.y); by += gridDim.y) {
+        const int y = by * blockDim.y + threadIdx.y;
+        if (y < h) out[(long)y * out_stride + x] = in[(long)(y + pad) * (w + 2 * pad) + x + pad];
+    }
 }
 
 // 2-D strided copy (block ROI extraction / stitching, src/convertRoutine.cpp:116-131, :143-161)
 __global__ void copy2d_kernel(const float *__restrict__ in, long in_stride, float *__restrict__ out,
                               long out_stride, int w, int h) {
-    int x = blockIdx.x * blockDim.x + threadIdx.x;
-    int y = blockIdx.y * blockDim.y + threadIdx.y;
-    if (x >= w || y >= h) return;
-    out[(long)y * out_stride + x] = in[(long)y * in_stride + x];
+    const int x = blockIdx.x * blockDim.x + threadIdx.x;
+    if (x >= w) return;
+    for (int by = blockIdx.y; by < row_blocks(h, blockDim.y); by += gridDim.y) {
+        const int y = by * blockDim.y + threadIdx.y;
+        if (y < h) out[(long)y * out_stride + x] = in[(long)y * in_stride + x];
+    }
 }
 
 // ---- the fp32 layer kernel --------------------------------------------------------------------
@@ -65,86 +77,89 @@ conv3x3_planar_fp32(const float *__restrict__ in, float *__restrict__ out,
     __shared__ __align__(16) float s_w[CK][9][CT];
 
     const int tx = threadIdx.x % TX, ty = threadIdx.x / TX;
-    const int x0 = blockIdx.x * TX, y0 = blockIdx.y * TY;
+    const int x0 = blockIdx.x * TX;
     const int co0 = blockIdx.z * CT;
     const long plane = (long)W * H;
 
-    float acc[CT];
+    for (int by = blockIdx.y; by < row_blocks(H, TY); by += gridDim.y) {   // block-uniform: the __syncthreads below stay legal
+        const int y0 = by * TY;
+        float acc[CT];
 #pragma unroll
-    for (int i = 0; i < CT; i++) acc[i] = 0.f;
+        for (int i = 0; i < CT; i++) acc[i] = 0.f;
 
-    for (int c0 = 0; c0 < Cin; c0 += CK) {
-        const int nck = min(CK, Cin - c0);
-        // stage the input tile (+1 halo, replicate at the plane border)
-        for (int idx = threadIdx.x; idx < nck * (TY + 2) * (TX + 2); idx += TX * TY) {
-            int ck = idx / ((TY + 2) * (TX + 2));
-            int r = idx % ((TY + 2) * (TX + 2));
-            int yy = r / (TX + 2), xx = r % (TX + 2);
-            int gy = min(max(y0 + yy - 1, 0), H - 1);
-            int gx = min(max(x0 + xx - 1, 0), W - 1);
-            s_in[ck][yy][xx] = __ldg(in + plane * (c0 + ck) + (long)gy * W + gx);
-        }
-        // stage the weights transposed to [ck][tap][co]
-        for (int idx = threadIdx.x; idx < nck * 9 * CT; idx += TX * TY) {
-            int co = idx / (nck * 9);
-            int r = idx % (nck * 9);
-            int ck = r / 9, t = r % 9;
-            float v = 0.f;
-            if (co0 + co < Cout) v = __ldg(wgt + ((long)(co0 + co) * Cin + c0 + ck) * 9 + t);
-            s_w[ck][t][co] = v;
-        }
-        __syncthreads();
-        for (int ck = 0; ck < nck; ck++) {
-            float v[9];
+        for (int c0 = 0; c0 < Cin; c0 += CK) {
+            const int nck = min(CK, Cin - c0);
+            // stage the input tile (+1 halo, replicate at the plane border)
+            for (int idx = threadIdx.x; idx < nck * (TY + 2) * (TX + 2); idx += TX * TY) {
+                int ck = idx / ((TY + 2) * (TX + 2));
+                int r = idx % ((TY + 2) * (TX + 2));
+                int yy = r / (TX + 2), xx = r % (TX + 2);
+                int gy = min(max(y0 + yy - 1, 0), H - 1);
+                int gx = min(max(x0 + xx - 1, 0), W - 1);
+                s_in[ck][yy][xx] = __ldg(in + plane * (c0 + ck) + (long)gy * W + gx);
+            }
+            // stage the weights transposed to [ck][tap][co]
+            for (int idx = threadIdx.x; idx < nck * 9 * CT; idx += TX * TY) {
+                int co = idx / (nck * 9);
+                int r = idx % (nck * 9);
+                int ck = r / 9, t = r % 9;
+                float v = 0.f;
+                if (co0 + co < Cout) v = __ldg(wgt + ((long)(co0 + co) * Cin + c0 + ck) * 9 + t);
+                s_w[ck][t][co] = v;
+            }
+            __syncthreads();
+            for (int ck = 0; ck < nck; ck++) {
+                float v[9];
 #pragma unroll
-            for (int ky = 0; ky < 3; ky++)
+                for (int ky = 0; ky < 3; ky++)
 #pragma unroll
-                for (int kx = 0; kx < 3; kx++) v[ky * 3 + kx] = s_in[ck][ty + ky][tx + kx];
-            if constexpr (CT % 4 == 0) {
+                    for (int kx = 0; kx < 3; kx++) v[ky * 3 + kx] = s_in[ck][ty + ky][tx + kx];
+                if constexpr (CT % 4 == 0) {
 #pragma unroll
-                for (int c4 = 0; c4 < CT / 4; c4++) {
-                    float4 t4 = *reinterpret_cast<const float4 *>(&s_w[ck][0][c4 * 4]);
-                    float t0 = t4.x * v[0], t1 = t4.y * v[0], t2 = t4.z * v[0], t3 = t4.w * v[0];
+                    for (int c4 = 0; c4 < CT / 4; c4++) {
+                        float4 t4 = *reinterpret_cast<const float4 *>(&s_w[ck][0][c4 * 4]);
+                        float t0 = t4.x * v[0], t1 = t4.y * v[0], t2 = t4.z * v[0], t3 = t4.w * v[0];
 #pragma unroll
-                    for (int t = 1; t < 9; t++) {
-                        float4 w4 = *reinterpret_cast<const float4 *>(&s_w[ck][t][c4 * 4]);
-                        t0 = fmaf(w4.x, v[t], t0);
-                        t1 = fmaf(w4.y, v[t], t1);
-                        t2 = fmaf(w4.z, v[t], t2);
-                        t3 = fmaf(w4.w, v[t], t3);
+                        for (int t = 1; t < 9; t++) {
+                            float4 w4 = *reinterpret_cast<const float4 *>(&s_w[ck][t][c4 * 4]);
+                            t0 = fmaf(w4.x, v[t], t0);
+                            t1 = fmaf(w4.y, v[t], t1);
+                            t2 = fmaf(w4.z, v[t], t2);
+                            t3 = fmaf(w4.w, v[t], t3);
+                        }
+                        acc[c4 * 4 + 0] += t0;
+                        acc[c4 * 4 + 1] += t1;
+                        acc[c4 * 4 + 2] += t2;
+                        acc[c4 * 4 + 3] += t3;
                     }
-                    acc[c4 * 4 + 0] += t0;
-                    acc[c4 * 4 + 1] += t1;
-                    acc[c4 * 4 + 2] += t2;
-                    acc[c4 * 4 + 3] += t3;
-                }
-            } else {
+                } else {
 #pragma unroll
-                for (int co = 0; co < CT; co++) {
-                    float t0 = s_w[ck][0][co] * v[0];
+                    for (int co = 0; co < CT; co++) {
+                        float t0 = s_w[ck][0][co] * v[0];
 #pragma unroll
-                    for (int t = 1; t < 9; t++) t0 = fmaf(s_w[ck][t][co], v[t], t0);
-                    acc[co] += t0;
+                        for (int t = 1; t < 9; t++) t0 = fmaf(s_w[ck][t][co], v[t], t0);
+                        acc[co] += t0;
+                    }
                 }
             }
+            __syncthreads();
         }
-        __syncthreads();
-    }
-    const int x = x0 + tx, y = y0 + ty;
-    if (x < W && y < H) {
+        const int x = x0 + tx, y = y0 + ty;
+        if (x < W && y < H) {
 #pragma unroll
-        for (int co = 0; co < CT; co++) {
-            if (co0 + co < Cout) {
-                float v = acc[co] + __ldg(bias + co0 + co);
-                float pos = fmaxf(v, 0.f), neg = fminf(v, 0.f);
-                out[plane * (co0 + co) + (long)y * W + x] = neg * 0.1f + pos;
+            for (int co = 0; co < CT; co++) {
+                if (co0 + co < Cout) {
+                    float v = acc[co] + __ldg(bias + co0 + co);
+                    float pos = fmaxf(v, 0.f), neg = fminf(v, 0.f);
+                    out[plane * (co0 + co) + (long)y * W + x] = neg * 0.1f + pos;
+                }
             }
         }
     }
 }
 
 // ---- launchers --------------------------------------------------------------------------------
-static inline dim3 grid2d(int w, int h, dim3 b) { return dim3((w + b.x - 1) / b.x, (h + b.y - 1) / b.y); }
+static inline dim3 grid2d(int w, int h, dim3 b) { return dim3((w + b.x - 1) / b.x, std::min<unsigned>((h + b.y - 1) / b.y, MAX_GRID_Y)); }
 
 cudaError_t launch_pad_replicate(const float *in, int w, int h, long in_stride_floats, int pad,
                                  int rows_above, int rows_below, float *out, cudaStream_t s) {
@@ -230,8 +245,7 @@ cudaError_t launch_copy2d(const float *in, long in_stride_floats, float *out, lo
 
 cudaError_t launch_conv3x3_fp32(const float *in, float *out, const float *wgt, const float *bias, int Cin, int Cout,
                                 int W, int H, cudaStream_t s) {
-    dim3 grid((W + TX - 1) / TX, (H + TY - 1) / TY, 1);
-    if (grid.y > 65535) return cudaErrorInvalidConfiguration;
+    dim3 grid((W + TX - 1) / TX, std::min<unsigned>((H + TY - 1) / TY, MAX_GRID_Y), 1);
     if (Cout > 16) {
         grid.z = (Cout + 31) / 32;
         conv3x3_planar_fp32<32><<<grid, TX * TY, 0, s>>>(in, out, wgt, bias, Cin, Cout, W, H);

@@ -60,12 +60,16 @@ uint16_t f32_to_f16_rn(float f);    // round-to-nearest-even, subnormals kept
 float f16_to_f32(uint16_t h);
 uint8_t f32_to_e4m3_rn(float f);    // OCP e4m3 (max 448, no inf), round-to-nearest-even, saturating (cvt.rn.satfinite.e4m3x2.f32)
 
+// The most rows a frame (a padded plane, band or packed frame that one layer pass covers) may have: the first layer, the
+// separate last layer, the gathers and the pack tile it in 8-row blocks on grid.y, which is at most 65535.
+constexpr long MAX_FRAME_ROWS = 8L * 65535;
+
 // geometry.cpp
 struct Config { int n_job = 4, block_w = 512, block_h = 512; };
 Config &config();
 int block_table(int w, int h, int bw, int bh, int n_model, int *table, int capacity, int *sc, int *sr);
 // Places the padded rectangles (w + 2 n_layers) x (h + 2 n_layers) of n independent planes side by side into frames of at most
-// scratch_limit / (max_channels * 4) pixels and 524 280 rows.  frame[i] = the plane's frame, or -1 when its rectangle fits no
+// scratch_limit / (max_channels * 4) pixels and MAX_FRAME_ROWS rows.  frame[i] = the plane's frame, or -1 when its rectangle fits no
 // frame (the caller converts it alone); (x0[i], y0[i]) = the rectangle's top-left corner.  Returns the frame count; fw / fh
 // receive the frame sizes.
 int plan_planes(int n, const int *widths, const int *heights, int n_layers, int max_channels, size_t scratch_limit, int *frame,
