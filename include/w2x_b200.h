@@ -290,6 +290,32 @@ W2X_API int w2x_convert_planes_device(w2x_ctx *ctx, const w2x_model *model, int 
                                       const int *widths, const int *heights, const size_t *in_strides, float *const *d_out,
                                       const size_t *out_strides);
 
+/* ---- a chain of conversions on one plane: noise reduction, then 2x scaling steps ------------------ */
+/* The reference's main loop (src/main.cpp:82-156) runs the Y plane through the noise model (:96) and then through k scale
+ * iterations, each a nearest-neighbour 2x resize followed by the scale model (:132-148).  Y after a step depends only on Y before
+ * it (split, merge and an exact 2x INTER_NEAREST resize copy values; the bicubic Y channel is overwritten at :148-154), so the
+ * whole sequence can run in one call that keeps the plane on the device between steps and never builds the 2x plane.
+ * Step k computes P_{k+1} = convertWithModels(models[k], U_k(P_k)), P_0 = in, U_k = identity (W2X_STEP_SAME) or the nearest 2x
+ * resize (W2X_STEP_UPSCALE2X); every P_{k+1} is bit-identical to w2x_convert_plane(ctx, models[k], U_k(P_k), ..., block_splitting)
+ * on the same context settings.  The output is (width << u) x (height << u), u = the number of upscaling steps.
+ * Before step k is queued, on_step(k, user) is called (if not NULL); then the step logs the progress lines w2x_convert_plane
+ * (host entry) or w2x_convert_plane_device (device entry) logs for its plane, block lines included.
+ * Every argument is checked before anything is queued; W2X_ERR_ARG names the step: n_steps < 1, a NULL models / kinds array or
+ * model, an unknown kind, a model that does not map 1 plane to 1 plane, an output size that overflows int, bad row strides
+ * (multiples of 4 bytes, >= the row) or NULL planes.  in and out must not overlap.
+ * HOST buffers, synchronous. */
+#define W2X_STEP_SAME 0        /* the model's output replaces the plane (noise pass, src/main.cpp:96) */
+#define W2X_STEP_UPSCALE2X 1   /* cv::resize INTER_NEAREST to 2w x 2h (src/main.cpp:132-140), then the model (:148) */
+typedef void (*w2x_step_fn)(int step, void *user);
+W2X_API int w2x_convert_chain(w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds,
+                              const float *in, int width, int height, size_t in_stride_bytes,
+                              float *out, size_t out_stride_bytes, int block_splitting, w2x_step_fn on_step, void *user);
+/* Same on DEVICE planes, asynchronous on the context's stream (w2x_ctx_set_stream). */
+W2X_API int w2x_convert_chain_device(w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds,
+                                     const float *d_in, int width, int height, size_t in_stride_bytes,
+                                     float *d_out, size_t out_stride_bytes, int block_splitting, w2x_step_fn on_step,
+                                     void *user);
+
 /* ---- one process, N GPUs ---------------------------------------------------------------------- */
 /* The sibling of the reference's -j (src/main.cpp:58-60, modelUtility::setNumberOfJobs): N contexts driven by
  * one host thread.  w2x_multi_convert_plane = w2x_convert_plane with the plane cut into N row bands and the
@@ -321,6 +347,7 @@ W2X_API int w2x_ctx_layer_times(w2x_ctx *ctx, int max_layers, float *ms, int *la
                                 int *n_layers_out, int reset);
 /* Name of the kernel family the last convert call used for `layer` ("fp32_direct",
  * "wgmma_f16x3", "wgmma_f16+f8x2", "wgmma_f16", each with "+last" when the last layer is folded in, "first_1xN",
+ * "first_1xN+up2x" (the first layer reading a half-resolution plane through the nearest 2x resize, w2x_convert_chain),
  * "last_Nx1", "last_gather"). */
 W2X_API const char *w2x_ctx_layer_kernel_name(const w2x_ctx *ctx, int layer);
 

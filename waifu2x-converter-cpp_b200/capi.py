@@ -18,6 +18,7 @@ _LIB_PATH = os.path.join(_HERE, "libw2x_b200.so")
 ENGINE_AUTO, ENGINE_FP32, ENGINE_TC = 0, 1, 2
 PRECISION_F16X3, PRECISION_F16_F8X2, PRECISION_F16 = 0, 1, 2
 WALK_FUSED, WALK_BLOCKS = 0, 1
+STEP_SAME, STEP_UPSCALE2X = 0, 1
 
 STATUS = {0: "W2X_OK", 1: "W2X_ERR_ARG", 2: "W2X_ERR_IO", 3: "W2X_ERR_PARSE", 4: "W2X_ERR_MODEL",
           5: "W2X_ERR_CUDA", 6: "W2X_ERR_NO_DEVICE", 7: "W2X_ERR_UNSUPPORTED", 8: "W2X_ERR_NOMEM"}
@@ -39,7 +40,7 @@ ABI_SYMBOLS = (
     "w2x_multi_set_precision", "w2x_multi_set_log", "w2x_multi_convert_plane", "w2x_multi_convert_tiles",
     "w2x_host_alloc", "w2x_host_free", "w2x_ctx_forget_model", "w2x_slab_create", "w2x_slab_destroy", "w2x_slab_export",
     "w2x_slab_connect", "w2x_slab_connect_local", "w2x_slab_convert", "w2x_slab_convert_async", "w2x_slab_synchronize",
-    "w2x_convert_planes", "w2x_convert_planes_device",
+    "w2x_convert_planes", "w2x_convert_planes_device", "w2x_convert_chain", "w2x_convert_chain_device",
 )
 BAND_BLOB_BYTES = 320
 
@@ -53,6 +54,7 @@ class W2xError(RuntimeError):
 
 _lib = None
 LOG_FN = C.CFUNCTYPE(None, C.c_char_p, C.c_void_p)
+STEP_FN = C.CFUNCTYPE(None, C.c_int, C.c_void_p)
 
 
 def lib_path() -> str:
@@ -141,6 +143,8 @@ def lib():
     pi, ps = C.POINTER(ci), C.POINTER(cs)
     L.w2x_convert_planes.argtypes = [vp, vp, ci, C.POINTER(vp), pi, pi, ps, C.POINTER(vp), ps]
     L.w2x_convert_planes_device.argtypes = [vp, vp, ci, C.POINTER(vp), pi, pi, ps, C.POINTER(vp), ps]
+    L.w2x_convert_chain.argtypes = [vp, ci, C.POINTER(vp), pi, vp, ci, ci, cs, vp, cs, ci, STEP_FN, vp]
+    L.w2x_convert_chain_device.argtypes = [vp, ci, C.POINTER(vp), pi, vp, ci, ci, cs, vp, cs, ci, STEP_FN, vp]
     L.w2x_debug_plan_planes.argtypes = [ci, pi, pi, ci, ci, cs, pi, pi, pi, pi, ci]
     L.w2x_multi_create.argtypes = [C.POINTER(ci), ci, C.POINTER(vp)]
     L.w2x_multi_destroy.argtypes = [vp]
@@ -435,6 +439,44 @@ class Context:
         _check(lib().w2x_convert_planes_device(self._h, model._h, n, (C.c_void_p * n)(*d_in), (C.c_int * n)(*widths),
                                                (C.c_int * n)(*heights), (C.c_size_t * n)(*in_strides),
                                                (C.c_void_p * n)(*d_out), (C.c_size_t * n)(*out_strides)))
+
+    # the reference's noise pass and 2x scale iterations on one plane (src/main.cpp:82-156), kept on the device between steps
+    @staticmethod
+    def _chain_args(steps, on_step):
+        steps = list(steps)
+        n = len(steps)
+        models = (C.c_void_p * max(n, 1))(*[m._h if m is not None else None for m, _ in steps])
+        kinds = (C.c_int * max(n, 1))(*[STEP_UPSCALE2X if up else STEP_SAME for _, up in steps])
+        cb = STEP_FN(lambda k, _u: on_step(k)) if on_step is not None else STEP_FN()
+        ups = sum(1 for _, up in steps if up)
+        return n, models, kinds, cb, ups
+
+    def convert_chain(self, steps, plane, out=None, block_splitting=True, on_step=None):
+        """steps: list of (model, upscale) pairs -- upscale=True resizes the plane to 2w x 2h (nearest) before the model.
+        plane: 2-D float32 array (a row-strided view is passed as it is) -> the last step's plane, (h << u) x (w << u) for u upscaling
+        steps; `out` may be such an array (strided views included), written in place.  on_step(k) is called before step k."""
+        x = np.asarray(plane, np.float32)
+        if x.ndim != 2:
+            raise ValueError("plane must be 2-D")
+        if x.strides[1] != 4 or x.strides[0] % 4 or x.strides[0] < x.shape[1] * 4:
+            x = np.ascontiguousarray(x)
+        h, w = x.shape
+        n, models, kinds, cb, ups = self._chain_args(steps, on_step)
+        if out is None:
+            out = np.empty((h << ups, w << ups), np.float32)
+        if out.ndim != 2 or out.dtype != np.float32 or out.strides[1] != 4 or out.strides[0] % 4:
+            raise ValueError("out must be a 2-D float32 array with unit column stride and a row stride that is a multiple of 4 bytes")
+        if out.shape != (h << ups, w << ups):
+            raise ValueError(f"out must have shape {(h << ups, w << ups)}")
+        _check(lib().w2x_convert_chain(self._h, n, models, kinds, C.c_void_p(x.ctypes.data), w, h, x.strides[0],
+                                       C.c_void_p(out.ctypes.data), out.strides[0], int(bool(block_splitting)), cb, None))
+        return out
+
+    def convert_chain_device(self, steps, d_in, w, h, in_stride_bytes, d_out, out_stride_bytes, block_splitting=True, on_step=None):
+        """Device pointers (ints); asynchronous on the context's stream.  The output is (w << u) x (h << u)."""
+        n, models, kinds, cb, _ = self._chain_args(steps, on_step)
+        _check(lib().w2x_convert_chain_device(self._h, n, models, kinds, C.c_void_p(d_in), w, h, in_stride_bytes, C.c_void_p(d_out),
+                                              out_stride_bytes, int(bool(block_splitting)), cb, None))
 
     # w2xc::Model::filter on host planes [n_in][h][w] -> [n_out][h][w]
     def filter_layer(self, model: Model, layer, in_planes):

@@ -14,6 +14,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <climits>
 #include <cstdlib>
 #include <cstring>
 #include <map>
@@ -230,7 +231,7 @@ int run_basic(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int engine, const 
         LayerTimer t(ctx, 0);
         const tc::FirstSource padded{src, src_stride, pw, ph, 0, 0, 0, 0};
         CU_CHECK(tc::launch_first(direct ? *direct : padded, pw, ph, L.w.data(), dm->b_host[0].data(), L.n_out, cur, ctx->stream, f8));
-        note_kernel(ctx, 0, "first_1xN");
+        note_kernel(ctx, 0, direct && direct->up2x ? "first_1xN+up2x" : "first_1xN");
         ctx->launches++;
     }
     const bool fuse = ctx->fuse_last && n >= 3 && !dm->last_w_t.empty();
@@ -282,15 +283,24 @@ int scratch_band_rows(const w2x_ctx *ctx, const w2x_model *m, int w, int h) {
     return (int)std::min<long>(h, max_rows);
 }
 
+// up2x (direct_in only): the plane is the nearest-neighbour 2x resize of direct_in, w x h its 2x size (see convert_device).
 int run_padded_plane(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int engine, const float *padp, int w, int h,
-                     float *dst, long dst_stride, const float *direct_in = nullptr, long in_stride = 0, int rows_above = 0, int rows_below = 0) {
+                     float *dst, long dst_stride, const float *direct_in = nullptr, long in_stride = 0, int rows_above = 0, int rows_below = 0,
+                     bool up2x = false) {
     const int n = (int)m->layers.size();
     const int pw = w + 2 * n;
     const int band = scratch_band_rows(ctx, m, w, h);
     for (int y0 = 0; y0 < h; y0 += band) {
         const int bh = std::min(band, h - y0);
         int rc;
-        if (direct_in) {
+        if (direct_in && up2x) {
+            // the band's 2x rows [y0, y0 + bh) seen from source row y0 >> 1: on an odd y0 the band is 2x row 1 of that source row
+            const int p = y0 & 1;
+            tc::FirstSource fs{direct_in + (long)(y0 >> 1) * in_stride, in_stride, w, bh + p, n, n - p, std::min(n, y0 + rows_above) - p,
+                               std::min(n, h - y0 - bh + rows_below)};
+            fs.up2x = true;
+            rc = run_basic(ctx, m, dm, engine, nullptr, 0, pw, bh + 2 * n, dst + (long)y0 * dst_stride, dst_stride, nullptr, &fs);
+        } else if (direct_in) {
             const tc::FirstSource fs{direct_in + (long)y0 * in_stride, in_stride, w, bh, n, n, std::min(n, y0 + rows_above), std::min(n, h - y0 - bh + rows_below)};
             rc = run_basic(ctx, m, dm, engine, nullptr, 0, pw, bh + 2 * n, dst + (long)y0 * dst_stride, dst_stride, nullptr, &fs);
         } else {
@@ -306,10 +316,21 @@ int check_ctx(w2x_ctx *ctx) {
     return W2X_OK;
 }
 
+// Row bands of w2x_convert_plane's host copy pipeline for a plane of width x height (1 = no pipeline: one upload, one pass,
+// one download).  The literal block walk keeps its own order, and a band needs 2n rows of its own.
+int host_copy_bands(const w2x_ctx *ctx, int n_model, int width, int height, int block_splitting) {
+    int nb = ctx->host_bands > 0 ? ctx->host_bands : std::min(4, height / 512);
+    const bool literal_walk = block_splitting && ctx->walk == W2X_WALK_BLOCKS && w2x_requires_splitting(width, height);
+    if (nb > 8) nb = 8;
+    if (nb < 2 || literal_walk || height / nb < 2 * n_model) return 1;
+    return nb;
+}
+
 int convert_device(w2x_ctx *ctx, const w2x_model *m, const float *d_in, int w, int h, size_t in_stride_bytes,
-                   int rows_above, int rows_below, float *d_out, size_t out_stride_bytes, int block_splitting) {
+                   int rows_above, int rows_below, float *d_out, size_t out_stride_bytes, int block_splitting, bool up2x) {
     if (!m || !d_in || !d_out || w < 1 || h < 1) return fail(W2X_ERR_ARG, "w2x_convert_plane: bad argument");
-    if (in_stride_bytes % 4 || out_stride_bytes % 4 || in_stride_bytes < (size_t)w * 4 || out_stride_bytes < (size_t)w * 4)
+    const int in_w = up2x ? (w + 1) / 2 : w;
+    if (in_stride_bytes % 4 || out_stride_bytes % 4 || in_stride_bytes < (size_t)in_w * 4 || out_stride_bytes < (size_t)w * 4)
         return fail(W2X_ERR_ARG, "w2x_convert_plane: row strides must be multiples of 4 bytes and >= width*4");
     if (m->layers.front().n_in != 1 || m->layers.back().n_out != 1)
         return fail(W2X_ERR_ARG, "w2x_convert_plane: model must map 1 plane to 1 plane");
@@ -328,13 +349,18 @@ int convert_device(w2x_ctx *ctx, const w2x_model *m, const float *d_in, int w, i
         // cv::copyMakeBorder (src/convertRoutine.cpp:35, :96) is folded into the first layer's loads: no padded copy of the plane
         if (split && !ctx->log_muted) emit_reference_progress(ctx, w, h, n, true);
         LogMute mute(ctx, split);
-        return run_padded_plane(ctx, m, dm, engine, nullptr, w, h, d_out, ostride, d_in, (long)(in_stride_bytes / 4), rows_above, rows_below);
+        return run_padded_plane(ctx, m, dm, engine, nullptr, w, h, d_out, ostride, d_in, (long)(in_stride_bytes / 4), rows_above, rows_below,
+                                up2x);
     }
     rc = ensure(reinterpret_cast<void **>(&ctx->pad_buf), &ctx->pad_bytes, (size_t)pw * ph * sizeof(float));
     if (rc) return rc;
     // cv::copyMakeBorder(in, temp, n, n, n, n, BORDER_REPLICATE)   (src/convertRoutine.cpp:35, :96)
-    CU_CHECK(launch_pad_replicate(d_in, w, h, (long)(in_stride_bytes / 4), n, std::min(rows_above, n),
-                                  std::min(rows_below, n), ctx->pad_buf, ctx->stream));
+    if (up2x)
+        CU_CHECK(launch_pad_upsample2x(d_in, w, h, (long)(in_stride_bytes / 4), n, std::min(rows_above, n), std::min(rows_below, n),
+                                       ctx->pad_buf, ctx->stream));
+    else
+        CU_CHECK(launch_pad_replicate(d_in, w, h, (long)(in_stride_bytes / 4), n, std::min(rows_above, n),
+                                      std::min(rows_below, n), ctx->pad_buf, ctx->stream));
     ctx->launches++;
     if (split && ctx->walk == W2X_WALK_BLOCKS) {
         // the literal block walk of convertWithModelsBlockSplit (src/convertRoutine.cpp:114-165)
@@ -439,6 +465,7 @@ void w2x_ctx_destroy(w2x_ctx *ctx) {
     for (int i = 0; i < 2; i++) {
         cudaFree(ctx->buf[i]);
         cudaFree(ctx->io_buf[i]);
+        cudaFree(ctx->chain_buf[i]);
     }
     cudaFree(ctx->pad_buf);
     cudaFree(ctx->plan_buf);
@@ -597,10 +624,8 @@ int w2x_convert_plane(w2x_ctx *ctx, const w2x_model *model, const float *in, int
     // layers of band i (copy engines + compute run concurrently); each band re-reads n real rows of context from its
     // neighbours, which keeps the result bit-identical to the single-pass path.
     const int n_model = model ? (int)model->layers.size() : 0;
-    int nb = ctx->host_bands > 0 ? ctx->host_bands : std::min(4, height / 512);
-    const bool literal_walk = block_splitting && ctx->walk == W2X_WALK_BLOCKS && w2x_requires_splitting(width, height);
-    if (nb > 8) nb = 8;
-    if (nb < 2 || literal_walk || !model || height / nb < 2 * n_model) {
+    const int nb = model ? host_copy_bands(ctx, n_model, width, height, block_splitting) : 1;
+    if (nb < 2) {
         CU_CHECK(cudaMemcpy2DAsync(ctx->io_buf[0], (size_t)width * 4, in, in_stride_bytes, (size_t)width * 4, (size_t)height,
                                    cudaMemcpyHostToDevice, ctx->stream));
         int rc = convert_device(ctx, model, ctx->io_buf[0], width, height, (size_t)width * 4, 0, 0, ctx->io_buf[1],
@@ -1201,6 +1226,188 @@ int w2x_convert_planes(w2x_ctx *ctx, const w2x_model *model, int n_planes, const
     rc = planes_host_pipeline(ctx, model, dm, n_planes, in, widths, heights, in_strides, out, out_strides);
     if (rc) {   // copies already queued still touch the caller's buffers and the staging: drain them first
         cudaStreamSynchronize(ctx->copy_in);
+        cudaStreamSynchronize(ctx->stream);
+        cudaStreamSynchronize(ctx->copy_out);
+    }
+    return rc;
+}
+
+}  // extern "C"
+
+// ---- chains of conversions on one plane (w2x_convert_chain*) ---------------------------------------------------------------
+// The reference's main loop (src/main.cpp:82-156) runs the Y plane through the noise model (:96) and then through k scale
+// iterations, each a nearest-neighbour 2x resize (:132-140) followed by the scale model (:148).  The Y plane after a step depends
+// only on the Y plane before it, so the whole sequence stays on the device: intermediate planes live in ctx->chain_buf, and an
+// upscaling step reads its half-resolution source through the first layer (or the padding kernel) instead of a 2x plane.
+namespace {
+struct ChainStep {
+    const w2x_model *m;
+    bool up;
+    int w, h;     // the step's OUTPUT size
+};
+
+// Every argument, before anything is queued: W2X_ERR_ARG naming the step it concerns.
+int check_chain(const char *fn, w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, const void *in, int width,
+                int height, size_t in_stride_bytes, const void *out, size_t out_stride_bytes, bool host, std::vector<ChainStep> *steps) {
+    if (check_ctx(ctx)) return W2X_ERR_ARG;
+    if (n_steps < 1) return fail(W2X_ERR_ARG, "%s: n_steps is %d: at least one step (step 0) is needed", fn, n_steps);
+    if (!models) return fail(W2X_ERR_ARG, "%s: step 0: NULL models array", fn);
+    if (!kinds) return fail(W2X_ERR_ARG, "%s: step 0: NULL kinds array", fn);
+    if (width < 1 || height < 1) return fail(W2X_ERR_ARG, "%s: step 0: input size %d x %d", fn, width, height);
+    if (!in) return fail(W2X_ERR_ARG, "%s: step 0: NULL input plane", fn);
+    if (in_stride_bytes % 4 || in_stride_bytes < (size_t)width * 4)
+        return fail(W2X_ERR_ARG, "%s: step 0: the input row stride must be a multiple of 4 bytes and >= width*4", fn);
+    long w = width, h = height;
+    steps->clear();
+    for (int k = 0; k < n_steps; k++) {
+        const w2x_model *m = models[k];
+        if (!m) return fail(W2X_ERR_ARG, "%s: step %d: NULL model", fn, k);
+        if (kinds[k] != W2X_STEP_SAME && kinds[k] != W2X_STEP_UPSCALE2X)
+            return fail(W2X_ERR_ARG, "%s: step %d: kind %d is neither W2X_STEP_SAME (0) nor W2X_STEP_UPSCALE2X (1)", fn, k, kinds[k]);
+        if (m->layers.front().n_in != 1 || m->layers.back().n_out != 1)
+            return fail(W2X_ERR_ARG, "%s: step %d: model must map 1 plane to 1 plane", fn, k);
+        if (kinds[k] == W2X_STEP_UPSCALE2X) {
+            w *= 2;
+            h *= 2;
+            if (w > INT_MAX || h > INT_MAX) return fail(W2X_ERR_ARG, "%s: step %d: the output size %ld x %ld overflows int", fn, k, w, h);
+        }
+        steps->push_back(ChainStep{m, kinds[k] == W2X_STEP_UPSCALE2X, (int)w, (int)h});
+    }
+    const int last = n_steps - 1;
+    if (!out) return fail(W2X_ERR_ARG, "%s: step %d: NULL output plane", fn, last);
+    if (out_stride_bytes % 4 || out_stride_bytes < (size_t)w * 4)
+        return fail(W2X_ERR_ARG, "%s: step %d: the output row stride must be a multiple of 4 bytes and >= width*4 (%ld)", fn, last, w * 4);
+    if (host) {   // device planes may alias in ways the host cannot see; host planes are checked
+        const char *i0 = static_cast<const char *>(in), *i1 = i0 + (size_t)(height - 1) * in_stride_bytes + (size_t)width * 4;
+        const char *o0 = static_cast<const char *>(out), *o1 = o0 + (size_t)(h - 1) * out_stride_bytes + (size_t)w * 4;
+        if (i0 < o1 && o0 < i1) return fail(W2X_ERR_ARG, "%s: step %d: the output plane overlaps the input plane", fn, last);
+    }
+    for (int k = 0; k < n_steps; k++) {   // engine choice (the tensor-core engine needs a 1->{32,64,128}...->1 chain)
+        if (pick_engine(ctx, (*steps)[(size_t)k].m) < 0) {
+            const std::string why = w2x_last_error();
+            return fail(W2X_ERR_UNSUPPORTED, "%s: step %d: %s", fn, k, why.c_str());
+        }
+    }
+    return W2X_OK;
+}
+
+// Sizes both intermediate buffers for the whole chain before the first step is queued (step k writes chain_buf[k & 1]).
+int reserve_chain(w2x_ctx *ctx, const std::vector<ChainStep> &steps) {
+    size_t need[2] = {0, 0};
+    for (size_t k = 0; k + 1 < steps.size(); k++) need[k & 1] = std::max(need[k & 1], (size_t)steps[k].w * steps[k].h * sizeof(float));
+    for (int i = 0; i < 2; i++) {
+        if (!need[i]) continue;
+        int rc = ensure(reinterpret_cast<void **>(&ctx->chain_buf[i]), &ctx->chain_bytes[i], need[i]);
+        if (rc) return rc;
+    }
+    return W2X_OK;
+}
+
+// One step on device planes, logging what the single-plane entry point would log for the step's plane: w2x_convert_plane (host)
+// emits the reference's sequence up front when its copy pipeline cuts the plane, w2x_convert_plane_device logs as it goes.
+int chain_step(w2x_ctx *ctx, const ChainStep &s, const float *src, size_t src_stride, float *dst, size_t dst_stride, int block_splitting,
+               bool host) {
+    const int n = (int)s.m->layers.size();
+    const bool pipelined = host && host_copy_bands(ctx, n, s.w, s.h, block_splitting) >= 2;
+    if (pipelined) emit_reference_progress(ctx, s.w, s.h, n, block_splitting && w2x_requires_splitting(s.w, s.h));
+    LogMute mute(ctx, pipelined);
+    return convert_device(ctx, s.m, src, s.w, s.h, src_stride, 0, 0, dst, dst_stride, block_splitting, s.up);
+}
+
+// Steps [0, n_dev) on the device: the first reads d_in, step k writes chain_buf[k & 1], the last of the whole chain writes d_out.
+int chain_device_steps(w2x_ctx *ctx, const std::vector<ChainStep> &steps, int n_dev, const float *d_in, size_t in_stride, float *d_out,
+                       size_t out_stride, int block_splitting, w2x_step_fn on_step, void *user, bool host) {
+    const float *cur = d_in;
+    size_t cur_stride = in_stride;
+    for (int k = 0; k < n_dev; k++) {
+        const ChainStep &s = steps[(size_t)k];
+        const bool last = k + 1 == (int)steps.size();
+        float *dst = last ? d_out : ctx->chain_buf[k & 1];
+        const size_t dst_stride = last ? out_stride : (size_t)s.w * sizeof(float);
+        if (on_step) on_step(k, user);
+        int rc = chain_step(ctx, s, cur, cur_stride, dst, dst_stride, block_splitting, host);
+        if (rc) return rc;
+        cur = dst;
+        cur_stride = dst_stride;
+    }
+    return W2X_OK;
+}
+
+// Host planes: one upload, the steps on the device, and the last step cut into the row bands of w2x_convert_plane's copy
+// pipeline when it would cut that plane, so that the download of band i overlaps the layers of band i + 1.  An upscaling step's
+// bands start on even 2x rows (the source row of a band's first row is then whole).
+int chain_host(w2x_ctx *ctx, const std::vector<ChainStep> &steps, const float *in, int width, int height, size_t in_stride_bytes, float *out,
+               size_t out_stride_bytes, int block_splitting, w2x_step_fn on_step, void *user) {
+    const ChainStep &L = steps.back();
+    const int n_steps = (int)steps.size(), n = (int)L.m->layers.size();
+    int rc = ensure(reinterpret_cast<void **>(&ctx->io_buf[0]), &ctx->io_bytes[0], (size_t)width * height * sizeof(float));
+    if (!rc) rc = ensure(reinterpret_cast<void **>(&ctx->io_buf[1]), &ctx->io_bytes[1], (size_t)L.w * L.h * sizeof(float));
+    if (!rc) rc = reserve_chain(ctx, steps);
+    if (rc) return rc;
+    CU_CHECK(cudaMemcpy2DAsync(ctx->io_buf[0], (size_t)width * 4, in, in_stride_bytes, (size_t)width * 4, (size_t)height, cudaMemcpyHostToDevice,
+                               ctx->stream));
+    const size_t in_dense = (size_t)width * 4, stage_stride = (size_t)L.w * 4;
+    const int nb = host_copy_bands(ctx, n, L.w, L.h, block_splitting);
+    if (nb < 2) {
+        rc = chain_device_steps(ctx, steps, n_steps, ctx->io_buf[0], in_dense, ctx->io_buf[1], stage_stride, block_splitting, on_step, user, true);
+        if (rc) return rc;
+        CU_CHECK(cudaMemcpy2DAsync(out, out_stride_bytes, ctx->io_buf[1], stage_stride, stage_stride, (size_t)L.h, cudaMemcpyDeviceToHost,
+                                   ctx->stream));
+        CU_CHECK(cudaStreamSynchronize(ctx->stream));
+        return W2X_OK;
+    }
+    rc = chain_device_steps(ctx, steps, n_steps - 1, ctx->io_buf[0], in_dense, nullptr, 0, block_splitting, on_step, user, true);
+    if (rc) return rc;
+    const float *src = n_steps == 1 ? ctx->io_buf[0] : ctx->chain_buf[(n_steps - 2) & 1];
+    const size_t src_stride = n_steps == 1 ? in_dense : (size_t)steps[(size_t)n_steps - 2].w * 4;
+    if (on_step) on_step(n_steps - 1, user);
+    emit_reference_progress(ctx, L.w, L.h, n, block_splitting && w2x_requires_splitting(L.w, L.h));
+    LogMute mute(ctx, true);
+    std::vector<int> r0((size_t)nb + 1);
+    for (int i = 0; i <= nb; i++) r0[(size_t)i] = (int)((long)L.h * i / nb) & (L.up ? ~1 : ~0);
+    for (int i = 0; i < nb; i++) {
+        const int y = r0[(size_t)i], rows = r0[(size_t)i + 1] - y;
+        const float *band_src = reinterpret_cast<const float *>(reinterpret_cast<const char *>(src) + (size_t)(L.up ? y / 2 : y) * src_stride);
+        rc = convert_device(ctx, L.m, band_src, L.w, rows, src_stride, i > 0 ? n : 0, i + 1 < nb ? n : 0, ctx->io_buf[1] + (size_t)y * L.w,
+                            stage_stride, 0, L.up);
+        if (rc) return rc;
+        CU_CHECK(cudaEventRecord(ctx->ev_done[i], ctx->stream));
+        CU_CHECK(cudaStreamWaitEvent(ctx->copy_out, ctx->ev_done[i], 0));
+        CU_CHECK(cudaMemcpy2DAsync(reinterpret_cast<char *>(out) + (size_t)y * out_stride_bytes, out_stride_bytes, ctx->io_buf[1] + (size_t)y * L.w,
+                                   stage_stride, stage_stride, (size_t)rows, cudaMemcpyDeviceToHost, ctx->copy_out));
+    }
+    CU_CHECK(cudaStreamSynchronize(ctx->copy_out));
+    CU_CHECK(cudaStreamSynchronize(ctx->stream));
+    return W2X_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int w2x_convert_chain_device(w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, const float *d_in, int width,
+                             int height, size_t in_stride_bytes, float *d_out, size_t out_stride_bytes, int block_splitting,
+                             w2x_step_fn on_step, void *user) {
+    std::vector<ChainStep> steps;
+    int rc = check_chain("w2x_convert_chain_device", ctx, n_steps, models, kinds, d_in, width, height, in_stride_bytes, d_out, out_stride_bytes,
+                         false, &steps);
+    if (rc) return rc;
+    DeviceGuard g(ctx->device);
+    NvtxRange nvtx("w2x convert chain");
+    rc = reserve_chain(ctx, steps);
+    if (rc) return rc;
+    return chain_device_steps(ctx, steps, n_steps, d_in, in_stride_bytes, d_out, out_stride_bytes, block_splitting, on_step, user, false);
+}
+
+int w2x_convert_chain(w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, const float *in, int width, int height,
+                      size_t in_stride_bytes, float *out, size_t out_stride_bytes, int block_splitting, w2x_step_fn on_step, void *user) {
+    std::vector<ChainStep> steps;
+    int rc = check_chain("w2x_convert_chain", ctx, n_steps, models, kinds, in, width, height, in_stride_bytes, out, out_stride_bytes, true,
+                         &steps);
+    if (rc) return rc;
+    DeviceGuard g(ctx->device);
+    NvtxRange nvtx("w2x convert chain");
+    rc = chain_host(ctx, steps, in, width, height, in_stride_bytes, out, out_stride_bytes, block_splitting, on_step, user);
+    if (rc) {   // copies already queued still touch the caller's buffers and the staging: drain them first
         cudaStreamSynchronize(ctx->stream);
         cudaStreamSynchronize(ctx->copy_out);
     }

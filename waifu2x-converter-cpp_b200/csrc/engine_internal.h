@@ -63,6 +63,8 @@ struct w2x_ctx {
     size_t pad_bytes = 0;
     float *io_buf[2] = {nullptr, nullptr};   // device staging for the host-buffer entry points
     size_t io_bytes[2] = {0, 0};
+    float *chain_buf[2] = {nullptr, nullptr};   // the planes between the steps of w2x_convert_chain*
+    size_t chain_bytes[2] = {0, 0};
     bool tc_ready = false;
     cudaStream_t copy_in = nullptr, copy_out = nullptr;   // host<->device copies of w2x_convert_plane overlap the compute stream
     cudaEvent_t ev_in[8] = {}, ev_done[8] = {};
@@ -138,9 +140,11 @@ void emit_reference_progress(w2x_ctx *ctx, int w, int h, int n_layers, bool spli
 // Only frame rows [out_y0, out_y0 + out_rows) are stored (out_rows < 0: the whole frame).
 int launch_layer_tc(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int li, const __half *in, __half *out, int pw, int ph,
                     bool fused, bool profile, int out_y0 = 0, int out_rows = -1);
-// convertWithModels on device buffers (rows_above / rows_below: real neighbour rows available around the band)
+// convertWithModels on device buffers (rows_above / rows_below: real neighbour rows available around the band).
+// up2x: the plane converted is the nearest-neighbour 2x resize of d_in, never materialised; w x h is its (2x) size, the row
+// counts are 2x rows, and a band of it starts on an even 2x row with d_in pointing at its first source row.
 int convert_device(w2x_ctx *ctx, const w2x_model *m, const float *d_in, int w, int h, size_t in_stride_bytes, int rows_above,
-                   int rows_below, float *d_out, size_t out_stride_bytes, int block_splitting);
+                   int rows_below, float *d_out, size_t out_stride_bytes, int block_splitting, bool up2x = false);
 
 int tiles_enqueue_compute(w2x_ctx *ctx, const w2x_model *model, const float *const *in_tiles, int n_tiles, int width, int height, size_t in_stride_bytes);
 int tiles_enqueue_download(w2x_ctx *ctx, float *const *out_tiles, int n_tiles, int width, int height, size_t out_stride_bytes);

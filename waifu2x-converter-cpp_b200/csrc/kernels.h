@@ -15,6 +15,11 @@ cudaError_t launch_pad_replicate(const float *in, int w, int h, long in_stride_f
 cudaError_t launch_pad_replicate_xy(const float *in, int w, int h, long in_stride_floats, int pad_x, int pad_top,
                                     int pad_bottom, int rows_above, int rows_below, float *out, cudaStream_t s,
                                     int skip_top = 0, int skip_bottom = 0);
+// launch_pad_replicate of the nearest-neighbour 2x resize of `in` (pixel (y, x) = in[y >> 1][x >> 1]) without materialising it:
+// w2 x h2 is the 2x plane (or a band of it starting on an even 2x row, `in` pointing at its first source row) and rows_above /
+// rows_below count real 2x rows beyond it.  Writes the dense (w2 + 2 pad) x (h2 + 2 pad) plane.
+cudaError_t launch_pad_upsample2x(const float *in, int w2, int h2, long in_stride_floats, int pad, int rows_above, int rows_below,
+                                  float *out, cudaStream_t s);
 // Peer-memory halo exchange (engine_band.cu): ONE kernel copies up to 8 row segments into the neighbour GPUs' frames,
 // publishes `value` in their flag words once every byte is visible system-wide, then waits until the neighbours have
 // published the same value here.  Flag values only grow, so nothing is ever reset.
@@ -53,11 +58,14 @@ cudaError_t init_kernels();
 // whose pixel (fy, fx) is the source plane's pixel (clamp(fy - pad_top), clamp(fx - pad_x)) -- i.e. cv::copyMakeBorder
 // (src/convertRoutine.cpp:35,96) is folded into the loads; pad_x = pad_top = 0 with w x h = pw x ph reads an already padded ROI.
 // rows_above / rows_below: real rows readable beyond the plane (row bands).  -> RECORD frame.
+// up2x: the source plane is the nearest-neighbour 2x resize of `in` (pixel (y, x) = in[y >> 1][x >> 1]); w, h, pad_top and the
+// row counts are in 2x rows / columns, `in` points at the source row holding 2x row 0 (see first_layer_kernel).
 // `wgt` ([C][9]) and `bias` ((float)bias) are HOST pointers: they travel as kernel parameters.
 struct FirstSource {
     const float *in;
     long stride_floats;
     int w, h, pad_x, pad_top, rows_above, rows_below;
+    bool up2x = false;
 };
 cudaError_t launch_first(const FirstSource &src, int pw, int ph, const float *wgt /*[C][9]*/, const float *bias, int cout, __half *out,
                          cudaStream_t s, int f8 = 0, int out_y0 = 0, int out_rows = -1);

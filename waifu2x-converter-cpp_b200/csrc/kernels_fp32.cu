@@ -41,6 +41,23 @@ __global__ void pad_replicate_kernel(const float *__restrict__ in, int w, int h,
     }
 }
 
+// The same padding of the nearest-neighbour 2x resize of `in` (cv::resize INTER_NEAREST to exactly twice the size,
+// src/main.cpp:135-139, whose pixel (y, x) is in[y >> 1][x >> 1]): w2 x h2 are the 2x plane's (or band's) size, the rows count
+// in 2x rows, and the band starts on an even 2x row, so that its first row is the first copy of in's row 0.
+__global__ void pad_upsample2x_kernel(const float *__restrict__ in, int w2, int h2, long in_stride, int pad, int rows_above,
+                                      int rows_below, float *__restrict__ out) {
+    const int W = w2 + 2 * pad, H = h2 + 2 * pad;
+    const int x = blockIdx.x * blockDim.x + threadIdx.x;
+    if (x >= W) return;
+    const int sx = min(max(x - pad, 0), w2 - 1) >> 1;
+    for (int by = blockIdx.y; by < row_blocks(H, blockDim.y); by += gridDim.y) {
+        const int y = by * blockDim.y + threadIdx.y;
+        if (y >= H) continue;
+        const int sy = min(max(y - pad, -rows_above), h2 - 1 + rows_below) >> 1;   // arithmetic shift: floor, also above the band
+        out[(long)y * W + x] = in[(long)sy * in_stride + sx];
+    }
+}
+
 // crop [pad, pad+h) x [pad, pad+w) of a dense (h+2pad) x (w+2pad) plane (src/convertRoutine.cpp:40-46)
 __global__ void crop_kernel(const float *__restrict__ in, int w, int h, int pad,
                             float *__restrict__ out, long out_stride) {
@@ -172,6 +189,14 @@ cudaError_t launch_pad_replicate_xy(const float *in, int w, int h, long in_strid
     dim3 b(32, 8);
     pad_replicate_kernel<<<grid2d(w + 2 * pad_x, h + pad_top + pad_bottom, b), b, 0, s>>>(
         in, w, h, in_stride_floats, pad_x, pad_top, pad_bottom, rows_above, rows_below, out, skip_top, skip_bottom);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_pad_upsample2x(const float *in, int w2, int h2, long in_stride_floats, int pad, int rows_above, int rows_below,
+                                  float *out, cudaStream_t s) {
+    dim3 b(32, 8);
+    pad_upsample2x_kernel<<<grid2d(w2 + 2 * pad, h2 + 2 * pad, b), b, 0, s>>>(in, w2, h2, in_stride_floats, pad, rows_above,
+                                                                               rows_below, out);
     return cudaGetLastError();
 }
 

@@ -160,8 +160,13 @@ static cudaError_t launch_first_c(const FirstSource &src, int pw, int ph, const 
     dim3 grid((pw + 31) / 32, (out_rows + 7) / 8);   // blocks tile the store window
     if (grid.y > 65535) return cudaErrorInvalidConfiguration;
     if (make_rec_map(&omap, out, COUT, pw, ph, 32, 8, out_y0, out_rows)) return cudaErrorInvalidValue;
-    if (f8) first_layer_kernel<COUT, true><<<grid, 256, FIRST_TILE_BYTES + 1024, s>>>(fs, pw, ph, out_y0, omap, prm);
-    else first_layer_kernel<COUT, false><<<grid, 256, FIRST_TILE_BYTES + 1024, s>>>(fs, pw, ph, out_y0, omap, prm);
+    if (src.up2x) {
+        if (f8) first_layer_kernel<COUT, true, true><<<grid, 256, FIRST_TILE_BYTES + 1024, s>>>(fs, pw, ph, out_y0, omap, prm);
+        else first_layer_kernel<COUT, false, true><<<grid, 256, FIRST_TILE_BYTES + 1024, s>>>(fs, pw, ph, out_y0, omap, prm);
+    } else {
+        if (f8) first_layer_kernel<COUT, true, false><<<grid, 256, FIRST_TILE_BYTES + 1024, s>>>(fs, pw, ph, out_y0, omap, prm);
+        else first_layer_kernel<COUT, false, false><<<grid, 256, FIRST_TILE_BYTES + 1024, s>>>(fs, pw, ph, out_y0, omap, prm);
+    }
     return cudaGetLastError();
 }
 

@@ -36,7 +36,11 @@ struct FirstSrc {
     int w, h, pad_x, pad_top, rows_above, rows_below;
 };
 
-template <int COUT, bool F8>
+// UP2X: the plane of w x h the frame pads is the nearest-neighbour 2x resize of `in` (cv::resize INTER_NEAREST to exactly twice
+// the size, src/main.cpp:135-139), never materialised: its pixel (y, x) is in[y >> 1][x >> 1].  Row 0 of that virtual plane is the
+// first copy of in's row 0, so a band starting on an odd 2x row has pad_top one smaller, rows_above one smaller and h one larger
+// than its even-row neighbour would (tc::FirstSource::up2x, set up by the engine).
+template <int COUT, bool F8, bool UP2X>
 __global__ void __launch_bounds__(256, 4)
 first_layer_kernel(const FirstSrc src, int pw, int ph, int out_y0, const __grid_constant__ CUtensorMap tmap_out,
                    const __grid_constant__ FirstParams<COUT> prm) {
@@ -53,7 +57,8 @@ first_layer_kernel(const FirstSrc src, int pw, int ph, int out_y0, const __grid_
             // being the replicate-padded input: clamp to the frame, then to the rows / columns that really exist
             const int fy = min(max(y + ky - 1, 0), ph - 1), fx = min(max(x + kx - 1, 0), pw - 1);
             const int sy = min(max(fy - src.pad_top, -src.rows_above), src.h - 1 + src.rows_below), sx = min(max(fx - src.pad_x, 0), src.w - 1);
-            v[ky * 3 + kx] = __ldg(src.in + (long)sy * src.in_stride + sx);
+            const int ry = UP2X ? sy >> 1 : sy, rx = UP2X ? sx >> 1 : sx;   // arithmetic shift: floor, also for the rows above
+            v[ky * 3 + kx] = __ldg(src.in + (long)ry * src.in_stride + rx);
         }
     const uint32_t r = (uint32_t)threadIdx.x;                            // pixel index inside the block = row of the staged image
     const uint32_t sw128 = r & 7u;

@@ -183,11 +183,56 @@ int main(int argc, char **argv) {
     w2xc::modelUtility::getInstance().setNumberOfJobs(std::atoi(cmd.get("jobs").c_str()));   // :79
     // (-j bounds the reference's filter threads; here it bounds the host image plumbing's row workers, the GPU does the filtering)
 
+    const bool noisePhase = mode == "noise" || mode == "noise_scale", scalePhase = mode == "scale" || mode == "noise_scale";
+    const int iterTimesTwiceScaling = static_cast<int>(std::ceil(std::log2(scaleRatio)));   // :107-108
+    std::vector<std::unique_ptr<w2xc::Model>> noiseModels, scaleModels;
+    if (noisePhase && !w2xc::modelUtility::generateModelFromJSON(modelDir + "/noise" + std::to_string(nrLevel) + "_model.json", noiseModels))
+        leave(-1);                                                                          // :88-89
+    // The Y plane after each pass depends only on the Y plane before it (split / merge / an exact 2x nearest resize copy values, the
+    // bicubic Y channel is overwritten at :148-154, U and V never feed back into Y).  So on one GPU the noise pass and every 2x
+    // iteration run as ONE chain that keeps Y on the device, while the bicubic iterations of U and V run here on the host.
+    // -m noise, --gpus n > 1 (w2x_multi_convert_plane), no usable device and a scale model that does not load keep the per-pass path below.
+    bool chained = false;
+    if (scalePhase && iterTimesTwiceScaling >= 1 && w2xc::modelUtility::tryGenerateModelFromJSON(modelDir + "/scale2.0x_model.json", scaleModels)) {
+        wait_for_gpu();
+        chained = w2xc::gpuRuntime::context() != nullptr && w2xc::gpuRuntime::multi() == nullptr;
+    }
+    if (chained) {
+        struct Progress {
+            bool noise;
+            int failedStep = -1;
+            static void step(int k, void *user) {                                           // stdout keeps the reference's line order
+                Progress *p = static_cast<Progress *>(user);
+                p->failedStep = k;
+                const int it = p->noise ? k : k + 1;                                        // 2x iteration number, 0 = the noise pass
+                if (it == 1) std::cout << "start scaling" << std::endl;                     // :123
+                if (it >= 1) std::cout << "#" << std::to_string(it) << " 2x scaling..." << std::endl;   // :129-130
+            }
+        } progress{noisePhase};
+        std::vector<w2xc::ChainStep> steps;
+        if (noisePhase) steps.push_back({&noiseModels, false});
+        for (int i = 0; i < iterTimesTwiceScaling; i++) steps.push_back({&scaleModels, true});
+        w2xc::Plane imageY = plane_of(image, 0), out;
+        // the bicubic iterations (:144) of U and V: w2ximg::resize computes every channel from that channel alone, so U and V do not
+        // depend on the Y values they are resized along with
+        std::thread colour([&] {
+            for (int i = 0; i < iterTimesTwiceScaling; i++) image = w2ximg::resize(image, image.width * 2, image.height * 2, w2ximg::CUBIC);
+        });
+        const double t0 = now();
+        const bool ok = w2xc::convertChainWithModels(imageY, out, steps, &Progress::step, &progress);
+        t_conv += now() - t0;
+        colour.join();
+        if (!ok) {
+            if (noisePhase && progress.failedStep <= 0) leave(-1);                          // the noise pass failed (see below)
+            std::cerr << "w2xc::convertWithModels : something error has occured.\nstop." << std::endl;
+            leave(1);
+        }
+        w2ximg::set_channel(image, 0, out.data, out.stride_bytes / 4);                    // merge, :98 and :154
+    }
+
     // ===== Noise Reduction Phase ===== (:82-100)
-    if (mode == "noise" || mode == "noise_scale") {
-        std::string modelFileName = modelDir + "/noise" + std::to_string(nrLevel) + "_model.json";
-        std::vector<std::unique_ptr<w2xc::Model>> models;
-        if (!w2xc::modelUtility::generateModelFromJSON(modelFileName, models)) leave(-1);
+    if (noisePhase && !chained) {
+        std::vector<std::unique_ptr<w2xc::Model>> &models = noiseModels;
         w2xc::Plane imageY = plane_of(image, 0), out;
         wait_for_gpu();
         const double t0 = now();
@@ -200,16 +245,15 @@ int main(int argc, char **argv) {
     }
 
     // ===== scaling phase ===== (:104-169)
-    if (mode == "scale" || mode == "noise_scale") {
-        int iterTimesTwiceScaling = static_cast<int>(std::ceil(std::log2(scaleRatio)));
+    if (scalePhase) {
         double shrinkRatio = 0.0;
         if (static_cast<int>(scaleRatio) != std::pow(2, iterTimesTwiceScaling))
             shrinkRatio = scaleRatio / std::pow(2.0, static_cast<double>(iterTimesTwiceScaling));
-        std::string modelFileName = modelDir + "/scale2.0x_model.json";
-        std::vector<std::unique_ptr<w2xc::Model>> models;
-        if (!w2xc::modelUtility::generateModelFromJSON(modelFileName, models)) leave(-1);
-        std::cout << "start scaling" << std::endl;
-        for (int nIteration = 0; nIteration < iterTimesTwiceScaling; nIteration++) {
+        std::vector<std::unique_ptr<w2xc::Model>> &models = scaleModels;
+        // :120-121 (when the quiet load above failed, this one fails again and reports it here, after the noise pass, as the reference does)
+        if (models.empty() && !w2xc::modelUtility::generateModelFromJSON(modelDir + "/scale2.0x_model.json", models)) leave(-1);
+        if (!chained) std::cout << "start scaling" << std::endl;
+        for (int nIteration = 0; nIteration < iterTimesTwiceScaling && !chained; nIteration++) {
             std::cout << "#" << std::to_string(nIteration + 1) << " 2x scaling..." << std::endl;
             const int w2 = image.width * 2, h2 = image.height * 2;
             w2xc::Plane imageY = plane_of_nearest(image, 0, w2, h2), out;                 // :135-139 (only the Y plane of the nearest image is used)

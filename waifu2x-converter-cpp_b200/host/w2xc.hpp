@@ -132,6 +132,7 @@ class Model {
     int layer_ = 0;
     friend class modelUtility;
     friend bool convertWithModels(Plane &, Plane &, std::vector<std::unique_ptr<Model>> &, bool);
+    friend const w2x_model *modelFileOf(std::vector<std::unique_ptr<Model>> &);
     Model(std::shared_ptr<w2x_model> f, int layer) : file_(std::move(f)), layer_(layer) {}
 
 public:
@@ -199,14 +200,12 @@ public:
     // static bool generateModelFromJSON(const std::string& fileName, std::vector<std::unique_ptr<Model>>& models)
     // (src/modelHandler.cpp:170-197): appends one Model per layer; false + message on failure.
     static bool generateModelFromJSON(const std::string &fileName, std::vector<std::unique_ptr<Model>> &models) {
-        w2x_model *m = take_prefetched(fileName);
-        if (!m && w2x_model_load_json(fileName.c_str(), &m) != W2X_OK) {
-            std::cerr << w2x_last_error() << std::endl;
-            return false;
-        }
-        std::shared_ptr<w2x_model> sp(m, w2x_model_free);
-        for (int i = 0; i < w2x_model_layer_count(m); i++) models.push_back(std::unique_ptr<Model>(new Model(sp, i)));
-        return true;
+        return load(fileName, models, true);
+    }
+    // Not in the reference: the same without the error message, for a caller that reports the failure later (by calling
+    // generateModelFromJSON again where the reference reports it).
+    static bool tryGenerateModelFromJSON(const std::string &fileName, std::vector<std::unique_ptr<Model>> &models) {
+        return load(fileName, models, false);
     }
     // Not in the reference: start reading + parsing a model file on a background thread (a 5.5 MB JSON file costs ~60 ms); a later
     // generateModelFromJSON(fileName, ...) of the same name takes the result.  Silent: if the background load failed, the
@@ -225,6 +224,16 @@ public:
     }
 
 private:
+    static bool load(const std::string &fileName, std::vector<std::unique_ptr<Model>> &models, bool report) {
+        w2x_model *m = take_prefetched(fileName);
+        if (!m && w2x_model_load_json(fileName.c_str(), &m) != W2X_OK) {
+            if (report) std::cerr << w2x_last_error() << std::endl;
+            return false;
+        }
+        std::shared_ptr<w2x_model> sp(m, w2x_model_free);
+        for (int i = 0; i < w2x_model_layer_count(m); i++) models.push_back(std::unique_ptr<Model>(new Model(sp, i)));
+        return true;
+    }
     static std::mutex &prefetch_mutex() { static std::mutex mu; return mu; }
     static std::map<std::string, std::future<w2x_model *>> &prefetched() {
         struct Holder {
@@ -281,6 +290,56 @@ inline bool convertWithModels(Plane &inputPlane, Plane &outputPlane, std::vector
     else
         rc = w2x_convert_plane(ctx, models[0]->file_.get(), inputPlane.data, inputPlane.width, inputPlane.height,
                                inputPlane.stride_bytes, outputPlane.data, outputPlane.stride_bytes, blockSplitting ? 1 : 0);
+    if (rc != W2X_OK) {
+        std::cerr << w2x_last_error() << std::endl;
+        return false;
+    }
+    return true;
+}
+
+// The model file whose layers `models` holds, in order (what generateModelFromJSON produced); nullptr + message otherwise.
+inline const w2x_model *modelFileOf(std::vector<std::unique_ptr<Model>> &models) {
+    if (models.empty()) return nullptr;
+    for (size_t i = 0; i < models.size(); i++)
+        if (models[i]->file_ != models[0]->file_ || models[i]->layer_ != (int)i ||
+            (int)models.size() != w2x_model_layer_count(models[0]->file_.get())) {
+            std::cerr << "Error : convertWithModels : models must be the layers of one model file, in order." << std::endl;
+            return nullptr;
+        }
+    return models[0]->file_.get();
+}
+
+// Not in the reference: the Y plane's passes of src/main.cpp:82-156 in ONE call -- steps[k] is a model (the layers of one model
+// file, as for convertWithModels) and whether the plane is first resized to 2w x 2h by cv::resize INTER_NEAREST (:132-140).  The
+// plane stays on the GPU between the steps and the 2x plane is never built; each step's result is bit-identical to
+// convertWithModels on the previous step's (resized) output.  onStep(k) runs before step k starts, then the step prints its
+// progress lines like convertWithModels.  outputPlane is (re)allocated to the final size.  One GPU only (w2x_convert_chain).
+struct ChainStep {
+    std::vector<std::unique_ptr<Model>> *models;
+    bool upscale2x;
+};
+inline bool convertChainWithModels(Plane &inputPlane, Plane &outputPlane, const std::vector<ChainStep> &steps,
+                                   void (*onStep)(int step, void *user), void *user, bool blockSplitting = true) {
+    w2x_ctx *ctx = gpuRuntime::context();
+    if (!ctx || steps.empty() || inputPlane.empty()) return false;
+    std::vector<const w2x_model *> files;
+    std::vector<int> kinds;
+    int w = inputPlane.width, h = inputPlane.height;
+    for (const ChainStep &s : steps) {
+        const w2x_model *f = s.models ? modelFileOf(*s.models) : nullptr;
+        if (!f) return false;
+        files.push_back(f);
+        kinds.push_back(s.upscale2x ? W2X_STEP_UPSCALE2X : W2X_STEP_SAME);
+        if (s.upscale2x) { w *= 2; h *= 2; }
+    }
+    if (outputPlane.data == inputPlane.data || outputPlane.width != w || outputPlane.height != h) outputPlane.create(w, h);
+    static struct Printer {
+        static void line(const char *l, void *) { std::cout << l << std::endl; }
+    } printer;
+    (void)printer;
+    w2x_ctx_set_log(ctx, &Printer::line, nullptr);
+    int rc = w2x_convert_chain(ctx, (int)steps.size(), files.data(), kinds.data(), inputPlane.data, inputPlane.width, inputPlane.height,
+                               inputPlane.stride_bytes, outputPlane.data, outputPlane.stride_bytes, blockSplitting ? 1 : 0, onStep, user);
     if (rc != W2X_OK) {
         std::cerr << w2x_last_error() << std::endl;
         return false;
