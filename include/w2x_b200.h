@@ -123,7 +123,8 @@ W2X_API int w2x_ctx_get_engine(const w2x_ctx *ctx);
 #define W2X_PRECISION_F16 2
 W2X_API int w2x_ctx_set_precision(w2x_ctx *ctx, int precision);
 W2X_API int w2x_ctx_get_precision(const w2x_ctx *ctx);
-/* Run on a caller-owned CUDA stream (cudaStream_t passed as void*); NULL = the ctx's own stream. */
+/* Run on a caller-owned CUDA stream (cudaStream_t passed as void*); NULL = the ctx's own stream.
+ * A host-buffer entry point starts its copies only after the work already queued on the context's stream. */
 W2X_API int w2x_ctx_set_stream(w2x_ctx *ctx, void *cuda_stream);
 /* Block until everything queued by this context has finished. */
 W2X_API int w2x_ctx_synchronize(w2x_ctx *ctx);

@@ -17,6 +17,7 @@
 #include <climits>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -326,6 +327,67 @@ int host_copy_bands(const w2x_ctx *ctx, int n_model, int width, int height, int 
     return nb;
 }
 
+// One group of a host-buffer call's copy pipeline: its uploads, the work that reads them (queued on the context's stream), and its
+// downloads.  Each copy is one cudaMemcpy2DAsync.
+struct HostGroup {
+    struct Copy { void *dst; size_t dst_pitch; const void *src; size_t src_pitch, row_bytes, rows; };
+    std::vector<Copy> up;
+    std::function<int()> compute;
+    std::vector<Copy> down;
+};
+
+// Runs the groups in order and returns once every download has landed.  One group runs on the context's stream alone.  With more,
+// uploads go on copy_in up to 8 groups ahead (ev_in / ev_done are 8 deep) and downloads on copy_out, so that the uploads of later
+// groups and the downloads of earlier ones overlap the compute of the current one.  The first upload waits for the work already
+// queued on the context's stream, which may still read the staging buffers.  On an error every stream is drained before returning:
+// queued copies still touch the caller's buffers and the staging.
+int run_host_groups(w2x_ctx *ctx, const std::vector<HostGroup> &groups) {
+    const int ng = (int)groups.size();
+    auto copy = [](const HostGroup::Copy &c, cudaMemcpyKind kind, cudaStream_t s) {
+        return cudaMemcpy2DAsync(c.dst, c.dst_pitch, c.src, c.src_pitch, c.row_bytes, c.rows, kind, s);
+    };
+    auto upload = [&](int gi) -> int {
+        if (groups[(size_t)gi].up.empty()) return W2X_OK;
+        for (auto &c : groups[(size_t)gi].up) CU_CHECK(copy(c, cudaMemcpyHostToDevice, ctx->copy_in));
+        CU_CHECK(cudaEventRecord(ctx->ev_in[gi % 8], ctx->copy_in));
+        return W2X_OK;
+    };
+    auto queue = [&]() -> int {
+        if (ng == 1) {
+            for (auto &c : groups[0].up) CU_CHECK(copy(c, cudaMemcpyHostToDevice, ctx->stream));
+            int rc = groups[0].compute();
+            if (rc) return rc;
+            for (auto &c : groups[0].down) CU_CHECK(copy(c, cudaMemcpyDeviceToHost, ctx->stream));
+            return W2X_OK;
+        }
+        CU_CHECK(cudaEventRecord(ctx->ev_done[0], ctx->stream));   // not recorded again before group 0's compute is queued
+        CU_CHECK(cudaStreamWaitEvent(ctx->copy_in, ctx->ev_done[0], 0));
+        int rc = W2X_OK;
+        for (int gi = 0; gi < std::min(8, ng) && !rc; gi++) rc = upload(gi);
+        for (int gi = 0; gi < ng && !rc; gi++) {
+            const HostGroup &G = groups[(size_t)gi];
+            if (!G.up.empty()) CU_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->ev_in[gi % 8], 0));
+            rc = G.compute();
+            if (rc) break;
+            CU_CHECK(cudaEventRecord(ctx->ev_done[gi % 8], ctx->stream));
+            CU_CHECK(cudaStreamWaitEvent(ctx->copy_out, ctx->ev_done[gi % 8], 0));
+            for (auto &c : G.down) CU_CHECK(copy(c, cudaMemcpyDeviceToHost, ctx->copy_out));
+            if (gi + 8 < ng) rc = upload(gi + 8);   // ev_in[gi % 8]'s previous record has been waited for above
+        }
+        return rc;
+    };
+    int rc = queue();
+    if (rc) {
+        cudaStreamSynchronize(ctx->copy_in);
+        cudaStreamSynchronize(ctx->stream);
+        cudaStreamSynchronize(ctx->copy_out);
+        return rc;
+    }
+    if (ng > 1) CU_CHECK(cudaStreamSynchronize(ctx->copy_out));
+    CU_CHECK(cudaStreamSynchronize(ctx->stream));
+    return W2X_OK;
+}
+
 int convert_device(w2x_ctx *ctx, const w2x_model *m, const float *d_in, int w, int h, size_t in_stride_bytes,
                    int rows_above, int rows_below, float *d_out, size_t out_stride_bytes, int block_splitting, bool up2x) {
     if (!m || !d_in || !d_out || w < 1 || h < 1) return fail(W2X_ERR_ARG, "w2x_convert_plane: bad argument");
@@ -611,63 +673,39 @@ int w2x_convert_band_device(w2x_ctx *ctx, const w2x_model *model, const float *d
 int w2x_convert_plane(w2x_ctx *ctx, const w2x_model *model, const float *in, int width, int height, size_t in_stride_bytes,
                       float *out, size_t out_stride_bytes, int block_splitting) {
     if (check_ctx(ctx)) return W2X_ERR_ARG;
-    if (!in || !out || width < 1 || height < 1) return fail(W2X_ERR_ARG, "w2x_convert_plane: bad argument");
+    if (!model || !in || !out || width < 1 || height < 1) return fail(W2X_ERR_ARG, "w2x_convert_plane: bad argument");
     if (in_stride_bytes < (size_t)width * 4 || out_stride_bytes < (size_t)width * 4)
         return fail(W2X_ERR_ARG, "w2x_convert_plane: row stride smaller than a row");
     DeviceGuard g(ctx->device);
-    const size_t bytes = (size_t)width * height * sizeof(float);
+    const size_t bytes = (size_t)width * height * sizeof(float), row = (size_t)width * 4;
     for (int i = 0; i < 2; i++) {
         int rc = ensure(reinterpret_cast<void **>(&ctx->io_buf[i]), &ctx->io_bytes[i], bytes);
         if (rc) return rc;
     }
+    float *din = ctx->io_buf[0], *dout = ctx->io_buf[1];
     // Large planes are cut into row bands so that the upload of band i+1 and the download of band i-1 overlap the
     // layers of band i (copy engines + compute run concurrently); each band re-reads n real rows of context from its
     // neighbours, which keeps the result bit-identical to the single-pass path.
-    const int n_model = model ? (int)model->layers.size() : 0;
-    const int nb = model ? host_copy_bands(ctx, n_model, width, height, block_splitting) : 1;
-    if (nb < 2) {
-        CU_CHECK(cudaMemcpy2DAsync(ctx->io_buf[0], (size_t)width * 4, in, in_stride_bytes, (size_t)width * 4, (size_t)height,
-                                   cudaMemcpyHostToDevice, ctx->stream));
-        int rc = convert_device(ctx, model, ctx->io_buf[0], width, height, (size_t)width * 4, 0, 0, ctx->io_buf[1],
-                                (size_t)width * 4, block_splitting);
-        if (rc) return rc;
-        CU_CHECK(cudaMemcpy2DAsync(out, out_stride_bytes, ctx->io_buf[1], (size_t)width * 4, (size_t)width * 4, (size_t)height,
-                                   cudaMemcpyDeviceToHost, ctx->stream));
-        CU_CHECK(cudaStreamSynchronize(ctx->stream));
-        return W2X_OK;
-    }
+    const int n_model = (int)model->layers.size();
+    const int nb = host_copy_bands(ctx, n_model, width, height, block_splitting);
     // the copy pipeline cuts the plane its own way: the reference's progress lines for this plane go out first
-    emit_reference_progress(ctx, width, height, n_model, block_splitting && w2x_requires_splitting(width, height));
-    LogMute mute(ctx, true);
-    std::vector<int> r0((size_t)nb + 1);
-    for (int i = 0; i <= nb; i++) r0[(size_t)i] = (int)((long)height * i / nb);
+    if (nb > 1) emit_reference_progress(ctx, width, height, n_model, block_splitting && w2x_requires_splitting(width, height));
+    LogMute mute(ctx, nb > 1);
+    std::vector<HostGroup> groups((size_t)nb);
     for (int i = 0; i < nb; i++) {
+        const int y = (int)((long)height * i / nb), y_end = (int)((long)height * (i + 1) / nb);
         // upload i carries band i plus the n rows of context band i needs from band i+1, so that band i waits for ITS upload only
-        const int y = i == 0 ? 0 : r0[(size_t)i] + n_model, y_end = i + 1 < nb ? r0[(size_t)i + 1] + n_model : height;
-        CU_CHECK(cudaMemcpy2DAsync(ctx->io_buf[0] + (size_t)y * width, (size_t)width * 4, reinterpret_cast<const char *>(in) + (size_t)y * in_stride_bytes,
-                                   in_stride_bytes, (size_t)width * 4, (size_t)(y_end - y), cudaMemcpyHostToDevice, ctx->copy_in));
-        CU_CHECK(cudaEventRecord(ctx->ev_in[i], ctx->copy_in));
+        const int u = i == 0 ? 0 : y + n_model, u_end = i + 1 < nb ? y_end + n_model : height;
+        groups[(size_t)i].up = {{din + (size_t)u * width, row, reinterpret_cast<const char *>(in) + (size_t)u * in_stride_bytes, in_stride_bytes,
+                                 row, (size_t)(u_end - u)}};
+        groups[(size_t)i].compute = [=] {
+            return convert_device(ctx, model, din + (size_t)y * width, width, y_end - y, row, i > 0 ? n_model : 0, i + 1 < nb ? n_model : 0,
+                                  dout + (size_t)y * width, row, nb > 1 ? 0 : block_splitting);
+        };
+        groups[(size_t)i].down = {{reinterpret_cast<char *>(out) + (size_t)y * out_stride_bytes, out_stride_bytes, dout + (size_t)y * width, row,
+                                   row, (size_t)(y_end - y)}};
     }
-    for (int i = 0; i < nb; i++) {
-        const int y = r0[(size_t)i], rows = r0[(size_t)i + 1] - y;
-        CU_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->ev_in[i], 0));
-        const int above = i > 0 ? n_model : 0, below = i + 1 < nb ? n_model : 0;
-        int rc = convert_device(ctx, model, ctx->io_buf[0] + (size_t)y * width, width, rows, (size_t)width * 4, above, below,
-                                ctx->io_buf[1] + (size_t)y * width, (size_t)width * 4, 0);
-        if (rc) {   // uploads / downloads already queued still touch the caller's buffers and the staging: drain them first
-            cudaStreamSynchronize(ctx->copy_in);
-            cudaStreamSynchronize(ctx->stream);
-            cudaStreamSynchronize(ctx->copy_out);
-            return rc;
-        }
-        CU_CHECK(cudaEventRecord(ctx->ev_done[i], ctx->stream));
-        CU_CHECK(cudaStreamWaitEvent(ctx->copy_out, ctx->ev_done[i], 0));
-        CU_CHECK(cudaMemcpy2DAsync(reinterpret_cast<char *>(out) + (size_t)y * out_stride_bytes, out_stride_bytes, ctx->io_buf[1] + (size_t)y * width,
-                                   (size_t)width * 4, (size_t)width * 4, (size_t)rows, cudaMemcpyDeviceToHost, ctx->copy_out));
-    }
-    CU_CHECK(cudaStreamSynchronize(ctx->copy_out));
-    CU_CHECK(cudaStreamSynchronize(ctx->stream));
-    return W2X_OK;
+    return run_host_groups(ctx, groups);
 }
 
 int w2x_filter_layer_device(w2x_ctx *ctx, const w2x_model *model, int layer, const float *d_in, float *d_out, int width,
@@ -725,26 +763,22 @@ int w2x_filter_layer(w2x_ctx *ctx, const w2x_model *model, int layer, const floa
         return fail(W2X_ERR_ARG, "w2x_filter_layer: %d output planes supplied, layer produces %d", n_out_planes, L.n_out);
     if (in_stride_bytes < (size_t)width * 4 || out_stride_bytes < (size_t)width * 4)
         return fail(W2X_ERR_ARG, "w2x_filter_layer: row stride smaller than a row");
-    DeviceGuard g(ctx->device);
-    const size_t plane = (size_t)width * height * sizeof(float);
-    int rc = ensure(reinterpret_cast<void **>(&ctx->io_buf[0]), &ctx->io_bytes[0], plane * (size_t)L.n_in);
-    if (rc) return rc;
-    rc = ensure(reinterpret_cast<void **>(&ctx->io_buf[1]), &ctx->io_bytes[1], plane * (size_t)L.n_out);
-    if (rc) return rc;
-    for (int i = 0; i < L.n_in; i++) {
+    for (int i = 0; i < L.n_in; i++)
         if (!in_planes[i]) return fail(W2X_ERR_ARG, "w2x_filter_layer: NULL input plane %d", i);
-        CU_CHECK(cudaMemcpy2DAsync(reinterpret_cast<char *>(ctx->io_buf[0]) + plane * (size_t)i, (size_t)width * 4, in_planes[i],
-                                   in_stride_bytes, (size_t)width * 4, (size_t)height, cudaMemcpyHostToDevice, ctx->stream));
-    }
-    rc = w2x_filter_layer_device(ctx, model, layer, ctx->io_buf[0], ctx->io_buf[1], width, height);
-    if (rc) return rc;
-    for (int i = 0; i < L.n_out; i++) {
+    for (int i = 0; i < L.n_out; i++)
         if (!out_planes[i]) return fail(W2X_ERR_ARG, "w2x_filter_layer: NULL output plane %d", i);
-        CU_CHECK(cudaMemcpy2DAsync(out_planes[i], out_stride_bytes, reinterpret_cast<char *>(ctx->io_buf[1]) + plane * (size_t)i,
-                                   (size_t)width * 4, (size_t)width * 4, (size_t)height, cudaMemcpyDeviceToHost, ctx->stream));
-    }
-    CU_CHECK(cudaStreamSynchronize(ctx->stream));
-    return W2X_OK;
+    DeviceGuard g(ctx->device);
+    const size_t plane = (size_t)width * height, row = (size_t)width * 4;
+    int rc = ensure(reinterpret_cast<void **>(&ctx->io_buf[0]), &ctx->io_bytes[0], plane * sizeof(float) * (size_t)L.n_in);
+    if (rc) return rc;
+    rc = ensure(reinterpret_cast<void **>(&ctx->io_buf[1]), &ctx->io_bytes[1], plane * sizeof(float) * (size_t)L.n_out);
+    if (rc) return rc;
+    float *din = ctx->io_buf[0], *dout = ctx->io_buf[1];
+    std::vector<HostGroup> groups(1);
+    for (int i = 0; i < L.n_in; i++) groups[0].up.push_back({din + plane * (size_t)i, row, in_planes[i], in_stride_bytes, row, (size_t)height});
+    groups[0].compute = [=] { return w2x_filter_layer_device(ctx, model, layer, din, dout, width, height); };
+    for (int i = 0; i < L.n_out; i++) groups[0].down.push_back({out_planes[i], out_stride_bytes, dout + plane * (size_t)i, row, row, (size_t)height});
+    return run_host_groups(ctx, groups);
 }
 
 // Page-locked host memory for planes: copies from / to it are truly asynchronous and run at the link rate (the reference's
@@ -965,13 +999,9 @@ void emit_planes_progress(w2x_ctx *ctx, const w2x_model *m, int n_planes, const 
     const int n = (int)m->layers.size();
     for (int i = 0; i < n_planes; i++) {
         int passes = 1;
-        if (frame[i] < 0) {
-            const int h = heights[i];
-            const int nb = std::min(8, ctx->host_bands > 0 ? ctx->host_bands : std::min(4, h / 512));
-            if (!(host && nb >= 2 && h / nb >= 2 * n)) {
-                const int band = scratch_band_rows(ctx, m, widths[i], h);
-                passes = (h + band - 1) / band;
-            }
+        if (frame[i] < 0 && !(host && host_copy_bands(ctx, n, widths[i], heights[i], 0) > 1)) {
+            const int band = scratch_band_rows(ctx, m, widths[i], heights[i]);
+            passes = (heights[i] + band - 1) / band;
         }
         for (int p = 0; p < passes; p++)
             for (int k = 1; k <= n; k++) logf(ctx, "Iteration #%d...", k);
@@ -1029,11 +1059,10 @@ int convert_planes_dev(w2x_ctx *ctx, const w2x_model *m, int n_planes, const flo
     return rc;
 }
 
-// Host planes, packed: dense device staging (plane i at the same offset in io_buf[0] and io_buf[1]); the uploads of later frames
-// and the downloads of earlier ones overlap the layers of the current one, as in w2x_convert_tiles.  A group is a frame or one
-// plane too large to pack.  Up to 8 uploads are queued ahead (ev_in / ev_done are 8 deep).
-int planes_host_pipeline(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int n_planes, const float *const *in, const int *widths,
-                         const int *heights, const size_t *in_strides, float *const *out, const size_t *out_strides) {
+// Host planes, packed: dense device staging (plane i at the same offset in io_buf[0] and io_buf[1]).  A group of the copy pipeline
+// is a frame or one plane too large to pack.
+int planes_host(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int n_planes, const float *const *in, const int *widths,
+                const int *heights, const size_t *in_strides, float *const *out, const size_t *out_strides) {
     PlanesPlan p;
     plan_for(ctx, m, n_planes, widths, heights, &p);
     emit_planes_progress(ctx, m, n_planes, widths, heights, p.frame.data(), true);
@@ -1044,93 +1073,87 @@ int planes_host_pipeline(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int n_p
         int rc = ensure(reinterpret_cast<void **>(&ctx->io_buf[i]), &ctx->io_bytes[i], off.back() * sizeof(float));
         if (rc) return rc;
     }
+    float *din = ctx->io_buf[0], *dout = ctx->io_buf[1];
     std::vector<FramePlan> frames = frames_for(p);
-    std::vector<std::vector<int>> groups(frames.size());
+    std::vector<HostGroup> groups(frames.size());
+    auto add_copies = [&](HostGroup &G, int i) {
+        const size_t row = (size_t)widths[i] * 4;
+        G.up.push_back({din + off[(size_t)i], row, in[i], in_strides[i], row, (size_t)heights[i]});
+        G.down.push_back({out[i], out_strides[i], dout + off[(size_t)i], row, row, (size_t)heights[i]});
+    };
     for (int i = 0; i < n_planes; i++) {
         const int f = p.frame[(size_t)i];
         if (f < 0) continue;
-        frames[(size_t)f].rect.push_back(tc::PlaneRect{ctx->io_buf[0] + off[(size_t)i], ctx->io_buf[1] + off[(size_t)i], widths[i], widths[i],
-                                                       widths[i], heights[i], p.x0[(size_t)i], p.y0[(size_t)i], 0});
-        groups[(size_t)f].push_back(i);
+        frames[(size_t)f].rect.push_back(tc::PlaneRect{din + off[(size_t)i], dout + off[(size_t)i], widths[i], widths[i], widths[i], heights[i],
+                                                       p.x0[(size_t)i], p.y0[(size_t)i], 0});
+        add_copies(groups[(size_t)f], i);
     }
-    for (int i = 0; i < n_planes; i++)
-        if (p.frame[(size_t)i] < 0) groups.push_back({i});
     std::vector<FrameDev> fd;
-    int rc = 0;
     if (!frames.empty()) {
-        rc = upload_frames(ctx, frames, &fd);
+        int rc = upload_frames(ctx, frames, &fd);
         if (!rc) rc = reserve_frames(ctx, m, fd);
         if (rc) return rc;
     }
-    const int n_groups = (int)groups.size();
-    auto upload = [&](int gi) -> int {
-        for (int i : groups[(size_t)gi])
-            CU_CHECK(cudaMemcpy2DAsync(ctx->io_buf[0] + off[(size_t)i], (size_t)widths[i] * 4, in[i], in_strides[i], (size_t)widths[i] * 4,
-                                       (size_t)heights[i], cudaMemcpyHostToDevice, ctx->copy_in));
-        CU_CHECK(cudaEventRecord(ctx->ev_in[gi % 8], ctx->copy_in));
-        return W2X_OK;
-    };
-    for (int gi = 0; gi < std::min(8, n_groups) && !rc; gi++) rc = upload(gi);
-    for (int gi = 0; gi < n_groups && !rc; gi++) {
-        CU_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->ev_in[gi % 8], 0));
-        if (gi < (int)fd.size()) {
-            rc = run_packed_frame(ctx, m, dm, fd[(size_t)gi]);
-        } else {
-            const int i = groups[(size_t)gi][0];
-            rc = convert_device(ctx, m, ctx->io_buf[0] + off[(size_t)i], widths[i], heights[i], (size_t)widths[i] * 4, 0, 0,
-                                ctx->io_buf[1] + off[(size_t)i], (size_t)widths[i] * 4, 0);
-        }
-        if (rc) break;
-        if (gi + 1 == (int)fd.size()) {   // the last kernel reading the frame tables is queued
-            CU_CHECK(cudaEventRecord(ctx->plan_ev, ctx->stream));
+    for (size_t f = 0; f < fd.size(); f++)
+        groups[f].compute = [&, f]() -> int {
+            int rc = run_packed_frame(ctx, m, dm, fd[f]);
+            if (rc || f + 1 < fd.size()) return rc;
+            CU_CHECK(cudaEventRecord(ctx->plan_ev, ctx->stream));   // the last kernel reading the frame tables is queued
             ctx->plan_ev_live = true;
-        }
-        CU_CHECK(cudaEventRecord(ctx->ev_done[gi % 8], ctx->stream));
-        CU_CHECK(cudaStreamWaitEvent(ctx->copy_out, ctx->ev_done[gi % 8], 0));
-        for (int i : groups[(size_t)gi])
-            CU_CHECK(cudaMemcpy2DAsync(out[i], out_strides[i], ctx->io_buf[1] + off[(size_t)i], (size_t)widths[i] * 4, (size_t)widths[i] * 4,
-                                       (size_t)heights[i], cudaMemcpyDeviceToHost, ctx->copy_out));
-        if (gi + 8 < n_groups) rc = upload(gi + 8);   // its event's previous record has been waited for above
+            return W2X_OK;
+        };
+    for (int i = 0; i < n_planes; i++) {
+        if (p.frame[(size_t)i] >= 0) continue;
+        groups.emplace_back();
+        add_copies(groups.back(), i);
+        groups.back().compute = [&, i] {
+            return convert_device(ctx, m, din + off[(size_t)i], widths[i], heights[i], (size_t)widths[i] * 4, 0, 0, dout + off[(size_t)i],
+                                  (size_t)widths[i] * 4, 0);
+        };
     }
-    if (rc) return rc;
-    CU_CHECK(cudaStreamSynchronize(ctx->copy_out));
-    CU_CHECK(cudaStreamSynchronize(ctx->stream));
-    return W2X_OK;
+    return run_host_groups(ctx, groups);
 }
 }  // namespace
 
 namespace w2x {
 namespace eng {
-// phase 1: uploads + the batched pass (results stay in the context's staging buffer); phase 2: downloads.  Split so that a
-// multi-GPU driver can queue phase 1 everywhere before a download into pageable memory blocks its thread.
-int tiles_enqueue_compute(w2x_ctx *ctx, const w2x_model *model, const float *const *in_tiles, int n_tiles, int width, int height, size_t in_stride_bytes) {
+// The host tiles of w2x_convert_tiles*, all checked before anything is queued.
+int check_tiles(w2x_ctx *ctx, const float *const *in_tiles, float *const *out_tiles, int n_tiles, int width, int height, size_t in_stride_bytes,
+                size_t out_stride_bytes) {
     if (check_ctx(ctx)) return W2X_ERR_ARG;
-    if (!in_tiles || n_tiles < 1 || width < 1 || height < 1) return fail(W2X_ERR_ARG, "w2x_convert_tiles: bad argument");
-    if (in_stride_bytes < (size_t)width * 4) return fail(W2X_ERR_ARG, "w2x_convert_tiles: row stride smaller than a row");
+    if (!in_tiles || !out_tiles || n_tiles < 1 || width < 1 || height < 1) return fail(W2X_ERR_ARG, "w2x_convert_tiles: bad argument");
+    if (in_stride_bytes < (size_t)width * 4 || out_stride_bytes < (size_t)width * 4)
+        return fail(W2X_ERR_ARG, "w2x_convert_tiles: row stride smaller than a row");
+    for (int t = 0; t < n_tiles; t++)
+        if (!in_tiles[t] || !out_tiles[t]) return fail(W2X_ERR_ARG, "w2x_convert_tiles: NULL tile %d", t);
+    return W2X_OK;
+}
+
+// phase 1: uploads + the batched pass (results stay in the context's staging buffer); phase 2: downloads.  Split so that a
+// multi-GPU driver can queue phase 1 everywhere before a download into pageable memory blocks its thread.  Phase 1 checks the
+// tiles of both phases.
+int tiles_enqueue_compute(w2x_ctx *ctx, const w2x_model *model, const float *const *in_tiles, float *const *out_tiles, int n_tiles, int width,
+                          int height, size_t in_stride_bytes, size_t out_stride_bytes) {
+    int rc = check_tiles(ctx, in_tiles, out_tiles, n_tiles, width, height, in_stride_bytes, out_stride_bytes);
+    if (rc) return rc;
     DeviceGuard g(ctx->device);
     const size_t tile_bytes = (size_t)width * height * sizeof(float);
     for (int i = 0; i < 2; i++) {
-        int rc = ensure(reinterpret_cast<void **>(&ctx->io_buf[i]), &ctx->io_bytes[i], tile_bytes * (size_t)n_tiles);
+        rc = ensure(reinterpret_cast<void **>(&ctx->io_buf[i]), &ctx->io_bytes[i], tile_bytes * (size_t)n_tiles);
         if (rc) return rc;
     }
-    for (int t = 0; t < n_tiles; t++) {
-        if (!in_tiles[t]) return fail(W2X_ERR_ARG, "w2x_convert_tiles: NULL tile %d", t);
+    for (int t = 0; t < n_tiles; t++)
         CU_CHECK(cudaMemcpy2DAsync(reinterpret_cast<char *>(ctx->io_buf[0]) + tile_bytes * (size_t)t, (size_t)width * 4, in_tiles[t], in_stride_bytes,
                                    (size_t)width * 4, (size_t)height, cudaMemcpyHostToDevice, ctx->stream));
-    }
     return convert_tiles_dev(ctx, model, ctx->io_buf[0], ctx->io_buf[1], n_tiles, width, height);
 }
 
 int tiles_enqueue_download(w2x_ctx *ctx, float *const *out_tiles, int n_tiles, int width, int height, size_t out_stride_bytes) {
-    if (check_ctx(ctx)) return W2X_ERR_ARG;
-    if (!out_tiles || out_stride_bytes < (size_t)width * 4) return fail(W2X_ERR_ARG, "w2x_convert_tiles: bad output argument");
     DeviceGuard g(ctx->device);
     const size_t tile_bytes = (size_t)width * height * sizeof(float);
-    for (int t = 0; t < n_tiles; t++) {
-        if (!out_tiles[t]) return fail(W2X_ERR_ARG, "w2x_convert_tiles: NULL tile %d", t);
+    for (int t = 0; t < n_tiles; t++)
         CU_CHECK(cudaMemcpy2DAsync(out_tiles[t], out_stride_bytes, reinterpret_cast<char *>(ctx->io_buf[1]) + tile_bytes * (size_t)t, (size_t)width * 4,
                                    (size_t)width * 4, (size_t)height, cudaMemcpyDeviceToHost, ctx->stream));
-    }
     return W2X_OK;
 }
 }  // namespace eng
@@ -1145,60 +1168,38 @@ int w2x_convert_tiles_device(w2x_ctx *ctx, const w2x_model *model, const float *
 
 int w2x_convert_tiles_async(w2x_ctx *ctx, const w2x_model *model, const float *const *in_tiles, float *const *out_tiles, int n_tiles,
                             int width, int height, size_t in_stride_bytes, size_t out_stride_bytes) {
-    int rc = tiles_enqueue_compute(ctx, model, in_tiles, n_tiles, width, height, in_stride_bytes);
+    int rc = tiles_enqueue_compute(ctx, model, in_tiles, out_tiles, n_tiles, width, height, in_stride_bytes, out_stride_bytes);
     if (rc) return rc;
     return tiles_enqueue_download(ctx, out_tiles, n_tiles, width, height, out_stride_bytes);
 }
 
 int w2x_convert_tiles(w2x_ctx *ctx, const w2x_model *model, const float *const *in_tiles, float *const *out_tiles, int n_tiles,
                       int width, int height, size_t in_stride_bytes, size_t out_stride_bytes) {
-    if (check_ctx(ctx)) return W2X_ERR_ARG;
+    int rc = check_tiles(ctx, in_tiles, out_tiles, n_tiles, width, height, in_stride_bytes, out_stride_bytes);
+    if (rc) return rc;
+    DeviceGuard g(ctx->device);
+    const size_t tile_px = (size_t)width * height, row = (size_t)width * 4;
+    for (int i = 0; i < 2; i++) {
+        rc = ensure(reinterpret_cast<void **>(&ctx->io_buf[i]), &ctx->io_bytes[i], tile_px * sizeof(float) * (size_t)n_tiles);
+        if (rc) return rc;
+    }
+    float *din = ctx->io_buf[0], *dout = ctx->io_buf[1];
     // Larger batches run as up to four groups: the uploads of group g+1 and the downloads of group g-1 overlap the layers of
     // group g (copy engines + compute), as the row bands of w2x_convert_plane do.  Tiles are independent, so the grouping
     // does not change a bit of any of them.
-    const int groups = n_tiles >= 8 ? std::min(4, n_tiles / 4) : 1;
-    if (groups < 2) {
-        int rc = w2x_convert_tiles_async(ctx, model, in_tiles, out_tiles, n_tiles, width, height, in_stride_bytes, out_stride_bytes);
-        int rc2 = w2x_ctx_synchronize(ctx);
-        return rc ? rc : rc2;
-    }
-    if (!in_tiles || !out_tiles || width < 1 || height < 1) return fail(W2X_ERR_ARG, "w2x_convert_tiles: bad argument");
-    if (in_stride_bytes < (size_t)width * 4 || out_stride_bytes < (size_t)width * 4)
-        return fail(W2X_ERR_ARG, "w2x_convert_tiles: row stride smaller than a row");
-    for (int t = 0; t < n_tiles; t++)
-        if (!in_tiles[t] || !out_tiles[t]) return fail(W2X_ERR_ARG, "w2x_convert_tiles: NULL tile %d", t);
-    DeviceGuard g(ctx->device);
-    const size_t tile_px = (size_t)width * height, tile_bytes = tile_px * sizeof(float);
-    for (int i = 0; i < 2; i++) {
-        int rc = ensure(reinterpret_cast<void **>(&ctx->io_buf[i]), &ctx->io_bytes[i], tile_bytes * (size_t)n_tiles);
-        if (rc) return rc;
-    }
-    auto first = [&](int gi) { return (int)((long)n_tiles * gi / groups); };
-    for (int gi = 0; gi < groups; gi++) {
-        for (int t = first(gi); t < first(gi + 1); t++)
-            CU_CHECK(cudaMemcpy2DAsync(ctx->io_buf[0] + tile_px * (size_t)t, (size_t)width * 4, in_tiles[t], in_stride_bytes, (size_t)width * 4,
-                                       (size_t)height, cudaMemcpyHostToDevice, ctx->copy_in));
-        CU_CHECK(cudaEventRecord(ctx->ev_in[gi], ctx->copy_in));
-    }
-    for (int gi = 0; gi < groups; gi++) {
-        const int t0 = first(gi), nt = first(gi + 1) - t0;
-        CU_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->ev_in[gi], 0));
-        int rc = convert_tiles_dev(ctx, model, ctx->io_buf[0] + tile_px * (size_t)t0, ctx->io_buf[1] + tile_px * (size_t)t0, nt, width, height);
-        if (rc) {   // copies already queued still touch the caller's buffers and the staging: drain them first
-            cudaStreamSynchronize(ctx->copy_in);
-            cudaStreamSynchronize(ctx->stream);
-            cudaStreamSynchronize(ctx->copy_out);
-            return rc;
+    const int ng = n_tiles >= 8 ? std::min(4, n_tiles / 4) : 1;
+    std::vector<HostGroup> groups((size_t)ng);
+    for (int gi = 0; gi < ng; gi++) {
+        const int t0 = (int)((long)n_tiles * gi / ng), t1 = (int)((long)n_tiles * (gi + 1) / ng);
+        for (int t = t0; t < t1; t++) {
+            groups[(size_t)gi].up.push_back({din + tile_px * (size_t)t, row, in_tiles[t], in_stride_bytes, row, (size_t)height});
+            groups[(size_t)gi].down.push_back({out_tiles[t], out_stride_bytes, dout + tile_px * (size_t)t, row, row, (size_t)height});
         }
-        CU_CHECK(cudaEventRecord(ctx->ev_done[gi], ctx->stream));
-        CU_CHECK(cudaStreamWaitEvent(ctx->copy_out, ctx->ev_done[gi], 0));
-        for (int t = t0; t < t0 + nt; t++)
-            CU_CHECK(cudaMemcpy2DAsync(out_tiles[t], out_stride_bytes, ctx->io_buf[1] + tile_px * (size_t)t, (size_t)width * 4, (size_t)width * 4,
-                                       (size_t)height, cudaMemcpyDeviceToHost, ctx->copy_out));
+        groups[(size_t)gi].compute = [=] {
+            return convert_tiles_dev(ctx, model, din + tile_px * (size_t)t0, dout + tile_px * (size_t)t0, t1 - t0, width, height);
+        };
     }
-    CU_CHECK(cudaStreamSynchronize(ctx->copy_out));
-    CU_CHECK(cudaStreamSynchronize(ctx->stream));
-    return W2X_OK;
+    return run_host_groups(ctx, groups);
 }
 
 int w2x_convert_planes_device(w2x_ctx *ctx, const w2x_model *model, int n_planes, const float *const *d_in, const int *widths,
@@ -1223,13 +1224,7 @@ int w2x_convert_planes(w2x_ctx *ctx, const w2x_model *model, int n_planes, const
             rc = w2x_convert_plane(ctx, model, in[i], widths[i], heights[i], in_strides[i], out[i], out_strides[i], 0);
         return rc;
     }
-    rc = planes_host_pipeline(ctx, model, dm, n_planes, in, widths, heights, in_strides, out, out_strides);
-    if (rc) {   // copies already queued still touch the caller's buffers and the staging: drain them first
-        cudaStreamSynchronize(ctx->copy_in);
-        cudaStreamSynchronize(ctx->stream);
-        cudaStreamSynchronize(ctx->copy_out);
-    }
-    return rc;
+    return planes_host(ctx, model, dm, n_planes, in, widths, heights, in_strides, out, out_strides);
 }
 
 }  // extern "C"
@@ -1333,9 +1328,9 @@ int chain_device_steps(w2x_ctx *ctx, const std::vector<ChainStep> &steps, int n_
     return W2X_OK;
 }
 
-// Host planes: one upload, the steps on the device, and the last step cut into the row bands of w2x_convert_plane's copy
-// pipeline when it would cut that plane, so that the download of band i overlaps the layers of band i + 1.  An upscaling step's
-// bands start on even 2x rows (the source row of a band's first row is then whole).
+// Host planes: one upload and the first n - 1 steps on the context's stream, then the last step as groups of the copy pipeline: the
+// row bands of w2x_convert_plane's when it would cut that plane, so that the download of band i overlaps the layers of band i + 1,
+// else one.  An upscaling step's bands start on even 2x rows (the source row of a band's first row is then whole).
 int chain_host(w2x_ctx *ctx, const std::vector<ChainStep> &steps, const float *in, int width, int height, size_t in_stride_bytes, float *out,
                size_t out_stride_bytes, int block_splitting, w2x_step_fn on_step, void *user) {
     const ChainStep &L = steps.back();
@@ -1344,41 +1339,33 @@ int chain_host(w2x_ctx *ctx, const std::vector<ChainStep> &steps, const float *i
     if (!rc) rc = ensure(reinterpret_cast<void **>(&ctx->io_buf[1]), &ctx->io_bytes[1], (size_t)L.w * L.h * sizeof(float));
     if (!rc) rc = reserve_chain(ctx, steps);
     if (rc) return rc;
-    CU_CHECK(cudaMemcpy2DAsync(ctx->io_buf[0], (size_t)width * 4, in, in_stride_bytes, (size_t)width * 4, (size_t)height, cudaMemcpyHostToDevice,
-                               ctx->stream));
     const size_t in_dense = (size_t)width * 4, stage_stride = (size_t)L.w * 4;
-    const int nb = host_copy_bands(ctx, n, L.w, L.h, block_splitting);
-    if (nb < 2) {
-        rc = chain_device_steps(ctx, steps, n_steps, ctx->io_buf[0], in_dense, ctx->io_buf[1], stage_stride, block_splitting, on_step, user, true);
-        if (rc) return rc;
-        CU_CHECK(cudaMemcpy2DAsync(out, out_stride_bytes, ctx->io_buf[1], stage_stride, stage_stride, (size_t)L.h, cudaMemcpyDeviceToHost,
-                                   ctx->stream));
-        CU_CHECK(cudaStreamSynchronize(ctx->stream));
-        return W2X_OK;
-    }
+    CU_CHECK(cudaMemcpy2DAsync(ctx->io_buf[0], in_dense, in, in_stride_bytes, in_dense, (size_t)height, cudaMemcpyHostToDevice, ctx->stream));
     rc = chain_device_steps(ctx, steps, n_steps - 1, ctx->io_buf[0], in_dense, nullptr, 0, block_splitting, on_step, user, true);
-    if (rc) return rc;
+    if (rc) {   // the upload may still read the caller's plane
+        cudaStreamSynchronize(ctx->stream);
+        return rc;
+    }
     const float *src = n_steps == 1 ? ctx->io_buf[0] : ctx->chain_buf[(n_steps - 2) & 1];
     const size_t src_stride = n_steps == 1 ? in_dense : (size_t)steps[(size_t)n_steps - 2].w * 4;
+    float *dout = ctx->io_buf[1];
     if (on_step) on_step(n_steps - 1, user);
-    emit_reference_progress(ctx, L.w, L.h, n, block_splitting && w2x_requires_splitting(L.w, L.h));
-    LogMute mute(ctx, true);
-    std::vector<int> r0((size_t)nb + 1);
-    for (int i = 0; i <= nb; i++) r0[(size_t)i] = (int)((long)L.h * i / nb) & (L.up ? ~1 : ~0);
+    const int nb = host_copy_bands(ctx, n, L.w, L.h, block_splitting);
+    if (nb > 1) emit_reference_progress(ctx, L.w, L.h, n, block_splitting && w2x_requires_splitting(L.w, L.h));
+    LogMute mute(ctx, nb > 1);
+    auto band_y = [&](int i) { return (int)((long)L.h * i / nb) & (L.up ? ~1 : ~0); };
+    std::vector<HostGroup> groups((size_t)nb);
     for (int i = 0; i < nb; i++) {
-        const int y = r0[(size_t)i], rows = r0[(size_t)i + 1] - y;
+        const int y = band_y(i), rows = band_y(i + 1) - y;
         const float *band_src = reinterpret_cast<const float *>(reinterpret_cast<const char *>(src) + (size_t)(L.up ? y / 2 : y) * src_stride);
-        rc = convert_device(ctx, L.m, band_src, L.w, rows, src_stride, i > 0 ? n : 0, i + 1 < nb ? n : 0, ctx->io_buf[1] + (size_t)y * L.w,
-                            stage_stride, 0, L.up);
-        if (rc) return rc;
-        CU_CHECK(cudaEventRecord(ctx->ev_done[i], ctx->stream));
-        CU_CHECK(cudaStreamWaitEvent(ctx->copy_out, ctx->ev_done[i], 0));
-        CU_CHECK(cudaMemcpy2DAsync(reinterpret_cast<char *>(out) + (size_t)y * out_stride_bytes, out_stride_bytes, ctx->io_buf[1] + (size_t)y * L.w,
-                                   stage_stride, stage_stride, (size_t)rows, cudaMemcpyDeviceToHost, ctx->copy_out));
+        groups[(size_t)i].compute = [=] {
+            return convert_device(ctx, L.m, band_src, L.w, rows, src_stride, i > 0 ? n : 0, i + 1 < nb ? n : 0, dout + (size_t)y * L.w, stage_stride,
+                                  nb > 1 ? 0 : block_splitting, L.up);
+        };
+        groups[(size_t)i].down = {{reinterpret_cast<char *>(out) + (size_t)y * out_stride_bytes, out_stride_bytes, dout + (size_t)y * L.w,
+                                   stage_stride, stage_stride, (size_t)rows}};
     }
-    CU_CHECK(cudaStreamSynchronize(ctx->copy_out));
-    CU_CHECK(cudaStreamSynchronize(ctx->stream));
-    return W2X_OK;
+    return run_host_groups(ctx, groups);
 }
 }  // namespace
 
@@ -1406,12 +1393,7 @@ int w2x_convert_chain(w2x_ctx *ctx, int n_steps, const w2x_model *const *models,
     if (rc) return rc;
     DeviceGuard g(ctx->device);
     NvtxRange nvtx("w2x convert chain");
-    rc = chain_host(ctx, steps, in, width, height, in_stride_bytes, out, out_stride_bytes, block_splitting, on_step, user);
-    if (rc) {   // copies already queued still touch the caller's buffers and the staging: drain them first
-        cudaStreamSynchronize(ctx->stream);
-        cudaStreamSynchronize(ctx->copy_out);
-    }
-    return rc;
+    return chain_host(ctx, steps, in, width, height, in_stride_bytes, out, out_stride_bytes, block_splitting, on_step, user);
 }
 
 }  // extern "C"

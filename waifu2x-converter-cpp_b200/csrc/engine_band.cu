@@ -704,7 +704,7 @@ int w2x_multi_convert_tiles(w2x_multi *m, const w2x_model *model, const float *c
     // queue every GPU's batch without waiting, then wait for all of them
     int rc = W2X_OK;
     for (int i = 0; i < nd && rc == W2X_OK; i++)
-        rc = tiles_enqueue_compute(m->ctx[(size_t)i], model, tin[(size_t)i].data(), (int)tin[(size_t)i].size(), width, height, in_stride_bytes);
+        rc = tiles_enqueue_compute(m->ctx[(size_t)i], model, tin[(size_t)i].data(), tout[(size_t)i].data(), (int)tin[(size_t)i].size(), width, height, in_stride_bytes, out_stride_bytes);
     for (int i = 0; i < nd && rc == W2X_OK; i++)
         rc = tiles_enqueue_download(m->ctx[(size_t)i], tout[(size_t)i].data(), (int)tout[(size_t)i].size(), width, height, out_stride_bytes);
     for (int i = 0; i < nd; i++) {

@@ -66,7 +66,7 @@ struct w2x_ctx {
     float *chain_buf[2] = {nullptr, nullptr};   // the planes between the steps of w2x_convert_chain*
     size_t chain_bytes[2] = {0, 0};
     bool tc_ready = false;
-    cudaStream_t copy_in = nullptr, copy_out = nullptr;   // host<->device copies of w2x_convert_plane overlap the compute stream
+    cudaStream_t copy_in = nullptr, copy_out = nullptr;   // host<->device copies of run_host_groups overlap the compute stream
     cudaEvent_t ev_in[8] = {}, ev_done[8] = {};
     int host_bands = 0;                                   // 0 = automatic (up to 4 bands of >= 512 rows), 1 = no pipelining
     void *plan_buf = nullptr;                             // device tables of the packed frames (w2x_convert_planes, w2x_convert_tiles)
@@ -146,7 +146,7 @@ int launch_layer_tc(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int li, cons
 int convert_device(w2x_ctx *ctx, const w2x_model *m, const float *d_in, int w, int h, size_t in_stride_bytes, int rows_above,
                    int rows_below, float *d_out, size_t out_stride_bytes, int block_splitting, bool up2x = false);
 
-int tiles_enqueue_compute(w2x_ctx *ctx, const w2x_model *model, const float *const *in_tiles, int n_tiles, int width, int height, size_t in_stride_bytes);
+int tiles_enqueue_compute(w2x_ctx *ctx, const w2x_model *model, const float *const *in_tiles, float *const *out_tiles, int n_tiles, int width, int height, size_t in_stride_bytes, size_t out_stride_bytes);
 int tiles_enqueue_download(w2x_ctx *ctx, float *const *out_tiles, int n_tiles, int width, int height, size_t out_stride_bytes);
 
 struct NvtxRange {    // a named range on the calling thread's timeline (nsys / ncu --nvtx), e.g. "w2x L3", "w2x halo exchange"
