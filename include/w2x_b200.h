@@ -130,6 +130,7 @@ W2X_API int w2x_ctx_set_stream(w2x_ctx *ctx, void *cuda_stream);
 W2X_API int w2x_ctx_synchronize(w2x_ctx *ctx);
 /* Progress lines exactly as the reference prints them to std::cout
  * ("Iteration #k..." src/convertRoutine.cpp:67, "start process block (c,r) ..." :133-134).
+ * A call prints its lines before it queues the work they describe, and a call rejected by its argument checks prints none.
  * NULL disables (default). */
 typedef void (*w2x_log_fn)(const char *line, void *user);
 W2X_API int w2x_ctx_set_log(w2x_ctx *ctx, w2x_log_fn fn, void *user);

@@ -106,38 +106,30 @@ void note_kernel(w2x_ctx *ctx, int layer, const char *name) {
 }
 
 void logf(w2x_ctx *ctx, const char *fmt, int a, int b = 0) {
-    if (!ctx->log || ctx->log_muted) return;
     char line[128];
     snprintf(line, sizeof line, fmt, a, b);
     ctx->log(line, ctx->log_user);
 }
 
+// The reference's blocks of a w x h plane for an n-layer model, 8 ints each (block_table); empty when the block size is too small.
+std::vector<int> blocks_of(int w, int h, int n) {
+    const Config &cfg = config();
+    const int nb = block_table(w, h, cfg.block_w, cfg.block_h, n, nullptr, 0, nullptr, nullptr);
+    std::vector<int> tab((size_t)std::max(nb, 0) * 8);
+    if (nb > 0) block_table(w, h, cfg.block_w, cfg.block_h, n, tab.data(), nb, nullptr, nullptr);
+    return tab;
+}
+
 // The progress lines the reference prints for one convertWithModels call (src/convertRoutine.cpp:67,133-134): per block
 // "start process block (c,r) ..." + one "Iteration #k..." per layer when the plane is split, else just the iterations.
-// The fused walk and the copy pipeline process the plane in other units, so they emit the reference's sequence up front.
 void emit_reference_progress(w2x_ctx *ctx, int w, int h, int n_layers, bool split) {
     if (!ctx->log) return;
-    int nb = 1;
-    std::vector<int> tab;
-    if (split) {
-        const Config &cfg = config();
-        nb = block_table(w, h, cfg.block_w, cfg.block_h, n_layers, nullptr, 0, nullptr, nullptr);
-        if (nb < 1) return;
-        tab.resize((size_t)nb * 8);
-        block_table(w, h, cfg.block_w, cfg.block_h, n_layers, tab.data(), nb, nullptr, nullptr);
-    }
-    for (int i = 0; i < nb; i++) {
-        if (split) logf(ctx, "start process block (%d,%d) ...", tab[(size_t)i * 8 + 1], tab[(size_t)i * 8]);
+    const std::vector<int> tab = split ? blocks_of(w, h, n_layers) : std::vector<int>(8);   // unsplit: one block without a line
+    for (size_t i = 0; i < tab.size(); i += 8) {
+        if (split) logf(ctx, "start process block (%d,%d) ...", tab[i + 1], tab[i]);
         for (int k = 1; k <= n_layers; k++) logf(ctx, "Iteration #%d...", k);
     }
 }
-
-struct LogMute {   // silences the per-launch lines while a caller that already emitted the reference's sequence runs the layers
-    w2x_ctx *ctx;
-    bool prev;
-    explicit LogMute(w2x_ctx *c, bool on) : ctx(c), prev(c->log_muted) { if (on) c->log_muted = true; }
-    ~LogMute() { ctx->log_muted = prev; }
-};
 
 int pick_engine(w2x_ctx *ctx, const w2x_model *m) {
     int e = ctx->engine;
@@ -202,7 +194,6 @@ int run_basic(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int engine, const 
         ctx->launches++;
         for (int li = 0; li < n; li++) {
             const Layer &L = m->layers[(size_t)li];
-            logf(ctx, "Iteration #%d...", li + 1);                                 // src/convertRoutine.cpp:67
             {
                 LayerTimer t(ctx, li);
                 CU_CHECK(launch_conv3x3_fp32(cur, nxt, dm->w[(size_t)li], dm->b[(size_t)li], L.n_in, L.n_out, pw, ph,
@@ -228,7 +219,6 @@ int run_basic(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int engine, const 
     __half *cur = static_cast<__half *>(ctx->buf[0]), *nxt = static_cast<__half *>(ctx->buf[1]);
     {
         const Layer &L = m->layers[0];
-        logf(ctx, "Iteration #%d...", 1);
         LayerTimer t(ctx, 0);
         const tc::FirstSource padded{src, src_stride, pw, ph, 0, 0, 0, 0};
         CU_CHECK(tc::launch_first(direct ? *direct : padded, pw, ph, L.w.data(), dm->b_host[0].data(), L.n_out, cur, ctx->stream, f8));
@@ -237,14 +227,12 @@ int run_basic(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int engine, const 
     }
     const bool fuse = ctx->fuse_last && n >= 3 && !dm->last_w_t.empty();
     for (int li = 1; li + 1 < n; li++) {
-        logf(ctx, "Iteration #%d...", li + 1);
         rc = launch_layer_tc(ctx, m, dm, li, cur, nxt, pw, ph, fuse && li == n - 2, true);
         if (rc) return rc;
         std::swap(cur, nxt);
     }
     {
         const Layer &L = m->layers[(size_t)n - 1];
-        logf(ctx, "Iteration #%d...", n);
         LayerTimer t(ctx, n - 1);
         if (fuse) {
             if (packed)
@@ -317,13 +305,17 @@ int check_ctx(w2x_ctx *ctx) {
     return W2X_OK;
 }
 
+// Whether a plane conversion walks the reference's blocks literally (convertWithModelsBlockSplit, src/convertRoutine.cpp:114-165).
+bool literal_walk(const w2x_ctx *ctx, int w, int h, int block_splitting) {
+    return block_splitting && ctx->walk == W2X_WALK_BLOCKS && w2x_requires_splitting(w, h);
+}
+
 // Row bands of w2x_convert_plane's host copy pipeline for a plane of width x height (1 = no pipeline: one upload, one pass,
 // one download).  The literal block walk keeps its own order, and a band needs 2n rows of its own.
 int host_copy_bands(const w2x_ctx *ctx, int n_model, int width, int height, int block_splitting) {
     int nb = ctx->host_bands > 0 ? ctx->host_bands : std::min(4, height / 512);
-    const bool literal_walk = block_splitting && ctx->walk == W2X_WALK_BLOCKS && w2x_requires_splitting(width, height);
     if (nb > 8) nb = 8;
-    if (nb < 2 || literal_walk || height / nb < 2 * n_model) return 1;
+    if (nb < 2 || literal_walk(ctx, width, height, block_splitting) || height / nb < 2 * n_model) return 1;
     return nb;
 }
 
@@ -388,29 +380,61 @@ int run_host_groups(w2x_ctx *ctx, const std::vector<HostGroup> &groups) {
     return W2X_OK;
 }
 
-int convert_device(w2x_ctx *ctx, const w2x_model *m, const float *d_in, int w, int h, size_t in_stride_bytes,
-                   int rows_above, int rows_below, float *d_out, size_t out_stride_bytes, int block_splitting, bool up2x) {
+// The literal walk needs every block inside the plane; block_table places columns by the block height, as the reference does, so
+// a non-square block size can put one past the plane's edge.
+int check_blocks(const w2x_ctx *ctx, int n, int w, int h, int block_splitting) {
+    if (!literal_walk(ctx, w, h, block_splitting)) return W2X_OK;
+    const std::vector<int> tab = blocks_of(w, h, n);
+    if (tab.empty()) return fail(W2X_ERR_ARG, "block size too small for a %d-layer model", n);
+    for (size_t i = 0; i < tab.size(); i += 8) {
+        const int *t = &tab[i];
+        if (t[6] + (t[3] - t[2]) - 2 * n > h || t[7] + (t[5] - t[4]) - 2 * n > w)
+            return fail(W2X_ERR_ARG, "block (%d,%d) does not fit the output plane (non-square block size?)", t[1], t[0]);
+    }
+    return W2X_OK;
+}
+
+// Every argument of a plane conversion on device buffers, before anything is printed or queued.
+int check_plane(w2x_ctx *ctx, const w2x_model *m, const float *d_in, int w, int h, size_t in_stride_bytes, const float *d_out,
+                size_t out_stride_bytes, int block_splitting) {
     if (!m || !d_in || !d_out || w < 1 || h < 1) return fail(W2X_ERR_ARG, "w2x_convert_plane: bad argument");
-    const int in_w = up2x ? (w + 1) / 2 : w;
-    if (in_stride_bytes % 4 || out_stride_bytes % 4 || in_stride_bytes < (size_t)in_w * 4 || out_stride_bytes < (size_t)w * 4)
+    if (in_stride_bytes % 4 || out_stride_bytes % 4 || in_stride_bytes < (size_t)w * 4 || out_stride_bytes < (size_t)w * 4)
         return fail(W2X_ERR_ARG, "w2x_convert_plane: row strides must be multiples of 4 bytes and >= width*4");
     if (m->layers.front().n_in != 1 || m->layers.back().n_out != 1)
         return fail(W2X_ERR_ARG, "w2x_convert_plane: model must map 1 plane to 1 plane");
+    if (pick_engine(ctx, m) < 0) return W2X_ERR_UNSUPPORTED;
+    return check_blocks(ctx, (int)m->layers.size(), w, h, block_splitting);
+}
+
+// The progress lines of one convertWithModels-equivalent plane of w x h (host: through w2x_convert_plane's copy pipeline).  A
+// plane the reference splits gets the reference's block sequence, whichever walk runs it; any other the layers' lines once when
+// the copy pipeline cuts it into bands, else once per scratch band of run_padded_plane.
+void emit_plane_progress(w2x_ctx *ctx, const w2x_model *m, int w, int h, int block_splitting, bool host) {
+    if (!ctx->log) return;
+    const int n = (int)m->layers.size();
+    if (block_splitting && w2x_requires_splitting(w, h)) return emit_reference_progress(ctx, w, h, n, true);
+    const int band = scratch_band_rows(ctx, m, w, h);
+    const int passes = host && host_copy_bands(ctx, n, w, h, 0) > 1 ? 1 : (h + band - 1) / band;
+    for (int p = 0; p < passes; p++) emit_reference_progress(ctx, w, h, n, false);
+}
+
+// convertWithModels on checked device buffers (rows_above / rows_below: real neighbour rows available around the band).  up2x: the
+// plane converted is the nearest-neighbour 2x resize of d_in, never materialised; w x h is its (2x) size, the row counts are 2x
+// rows, and a band of it starts on an even 2x row with d_in pointing at its first source row.
+int convert_device(w2x_ctx *ctx, const w2x_model *m, const float *d_in, int w, int h, size_t in_stride_bytes,
+                   int rows_above, int rows_below, float *d_out, size_t out_stride_bytes, int block_splitting, bool up2x = false) {
     DeviceGuard g(ctx->device);
     NvtxRange nvtx("w2x convertWithModels");
     const int engine = pick_engine(ctx, m);
-    if (engine < 0) return W2X_ERR_UNSUPPORTED;
     DevModel *dm = nullptr;
     int rc = get_dev_model(ctx, m, &dm);
     if (rc) return rc;
     const int n = (int)m->layers.size();
     const int pw = w + 2 * n, ph = h + 2 * n;
     const long ostride = (long)(out_stride_bytes / 4);
-    const bool split = block_splitting && w2x_requires_splitting(w, h);
-    if (engine == W2X_ENGINE_TC && !(split && ctx->walk == W2X_WALK_BLOCKS)) {
+    const bool literal = literal_walk(ctx, w, h, block_splitting);
+    if (engine == W2X_ENGINE_TC && !literal) {
         // cv::copyMakeBorder (src/convertRoutine.cpp:35, :96) is folded into the first layer's loads: no padded copy of the plane
-        if (split && !ctx->log_muted) emit_reference_progress(ctx, w, h, n, true);
-        LogMute mute(ctx, split);
         return run_padded_plane(ctx, m, dm, engine, nullptr, w, h, d_out, ostride, d_in, (long)(in_stride_bytes / 4), rows_above, rows_below,
                                 up2x);
     }
@@ -424,27 +448,16 @@ int convert_device(w2x_ctx *ctx, const w2x_model *m, const float *d_in, int w, i
         CU_CHECK(launch_pad_replicate(d_in, w, h, (long)(in_stride_bytes / 4), n, std::min(rows_above, n),
                                       std::min(rows_below, n), ctx->pad_buf, ctx->stream));
     ctx->launches++;
-    if (split && ctx->walk == W2X_WALK_BLOCKS) {
-        // the literal block walk of convertWithModelsBlockSplit (src/convertRoutine.cpp:114-165)
-        const Config &cfg = config();
-        int nb = block_table(w, h, cfg.block_w, cfg.block_h, n, nullptr, 0, nullptr, nullptr);
-        if (nb < 0) return fail(W2X_ERR_ARG, "block size too small for a %d-layer model", n);
-        std::vector<int> tab((size_t)nb * 8);
-        block_table(w, h, cfg.block_w, cfg.block_h, n, tab.data(), nb, nullptr, nullptr);
-        for (int i = 0; i < nb; i++) {
-            const int *t = &tab[(size_t)i * 8];
-            logf(ctx, "start process block (%d,%d) ...", t[1], t[0]);              // :133-134 prints (c,r)
-            const int bw_i = t[5] - t[4], bh_i = t[3] - t[2];
-            if (t[6] + bh_i - 2 * n > h || t[7] + bw_i - 2 * n > w)
-                return fail(W2X_ERR_ARG, "block (%d,%d) does not fit the output plane (non-square block size?)", t[1], t[0]);
-            rc = run_basic(ctx, m, dm, engine, ctx->pad_buf + (long)t[2] * pw + t[4], pw, bw_i, bh_i,
+    if (literal) {   // check_blocks has seen every block fit
+        const std::vector<int> tab = blocks_of(w, h, n);
+        for (size_t i = 0; i < tab.size(); i += 8) {
+            const int *t = &tab[i];
+            rc = run_basic(ctx, m, dm, engine, ctx->pad_buf + (long)t[2] * pw + t[4], pw, t[5] - t[4], t[3] - t[2],
                            d_out + (long)t[6] * ostride + t[7], ostride);
             if (rc) return rc;
         }
         return W2X_OK;
     }
-    if (split && !ctx->log_muted) emit_reference_progress(ctx, w, h, n, true);     // fused walk: the reference's per-block lines, up front
-    LogMute mute(ctx, split);
     return run_padded_plane(ctx, m, dm, engine, ctx->pad_buf, w, h, d_out, ostride);
 }
 
@@ -654,6 +667,9 @@ W2X_API int w2x_debug_set_fuse_last(w2x_ctx *ctx, int on) {
 int w2x_convert_plane_device(w2x_ctx *ctx, const w2x_model *model, const float *d_in, int width, int height,
                              size_t in_stride_bytes, float *d_out, size_t out_stride_bytes, int block_splitting) {
     if (check_ctx(ctx)) return W2X_ERR_ARG;
+    int rc = check_plane(ctx, model, d_in, width, height, in_stride_bytes, d_out, out_stride_bytes, block_splitting);
+    if (rc) return rc;
+    emit_plane_progress(ctx, model, width, height, block_splitting, false);
     return convert_device(ctx, model, d_in, width, height, in_stride_bytes, 0, 0, d_out, out_stride_bytes, block_splitting);
 }
 
@@ -666,6 +682,9 @@ int w2x_convert_band_device(w2x_ctx *ctx, const w2x_model *model, const float *d
                     model->layers.size());
     if (!d_in) return fail(W2X_ERR_ARG, "w2x_convert_band_device: NULL input");
     const float *band0 = d_in + (size_t)rows_above * (in_stride_bytes / 4);
+    int rc = check_plane(ctx, model, band0, width, band_height, in_stride_bytes, d_out, out_stride_bytes, 0);
+    if (rc) return rc;
+    emit_plane_progress(ctx, model, width, band_height, 0, false);
     return convert_device(ctx, model, band0, width, band_height, in_stride_bytes, rows_above, rows_below, d_out,
                           out_stride_bytes, 0);
 }
@@ -676,21 +695,19 @@ int w2x_convert_plane(w2x_ctx *ctx, const w2x_model *model, const float *in, int
     if (!model || !in || !out || width < 1 || height < 1) return fail(W2X_ERR_ARG, "w2x_convert_plane: bad argument");
     if (in_stride_bytes < (size_t)width * 4 || out_stride_bytes < (size_t)width * 4)
         return fail(W2X_ERR_ARG, "w2x_convert_plane: row stride smaller than a row");
-    DeviceGuard g(ctx->device);
     const size_t bytes = (size_t)width * height * sizeof(float), row = (size_t)width * 4;
-    for (int i = 0; i < 2; i++) {
-        int rc = ensure(reinterpret_cast<void **>(&ctx->io_buf[i]), &ctx->io_bytes[i], bytes);
-        if (rc) return rc;
-    }
+    int rc = check_plane(ctx, model, in, width, height, row, out, row, block_splitting);   // the rest, on the dense staged planes
+    if (rc) return rc;
+    emit_plane_progress(ctx, model, width, height, block_splitting, true);
+    DeviceGuard g(ctx->device);
+    for (int i = 0; i < 2 && !rc; i++) rc = ensure(reinterpret_cast<void **>(&ctx->io_buf[i]), &ctx->io_bytes[i], bytes);
+    if (rc) return rc;
     float *din = ctx->io_buf[0], *dout = ctx->io_buf[1];
     // Large planes are cut into row bands so that the upload of band i+1 and the download of band i-1 overlap the
     // layers of band i (copy engines + compute run concurrently); each band re-reads n real rows of context from its
     // neighbours, which keeps the result bit-identical to the single-pass path.
     const int n_model = (int)model->layers.size();
     const int nb = host_copy_bands(ctx, n_model, width, height, block_splitting);
-    // the copy pipeline cuts the plane its own way: the reference's progress lines for this plane go out first
-    if (nb > 1) emit_reference_progress(ctx, width, height, n_model, block_splitting && w2x_requires_splitting(width, height));
-    LogMute mute(ctx, nb > 1);
     std::vector<HostGroup> groups((size_t)nb);
     for (int i = 0; i < nb; i++) {
         const int y = (int)((long)height * i / nb), y_end = (int)((long)height * (i + 1) / nb);
@@ -945,12 +962,14 @@ int convert_tiles_dev(w2x_ctx *ctx, const w2x_model *m, const float *d_in, float
     if (rc) return rc;
     const int n = (int)m->layers.size();
     const int pw = w + 2 * n, ph = h + 2 * n;
-    if (packs_frames(ctx, m, dm, engine)) {
-        // tiles per frame: what the scratch limit (one frame of maxc channels, 4 bytes per element) and MAX_FRAME_ROWS allow; the
-        // tiles of a frame are stacked vertically, each padded like cv::copyMakeBorder (src/convertRoutine.cpp:35) by the pack
-        const size_t per_tile = (size_t)max_channels(m) * pw * ph * 4;
-        const size_t fit = std::min(ctx->scratch_limit / per_tile, (size_t)(MAX_FRAME_ROWS / ph));
-        const int group = (int)std::max<size_t>(1, std::min<size_t>((size_t)n_tiles, fit));
+    const bool packed = packs_frames(ctx, m, dm, engine);
+    // tiles per frame (1 unpacked): what the scratch limit (one frame of maxc channels, 4 bytes per element) and MAX_FRAME_ROWS allow;
+    // the tiles of a frame are stacked vertically, each padded like cv::copyMakeBorder (src/convertRoutine.cpp:35) by the pack
+    const size_t per_tile = (size_t)max_channels(m) * pw * ph * 4;
+    const size_t fit = std::min(ctx->scratch_limit / per_tile, (size_t)(MAX_FRAME_ROWS / ph));
+    const int group = packed ? (int)std::max<size_t>(1, std::min<size_t>((size_t)n_tiles, fit)) : 1;
+    for (int t0 = 0; t0 < n_tiles; t0 += group) emit_reference_progress(ctx, w, h, n, false);   // the layers run once per frame
+    if (packed) {
         std::vector<FramePlan> frames;
         for (int t0 = 0; t0 < n_tiles; t0 += group) {
             FramePlan f;
@@ -991,21 +1010,10 @@ int check_planes(const char *fn, const w2x_model *m, int n_planes, const float *
     return W2X_OK;
 }
 
-// The progress lines of the whole call, plane by plane in order, as the single-plane entry point (w2x_convert_plane with
-// host = true, else w2x_convert_plane_device) would log them with block_splitting = 0: one "Iteration #k..." per layer, per
-// scratch band of a plane too large to pack (the host entry point's copy pipeline logs a plane it cuts once).
-void emit_planes_progress(w2x_ctx *ctx, const w2x_model *m, int n_planes, const int *widths, const int *heights, const int *frame, bool host) {
-    if (!ctx->log || ctx->log_muted) return;
-    const int n = (int)m->layers.size();
-    for (int i = 0; i < n_planes; i++) {
-        int passes = 1;
-        if (frame[i] < 0 && !(host && host_copy_bands(ctx, n, widths[i], heights[i], 0) > 1)) {
-            const int band = scratch_band_rows(ctx, m, widths[i], heights[i]);
-            passes = (heights[i] + band - 1) / band;
-        }
-        for (int p = 0; p < passes; p++)
-            for (int k = 1; k <= n; k++) logf(ctx, "Iteration #%d...", k);
-    }
+// The lines of the whole call, plane by plane, as the single-plane entry point prints them with block_splitting = 0.  A packed
+// plane's padded rectangle fits the scratch limit and MAX_FRAME_ROWS (plan_planes), so it is one scratch band: its lines come once.
+void emit_planes_progress(w2x_ctx *ctx, const w2x_model *m, int n_planes, const int *widths, const int *heights, bool host) {
+    for (int i = 0; i < n_planes; i++) emit_plane_progress(ctx, m, widths[i], heights[i], 0, host);
 }
 
 struct PlanesPlan {
@@ -1035,6 +1043,7 @@ int convert_planes_dev(w2x_ctx *ctx, const w2x_model *m, int n_planes, const flo
     DeviceGuard g(ctx->device);
     const int engine = pick_engine(ctx, m);
     if (engine < 0) return W2X_ERR_UNSUPPORTED;
+    emit_planes_progress(ctx, m, n_planes, widths, heights, false);
     DevModel *dm = nullptr;
     rc = get_dev_model(ctx, m, &dm);
     if (rc) return rc;
@@ -1045,8 +1054,6 @@ int convert_planes_dev(w2x_ctx *ctx, const w2x_model *m, int n_planes, const flo
     }
     PlanesPlan p;
     plan_for(ctx, m, n_planes, widths, heights, &p);
-    emit_planes_progress(ctx, m, n_planes, widths, heights, p.frame.data(), false);
-    LogMute mute(ctx, true);
     std::vector<FramePlan> frames = frames_for(p);
     for (int i = 0; i < n_planes; i++)
         if (p.frame[(size_t)i] >= 0)
@@ -1065,8 +1072,6 @@ int planes_host(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int n_planes, co
                 const int *heights, const size_t *in_strides, float *const *out, const size_t *out_strides) {
     PlanesPlan p;
     plan_for(ctx, m, n_planes, widths, heights, &p);
-    emit_planes_progress(ctx, m, n_planes, widths, heights, p.frame.data(), true);
-    LogMute mute(ctx, true);
     std::vector<size_t> off((size_t)n_planes + 1, 0);
     for (int i = 0; i < n_planes; i++) off[(size_t)i + 1] = off[(size_t)i] + (size_t)widths[i] * heights[i];
     for (int i = 0; i < 2; i++) {
@@ -1224,6 +1229,7 @@ int w2x_convert_planes(w2x_ctx *ctx, const w2x_model *model, int n_planes, const
             rc = w2x_convert_plane(ctx, model, in[i], widths[i], heights[i], in_strides[i], out[i], out_strides[i], 0);
         return rc;
     }
+    emit_planes_progress(ctx, model, n_planes, widths, heights, true);
     return planes_host(ctx, model, dm, n_planes, in, widths, heights, in_strides, out, out_strides);
 }
 
@@ -1243,7 +1249,8 @@ struct ChainStep {
 
 // Every argument, before anything is queued: W2X_ERR_ARG naming the step it concerns.
 int check_chain(const char *fn, w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, const void *in, int width,
-                int height, size_t in_stride_bytes, const void *out, size_t out_stride_bytes, bool host, std::vector<ChainStep> *steps) {
+                int height, size_t in_stride_bytes, const void *out, size_t out_stride_bytes, int block_splitting, bool host,
+                std::vector<ChainStep> *steps) {
     if (check_ctx(ctx)) return W2X_ERR_ARG;
     if (n_steps < 1) return fail(W2X_ERR_ARG, "%s: n_steps is %d: at least one step (step 0) is needed", fn, n_steps);
     if (!models) return fail(W2X_ERR_ARG, "%s: step 0: NULL models array", fn);
@@ -1277,10 +1284,12 @@ int check_chain(const char *fn, w2x_ctx *ctx, int n_steps, const w2x_model *cons
         const char *o0 = static_cast<const char *>(out), *o1 = o0 + (size_t)(h - 1) * out_stride_bytes + (size_t)w * 4;
         if (i0 < o1 && o0 < i1) return fail(W2X_ERR_ARG, "%s: step %d: the output plane overlaps the input plane", fn, last);
     }
-    for (int k = 0; k < n_steps; k++) {   // engine choice (the tensor-core engine needs a 1->{32,64,128}...->1 chain)
-        if (pick_engine(ctx, (*steps)[(size_t)k].m) < 0) {
+    for (int k = 0; k < n_steps; k++) {   // engine choice (the tensor-core engine needs a 1->{32,64,128}...->1 chain), literal walk
+        const ChainStep &s = (*steps)[(size_t)k];
+        const int rc = pick_engine(ctx, s.m) < 0 ? W2X_ERR_UNSUPPORTED : check_blocks(ctx, (int)s.m->layers.size(), s.w, s.h, block_splitting);
+        if (rc) {
             const std::string why = w2x_last_error();
-            return fail(W2X_ERR_UNSUPPORTED, "%s: step %d: %s", fn, k, why.c_str());
+            return fail(rc, "%s: step %d: %s", fn, k, why.c_str());
         }
     }
     return W2X_OK;
@@ -1298,18 +1307,8 @@ int reserve_chain(w2x_ctx *ctx, const std::vector<ChainStep> &steps) {
     return W2X_OK;
 }
 
-// One step on device planes, logging what the single-plane entry point would log for the step's plane: w2x_convert_plane (host)
-// emits the reference's sequence up front when its copy pipeline cuts the plane, w2x_convert_plane_device logs as it goes.
-int chain_step(w2x_ctx *ctx, const ChainStep &s, const float *src, size_t src_stride, float *dst, size_t dst_stride, int block_splitting,
-               bool host) {
-    const int n = (int)s.m->layers.size();
-    const bool pipelined = host && host_copy_bands(ctx, n, s.w, s.h, block_splitting) >= 2;
-    if (pipelined) emit_reference_progress(ctx, s.w, s.h, n, block_splitting && w2x_requires_splitting(s.w, s.h));
-    LogMute mute(ctx, pipelined);
-    return convert_device(ctx, s.m, src, s.w, s.h, src_stride, 0, 0, dst, dst_stride, block_splitting, s.up);
-}
-
 // Steps [0, n_dev) on the device: the first reads d_in, step k writes chain_buf[k & 1], the last of the whole chain writes d_out.
+// Each prints the lines of w2x_convert_plane (host) or w2x_convert_plane_device for its plane.
 int chain_device_steps(w2x_ctx *ctx, const std::vector<ChainStep> &steps, int n_dev, const float *d_in, size_t in_stride, float *d_out,
                        size_t out_stride, int block_splitting, w2x_step_fn on_step, void *user, bool host) {
     const float *cur = d_in;
@@ -1320,7 +1319,8 @@ int chain_device_steps(w2x_ctx *ctx, const std::vector<ChainStep> &steps, int n_
         float *dst = last ? d_out : ctx->chain_buf[k & 1];
         const size_t dst_stride = last ? out_stride : (size_t)s.w * sizeof(float);
         if (on_step) on_step(k, user);
-        int rc = chain_step(ctx, s, cur, cur_stride, dst, dst_stride, block_splitting, host);
+        emit_plane_progress(ctx, s.m, s.w, s.h, block_splitting, host);
+        int rc = convert_device(ctx, s.m, cur, s.w, s.h, cur_stride, 0, 0, dst, dst_stride, block_splitting, s.up);
         if (rc) return rc;
         cur = dst;
         cur_stride = dst_stride;
@@ -1350,9 +1350,8 @@ int chain_host(w2x_ctx *ctx, const std::vector<ChainStep> &steps, const float *i
     const size_t src_stride = n_steps == 1 ? in_dense : (size_t)steps[(size_t)n_steps - 2].w * 4;
     float *dout = ctx->io_buf[1];
     if (on_step) on_step(n_steps - 1, user);
+    emit_plane_progress(ctx, L.m, L.w, L.h, block_splitting, true);
     const int nb = host_copy_bands(ctx, n, L.w, L.h, block_splitting);
-    if (nb > 1) emit_reference_progress(ctx, L.w, L.h, n, block_splitting && w2x_requires_splitting(L.w, L.h));
-    LogMute mute(ctx, nb > 1);
     auto band_y = [&](int i) { return (int)((long)L.h * i / nb) & (L.up ? ~1 : ~0); };
     std::vector<HostGroup> groups((size_t)nb);
     for (int i = 0; i < nb; i++) {
@@ -1376,7 +1375,7 @@ int w2x_convert_chain_device(w2x_ctx *ctx, int n_steps, const w2x_model *const *
                              w2x_step_fn on_step, void *user) {
     std::vector<ChainStep> steps;
     int rc = check_chain("w2x_convert_chain_device", ctx, n_steps, models, kinds, d_in, width, height, in_stride_bytes, d_out, out_stride_bytes,
-                         false, &steps);
+                         block_splitting, false, &steps);
     if (rc) return rc;
     DeviceGuard g(ctx->device);
     NvtxRange nvtx("w2x convert chain");
@@ -1388,8 +1387,8 @@ int w2x_convert_chain_device(w2x_ctx *ctx, int n_steps, const w2x_model *const *
 int w2x_convert_chain(w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, const float *in, int width, int height,
                       size_t in_stride_bytes, float *out, size_t out_stride_bytes, int block_splitting, w2x_step_fn on_step, void *user) {
     std::vector<ChainStep> steps;
-    int rc = check_chain("w2x_convert_chain", ctx, n_steps, models, kinds, in, width, height, in_stride_bytes, out, out_stride_bytes, true,
-                         &steps);
+    int rc = check_chain("w2x_convert_chain", ctx, n_steps, models, kinds, in, width, height, in_stride_bytes, out, out_stride_bytes,
+                         block_splitting, true, &steps);
     if (rc) return rc;
     DeviceGuard g(ctx->device);
     NvtxRange nvtx("w2x convert chain");

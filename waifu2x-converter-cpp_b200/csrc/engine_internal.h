@@ -49,7 +49,6 @@ struct w2x_ctx {
     size_t scratch_limit = (size_t)16 << 30;
     w2x_log_fn log = nullptr;
     void *log_user = nullptr;
-    bool log_muted = false;            // the reference's line sequence of the current call has already been emitted
     uint64_t launches = 0;
     bool timing = false;
     std::vector<w2x::eng::TimedSpan> spans;
@@ -140,11 +139,6 @@ void emit_reference_progress(w2x_ctx *ctx, int w, int h, int n_layers, bool spli
 // Only frame rows [out_y0, out_y0 + out_rows) are stored (out_rows < 0: the whole frame).
 int launch_layer_tc(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int li, const __half *in, __half *out, int pw, int ph,
                     bool fused, bool profile, int out_y0 = 0, int out_rows = -1);
-// convertWithModels on device buffers (rows_above / rows_below: real neighbour rows available around the band).
-// up2x: the plane converted is the nearest-neighbour 2x resize of d_in, never materialised; w x h is its (2x) size, the row
-// counts are 2x rows, and a band of it starts on an even 2x row with d_in pointing at its first source row.
-int convert_device(w2x_ctx *ctx, const w2x_model *m, const float *d_in, int w, int h, size_t in_stride_bytes, int rows_above,
-                   int rows_below, float *d_out, size_t out_stride_bytes, int block_splitting, bool up2x = false);
 
 int tiles_enqueue_compute(w2x_ctx *ctx, const w2x_model *model, const float *const *in_tiles, float *const *out_tiles, int n_tiles, int width, int height, size_t in_stride_bytes, size_t out_stride_bytes);
 int tiles_enqueue_download(w2x_ctx *ctx, float *const *out_tiles, int n_tiles, int width, int height, size_t out_stride_bytes);
