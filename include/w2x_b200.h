@@ -318,6 +318,35 @@ W2X_API int w2x_convert_chain_device(w2x_ctx *ctx, int n_steps, const w2x_model 
                                      float *d_out, size_t out_stride_bytes, int block_splitting, w2x_step_fn on_step,
                                      void *user);
 
+/* ---- a chain of conversions on a collection of planes of any sizes ------------------------------------ */
+/* w2x_convert_chain for every plane of a w2x_convert_planes collection, in one call: the default noise_scale mode of a sprite set,
+ * say.  Step k maps every plane P to convertWithModels(models[k], U_k(P)), U_k as in w2x_convert_chain, with block splitting off;
+ * plane i comes out (widths[i] << u) x (heights[i] << u), u = the number of W2X_STEP_UPSCALE2X steps.  Every output is
+ * bit-identical to w2x_convert_chain(..., block_splitting = 0) on that plane alone, and to the per-step loop of w2x_convert_planes
+ * on the resized planes, on the same context settings.  Each step packs its planes into frames as w2x_convert_planes does, planned
+ * on the step's output sizes (a plane may pack at one step and be converted alone after a 2x step); an upscaling step packs
+ * straight from the half-resolution planes and never builds the 2x ones.  With n_steps == 1 and W2X_STEP_SAME this is
+ * w2x_convert_planes: same bits, same progress lines, same launches.
+ * Before step k is queued, on_step(k, user) is called (if not NULL); then the step logs the lines w2x_convert_planes (host entry) or
+ * w2x_convert_planes_device (device entry) logs for its planes, in plane order.
+ * Every argument is checked before anything is printed, allocated or queued; W2X_ERR_ARG names the step or the plane: n_steps or
+ * n_planes < 1, a NULL array, model or plane, an unknown kind, a model that does not map 1 plane to 1 plane, an output size that
+ * overflows int, row strides that are not multiples of 4 bytes or shorter than the plane's input (in_strides) or output
+ * (out_strides) row.  A model the engine refuses gives W2X_ERR_UNSUPPORTED naming the step.  Planes must not overlap one another's
+ * outputs (as in w2x_convert_planes).
+ * Device memory: two buffers of the context, each holding one step's outputs for the whole collection (only with 2 steps and
+ * more), plus the frame scratch of w2x_convert_planes; the host entry also stages every input and every output plane on the device.
+ * All of it is reserved before the first copy or launch: W2X_ERR_NOMEM leaves nothing queued.
+ * HOST buffers, synchronous; uploads overlap the first step and downloads the last. */
+W2X_API int w2x_convert_planes_chain(w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, int n_planes,
+                                     const float *const *in, const int *widths, const int *heights, const size_t *in_strides,
+                                     float *const *out, const size_t *out_strides, w2x_step_fn on_step, void *user);
+/* Same on DEVICE planes (the pointer, size and stride arrays themselves are host arrays), asynchronous on the context's stream. */
+W2X_API int w2x_convert_planes_chain_device(w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds,
+                                            int n_planes, const float *const *d_in, const int *widths, const int *heights,
+                                            const size_t *in_strides, float *const *d_out, const size_t *out_strides,
+                                            w2x_step_fn on_step, void *user);
+
 /* ---- one process, N GPUs ---------------------------------------------------------------------- */
 /* The sibling of the reference's -j (src/main.cpp:58-60, modelUtility::setNumberOfJobs): N contexts driven by
  * one host thread.  w2x_multi_convert_plane = w2x_convert_plane with the plane cut into N row bands and the

@@ -41,6 +41,7 @@ ABI_SYMBOLS = (
     "w2x_host_alloc", "w2x_host_free", "w2x_ctx_forget_model", "w2x_slab_create", "w2x_slab_destroy", "w2x_slab_export",
     "w2x_slab_connect", "w2x_slab_connect_local", "w2x_slab_convert", "w2x_slab_convert_async", "w2x_slab_synchronize",
     "w2x_convert_planes", "w2x_convert_planes_device", "w2x_convert_chain", "w2x_convert_chain_device",
+    "w2x_convert_planes_chain", "w2x_convert_planes_chain_device",
 )
 BAND_BLOB_BYTES = 320
 
@@ -145,6 +146,8 @@ def lib():
     L.w2x_convert_planes_device.argtypes = [vp, vp, ci, C.POINTER(vp), pi, pi, ps, C.POINTER(vp), ps]
     L.w2x_convert_chain.argtypes = [vp, ci, C.POINTER(vp), pi, vp, ci, ci, cs, vp, cs, ci, STEP_FN, vp]
     L.w2x_convert_chain_device.argtypes = [vp, ci, C.POINTER(vp), pi, vp, ci, ci, cs, vp, cs, ci, STEP_FN, vp]
+    L.w2x_convert_planes_chain.argtypes = [vp, ci, C.POINTER(vp), pi, ci, C.POINTER(vp), pi, pi, ps, C.POINTER(vp), ps, STEP_FN, vp]
+    L.w2x_convert_planes_chain_device.argtypes = [vp, ci, C.POINTER(vp), pi, ci, C.POINTER(vp), pi, pi, ps, C.POINTER(vp), ps, STEP_FN, vp]
     L.w2x_debug_plan_planes.argtypes = [ci, pi, pi, ci, ci, cs, pi, pi, pi, pi, ci]
     L.w2x_multi_create.argtypes = [C.POINTER(ci), ci, C.POINTER(vp)]
     L.w2x_multi_destroy.argtypes = [vp]
@@ -417,21 +420,28 @@ class Context:
     def convert_planes(self, model: Model, planes, out=None):
         """planes: 2-D float32 arrays (row-strided views are passed as they are) -> list of outputs; `out` may be a list of
         2-D float32 arrays of the same shapes (strided views included), written in place."""
+        xs, ip, ws, hs, ist, out, op, ost = self._planes_args(planes, out, 0)
+        _check(lib().w2x_convert_planes(self._h, model._h, len(xs), ip, ws, hs, ist, op, ost))
+        return out
+
+    @staticmethod
+    def _planes_args(planes, out, ups):
+        """inputs and outputs of a planes call whose planes come out (h << ups) x (w << ups)"""
         def fix(p):
             x = np.asarray(p, np.float32)
             if x.ndim == 2 and (x.strides[1] != 4 or x.strides[0] % 4 or x.strides[0] < x.shape[1] * 4):
                 x = np.ascontiguousarray(x)
             return x
         xs, ip, ws, hs, ist = _plane_arrays(planes, fix)
+        shapes = [(x.shape[0] << ups, x.shape[1] << ups) for x in xs]
         if out is None:
-            out = [np.empty(x.shape, np.float32) for x in xs]
-        if len(out) != len(xs) or any(o.shape != x.shape for o, x in zip(out, xs)):
-            raise ValueError("out must hold one array per plane, of the plane's shape")
+            out = [np.empty(s, np.float32) for s in shapes]
+        if len(out) != len(xs) or any(o.shape != s for o, s in zip(out, shapes)):
+            raise ValueError("out must hold one array per plane, of the plane's shape" + (" upscaled" if ups else ""))
         if any(o.strides[1] != 4 or o.strides[0] % 4 for o in out):
             raise ValueError("out arrays need unit column stride and row strides that are multiples of 4 bytes")
         _, op, _, _, ost = _plane_arrays(out, lambda o: o)
-        _check(lib().w2x_convert_planes(self._h, model._h, len(xs), ip, ws, hs, ist, op, ost))
-        return out
+        return xs, ip, ws, hs, ist, out, op, ost
 
     def convert_planes_device(self, model: Model, d_in, widths, heights, in_strides, d_out, out_strides):
         """Device pointers (ints) and host lists of sizes / row strides in bytes; asynchronous on the context's stream."""
@@ -477,6 +487,24 @@ class Context:
         n, models, kinds, cb, _ = self._chain_args(steps, on_step)
         _check(lib().w2x_convert_chain_device(self._h, n, models, kinds, C.c_void_p(d_in), w, h, in_stride_bytes, C.c_void_p(d_out),
                                               out_stride_bytes, int(bool(block_splitting)), cb, None))
+
+    # convert_chain for every plane of a convert_planes collection, each step packing the planes into frames
+    def convert_planes_chain(self, steps, planes, out=None, on_step=None):
+        """steps: (model, upscale) pairs as in convert_chain; planes: 2-D float32 arrays as in convert_planes -> list of outputs,
+        plane i (h << u) x (w << u) for u upscaling steps; `out` may be a list of such arrays (strided views included), written in
+        place.  on_step(k) is called before step k."""
+        n, models, kinds, cb, ups = self._chain_args(steps, on_step)
+        xs, ip, ws, hs, ist, out, op, ost = self._planes_args(planes, out, ups)
+        _check(lib().w2x_convert_planes_chain(self._h, n, models, kinds, len(xs), ip, ws, hs, ist, op, ost, cb, None))
+        return out
+
+    def convert_planes_chain_device(self, steps, d_in, widths, heights, in_strides, d_out, out_strides, on_step=None):
+        """Device pointers (ints) and host lists of input sizes / row strides in bytes; asynchronous on the context's stream."""
+        n, models, kinds, cb, _ = self._chain_args(steps, on_step)
+        k = len(d_in)
+        _check(lib().w2x_convert_planes_chain_device(self._h, n, models, kinds, k, (C.c_void_p * k)(*d_in), (C.c_int * k)(*widths),
+                                                     (C.c_int * k)(*heights), (C.c_size_t * k)(*in_strides),
+                                                     (C.c_void_p * k)(*d_out), (C.c_size_t * k)(*out_strides), cb, None))
 
     # w2xc::Model::filter on host planes [n_in][h][w] -> [n_out][h][w]
     def filter_layer(self, model: Model, layer, in_planes):

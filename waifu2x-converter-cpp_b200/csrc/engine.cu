@@ -919,21 +919,23 @@ int upload_frames(w2x_ctx *ctx, std::vector<FramePlan> &frames, std::vector<Fram
     return W2X_OK;
 }
 
-// Sizes the scratch for the largest frame once, so that no buffer is reallocated between frames.
-int reserve_frames(w2x_ctx *ctx, const w2x_model *m, const std::vector<FrameDev> &frames) {
+// Sizes the scratch for the largest of frames [f0, f1) of a model of maxc channels once, so that no buffer is reallocated between
+// frames.
+int reserve_frames(w2x_ctx *ctx, const std::vector<FramePlan> &frames, size_t f0, size_t f1, int maxc) {
     size_t px = 0;
-    for (auto &f : frames) px = std::max(px, (size_t)f.fw * f.fh);
+    for (size_t f = f0; f < f1; f++) px = std::max(px, (size_t)frames[f].fw * frames[f].fh);
     int rc = ensure(reinterpret_cast<void **>(&ctx->pad_buf), &ctx->pad_bytes, px * sizeof(float));
-    for (int i = 0; i < 2 && !rc; i++) rc = ensure(&ctx->buf[i], &ctx->buf_bytes[i], px * (size_t)max_channels(m) * 4);
+    for (int i = 0; i < 2 && !rc; i++) rc = ensure(&ctx->buf[i], &ctx->buf_bytes[i], px * (size_t)maxc * 4);
     return rc;
 }
 
-// One packed frame: the pack, the layers on the whole frame, the gather -- n + 1 launches whatever the number of planes.
-int run_packed_frame(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, const FrameDev &f) {
+// One packed frame: the pack, the layers on the whole frame, the gather -- n + 1 launches whatever the number of planes.  up2x: the
+// frame's planes are the nearest-neighbour 2x resizes of their sources (tc::launch_pack_planes).
+int run_packed_frame(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, const FrameDev &f, bool up2x = false) {
     const int n = (int)m->layers.size();
     int rc = ensure(reinterpret_cast<void **>(&ctx->pad_buf), &ctx->pad_bytes, (size_t)f.fw * f.fh * sizeof(float));
     if (rc) return rc;
-    CU_CHECK(tc::launch_pack_planes(f.rect, f.shelf_y0, f.shelf_first, f.n_shelf, n, f.fw, f.fh, ctx->pad_buf, ctx->stream));
+    CU_CHECK(tc::launch_pack_planes(f.rect, f.shelf_y0, f.shelf_first, f.n_shelf, n, f.fw, f.fh, up2x, ctx->pad_buf, ctx->stream));
     ctx->launches++;
     const PackedGather g{f.rect, f.n_rect, f.n_blocks};
     return run_basic(ctx, m, dm, W2X_ENGINE_TC, ctx->pad_buf, f.fw, f.fw, f.fh, nullptr, 0, &g);
@@ -941,8 +943,8 @@ int run_packed_frame(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, const Frame
 
 int run_packed_frames(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, std::vector<FramePlan> &frames) {
     std::vector<FrameDev> fd;
-    int rc = upload_frames(ctx, frames, &fd);
-    if (!rc) rc = reserve_frames(ctx, m, fd);
+    int rc = reserve_frames(ctx, frames, 0, frames.size(), max_channels(m));
+    if (!rc) rc = upload_frames(ctx, frames, &fd);
     for (size_t f = 0; f < fd.size() && !rc; f++) rc = run_packed_frame(ctx, m, dm, fd[f]);
     if (rc) return rc;
     CU_CHECK(cudaEventRecord(ctx->plan_ev, ctx->stream));
@@ -994,18 +996,30 @@ int convert_tiles_dev(w2x_ctx *ctx, const w2x_model *m, const float *d_in, float
     return W2X_OK;
 }
 
-// ---- independent planes of any sizes (w2x_convert_planes*) ------------------------------------------------------------------
-int check_planes(const char *fn, const w2x_model *m, int n_planes, const float *const *in, const int *widths, const int *heights,
-                 const size_t *in_strides, float *const *out, const size_t *out_strides) {
-    if (!m) return fail(W2X_ERR_ARG, "%s: NULL model", fn);
+// ---- independent planes of any sizes (w2x_convert_planes*), also through a chain of steps (w2x_convert_planes_chain*) ---------
+// The plane arrays: plane i is widths[i] x heights[i] at in[i] and comes out (widths[i] << u) x (heights[i] << u) at out[i], u being
+// the number of 2x steps; row strides in bytes.
+int check_plane_arrays(const char *fn, int n_planes, const float *const *in, const int *widths, const int *heights, const size_t *in_strides,
+                       float *const *out, const size_t *out_strides, int u) {
     if (n_planes < 1) return fail(W2X_ERR_ARG, "%s: n_planes is %d, at least 1 plane is needed", fn, n_planes);
     if (!in || !widths || !heights || !in_strides || !out || !out_strides) return fail(W2X_ERR_ARG, "%s: NULL array argument", fn);
     for (int i = 0; i < n_planes; i++) {
         if (!in[i] || !out[i]) return fail(W2X_ERR_ARG, "%s: plane %d: NULL %s pointer", fn, i, in[i] ? "output" : "input");
         if (widths[i] < 1 || heights[i] < 1) return fail(W2X_ERR_ARG, "%s: plane %d: size %d x %d", fn, i, widths[i], heights[i]);
-        if (in_strides[i] % 4 || out_strides[i] % 4 || in_strides[i] < (size_t)widths[i] * 4 || out_strides[i] < (size_t)widths[i] * 4)
+        if (u > 30 || ((long)widths[i] << u) > INT_MAX || ((long)heights[i] << u) > INT_MAX)
+            return fail(W2X_ERR_ARG, "%s: plane %d: %d x %d after %d 2x steps overflows int", fn, i, widths[i], heights[i], u);
+        const size_t out_row = ((size_t)widths[i] << u) * 4;
+        if (in_strides[i] % 4 || out_strides[i] % 4 || in_strides[i] < (size_t)widths[i] * 4 || out_strides[i] < out_row)
             return fail(W2X_ERR_ARG, "%s: plane %d: row strides must be multiples of 4 bytes and >= width*4", fn, i);
     }
+    return W2X_OK;
+}
+
+int check_planes(const char *fn, const w2x_model *m, int n_planes, const float *const *in, const int *widths, const int *heights,
+                 const size_t *in_strides, float *const *out, const size_t *out_strides) {
+    if (!m) return fail(W2X_ERR_ARG, "%s: NULL model", fn);
+    int rc = check_plane_arrays(fn, n_planes, in, widths, heights, in_strides, out, out_strides, 0);
+    if (rc) return rc;
     if (m->layers.front().n_in != 1 || m->layers.back().n_out != 1) return fail(W2X_ERR_ARG, "%s: model must map 1 plane to 1 plane", fn);
     return W2X_OK;
 }
@@ -1036,85 +1050,218 @@ std::vector<FramePlan> frames_for(const PlanesPlan &p) {
     return frames;
 }
 
-int convert_planes_dev(w2x_ctx *ctx, const w2x_model *m, int n_planes, const float *const *d_in, const int *widths, const int *heights,
-                       const size_t *in_strides, float *const *d_out, const size_t *out_strides) {
-    int rc = check_planes("w2x_convert_planes_device", m, n_planes, d_in, widths, heights, in_strides, d_out, out_strides);
-    if (rc) return rc;
-    DeviceGuard g(ctx->device);
-    const int engine = pick_engine(ctx, m);
-    if (engine < 0) return W2X_ERR_UNSUPPORTED;
-    emit_planes_progress(ctx, m, n_planes, widths, heights, false);
+// One step of a planes call: every plane through one model, after the nearest 2x resize when `up`.
+struct PlaneIO { const float *src; size_t src_stride; float *dst; size_t dst_stride; };   // row strides in bytes
+struct PlanesStep {
+    const w2x_model *m;
+    bool up;
+    std::vector<int> w, h;              // the step's output sizes
     DevModel *dm = nullptr;
-    rc = get_dev_model(ctx, m, &dm);
-    if (rc) return rc;
-    if (!packs_frames(ctx, m, dm, engine)) {
-        for (int i = 0; i < n_planes && !rc; i++)
-            rc = convert_device(ctx, m, d_in[i], widths[i], heights[i], in_strides[i], 0, 0, d_out[i], out_strides[i], 0);
-        return rc;
+    bool packed = false;                // packs_frames: frames plus planes too large to pack, else every plane alone
+    PlanesPlan plan;                    // packed: each plane's frame (-1: converted alone) and place
+    size_t f0 = 0;                      // packed: index of its frame 0 in the call's frame table
+    std::vector<PlaneIO> io;            // each plane's source and destination at this step
+};
+
+std::vector<PlanesStep> one_step(const w2x_model *m, int n_planes, const int *widths, const int *heights) {
+    std::vector<PlanesStep> steps(1, PlanesStep{});
+    steps[0].m = m;
+    steps[0].up = false;
+    steps[0].w.assign(widths, widths + n_planes);
+    steps[0].h.assign(heights, heights + n_planes);
+    return steps;
+}
+
+// Every argument of w2x_convert_planes_chain*, before anything is printed, allocated or queued: W2X_ERR_ARG naming the step or the
+// plane it concerns, W2X_ERR_UNSUPPORTED naming the step whose model the engine refuses.
+int check_planes_chain(const char *fn, w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, int n_planes,
+                       const float *const *in, const int *widths, const int *heights, const size_t *in_strides, float *const *out,
+                       const size_t *out_strides, std::vector<PlanesStep> *steps) {
+    if (check_ctx(ctx)) return W2X_ERR_ARG;
+    if (n_steps < 1) return fail(W2X_ERR_ARG, "%s: n_steps is %d: at least one step (step 0) is needed", fn, n_steps);
+    if (!models) return fail(W2X_ERR_ARG, "%s: step 0: NULL models array", fn);
+    if (!kinds) return fail(W2X_ERR_ARG, "%s: step 0: NULL kinds array", fn);
+    int u = 0;
+    for (int k = 0; k < n_steps; k++) {
+        const w2x_model *m = models[k];
+        if (!m) return fail(W2X_ERR_ARG, "%s: step %d: NULL model", fn, k);
+        if (kinds[k] != W2X_STEP_SAME && kinds[k] != W2X_STEP_UPSCALE2X)
+            return fail(W2X_ERR_ARG, "%s: step %d: kind %d is neither W2X_STEP_SAME (0) nor W2X_STEP_UPSCALE2X (1)", fn, k, kinds[k]);
+        if (m->layers.front().n_in != 1 || m->layers.back().n_out != 1)
+            return fail(W2X_ERR_ARG, "%s: step %d: model must map 1 plane to 1 plane", fn, k);
+        if (kinds[k] == W2X_STEP_UPSCALE2X) u++;
     }
-    PlanesPlan p;
-    plan_for(ctx, m, n_planes, widths, heights, &p);
-    std::vector<FramePlan> frames = frames_for(p);
+    int rc = check_plane_arrays(fn, n_planes, in, widths, heights, in_strides, out, out_strides, u);
+    if (rc) return rc;
+    for (int k = 0; k < n_steps; k++)
+        if (pick_engine(ctx, models[k]) < 0) {
+            const std::string why = w2x_last_error();
+            return fail(W2X_ERR_UNSUPPORTED, "%s: step %d: %s", fn, k, why.c_str());
+        }
+    std::vector<int> w(widths, widths + n_planes), h(heights, heights + n_planes);
+    steps->assign((size_t)n_steps, PlanesStep{});
+    for (int k = 0; k < n_steps; k++) {
+        PlanesStep &s = (*steps)[(size_t)k];
+        s.m = models[k];
+        s.up = kinds[k] == W2X_STEP_UPSCALE2X;
+        if (s.up)
+            for (int i = 0; i < n_planes; i++) w[(size_t)i] *= 2, h[(size_t)i] *= 2;
+        s.w = w;
+        s.h = h;
+    }
+    return W2X_OK;
+}
+
+// Everything before the first copy or launch: the models on the device; where each plane comes from and goes to at each step (step
+// 0 reads ends[i].src, the last step writes ends[i].dst, step k < last writes its outputs densely into chain_buf[k & 1]); each
+// packed step's frame plan, made on its OUTPUT sizes, so that a plane may pack at one step and be converted alone after a 2x step;
+// the intermediate buffers and the frame scratch; then ONE upload of every step's frame tables, so that no step waits for the host.
+int prepare_planes(w2x_ctx *ctx, std::vector<PlanesStep> &steps, const std::vector<PlaneIO> &ends, std::vector<FrameDev> *fd) {
+    const size_t n_planes = ends.size(), last = steps.size() - 1;
+    size_t need[2] = {0, 0};
+    for (size_t k = 0; k < last; k++) {
+        size_t px = 0;
+        for (size_t i = 0; i < n_planes; i++) px += (size_t)steps[k].w[i] * steps[k].h[i];
+        need[k & 1] = std::max(need[k & 1], px * sizeof(float));
+    }
+    for (int i = 0; i < 2; i++) {
+        if (!need[i]) continue;
+        int rc = ensure(reinterpret_cast<void **>(&ctx->chain_buf[i]), &ctx->chain_bytes[i], need[i]);
+        if (rc) return rc;
+    }
+    std::vector<FramePlan> frames;
+    for (size_t k = 0; k <= last; k++) {
+        PlanesStep &s = steps[k];
+        int rc = get_dev_model(ctx, s.m, &s.dm);
+        if (rc) return rc;
+        s.packed = packs_frames(ctx, s.m, s.dm, pick_engine(ctx, s.m));
+        s.io.resize(n_planes);
+        size_t off = 0;
+        for (size_t i = 0; i < n_planes; i++) {
+            PlaneIO &p = s.io[i];
+            p.src = k == 0 ? ends[i].src : steps[k - 1].io[i].dst;
+            p.src_stride = k == 0 ? ends[i].src_stride : steps[k - 1].io[i].dst_stride;
+            p.dst = k == last ? ends[i].dst : ctx->chain_buf[k & 1] + off;
+            p.dst_stride = k == last ? ends[i].dst_stride : (size_t)s.w[i] * sizeof(float);
+            off += (size_t)s.w[i] * s.h[i];
+        }
+        if (!s.packed) continue;
+        plan_for(ctx, s.m, (int)n_planes, s.w.data(), s.h.data(), &s.plan);
+        s.f0 = frames.size();
+        for (FramePlan &f : frames_for(s.plan)) frames.push_back(std::move(f));
+        for (size_t i = 0; i < n_planes; i++) {
+            const int f = s.plan.frame[i];
+            if (f >= 0)
+                frames[s.f0 + (size_t)f].rect.push_back(tc::PlaneRect{s.io[i].src, s.io[i].dst, (long)(s.io[i].src_stride / 4), (long)(s.io[i].dst_stride / 4),
+                                                                      s.w[i], s.h[i], s.plan.x0[i], s.plan.y0[i], 0});
+        }
+        rc = reserve_frames(ctx, frames, s.f0, frames.size(), max_channels(s.m));
+        if (rc) return rc;
+    }
+    return frames.empty() ? W2X_OK : upload_frames(ctx, frames, fd);
+}
+
+// A unit of work of one step: one packed frame (n + 1 launches for all its planes), or one plane converted alone by the single-plane
+// step code of w2x_convert_chain (too large to pack, or a step that does not pack).  A step's units: its frames, then its other
+// planes, each in order.
+struct PlanesUnit { int frame; std::vector<int> planes; };
+std::vector<PlanesUnit> units_of(const PlanesStep &s) {
+    std::vector<PlanesUnit> units;
+    const int n_planes = (int)s.w.size();
+    if (s.packed) {
+        units.resize((size_t)s.plan.n_frames);
+        for (int f = 0; f < s.plan.n_frames; f++) units[(size_t)f].frame = f;
+        for (int i = 0; i < n_planes; i++)
+            if (s.plan.frame[(size_t)i] >= 0) units[(size_t)s.plan.frame[(size_t)i]].planes.push_back(i);
+    }
     for (int i = 0; i < n_planes; i++)
-        if (p.frame[(size_t)i] >= 0)
-            frames[(size_t)p.frame[(size_t)i]].rect.push_back(tc::PlaneRect{d_in[i], d_out[i], (long)(in_strides[i] / 4), (long)(out_strides[i] / 4),
-                                                                            widths[i], heights[i], p.x0[(size_t)i], p.y0[(size_t)i], 0});
-    if (!frames.empty()) rc = run_packed_frames(ctx, m, dm, frames);
-    for (int i = 0; i < n_planes && !rc; i++)   // too large to pack: the single-plane path, which fills the GPU by itself
-        if (p.frame[(size_t)i] < 0)
-            rc = convert_device(ctx, m, d_in[i], widths[i], heights[i], in_strides[i], 0, 0, d_out[i], out_strides[i], 0);
+        if (!s.packed || s.plan.frame[(size_t)i] < 0) units.push_back(PlanesUnit{-1, {i}});
+    return units;
+}
+
+int run_unit(w2x_ctx *ctx, const PlanesStep &s, const std::vector<FrameDev> &fd, const PlanesUnit &u) {
+    if (u.frame < 0) {
+        const int i = u.planes[0];
+        const PlaneIO &p = s.io[(size_t)i];
+        return convert_device(ctx, s.m, p.src, s.w[(size_t)i], s.h[(size_t)i], p.src_stride, 0, 0, p.dst, p.dst_stride, 0, s.up);
+    }
+    const size_t f = s.f0 + (size_t)u.frame;
+    int rc = run_packed_frame(ctx, s.m, s.dm, fd[f], s.up);
+    if (rc || f + 1 < fd.size()) return rc;
+    CU_CHECK(cudaEventRecord(ctx->plan_ev, ctx->stream));   // the last kernel reading the frame tables is queued
+    ctx->plan_ev_live = true;
+    return W2X_OK;
+}
+
+// on_step(k), then the lines the planes entry point prints for the step's (resized) planes.
+void begin_step(w2x_ctx *ctx, const std::vector<PlanesStep> &steps, size_t k, w2x_step_fn on_step, void *user, bool host) {
+    if (on_step) on_step((int)k, user);
+    const PlanesStep &s = steps[k];
+    emit_planes_progress(ctx, s.m, (int)s.w.size(), s.w.data(), s.h.data(), host);
+}
+
+// Device planes, checked: the steps in order on the context's stream.
+int planes_device(w2x_ctx *ctx, std::vector<PlanesStep> &steps, const float *const *d_in, const size_t *in_strides, float *const *d_out,
+                  const size_t *out_strides, w2x_step_fn on_step, void *user) {
+    std::vector<PlaneIO> ends(steps[0].w.size());
+    for (size_t i = 0; i < ends.size(); i++) ends[i] = PlaneIO{d_in[i], in_strides[i], d_out[i], out_strides[i]};
+    std::vector<FrameDev> fd;
+    int rc = prepare_planes(ctx, steps, ends, &fd);
+    for (size_t k = 0; k < steps.size() && !rc; k++) {
+        begin_step(ctx, steps, k, on_step, user, false);
+        for (const PlanesUnit &u : units_of(steps[k]))
+            if ((rc = run_unit(ctx, steps[k], fd, u))) break;
+    }
     return rc;
 }
 
-// Host planes, packed: dense device staging (plane i at the same offset in io_buf[0] and io_buf[1]).  A group of the copy pipeline
-// is a frame or one plane too large to pack.
-int planes_host(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int n_planes, const float *const *in, const int *widths,
-                const int *heights, const size_t *in_strides, float *const *out, const size_t *out_strides) {
-    PlanesPlan p;
-    plan_for(ctx, m, n_planes, widths, heights, &p);
-    std::vector<size_t> off((size_t)n_planes + 1, 0);
-    for (int i = 0; i < n_planes; i++) off[(size_t)i + 1] = off[(size_t)i] + (size_t)widths[i] * heights[i];
-    for (int i = 0; i < 2; i++) {
-        int rc = ensure(reinterpret_cast<void **>(&ctx->io_buf[i]), &ctx->io_bytes[i], off.back() * sizeof(float));
-        if (rc) return rc;
+// Host planes, checked: dense device staging, inputs in io_buf[0] and outputs in io_buf[1], and ONE run of the copy pipeline.  Each
+// unit of step 0 is a group carrying its planes' uploads, each step between the first and the last one compute-only group, each unit
+// of the last step a group carrying its planes' downloads: uploads overlap the first step and downloads the last.
+int planes_host(w2x_ctx *ctx, std::vector<PlanesStep> &steps, const float *const *in, const int *widths, const int *heights,
+                const size_t *in_strides, float *const *out, const size_t *out_strides, w2x_step_fn on_step, void *user) {
+    const PlanesStep &L = steps.back();
+    const size_t n_planes = L.w.size(), last = steps.size() - 1;
+    std::vector<size_t> in_off(n_planes + 1, 0), out_off(n_planes + 1, 0);
+    for (size_t i = 0; i < n_planes; i++) {
+        in_off[i + 1] = in_off[i] + (size_t)widths[i] * heights[i];
+        out_off[i + 1] = out_off[i] + (size_t)L.w[i] * L.h[i];
     }
+    int rc = ensure(reinterpret_cast<void **>(&ctx->io_buf[0]), &ctx->io_bytes[0], in_off.back() * sizeof(float));
+    if (!rc) rc = ensure(reinterpret_cast<void **>(&ctx->io_buf[1]), &ctx->io_bytes[1], out_off.back() * sizeof(float));
+    if (rc) return rc;
     float *din = ctx->io_buf[0], *dout = ctx->io_buf[1];
-    std::vector<FramePlan> frames = frames_for(p);
-    std::vector<HostGroup> groups(frames.size());
-    auto add_copies = [&](HostGroup &G, int i) {
-        const size_t row = (size_t)widths[i] * 4;
-        G.up.push_back({din + off[(size_t)i], row, in[i], in_strides[i], row, (size_t)heights[i]});
-        G.down.push_back({out[i], out_strides[i], dout + off[(size_t)i], row, row, (size_t)heights[i]});
-    };
-    for (int i = 0; i < n_planes; i++) {
-        const int f = p.frame[(size_t)i];
-        if (f < 0) continue;
-        frames[(size_t)f].rect.push_back(tc::PlaneRect{din + off[(size_t)i], dout + off[(size_t)i], widths[i], widths[i], widths[i], heights[i],
-                                                       p.x0[(size_t)i], p.y0[(size_t)i], 0});
-        add_copies(groups[(size_t)f], i);
-    }
+    std::vector<PlaneIO> ends(n_planes);
+    for (size_t i = 0; i < n_planes; i++) ends[i] = PlaneIO{din + in_off[i], (size_t)widths[i] * 4, dout + out_off[i], (size_t)L.w[i] * 4};
     std::vector<FrameDev> fd;
-    if (!frames.empty()) {
-        int rc = upload_frames(ctx, frames, &fd);
-        if (!rc) rc = reserve_frames(ctx, m, fd);
-        if (rc) return rc;
-    }
-    for (size_t f = 0; f < fd.size(); f++)
-        groups[f].compute = [&, f]() -> int {
-            int rc = run_packed_frame(ctx, m, dm, fd[f]);
-            if (rc || f + 1 < fd.size()) return rc;
-            CU_CHECK(cudaEventRecord(ctx->plan_ev, ctx->stream));   // the last kernel reading the frame tables is queued
-            ctx->plan_ev_live = true;
-            return W2X_OK;
-        };
-    for (int i = 0; i < n_planes; i++) {
-        if (p.frame[(size_t)i] >= 0) continue;
-        groups.emplace_back();
-        add_copies(groups.back(), i);
-        groups.back().compute = [&, i] {
-            return convert_device(ctx, m, din + off[(size_t)i], widths[i], heights[i], (size_t)widths[i] * 4, 0, 0, dout + off[(size_t)i],
-                                  (size_t)widths[i] * 4, 0);
-        };
+    rc = prepare_planes(ctx, steps, ends, &fd);
+    if (rc) return rc;
+    std::vector<HostGroup> groups;
+    for (size_t k = 0; k <= last; k++) {
+        if (k > 0 && k < last) {
+            groups.emplace_back();
+            groups.back().compute = [&, k]() -> int {
+                begin_step(ctx, steps, k, on_step, user, true);
+                for (const PlanesUnit &u : units_of(steps[k]))
+                    if (int r = run_unit(ctx, steps[k], fd, u)) return r;
+                return W2X_OK;
+            };
+            continue;
+        }
+        const std::vector<PlanesUnit> units = units_of(steps[k]);
+        for (size_t j = 0; j < units.size(); j++) {
+            HostGroup G;
+            for (int i : units[j].planes) {
+                const size_t row = (size_t)widths[i] * 4, out_row = (size_t)L.w[(size_t)i] * 4;
+                if (k == 0) G.up.push_back({din + in_off[(size_t)i], row, in[i], in_strides[i], row, (size_t)heights[i]});
+                if (k == last) G.down.push_back({out[i], out_strides[i], dout + out_off[(size_t)i], out_row, out_row, (size_t)L.h[(size_t)i]});
+            }
+            G.compute = [&, k, j, u = units[j]] {
+                if (j == 0) begin_step(ctx, steps, k, on_step, user, true);
+                return run_unit(ctx, steps[k], fd, u);
+            };
+            groups.push_back(std::move(G));
+        }
     }
     return run_host_groups(ctx, groups);
 }
@@ -1210,7 +1357,12 @@ int w2x_convert_tiles(w2x_ctx *ctx, const w2x_model *model, const float *const *
 int w2x_convert_planes_device(w2x_ctx *ctx, const w2x_model *model, int n_planes, const float *const *d_in, const int *widths,
                               const int *heights, const size_t *in_strides, float *const *d_out, const size_t *out_strides) {
     if (check_ctx(ctx)) return W2X_ERR_ARG;
-    return convert_planes_dev(ctx, model, n_planes, d_in, widths, heights, in_strides, d_out, out_strides);
+    int rc = check_planes("w2x_convert_planes_device", model, n_planes, d_in, widths, heights, in_strides, d_out, out_strides);
+    if (rc) return rc;
+    DeviceGuard g(ctx->device);
+    if (pick_engine(ctx, model) < 0) return W2X_ERR_UNSUPPORTED;
+    std::vector<PlanesStep> steps = one_step(model, n_planes, widths, heights);
+    return planes_device(ctx, steps, d_in, in_strides, d_out, out_strides, nullptr, nullptr);
 }
 
 int w2x_convert_planes(w2x_ctx *ctx, const w2x_model *model, int n_planes, const float *const *in, const int *widths,
@@ -1219,18 +1371,33 @@ int w2x_convert_planes(w2x_ctx *ctx, const w2x_model *model, int n_planes, const
     int rc = check_planes("w2x_convert_planes", model, n_planes, in, widths, heights, in_strides, out, out_strides);
     if (rc) return rc;
     DeviceGuard g(ctx->device);
-    const int engine = pick_engine(ctx, model);
-    if (engine < 0) return W2X_ERR_UNSUPPORTED;
-    DevModel *dm = nullptr;
-    rc = get_dev_model(ctx, model, &dm);
+    if (pick_engine(ctx, model) < 0) return W2X_ERR_UNSUPPORTED;
+    std::vector<PlanesStep> steps = one_step(model, n_planes, widths, heights);
+    return planes_host(ctx, steps, in, widths, heights, in_strides, out, out_strides, nullptr, nullptr);
+}
+
+int w2x_convert_planes_chain_device(w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, int n_planes,
+                                    const float *const *d_in, const int *widths, const int *heights, const size_t *in_strides,
+                                    float *const *d_out, const size_t *out_strides, w2x_step_fn on_step, void *user) {
+    std::vector<PlanesStep> steps;
+    int rc = check_planes_chain("w2x_convert_planes_chain_device", ctx, n_steps, models, kinds, n_planes, d_in, widths, heights, in_strides,
+                                d_out, out_strides, &steps);
     if (rc) return rc;
-    if (!packs_frames(ctx, model, dm, engine)) {
-        for (int i = 0; i < n_planes && !rc; i++)
-            rc = w2x_convert_plane(ctx, model, in[i], widths[i], heights[i], in_strides[i], out[i], out_strides[i], 0);
-        return rc;
-    }
-    emit_planes_progress(ctx, model, n_planes, widths, heights, true);
-    return planes_host(ctx, model, dm, n_planes, in, widths, heights, in_strides, out, out_strides);
+    DeviceGuard g(ctx->device);
+    NvtxRange nvtx("w2x convert planes chain");
+    return planes_device(ctx, steps, d_in, in_strides, d_out, out_strides, on_step, user);
+}
+
+int w2x_convert_planes_chain(w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, int n_planes,
+                             const float *const *in, const int *widths, const int *heights, const size_t *in_strides, float *const *out,
+                             const size_t *out_strides, w2x_step_fn on_step, void *user) {
+    std::vector<PlanesStep> steps;
+    int rc = check_planes_chain("w2x_convert_planes_chain", ctx, n_steps, models, kinds, n_planes, in, widths, heights, in_strides, out,
+                                out_strides, &steps);
+    if (rc) return rc;
+    DeviceGuard g(ctx->device);
+    NvtxRange nvtx("w2x convert planes chain");
+    return planes_host(ctx, steps, in, widths, heights, in_strides, out, out_strides, on_step, user);
 }
 
 }  // extern "C"

@@ -103,8 +103,10 @@ struct PlaneRect {
     int blk0;            // first gather block: plane i owns blocks [blk0_i, blk0_i + ceil(w/32) * ceil(h/8))
 };
 // The frame's padded fp32 image (fw x fh, dense): replicate-padded planes inside the rectangles, 0 elsewhere.  One launch.
+// up2x: every rectangle's plane is the nearest-neighbour 2x resize of its src (pixel (y, x) = src[y >> 1][x >> 1]); w, h are the
+// 2x sizes and src_stride is the half-resolution plane's.
 cudaError_t launch_pack_planes(const PlaneRect *rect, const int *shelf_y0, const int *shelf_first, int n_shelf, int pad, int fw,
-                               int fh, float *frame, cudaStream_t s);
+                               int fh, bool up2x, float *frame, cudaStream_t s);
 // The fused last layer's output for every plane of the frame, from its tap partials ([fh][fw][12]).  One launch of n_blocks.
 cudaError_t launch_gather_planes(const float *partial, int fw, const PlaneRect *rect, int n_rect, int n_blocks, float bias, int pad,
                                  cudaStream_t s);

@@ -216,11 +216,12 @@ cudaError_t launch_last_gather_xy(const float *partial, int pw, int ph, float bi
 }
 
 cudaError_t launch_pack_planes(const PlaneRect *rect, const int *shelf_y0, const int *shelf_first, int n_shelf, int pad, int fw,
-                               int fh, float *frame, cudaStream_t s) {
+                               int fh, bool up2x, float *frame, cudaStream_t s) {
     if (n_shelf < 1 || fw < 1 || fh < 1) return cudaErrorInvalidValue;
     dim3 grid((fw + 31) / 32, (fh + 7) / 8);
     if (grid.y > 65535) return cudaErrorInvalidConfiguration;
-    pack_planes_kernel<<<grid, 256, 0, s>>>(rect, shelf_y0, shelf_first, n_shelf, pad, fw, fh, frame);
+    if (up2x) pack_planes_kernel<true><<<grid, 256, 0, s>>>(rect, shelf_y0, shelf_first, n_shelf, pad, fw, fh, frame);
+    else pack_planes_kernel<false><<<grid, 256, 0, s>>>(rect, shelf_y0, shelf_first, n_shelf, pad, fw, fh, frame);
     return cudaGetLastError();
 }
 

@@ -204,6 +204,9 @@ last_gather_kernel(const float *__restrict__ partial, int pw, int ph, float bias
 
 // Frame pixel (y, x) of the padded fp32 image: cv::copyMakeBorder(plane, pad, BORDER_REPLICATE) (src/convertRoutine.cpp:35)
 // inside a rectangle, 0 everywhere else.  One thread per frame pixel, 32 x 8 per block.
+// UP2X: the plane of R.w x R.h is the nearest-neighbour 2x resize of R.src (src/main.cpp:135-139), never materialised: its pixel
+// (y, x) is src[y >> 1][x >> 1], as in first_layer_kernel<..., true> and pad_upsample2x_kernel.
+template <bool UP2X>
 __global__ void __launch_bounds__(256)
 pack_planes_kernel(const PlaneRect *__restrict__ rect, const int *__restrict__ shelf_y0, const int *__restrict__ shelf_first,
                    int n_shelf, int pad, int fw, int fh, float *__restrict__ frame) {
@@ -226,7 +229,7 @@ pack_planes_kernel(const PlaneRect *__restrict__ rect, const int *__restrict__ s
     float v = 0.f;
     if (px >= 0 && py >= 0 && px < R.w + 2 * pad && py < R.h + 2 * pad) {
         const int sx = min(max(px - pad, 0), R.w - 1), sy = min(max(py - pad, 0), R.h - 1);
-        v = __ldg(R.src + (long)sy * R.src_stride + sx);
+        v = __ldg(R.src + (long)(UP2X ? sy >> 1 : sy) * R.src_stride + (UP2X ? sx >> 1 : sx));
     }
     frame[(size_t)y * fw + x] = v;
 }
