@@ -100,7 +100,9 @@ W2X_API int w2x_block_table(int width, int height, int n_model, int *table, int 
 W2X_API int w2x_ctx_create(int device, w2x_ctx **out_ctx);
 W2X_API void w2x_ctx_destroy(w2x_ctx *ctx);
 /* A context caches device copies of every model it has converted with; this drops one model's copies
- * (call before w2x_model_free when a long-lived context cycles through many models). */
+ * (call before w2x_model_free when a long-lived context cycles through many models).  Returns W2X_ERR_ARG, and keeps
+ * the copies, while band sessions on this context use the model: w2x_band_* sessions, the sub-bands of w2x_slab_*
+ * and the plan w2x_multi_convert_plane keeps for its last (model, width, height).  Destroy those first. */
 W2X_API int w2x_ctx_forget_model(w2x_ctx *ctx, const w2x_model *model);
 W2X_API int w2x_ctx_set_engine(w2x_ctx *ctx, int engine);
 W2X_API int w2x_ctx_get_engine(const w2x_ctx *ctx);

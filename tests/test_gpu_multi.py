@@ -6,7 +6,9 @@ multi-GPU runs use, only the "neighbour" lives on the same GPU (separate context
   * w2x_band_connect_local + w2x_band_run: row bands with the per-layer halo exchange done INSIDE the library through
     peer-mapped frames (one exchange kernel per layer: rows, flag, wait) reproduce the whole-plane bits;
   * w2x_multi_*: the one-process N-context driver (both in tools/multi_selftest.py, which also runs on N GPUs);
-  * w2x_band_export / w2x_band_connect: the same between PROCESSES over CUDA IPC (what bench.py's torchrun ranks do).
+  * w2x_band_export / w2x_band_connect: the same between PROCESSES over CUDA IPC.
+These are one fixed configuration per mechanism; test_band_exchange.py covers the shapes, precisions and edges (thin
+bands, odd frame widths, slab sub-band layouts, bench.py's slab export / connect path, the multi plan cache) bit for bit.
 """
 import os
 import subprocess

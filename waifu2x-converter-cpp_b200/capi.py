@@ -632,6 +632,16 @@ class Multi:
 
     def set_precision(self, precision): _check(lib().w2x_multi_set_precision(self._h, precision))
 
+    def set_log(self, fn):
+        """fn(str) receives the reference's progress lines of every call; None disables."""
+        self._log_cb = LOG_FN() if fn is None else LOG_FN(lambda line, _u: fn(line.decode()))
+        _check(lib().w2x_multi_set_log(self._h, self._log_cb, None))
+
+    def forget_model(self, model: Model):
+        """w2x_ctx_forget_model on every device's context"""
+        for i in range(lib().w2x_multi_device_count(self._h)):
+            _check(lib().w2x_ctx_forget_model(lib().w2x_multi_ctx(self._h, i), model._h))
+
     def convert_plane(self, model: Model, plane, block_splitting=True, out=None):
         x = np.ascontiguousarray(plane, np.float32)
         h, w = x.shape

@@ -519,12 +519,17 @@ static void free_dev_model(DevModel &dm) {
 }
 
 // Drops the context's device copies of a model (weights, packed operands); call it before w2x_model_free in a long-lived
-// context that cycles through many models.  The next conversion with the same model uploads it again.
+// context that cycles through many models.  The next conversion with the same model uploads it again.  Refused while band
+// sessions (w2x_band_*, the sub-bands of w2x_slab_*, the cached plan of w2x_multi_*) hold the copies: their passes launch
+// with them, and a pass cannot upload them again without stalling the neighbours that wait in the exchange kernel.
 int w2x_ctx_forget_model(w2x_ctx *ctx, const w2x_model *model) {
     if (check_ctx(ctx)) return W2X_ERR_ARG;
     if (!model) return fail(W2X_ERR_ARG, "w2x_ctx_forget_model: NULL model");
     auto it = ctx->models.find(model->uid);
     if (it == ctx->models.end()) return W2X_OK;
+    if (it->second.band_sessions > 0)
+        return fail(W2X_ERR_ARG, "w2x_ctx_forget_model: %d band session(s) on this context still use the model; destroy them first",
+                    it->second.band_sessions);
     DeviceGuard g(ctx->device);
     CU_CHECK(cudaStreamSynchronize(ctx->stream));
     free_dev_model(it->second);

@@ -60,6 +60,7 @@ constexpr uint32_t BLOB_MAGIC = 0x77327862u;   // "w2xb"
 struct BandBlob {                              // what w2x_band_export hands to the neighbour ranks
     uint32_t magic;
     int32_t pw, hf, n;
+    int32_t precision;                         // the exchanged records' format (W2X_PRECISION_*)
     uint64_t act_bytes;
     cudaIpcMemHandle_t pad, act0, act1, flags;
 };
@@ -121,6 +122,7 @@ int w2x_band_create(w2x_ctx *ctx, const w2x_model *model, int width, int band_ro
     if ((e = cudaMalloc(&b->flags, 64)) != cudaSuccess) return cleanup(e);
     if ((e = cudaMemset(b->flags, 0, 64)) != cudaSuccess) return cleanup(e);
     if ((e = cudaDeviceSynchronize()) != cudaSuccess) return cleanup(e);       // the flag words are zero before a neighbour can write them
+    b->dm->band_sessions++;                                                    // w2x_ctx_forget_model refuses until w2x_band_destroy
     *out_band = b.release();
     return W2X_OK;
 }
@@ -143,6 +145,7 @@ void w2x_band_destroy(w2x_band *band) {
         cudaFree(band->flags);
         cudaGetLastError();
     }
+    if (band->dm) band->dm->band_sessions--;
     delete band;
 }
 
@@ -257,6 +260,7 @@ int w2x_band_export(w2x_band *band, void *blob) {
     bl.pw = band->pw;
     bl.hf = band->hf;
     bl.n = band->n;
+    bl.precision = band->ctx->precision;
     bl.act_bytes = band->act_bytes;
     CU_CHECK(cudaIpcGetMemHandle(&bl.pad, band->pad));
     CU_CHECK(cudaIpcGetMemHandle(&bl.act0, band->act[0]));
@@ -276,8 +280,8 @@ int w2x_band_connect(w2x_band *band, const void *up_blob, const void *down_blob)
         if (!blobs[side]) continue;
         BandBlob bl;
         std::memcpy(&bl, blobs[side], sizeof bl);
-        if (bl.magic != BLOB_MAGIC || bl.pw != band->pw || bl.n != band->n || bl.hf < 3)
-            return fail(W2X_ERR_ARG, "w2x_band_connect: the %s neighbour's session does not match (width / model)", side ? "down" : "up");
+        if (bl.magic != BLOB_MAGIC || bl.pw != band->pw || bl.n != band->n || bl.precision != band->ctx->precision || bl.hf < 3)
+            return fail(W2X_ERR_ARG, "w2x_band_connect: the %s neighbour's session does not match (width / model / precision)", side ? "down" : "up");
         w2x_band::Peer &p = band->peer[side];
         void *q = nullptr;
         CU_CHECK(cudaIpcOpenMemHandle(&q, bl.pad, cudaIpcMemLazyEnablePeerAccess));

@@ -29,6 +29,7 @@ struct DevModel {                       // device-resident copy of one model
     std::vector<uint8_t *> pack8;       // same for the "f8" flavour (fp16 main product + e4m3 corrections)
     std::vector<float> out_scale;       // 1 / (wscale * ACT_SCALE)
     std::vector<float> last_w_t;        // HOST: last layer's weights transposed to [9][Cin] (fused last layer, passed as kernel parameters)
+    int band_sessions = 0;              // live w2x_band sessions that launch with these copies (w2x_ctx_forget_model refuses while > 0)
 };
 
 struct TimedSpan { int layer; cudaEvent_t e0, e1; };
