@@ -1029,12 +1029,6 @@ int check_planes(const char *fn, const w2x_model *m, int n_planes, const float *
     return W2X_OK;
 }
 
-// The lines of the whole call, plane by plane, as the single-plane entry point prints them with block_splitting = 0.  A packed
-// plane's padded rectangle fits the scratch limit and MAX_FRAME_ROWS (plan_planes), so it is one scratch band: its lines come once.
-void emit_planes_progress(w2x_ctx *ctx, const w2x_model *m, int n_planes, const int *widths, const int *heights, bool host) {
-    for (int i = 0; i < n_planes; i++) emit_plane_progress(ctx, m, widths[i], heights[i], 0, host);
-}
-
 struct PlanesPlan {
     std::vector<int> frame, x0, y0, fw, fh;
     int n_frames = 0;
@@ -1055,9 +1049,10 @@ std::vector<FramePlan> frames_for(const PlanesPlan &p) {
     return frames;
 }
 
-// One step of a planes call: every plane through one model, after the nearest 2x resize when `up`.
+// One step of a chain (w2x_convert_chain*, w2x_convert_planes*): every plane through one model, after the nearest 2x resize when
+// `up`.  A single-plane chain is a collection of one plane.
 struct PlaneIO { const float *src; size_t src_stride; float *dst; size_t dst_stride; };   // row strides in bytes
-struct PlanesStep {
+struct Step {
     const w2x_model *m;
     bool up;
     std::vector<int> w, h;              // the step's output sizes
@@ -1068,20 +1063,32 @@ struct PlanesStep {
     std::vector<PlaneIO> io;            // each plane's source and destination at this step
 };
 
-std::vector<PlanesStep> one_step(const w2x_model *m, int n_planes, const int *widths, const int *heights) {
-    std::vector<PlanesStep> steps(1, PlanesStep{});
-    steps[0].m = m;
-    steps[0].up = false;
-    steps[0].w.assign(widths, widths + n_planes);
-    steps[0].h.assign(heights, heights + n_planes);
+// The steps of checked arguments, each with its output size per plane.
+std::vector<Step> step_table(int n_steps, const w2x_model *const *models, const int *kinds, int n_planes, const int *widths, const int *heights) {
+    std::vector<int> w(widths, widths + n_planes), h(heights, heights + n_planes);
+    std::vector<Step> steps((size_t)n_steps);
+    for (int k = 0; k < n_steps; k++) {
+        Step &s = steps[(size_t)k];
+        s.m = models[k];
+        s.up = kinds[k] == W2X_STEP_UPSCALE2X;
+        if (s.up)
+            for (int i = 0; i < n_planes; i++) w[(size_t)i] *= 2, h[(size_t)i] *= 2;
+        s.w = w;
+        s.h = h;
+    }
     return steps;
 }
 
-// Every argument of w2x_convert_planes_chain*, before anything is printed, allocated or queued: W2X_ERR_ARG naming the step or the
-// plane it concerns, W2X_ERR_UNSUPPORTED naming the step whose model the engine refuses.
-int check_planes_chain(const char *fn, w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, int n_planes,
-                       const float *const *in, const int *widths, const int *heights, const size_t *in_strides, float *const *out,
-                       const size_t *out_strides, std::vector<PlanesStep> *steps) {
+std::vector<Step> one_step(const w2x_model *m, int n_planes, const int *widths, const int *heights) {
+    const int same = W2X_STEP_SAME;
+    return step_table(1, &m, &same, n_planes, widths, heights);
+}
+
+// Every argument of a chain call, before anything is printed, allocated or queued, in this order: the step arrays (W2X_ERR_ARG
+// naming the step); the caller's planes, by check_planes(number of 2x steps); each step's engine (W2X_ERR_UNSUPPORTED naming the
+// step) and, with block_splitting, its literal walk on every plane (W2X_ERR_ARG naming the step).  Then *steps is the step table.
+int check_steps(const char *fn, w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, int n_planes, const int *widths,
+                const int *heights, int block_splitting, const std::function<int(int)> &check_planes, std::vector<Step> *steps) {
     if (check_ctx(ctx)) return W2X_ERR_ARG;
     if (n_steps < 1) return fail(W2X_ERR_ARG, "%s: n_steps is %d: at least one step (step 0) is needed", fn, n_steps);
     if (!models) return fail(W2X_ERR_ARG, "%s: step 0: NULL models array", fn);
@@ -1096,32 +1103,36 @@ int check_planes_chain(const char *fn, w2x_ctx *ctx, int n_steps, const w2x_mode
             return fail(W2X_ERR_ARG, "%s: step %d: model must map 1 plane to 1 plane", fn, k);
         if (kinds[k] == W2X_STEP_UPSCALE2X) u++;
     }
-    int rc = check_plane_arrays(fn, n_planes, in, widths, heights, in_strides, out, out_strides, u);
+    int rc = check_planes(u);
     if (rc) return rc;
-    for (int k = 0; k < n_steps; k++)
-        if (pick_engine(ctx, models[k]) < 0) {
+    *steps = step_table(n_steps, models, kinds, n_planes, widths, heights);
+    for (int k = 0; k < n_steps; k++) {   // engine choice (the tensor-core engine needs a 1->{32,64,128}...->1 chain), literal walk
+        const Step &s = (*steps)[(size_t)k];
+        rc = pick_engine(ctx, s.m) < 0 ? W2X_ERR_UNSUPPORTED : W2X_OK;
+        for (int i = 0; i < n_planes && !rc; i++) rc = check_blocks(ctx, (int)s.m->layers.size(), s.w[(size_t)i], s.h[(size_t)i], block_splitting);
+        if (rc) {
             const std::string why = w2x_last_error();
-            return fail(W2X_ERR_UNSUPPORTED, "%s: step %d: %s", fn, k, why.c_str());
+            return fail(rc, "%s: step %d: %s", fn, k, why.c_str());
         }
-    std::vector<int> w(widths, widths + n_planes), h(heights, heights + n_planes);
-    steps->assign((size_t)n_steps, PlanesStep{});
-    for (int k = 0; k < n_steps; k++) {
-        PlanesStep &s = (*steps)[(size_t)k];
-        s.m = models[k];
-        s.up = kinds[k] == W2X_STEP_UPSCALE2X;
-        if (s.up)
-            for (int i = 0; i < n_planes; i++) w[(size_t)i] *= 2, h[(size_t)i] *= 2;
-        s.w = w;
-        s.h = h;
     }
     return W2X_OK;
 }
 
+// Every argument of w2x_convert_planes_chain*: the steps, and the planes by check_plane_arrays (W2X_ERR_ARG naming the plane).
+int check_planes_chain(const char *fn, w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, int n_planes,
+                       const float *const *in, const int *widths, const int *heights, const size_t *in_strides, float *const *out,
+                       const size_t *out_strides, std::vector<Step> *steps) {
+    return check_steps(fn, ctx, n_steps, models, kinds, n_planes, widths, heights, 0, [&](int u) {
+        return check_plane_arrays(fn, n_planes, in, widths, heights, in_strides, out, out_strides, u);
+    }, steps);
+}
+
 // Everything before the first copy or launch: the models on the device; where each plane comes from and goes to at each step (step
-// 0 reads ends[i].src, the last step writes ends[i].dst, step k < last writes its outputs densely into chain_buf[k & 1]); each
-// packed step's frame plan, made on its OUTPUT sizes, so that a plane may pack at one step and be converted alone after a 2x step;
-// the intermediate buffers and the frame scratch; then ONE upload of every step's frame tables, so that no step waits for the host.
-int prepare_planes(w2x_ctx *ctx, std::vector<PlanesStep> &steps, const std::vector<PlaneIO> &ends, std::vector<FrameDev> *fd) {
+// 0 reads ends[i].src, the last step writes ends[i].dst, step k < last writes its outputs densely into chain_buf[k & 1]); with
+// `pack`, each step that packs_frames allows is planned into frames on its OUTPUT sizes, so that a plane may pack at one step and be
+// converted alone after a 2x step (without, every plane is converted alone); the intermediate buffers and the frame scratch; then ONE
+// upload of every step's frame tables, so that no step waits for the host.
+int prepare_planes(w2x_ctx *ctx, std::vector<Step> &steps, const std::vector<PlaneIO> &ends, bool pack, std::vector<FrameDev> *fd) {
     const size_t n_planes = ends.size(), last = steps.size() - 1;
     size_t need[2] = {0, 0};
     for (size_t k = 0; k < last; k++) {
@@ -1136,10 +1147,10 @@ int prepare_planes(w2x_ctx *ctx, std::vector<PlanesStep> &steps, const std::vect
     }
     std::vector<FramePlan> frames;
     for (size_t k = 0; k <= last; k++) {
-        PlanesStep &s = steps[k];
+        Step &s = steps[k];
         int rc = get_dev_model(ctx, s.m, &s.dm);
         if (rc) return rc;
-        s.packed = packs_frames(ctx, s.m, s.dm, pick_engine(ctx, s.m));
+        s.packed = pack && packs_frames(ctx, s.m, s.dm, pick_engine(ctx, s.m));
         s.io.resize(n_planes);
         size_t off = 0;
         for (size_t i = 0; i < n_planes; i++) {
@@ -1166,11 +1177,10 @@ int prepare_planes(w2x_ctx *ctx, std::vector<PlanesStep> &steps, const std::vect
     return frames.empty() ? W2X_OK : upload_frames(ctx, frames, fd);
 }
 
-// A unit of work of one step: one packed frame (n + 1 launches for all its planes), or one plane converted alone by the single-plane
-// step code of w2x_convert_chain (too large to pack, or a step that does not pack).  A step's units: its frames, then its other
-// planes, each in order.
+// A unit of work of one step: one packed frame (n + 1 launches for all its planes), or one plane converted alone by convert_device
+// (too large to pack, or a step that does not pack).  A step's units: its frames, then its other planes, each in order.
 struct PlanesUnit { int frame; std::vector<int> planes; };
-std::vector<PlanesUnit> units_of(const PlanesStep &s) {
+std::vector<PlanesUnit> units_of(const Step &s) {
     std::vector<PlanesUnit> units;
     const int n_planes = (int)s.w.size();
     if (s.packed) {
@@ -1184,11 +1194,11 @@ std::vector<PlanesUnit> units_of(const PlanesStep &s) {
     return units;
 }
 
-int run_unit(w2x_ctx *ctx, const PlanesStep &s, const std::vector<FrameDev> &fd, const PlanesUnit &u) {
+int run_unit(w2x_ctx *ctx, const Step &s, const std::vector<FrameDev> &fd, const PlanesUnit &u, int block_splitting) {
     if (u.frame < 0) {
         const int i = u.planes[0];
         const PlaneIO &p = s.io[(size_t)i];
-        return convert_device(ctx, s.m, p.src, s.w[(size_t)i], s.h[(size_t)i], p.src_stride, 0, 0, p.dst, p.dst_stride, 0, s.up);
+        return convert_device(ctx, s.m, p.src, s.w[(size_t)i], s.h[(size_t)i], p.src_stride, 0, 0, p.dst, p.dst_stride, block_splitting, s.up);
     }
     const size_t f = s.f0 + (size_t)u.frame;
     int rc = run_packed_frame(ctx, s.m, s.dm, fd[f], s.up);
@@ -1198,34 +1208,42 @@ int run_unit(w2x_ctx *ctx, const PlanesStep &s, const std::vector<FrameDev> &fd,
     return W2X_OK;
 }
 
-// on_step(k), then the lines the planes entry point prints for the step's (resized) planes.
-void begin_step(w2x_ctx *ctx, const std::vector<PlanesStep> &steps, size_t k, w2x_step_fn on_step, void *user, bool host) {
+// on_step(k), then the step's (resized) planes' lines, plane by plane, as the single-plane entry point prints them.  A packed
+// plane's padded rectangle fits the scratch limit and MAX_FRAME_ROWS (plan_planes), so it is one scratch band: its lines come once.
+void begin_step(w2x_ctx *ctx, const std::vector<Step> &steps, size_t k, int block_splitting, w2x_step_fn on_step, void *user, bool host) {
     if (on_step) on_step((int)k, user);
-    const PlanesStep &s = steps[k];
-    emit_planes_progress(ctx, s.m, (int)s.w.size(), s.w.data(), s.h.data(), host);
+    const Step &s = steps[k];
+    for (size_t i = 0; i < s.w.size(); i++) emit_plane_progress(ctx, s.m, s.w[i], s.h[i], block_splitting, host);
 }
 
-// Device planes, checked: the steps in order on the context's stream.
-int planes_device(w2x_ctx *ctx, std::vector<PlanesStep> &steps, const float *const *d_in, const size_t *in_strides, float *const *d_out,
-                  const size_t *out_strides, w2x_step_fn on_step, void *user) {
+// Steps [k0, k1) of prepared steps, in order on the context's stream.
+int run_steps(w2x_ctx *ctx, const std::vector<Step> &steps, const std::vector<FrameDev> &fd, size_t k0, size_t k1, int block_splitting,
+              w2x_step_fn on_step, void *user, bool host) {
+    for (size_t k = k0; k < k1; k++) {
+        begin_step(ctx, steps, k, block_splitting, on_step, user, host);
+        for (const PlanesUnit &u : units_of(steps[k]))
+            if (int rc = run_unit(ctx, steps[k], fd, u, block_splitting)) return rc;
+    }
+    return W2X_OK;
+}
+
+// Device planes, checked: the steps in order on the context's stream (pack: see prepare_planes).
+int planes_device(w2x_ctx *ctx, std::vector<Step> &steps, const float *const *d_in, const size_t *in_strides, float *const *d_out,
+                  const size_t *out_strides, bool pack, int block_splitting, w2x_step_fn on_step, void *user) {
     std::vector<PlaneIO> ends(steps[0].w.size());
     for (size_t i = 0; i < ends.size(); i++) ends[i] = PlaneIO{d_in[i], in_strides[i], d_out[i], out_strides[i]};
     std::vector<FrameDev> fd;
-    int rc = prepare_planes(ctx, steps, ends, &fd);
-    for (size_t k = 0; k < steps.size() && !rc; k++) {
-        begin_step(ctx, steps, k, on_step, user, false);
-        for (const PlanesUnit &u : units_of(steps[k]))
-            if ((rc = run_unit(ctx, steps[k], fd, u))) break;
-    }
-    return rc;
+    int rc = prepare_planes(ctx, steps, ends, pack, &fd);
+    if (rc) return rc;
+    return run_steps(ctx, steps, fd, 0, steps.size(), block_splitting, on_step, user, false);
 }
 
 // Host planes, checked: dense device staging, inputs in io_buf[0] and outputs in io_buf[1], and ONE run of the copy pipeline.  Each
 // unit of step 0 is a group carrying its planes' uploads, each step between the first and the last one compute-only group, each unit
 // of the last step a group carrying its planes' downloads: uploads overlap the first step and downloads the last.
-int planes_host(w2x_ctx *ctx, std::vector<PlanesStep> &steps, const float *const *in, const int *widths, const int *heights,
+int planes_host(w2x_ctx *ctx, std::vector<Step> &steps, const float *const *in, const int *widths, const int *heights,
                 const size_t *in_strides, float *const *out, const size_t *out_strides, w2x_step_fn on_step, void *user) {
-    const PlanesStep &L = steps.back();
+    const Step &L = steps.back();
     const size_t n_planes = L.w.size(), last = steps.size() - 1;
     std::vector<size_t> in_off(n_planes + 1, 0), out_off(n_planes + 1, 0);
     for (size_t i = 0; i < n_planes; i++) {
@@ -1239,18 +1257,13 @@ int planes_host(w2x_ctx *ctx, std::vector<PlanesStep> &steps, const float *const
     std::vector<PlaneIO> ends(n_planes);
     for (size_t i = 0; i < n_planes; i++) ends[i] = PlaneIO{din + in_off[i], (size_t)widths[i] * 4, dout + out_off[i], (size_t)L.w[i] * 4};
     std::vector<FrameDev> fd;
-    rc = prepare_planes(ctx, steps, ends, &fd);
+    rc = prepare_planes(ctx, steps, ends, true, &fd);
     if (rc) return rc;
     std::vector<HostGroup> groups;
     for (size_t k = 0; k <= last; k++) {
         if (k > 0 && k < last) {
             groups.emplace_back();
-            groups.back().compute = [&, k]() -> int {
-                begin_step(ctx, steps, k, on_step, user, true);
-                for (const PlanesUnit &u : units_of(steps[k]))
-                    if (int r = run_unit(ctx, steps[k], fd, u)) return r;
-                return W2X_OK;
-            };
+            groups.back().compute = [&, k] { return run_steps(ctx, steps, fd, k, k + 1, 0, on_step, user, true); };
             continue;
         }
         const std::vector<PlanesUnit> units = units_of(steps[k]);
@@ -1262,8 +1275,8 @@ int planes_host(w2x_ctx *ctx, std::vector<PlanesStep> &steps, const float *const
                 if (k == last) G.down.push_back({out[i], out_strides[i], dout + out_off[(size_t)i], out_row, out_row, (size_t)L.h[(size_t)i]});
             }
             G.compute = [&, k, j, u = units[j]] {
-                if (j == 0) begin_step(ctx, steps, k, on_step, user, true);
-                return run_unit(ctx, steps[k], fd, u);
+                if (j == 0) begin_step(ctx, steps, k, 0, on_step, user, true);
+                return run_unit(ctx, steps[k], fd, u, 0);
             };
             groups.push_back(std::move(G));
         }
@@ -1366,8 +1379,8 @@ int w2x_convert_planes_device(w2x_ctx *ctx, const w2x_model *model, int n_planes
     if (rc) return rc;
     DeviceGuard g(ctx->device);
     if (pick_engine(ctx, model) < 0) return W2X_ERR_UNSUPPORTED;
-    std::vector<PlanesStep> steps = one_step(model, n_planes, widths, heights);
-    return planes_device(ctx, steps, d_in, in_strides, d_out, out_strides, nullptr, nullptr);
+    std::vector<Step> steps = one_step(model, n_planes, widths, heights);
+    return planes_device(ctx, steps, d_in, in_strides, d_out, out_strides, true, 0, nullptr, nullptr);
 }
 
 int w2x_convert_planes(w2x_ctx *ctx, const w2x_model *model, int n_planes, const float *const *in, const int *widths,
@@ -1377,26 +1390,26 @@ int w2x_convert_planes(w2x_ctx *ctx, const w2x_model *model, int n_planes, const
     if (rc) return rc;
     DeviceGuard g(ctx->device);
     if (pick_engine(ctx, model) < 0) return W2X_ERR_UNSUPPORTED;
-    std::vector<PlanesStep> steps = one_step(model, n_planes, widths, heights);
+    std::vector<Step> steps = one_step(model, n_planes, widths, heights);
     return planes_host(ctx, steps, in, widths, heights, in_strides, out, out_strides, nullptr, nullptr);
 }
 
 int w2x_convert_planes_chain_device(w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, int n_planes,
                                     const float *const *d_in, const int *widths, const int *heights, const size_t *in_strides,
                                     float *const *d_out, const size_t *out_strides, w2x_step_fn on_step, void *user) {
-    std::vector<PlanesStep> steps;
+    std::vector<Step> steps;
     int rc = check_planes_chain("w2x_convert_planes_chain_device", ctx, n_steps, models, kinds, n_planes, d_in, widths, heights, in_strides,
                                 d_out, out_strides, &steps);
     if (rc) return rc;
     DeviceGuard g(ctx->device);
     NvtxRange nvtx("w2x convert planes chain");
-    return planes_device(ctx, steps, d_in, in_strides, d_out, out_strides, on_step, user);
+    return planes_device(ctx, steps, d_in, in_strides, d_out, out_strides, true, 0, on_step, user);
 }
 
 int w2x_convert_planes_chain(w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, int n_planes,
                              const float *const *in, const int *widths, const int *heights, const size_t *in_strides, float *const *out,
                              const size_t *out_strides, w2x_step_fn on_step, void *user) {
-    std::vector<PlanesStep> steps;
+    std::vector<Step> steps;
     int rc = check_planes_chain("w2x_convert_planes_chain", ctx, n_steps, models, kinds, n_planes, in, widths, heights, in_strides, out,
                                 out_strides, &steps);
     if (rc) return rc;
@@ -1412,129 +1425,75 @@ int w2x_convert_planes_chain(w2x_ctx *ctx, int n_steps, const w2x_model *const *
 // iterations, each a nearest-neighbour 2x resize (:132-140) followed by the scale model (:148).  The Y plane after a step depends
 // only on the Y plane before it, so the whole sequence stays on the device: intermediate planes live in ctx->chain_buf, and an
 // upscaling step reads its half-resolution source through the first layer (or the padding kernel) instead of a 2x plane.
+// The steps run as those of w2x_convert_planes_chain* on a collection of one plane that never packs into a frame: each step is one
+// convert_device call with the caller's block_splitting.
 namespace {
-struct ChainStep {
-    const w2x_model *m;
-    bool up;
-    int w, h;     // the step's OUTPUT size
-};
-
-// Every argument, before anything is queued: W2X_ERR_ARG naming the step it concerns.
+// Every argument of w2x_convert_chain*: the steps, then the plane, W2X_ERR_ARG naming the step it concerns.
 int check_chain(const char *fn, w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, const void *in, int width,
                 int height, size_t in_stride_bytes, const void *out, size_t out_stride_bytes, int block_splitting, bool host,
-                std::vector<ChainStep> *steps) {
-    if (check_ctx(ctx)) return W2X_ERR_ARG;
-    if (n_steps < 1) return fail(W2X_ERR_ARG, "%s: n_steps is %d: at least one step (step 0) is needed", fn, n_steps);
-    if (!models) return fail(W2X_ERR_ARG, "%s: step 0: NULL models array", fn);
-    if (!kinds) return fail(W2X_ERR_ARG, "%s: step 0: NULL kinds array", fn);
-    if (width < 1 || height < 1) return fail(W2X_ERR_ARG, "%s: step 0: input size %d x %d", fn, width, height);
-    if (!in) return fail(W2X_ERR_ARG, "%s: step 0: NULL input plane", fn);
-    if (in_stride_bytes % 4 || in_stride_bytes < (size_t)width * 4)
-        return fail(W2X_ERR_ARG, "%s: step 0: the input row stride must be a multiple of 4 bytes and >= width*4", fn);
-    long w = width, h = height;
-    steps->clear();
-    for (int k = 0; k < n_steps; k++) {
-        const w2x_model *m = models[k];
-        if (!m) return fail(W2X_ERR_ARG, "%s: step %d: NULL model", fn, k);
-        if (kinds[k] != W2X_STEP_SAME && kinds[k] != W2X_STEP_UPSCALE2X)
-            return fail(W2X_ERR_ARG, "%s: step %d: kind %d is neither W2X_STEP_SAME (0) nor W2X_STEP_UPSCALE2X (1)", fn, k, kinds[k]);
-        if (m->layers.front().n_in != 1 || m->layers.back().n_out != 1)
-            return fail(W2X_ERR_ARG, "%s: step %d: model must map 1 plane to 1 plane", fn, k);
-        if (kinds[k] == W2X_STEP_UPSCALE2X) {
-            w *= 2;
-            h *= 2;
-            if (w > INT_MAX || h > INT_MAX) return fail(W2X_ERR_ARG, "%s: step %d: the output size %ld x %ld overflows int", fn, k, w, h);
+                std::vector<Step> *steps) {
+    return check_steps(fn, ctx, n_steps, models, kinds, 1, &width, &height, block_splitting, [&](int) -> int {
+        if (width < 1 || height < 1) return fail(W2X_ERR_ARG, "%s: step 0: input size %d x %d", fn, width, height);
+        if (!in) return fail(W2X_ERR_ARG, "%s: step 0: NULL input plane", fn);
+        if (in_stride_bytes % 4 || in_stride_bytes < (size_t)width * 4)
+            return fail(W2X_ERR_ARG, "%s: step 0: the input row stride must be a multiple of 4 bytes and >= width*4", fn);
+        long w = width, h = height;
+        for (int k = 0; k < n_steps; k++)
+            if (kinds[k] == W2X_STEP_UPSCALE2X) {
+                w *= 2;
+                h *= 2;
+                if (w > INT_MAX || h > INT_MAX) return fail(W2X_ERR_ARG, "%s: step %d: the output size %ld x %ld overflows int", fn, k, w, h);
+            }
+        const int last = n_steps - 1;
+        if (!out) return fail(W2X_ERR_ARG, "%s: step %d: NULL output plane", fn, last);
+        if (out_stride_bytes % 4 || out_stride_bytes < (size_t)w * 4)
+            return fail(W2X_ERR_ARG, "%s: step %d: the output row stride must be a multiple of 4 bytes and >= width*4 (%ld)", fn, last, w * 4);
+        if (host) {   // device planes may alias in ways the host cannot see; host planes are checked
+            const char *i0 = static_cast<const char *>(in), *i1 = i0 + (size_t)(height - 1) * in_stride_bytes + (size_t)width * 4;
+            const char *o0 = static_cast<const char *>(out), *o1 = o0 + (size_t)(h - 1) * out_stride_bytes + (size_t)w * 4;
+            if (i0 < o1 && o0 < i1) return fail(W2X_ERR_ARG, "%s: step %d: the output plane overlaps the input plane", fn, last);
         }
-        steps->push_back(ChainStep{m, kinds[k] == W2X_STEP_UPSCALE2X, (int)w, (int)h});
-    }
-    const int last = n_steps - 1;
-    if (!out) return fail(W2X_ERR_ARG, "%s: step %d: NULL output plane", fn, last);
-    if (out_stride_bytes % 4 || out_stride_bytes < (size_t)w * 4)
-        return fail(W2X_ERR_ARG, "%s: step %d: the output row stride must be a multiple of 4 bytes and >= width*4 (%ld)", fn, last, w * 4);
-    if (host) {   // device planes may alias in ways the host cannot see; host planes are checked
-        const char *i0 = static_cast<const char *>(in), *i1 = i0 + (size_t)(height - 1) * in_stride_bytes + (size_t)width * 4;
-        const char *o0 = static_cast<const char *>(out), *o1 = o0 + (size_t)(h - 1) * out_stride_bytes + (size_t)w * 4;
-        if (i0 < o1 && o0 < i1) return fail(W2X_ERR_ARG, "%s: step %d: the output plane overlaps the input plane", fn, last);
-    }
-    for (int k = 0; k < n_steps; k++) {   // engine choice (the tensor-core engine needs a 1->{32,64,128}...->1 chain), literal walk
-        const ChainStep &s = (*steps)[(size_t)k];
-        const int rc = pick_engine(ctx, s.m) < 0 ? W2X_ERR_UNSUPPORTED : check_blocks(ctx, (int)s.m->layers.size(), s.w, s.h, block_splitting);
-        if (rc) {
-            const std::string why = w2x_last_error();
-            return fail(rc, "%s: step %d: %s", fn, k, why.c_str());
-        }
-    }
-    return W2X_OK;
+        return W2X_OK;
+    }, steps);
 }
 
-// Sizes both intermediate buffers for the whole chain before the first step is queued (step k writes chain_buf[k & 1]).
-int reserve_chain(w2x_ctx *ctx, const std::vector<ChainStep> &steps) {
-    size_t need[2] = {0, 0};
-    for (size_t k = 0; k + 1 < steps.size(); k++) need[k & 1] = std::max(need[k & 1], (size_t)steps[k].w * steps[k].h * sizeof(float));
-    for (int i = 0; i < 2; i++) {
-        if (!need[i]) continue;
-        int rc = ensure(reinterpret_cast<void **>(&ctx->chain_buf[i]), &ctx->chain_bytes[i], need[i]);
-        if (rc) return rc;
-    }
-    return W2X_OK;
-}
-
-// Steps [0, n_dev) on the device: the first reads d_in, step k writes chain_buf[k & 1], the last of the whole chain writes d_out.
-// Each prints the lines of w2x_convert_plane (host) or w2x_convert_plane_device for its plane.
-int chain_device_steps(w2x_ctx *ctx, const std::vector<ChainStep> &steps, int n_dev, const float *d_in, size_t in_stride, float *d_out,
-                       size_t out_stride, int block_splitting, w2x_step_fn on_step, void *user, bool host) {
-    const float *cur = d_in;
-    size_t cur_stride = in_stride;
-    for (int k = 0; k < n_dev; k++) {
-        const ChainStep &s = steps[(size_t)k];
-        const bool last = k + 1 == (int)steps.size();
-        float *dst = last ? d_out : ctx->chain_buf[k & 1];
-        const size_t dst_stride = last ? out_stride : (size_t)s.w * sizeof(float);
-        if (on_step) on_step(k, user);
-        emit_plane_progress(ctx, s.m, s.w, s.h, block_splitting, host);
-        int rc = convert_device(ctx, s.m, cur, s.w, s.h, cur_stride, 0, 0, dst, dst_stride, block_splitting, s.up);
-        if (rc) return rc;
-        cur = dst;
-        cur_stride = dst_stride;
-    }
-    return W2X_OK;
-}
-
-// Host planes: one upload and the first n - 1 steps on the context's stream, then the last step as groups of the copy pipeline: the
-// row bands of w2x_convert_plane's when it would cut that plane, so that the download of band i overlaps the layers of band i + 1,
-// else one.  An upscaling step's bands start on even 2x rows (the source row of a band's first row is then whole).
-int chain_host(w2x_ctx *ctx, const std::vector<ChainStep> &steps, const float *in, int width, int height, size_t in_stride_bytes, float *out,
+// Host plane, staged densely in io_buf[0] (input) and io_buf[1] (output): one upload and steps 0 ... n - 2 on the context's stream,
+// then the last step as groups of the copy pipeline: the row bands of w2x_convert_plane's when it would cut that plane, so that the
+// download of band i overlaps the layers of band i + 1, else one.  An upscaling step's bands start on even 2x rows (the source row of
+// a band's first row is then whole).
+int chain_host(w2x_ctx *ctx, std::vector<Step> &steps, const float *in, int width, int height, size_t in_stride_bytes, float *out,
                size_t out_stride_bytes, int block_splitting, w2x_step_fn on_step, void *user) {
-    const ChainStep &L = steps.back();
-    const int n_steps = (int)steps.size(), n = (int)L.m->layers.size();
+    const size_t last = steps.size() - 1;
+    const w2x_model *m = steps[last].m;
+    const bool up = steps[last].up;
+    const int n = (int)m->layers.size(), w = steps[last].w[0], h = steps[last].h[0];
+    const size_t in_dense = (size_t)width * 4;
     int rc = ensure(reinterpret_cast<void **>(&ctx->io_buf[0]), &ctx->io_bytes[0], (size_t)width * height * sizeof(float));
-    if (!rc) rc = ensure(reinterpret_cast<void **>(&ctx->io_buf[1]), &ctx->io_bytes[1], (size_t)L.w * L.h * sizeof(float));
-    if (!rc) rc = reserve_chain(ctx, steps);
+    if (!rc) rc = ensure(reinterpret_cast<void **>(&ctx->io_buf[1]), &ctx->io_bytes[1], (size_t)w * h * sizeof(float));
+    std::vector<FrameDev> fd;
+    if (!rc) rc = prepare_planes(ctx, steps, {PlaneIO{ctx->io_buf[0], in_dense, ctx->io_buf[1], (size_t)w * 4}}, false, &fd);
     if (rc) return rc;
-    const size_t in_dense = (size_t)width * 4, stage_stride = (size_t)L.w * 4;
     CU_CHECK(cudaMemcpy2DAsync(ctx->io_buf[0], in_dense, in, in_stride_bytes, in_dense, (size_t)height, cudaMemcpyHostToDevice, ctx->stream));
-    rc = chain_device_steps(ctx, steps, n_steps - 1, ctx->io_buf[0], in_dense, nullptr, 0, block_splitting, on_step, user, true);
+    rc = run_steps(ctx, steps, fd, 0, last, block_splitting, on_step, user, true);
     if (rc) {   // the upload may still read the caller's plane
         cudaStreamSynchronize(ctx->stream);
         return rc;
     }
-    const float *src = n_steps == 1 ? ctx->io_buf[0] : ctx->chain_buf[(n_steps - 2) & 1];
-    const size_t src_stride = n_steps == 1 ? in_dense : (size_t)steps[(size_t)n_steps - 2].w * 4;
-    float *dout = ctx->io_buf[1];
-    if (on_step) on_step(n_steps - 1, user);
-    emit_plane_progress(ctx, L.m, L.w, L.h, block_splitting, true);
-    const int nb = host_copy_bands(ctx, n, L.w, L.h, block_splitting);
-    auto band_y = [&](int i) { return (int)((long)L.h * i / nb) & (L.up ? ~1 : ~0); };
+    const PlaneIO io = steps[last].io[0];
+    begin_step(ctx, steps, last, block_splitting, on_step, user, true);
+    const int nb = host_copy_bands(ctx, n, w, h, block_splitting);
+    auto band_y = [&](int i) { return (int)((long)h * i / nb) & (up ? ~1 : ~0); };
     std::vector<HostGroup> groups((size_t)nb);
     for (int i = 0; i < nb; i++) {
         const int y = band_y(i), rows = band_y(i + 1) - y;
-        const float *band_src = reinterpret_cast<const float *>(reinterpret_cast<const char *>(src) + (size_t)(L.up ? y / 2 : y) * src_stride);
+        const float *band_src = reinterpret_cast<const float *>(reinterpret_cast<const char *>(io.src) + (size_t)(up ? y / 2 : y) * io.src_stride);
+        float *band_dst = io.dst + (size_t)y * w;
         groups[(size_t)i].compute = [=] {
-            return convert_device(ctx, L.m, band_src, L.w, rows, src_stride, i > 0 ? n : 0, i + 1 < nb ? n : 0, dout + (size_t)y * L.w, stage_stride,
-                                  nb > 1 ? 0 : block_splitting, L.up);
+            return convert_device(ctx, m, band_src, w, rows, io.src_stride, i > 0 ? n : 0, i + 1 < nb ? n : 0, band_dst, io.dst_stride,
+                                  nb > 1 ? 0 : block_splitting, up);
         };
-        groups[(size_t)i].down = {{reinterpret_cast<char *>(out) + (size_t)y * out_stride_bytes, out_stride_bytes, dout + (size_t)y * L.w,
-                                   stage_stride, stage_stride, (size_t)rows}};
+        groups[(size_t)i].down = {{reinterpret_cast<char *>(out) + (size_t)y * out_stride_bytes, out_stride_bytes, band_dst, io.dst_stride,
+                                   io.dst_stride, (size_t)rows}};
     }
     return run_host_groups(ctx, groups);
 }
@@ -1545,20 +1504,18 @@ extern "C" {
 int w2x_convert_chain_device(w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, const float *d_in, int width,
                              int height, size_t in_stride_bytes, float *d_out, size_t out_stride_bytes, int block_splitting,
                              w2x_step_fn on_step, void *user) {
-    std::vector<ChainStep> steps;
+    std::vector<Step> steps;
     int rc = check_chain("w2x_convert_chain_device", ctx, n_steps, models, kinds, d_in, width, height, in_stride_bytes, d_out, out_stride_bytes,
                          block_splitting, false, &steps);
     if (rc) return rc;
     DeviceGuard g(ctx->device);
     NvtxRange nvtx("w2x convert chain");
-    rc = reserve_chain(ctx, steps);
-    if (rc) return rc;
-    return chain_device_steps(ctx, steps, n_steps, d_in, in_stride_bytes, d_out, out_stride_bytes, block_splitting, on_step, user, false);
+    return planes_device(ctx, steps, &d_in, &in_stride_bytes, &d_out, &out_stride_bytes, false, block_splitting, on_step, user);
 }
 
 int w2x_convert_chain(w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, const float *in, int width, int height,
                       size_t in_stride_bytes, float *out, size_t out_stride_bytes, int block_splitting, w2x_step_fn on_step, void *user) {
-    std::vector<ChainStep> steps;
+    std::vector<Step> steps;
     int rc = check_chain("w2x_convert_chain", ctx, n_steps, models, kinds, in, width, height, in_stride_bytes, out, out_stride_bytes,
                          block_splitting, true, &steps);
     if (rc) return rc;
