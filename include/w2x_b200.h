@@ -310,6 +310,20 @@ W2X_API int w2x_convert_planes_device(w2x_ctx *ctx, const w2x_model *model, int 
  * HOST buffers, synchronous. */
 #define W2X_STEP_SAME 0        /* the model's output replaces the plane (noise pass, src/main.cpp:96) */
 #define W2X_STEP_UPSCALE2X 1   /* cv::resize INTER_NEAREST to 2w x 2h (src/main.cpp:132-140), then the model (:148) */
+/* Test-time augmentation, OR-ed into a step's kind (valid kinds: 0, 1, 4, 5): average the step over the 8 flips / transposes of its
+ * plane(s), the "-tta" switch of later waifu2x front ends.  It damps the orientation bias of the SRCNN output (ringing along edges)
+ * at 8x the layer work.  Variant j = 0..7 of a w x h plane X, with t = bit 2, fy = bit 1 and fx = bit 0 of j, is W' x H' =
+ * (t ? h : w) x (t ? w : h) and V_j[y][x] = X[r][c], x' = fx ? W'-1-x : x, y' = fy ? H'-1-y : y, (r, c) = t ? (x', y') : (y', x');
+ * V_0 = X.  The step maps P to (((O_0 + O_1) + O_2) + ... + O_7) * 0.125f in fp32, left to right, where O_j is
+ * convertWithModels(models[k], V_j(U_k(P))) carried back through the same index map (out[r][c] = O_j[y][x]).  Every O_j is
+ * bit-identical to w2x_convert_plane(block_splitting = 0) on V_j(U_k(P)) on the same context settings, so the step is bit-identical
+ * to 8 such calls and an fp32 sum in that order.  The nearest 2x resize commutes with every V_j, so an upscaling TTA step
+ * transforms the half-resolution plane and never builds the 2x one.  w2x_convert_planes_chain* packs the 8n variants of its n
+ * planes into frames; w2x_convert_chain* converts each variant alone with the caller's block_splitting.  A TTA step logs the lines
+ * of the same step without the flag, and launches what the plain step launches on the 8n variant planes, plus 2 (building the
+ * variants, and the mean).  Its buffers (the 8 variants of every plane, their 8 outputs, the frame scratch) are reserved before
+ * the first copy or launch, like every other buffer of the call. */
+#define W2X_STEP_TTA 4
 typedef void (*w2x_step_fn)(int step, void *user);
 W2X_API int w2x_convert_chain(w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds,
                               const float *in, int width, int height, size_t in_stride_bytes,

@@ -18,7 +18,7 @@ _LIB_PATH = os.path.join(_HERE, "libw2x_b200.so")
 ENGINE_AUTO, ENGINE_FP32, ENGINE_TC = 0, 1, 2
 PRECISION_F16X3, PRECISION_F16_F8X2, PRECISION_F16 = 0, 1, 2
 WALK_FUSED, WALK_BLOCKS = 0, 1
-STEP_SAME, STEP_UPSCALE2X = 0, 1
+STEP_SAME, STEP_UPSCALE2X, STEP_TTA = 0, 1, 4
 
 STATUS = {0: "W2X_OK", 1: "W2X_ERR_ARG", 2: "W2X_ERR_IO", 3: "W2X_ERR_PARSE", 4: "W2X_ERR_MODEL",
           5: "W2X_ERR_CUDA", 6: "W2X_ERR_NO_DEVICE", 7: "W2X_ERR_UNSUPPORTED", 8: "W2X_ERR_NOMEM"}
@@ -453,16 +453,18 @@ class Context:
     # the reference's noise pass and 2x scale iterations on one plane (src/main.cpp:82-156), kept on the device between steps
     @staticmethod
     def _chain_args(steps, on_step):
-        steps = list(steps)
+        """steps: (model, upscale) pairs or (model, upscale, tta) triples"""
+        steps = [(s[0], bool(s[1]), bool(s[2]) if len(s) > 2 else False) for s in steps]
         n = len(steps)
-        models = (C.c_void_p * max(n, 1))(*[m._h if m is not None else None for m, _ in steps])
-        kinds = (C.c_int * max(n, 1))(*[STEP_UPSCALE2X if up else STEP_SAME for _, up in steps])
+        models = (C.c_void_p * max(n, 1))(*[m._h if m is not None else None for m, _, _ in steps])
+        kinds = (C.c_int * max(n, 1))(*[(STEP_UPSCALE2X if up else STEP_SAME) | (STEP_TTA if tta else 0) for _, up, tta in steps])
         cb = STEP_FN(lambda k, _u: on_step(k)) if on_step is not None else STEP_FN()
-        ups = sum(1 for _, up in steps if up)
+        ups = sum(1 for _, up, _ in steps if up)
         return n, models, kinds, cb, ups
 
     def convert_chain(self, steps, plane, out=None, block_splitting=True, on_step=None):
-        """steps: list of (model, upscale) pairs -- upscale=True resizes the plane to 2w x 2h (nearest) before the model.
+        """steps: list of (model, upscale) pairs -- upscale=True resizes the plane to 2w x 2h (nearest) before the model -- or
+        (model, upscale, tta) triples -- tta=True averages the step over the plane's 8 flips and transposes (W2X_STEP_TTA).
         plane: 2-D float32 array (a row-strided view is passed as it is) -> the last step's plane, (h << u) x (w << u) for u upscaling
         steps; `out` may be such an array (strided views included), written in place.  on_step(k) is called before step k."""
         x = np.asarray(plane, np.float32)
@@ -490,7 +492,7 @@ class Context:
 
     # convert_chain for every plane of a convert_planes collection, each step packing the planes into frames
     def convert_planes_chain(self, steps, planes, out=None, on_step=None):
-        """steps: (model, upscale) pairs as in convert_chain; planes: 2-D float32 arrays as in convert_planes -> list of outputs,
+        """steps: (model, upscale) pairs or (model, upscale, tta) triples as in convert_chain; planes: 2-D float32 arrays as in convert_planes -> list of outputs,
         plane i (h << u) x (w << u) for u upscaling steps; `out` may be a list of such arrays (strided views included), written in
         place.  on_step(k) is called before step k."""
         n, models, kinds, cb, ups = self._chain_args(steps, on_step)

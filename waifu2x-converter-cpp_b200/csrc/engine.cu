@@ -546,6 +546,7 @@ void w2x_ctx_destroy(w2x_ctx *ctx) {
         cudaFree(ctx->buf[i]);
         cudaFree(ctx->io_buf[i]);
         cudaFree(ctx->chain_buf[i]);
+        cudaFree(ctx->tta_buf[i]);
     }
     cudaFree(ctx->pad_buf);
     cudaFree(ctx->plan_buf);
@@ -875,9 +876,11 @@ struct FrameDev {                   // the same frame with its table in ctx->pla
 };
 
 // Puts each frame's rectangles in shelf order, numbers their gather blocks and uploads all tables in ONE copy on the context's
-// stream.  The copy waits for the kernels of an earlier call that still read the buffer (plan_ev), and its source is pageable
-// memory, so it is staged before cudaMemcpyAsync returns and the host vectors may go at once.
-int upload_frames(w2x_ctx *ctx, std::vector<FramePlan> &frames, std::vector<FrameDev> *out) {
+// stream, `tta` (the tables of the TTA kernels, at *tta_dev) after them.  The copy waits for the kernels of an earlier call that still
+// read the buffer (plan_ev), and its source is pageable memory, so it is staged before cudaMemcpyAsync returns and the host vectors
+// may go at once.
+int upload_frames(w2x_ctx *ctx, std::vector<FramePlan> &frames, std::vector<FrameDev> *out, const std::vector<TtaPlane> &tta = {},
+                  const TtaPlane **tta_dev = nullptr) {
     auto align = [](size_t b) { return (b + 15) & ~(size_t)15; };
     std::vector<char> blob;
     std::vector<size_t> off_rect, off_shelf;
@@ -910,11 +913,17 @@ int upload_frames(w2x_ctx *ctx, std::vector<FramePlan> &frames, std::vector<Fram
         std::memcpy(blob.data() + off_shelf.back(), sy.data(), sy.size() * sizeof(int));
         std::memcpy(blob.data() + off_shelf.back() + sy.size() * sizeof(int), sf.data(), sf.size() * sizeof(int));
     }
+    const size_t off_tta = align(blob.size());
+    if (!tta.empty()) {
+        blob.resize(off_tta + tta.size() * sizeof(TtaPlane));
+        std::memcpy(blob.data() + off_tta, tta.data(), tta.size() * sizeof(TtaPlane));
+    }
     if (ctx->plan_ev_live) CU_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->plan_ev, 0));
     int rc = ensure(&ctx->plan_buf, &ctx->plan_bytes, blob.size());
     if (rc) return rc;
     CU_CHECK(cudaMemcpyAsync(ctx->plan_buf, blob.data(), blob.size(), cudaMemcpyHostToDevice, ctx->stream));
     const char *base = static_cast<const char *>(ctx->plan_buf);
+    if (tta_dev) *tta_dev = reinterpret_cast<const TtaPlane *>(base + off_tta);
     for (size_t f = 0; f < frames.size(); f++) {
         FrameDev &d = (*out)[f];
         d.rect = reinterpret_cast<const tc::PlaneRect *>(base + off_rect[f]);
@@ -1055,26 +1064,43 @@ struct PlaneIO { const float *src; size_t src_stride; float *dst; size_t dst_str
 struct Step {
     const w2x_model *m;
     bool up;
+    bool tta = false;                   // W2X_STEP_TTA: the model runs on the 8 variants of every plane, the mean is the output
     std::vector<int> w, h;              // the step's output sizes
     DevModel *dm = nullptr;
     bool packed = false;                // packs_frames: frames plus planes too large to pack, else every plane alone
-    PlanesPlan plan;                    // packed: each plane's frame (-1: converted alone) and place
+    PlanesPlan plan;                    // packed: each converted plane's frame (-1: converted alone) and place
     size_t f0 = 0;                      // packed: index of its frame 0 in the call's frame table
     std::vector<PlaneIO> io;            // each plane's source and destination at this step
+    // tta: the 8n planes the model converts -- variant j of plane i at 8 i + j, its output vw x vh -- with their sources in
+    // ctx->tta_buf[0] and outputs in ctx->tta_buf[1], and the tables of the variants and the mean kernel (tiles: their blocks)
+    std::vector<int> vw, vh;
+    std::vector<PlaneIO> vio;
+    const TtaPlane *vtab = nullptr, *mtab = nullptr;
+    int vtiles = 0, mtiles = 0;
+    // the planes the model converts
+    const std::vector<int> &cw() const { return tta ? vw : w; }
+    const std::vector<int> &ch() const { return tta ? vh : h; }
+    const std::vector<PlaneIO> &cio() const { return tta ? vio : io; }
 };
 
-// The steps of checked arguments, each with its output size per plane.
+// The steps of checked arguments, each with its output size per plane (and, for a TTA step, per variant).
 std::vector<Step> step_table(int n_steps, const w2x_model *const *models, const int *kinds, int n_planes, const int *widths, const int *heights) {
     std::vector<int> w(widths, widths + n_planes), h(heights, heights + n_planes);
     std::vector<Step> steps((size_t)n_steps);
     for (int k = 0; k < n_steps; k++) {
         Step &s = steps[(size_t)k];
         s.m = models[k];
-        s.up = kinds[k] == W2X_STEP_UPSCALE2X;
+        s.up = (kinds[k] & W2X_STEP_UPSCALE2X) != 0;
+        s.tta = (kinds[k] & W2X_STEP_TTA) != 0;
         if (s.up)
             for (int i = 0; i < n_planes; i++) w[(size_t)i] *= 2, h[(size_t)i] *= 2;
         s.w = w;
         s.h = h;
+        for (int i = 0; i < n_planes && s.tta; i++)
+            for (int j = 0; j < 8; j++) {
+                s.vw.push_back(j & 4 ? h[(size_t)i] : w[(size_t)i]);
+                s.vh.push_back(j & 4 ? w[(size_t)i] : h[(size_t)i]);
+            }
     }
     return steps;
 }
@@ -1097,11 +1123,12 @@ int check_steps(const char *fn, w2x_ctx *ctx, int n_steps, const w2x_model *cons
     for (int k = 0; k < n_steps; k++) {
         const w2x_model *m = models[k];
         if (!m) return fail(W2X_ERR_ARG, "%s: step %d: NULL model", fn, k);
-        if (kinds[k] != W2X_STEP_SAME && kinds[k] != W2X_STEP_UPSCALE2X)
-            return fail(W2X_ERR_ARG, "%s: step %d: kind %d is neither W2X_STEP_SAME (0) nor W2X_STEP_UPSCALE2X (1)", fn, k, kinds[k]);
+        if (kinds[k] & ~(W2X_STEP_UPSCALE2X | W2X_STEP_TTA))
+            return fail(W2X_ERR_ARG, "%s: step %d: kind %d is neither W2X_STEP_SAME (0) nor W2X_STEP_UPSCALE2X (1), each optionally | W2X_STEP_TTA (4)",
+                        fn, k, kinds[k]);
         if (m->layers.front().n_in != 1 || m->layers.back().n_out != 1)
             return fail(W2X_ERR_ARG, "%s: step %d: model must map 1 plane to 1 plane", fn, k);
-        if (kinds[k] == W2X_STEP_UPSCALE2X) u++;
+        if (kinds[k] & W2X_STEP_UPSCALE2X) u++;
     }
     int rc = check_planes(u);
     if (rc) return rc;
@@ -1109,7 +1136,7 @@ int check_steps(const char *fn, w2x_ctx *ctx, int n_steps, const w2x_model *cons
     for (int k = 0; k < n_steps; k++) {   // engine choice (the tensor-core engine needs a 1->{32,64,128}...->1 chain), literal walk
         const Step &s = (*steps)[(size_t)k];
         rc = pick_engine(ctx, s.m) < 0 ? W2X_ERR_UNSUPPORTED : W2X_OK;
-        for (int i = 0; i < n_planes && !rc; i++) rc = check_blocks(ctx, (int)s.m->layers.size(), s.w[(size_t)i], s.h[(size_t)i], block_splitting);
+        for (size_t i = 0; i < s.cw().size() && !rc; i++) rc = check_blocks(ctx, (int)s.m->layers.size(), s.cw()[i], s.ch()[i], block_splitting);
         if (rc) {
             const std::string why = w2x_last_error();
             return fail(rc, "%s: step %d: %s", fn, k, why.c_str());
@@ -1132,20 +1159,34 @@ int check_planes_chain(const char *fn, w2x_ctx *ctx, int n_steps, const w2x_mode
 // `pack`, each step that packs_frames allows is planned into frames on its OUTPUT sizes, so that a plane may pack at one step and be
 // converted alone after a 2x step (without, every plane is converted alone); the intermediate buffers and the frame scratch; then ONE
 // upload of every step's frame tables, so that no step waits for the host.
+// A TTA step converts the 8n variant planes instead (variant j of plane i: 8 i + j), dense in tta_buf[0] (an upscaling step's
+// variants are those of its half-resolution sources: the nearest 2x resize commutes with every flip and transpose) with their outputs
+// dense in tta_buf[1]; with `pack` those are what its frames are planned on.  Its kernel tables go up with the frame tables.
 int prepare_planes(w2x_ctx *ctx, std::vector<Step> &steps, const std::vector<PlaneIO> &ends, bool pack, std::vector<FrameDev> *fd) {
     const size_t n_planes = ends.size(), last = steps.size() - 1;
-    size_t need[2] = {0, 0};
-    for (size_t k = 0; k < last; k++) {
+    size_t need[2] = {0, 0}, tta_need[2] = {0, 0};
+    for (size_t k = 0; k <= last; k++) {
         size_t px = 0;
         for (size_t i = 0; i < n_planes; i++) px += (size_t)steps[k].w[i] * steps[k].h[i];
-        need[k & 1] = std::max(need[k & 1], px * sizeof(float));
+        if (k < last) need[k & 1] = std::max(need[k & 1], px * sizeof(float));
+        if (steps[k].tta) {
+            tta_need[0] = std::max(tta_need[0], 8 * (steps[k].up ? px / 4 : px) * sizeof(float));
+            tta_need[1] = std::max(tta_need[1], 8 * px * sizeof(float));
+        }
     }
     for (int i = 0; i < 2; i++) {
         if (!need[i]) continue;
         int rc = ensure(reinterpret_cast<void **>(&ctx->chain_buf[i]), &ctx->chain_bytes[i], need[i]);
         if (rc) return rc;
     }
+    for (int i = 0; i < 2; i++) {
+        if (!tta_need[i]) continue;
+        int rc = ensure(reinterpret_cast<void **>(&ctx->tta_buf[i]), &ctx->tta_bytes[i], tta_need[i]);
+        if (rc) return rc;
+    }
     std::vector<FramePlan> frames;
+    std::vector<TtaPlane> tta;
+    std::vector<size_t> tab0(steps.size());   // a TTA step's variants table at tta[tab0], its mean table right after it
     for (size_t k = 0; k <= last; k++) {
         Step &s = steps[k];
         int rc = get_dev_model(ctx, s.m, &s.dm);
@@ -1161,28 +1202,62 @@ int prepare_planes(w2x_ctx *ctx, std::vector<Step> &steps, const std::vector<Pla
             p.dst_stride = k == last ? ends[i].dst_stride : (size_t)s.w[i] * sizeof(float);
             off += (size_t)s.w[i] * s.h[i];
         }
+        if (s.tta) {
+            auto tiles = [](int w, int h) { return ((w + 31) / 32) * ((h + 31) / 32); };
+            s.vio.resize(8 * n_planes);
+            tab0[k] = tta.size();
+            size_t in_off = 0, out_off = 0;
+            for (size_t i = 0; i < n_planes; i++) {   // the variants kernel: plane -> its 8 variants
+                const int sw = s.up ? s.w[i] / 2 : s.w[i], sh = s.up ? s.h[i] / 2 : s.h[i];
+                const size_t in_px = (size_t)sw * sh, out_px = (size_t)s.w[i] * s.h[i];
+                tta.push_back(TtaPlane{s.io[i].src, ctx->tta_buf[0] + in_off, nullptr, (long)(s.io[i].src_stride / 4), 0, sw, sh, s.vtiles});
+                s.vtiles += tiles(sw, sh);
+                for (int j = 0; j < 8; j++)
+                    s.vio[8 * i + j] = PlaneIO{ctx->tta_buf[0] + in_off + j * in_px, (size_t)(j & 4 ? sh : sw) * sizeof(float),
+                                               ctx->tta_buf[1] + out_off + j * out_px, (size_t)s.vw[8 * i + j] * sizeof(float)};
+                in_off += 8 * in_px;
+                out_off += 8 * out_px;
+            }
+            out_off = 0;
+            for (size_t i = 0; i < n_planes; i++) {   // the mean kernel: 8 variant outputs -> the step's output
+                tta.push_back(TtaPlane{nullptr, ctx->tta_buf[1] + out_off, s.io[i].dst, 0, (long)(s.io[i].dst_stride / 4), s.w[i], s.h[i], s.mtiles});
+                s.mtiles += tiles(s.w[i], s.h[i]);
+                out_off += 8 * (size_t)s.w[i] * s.h[i];
+            }
+        }
         if (!s.packed) continue;
-        plan_for(ctx, s.m, (int)n_planes, s.w.data(), s.h.data(), &s.plan);
+        const std::vector<int> &cw = s.cw(), &ch = s.ch();
+        const std::vector<PlaneIO> &cio = s.cio();
+        plan_for(ctx, s.m, (int)cw.size(), cw.data(), ch.data(), &s.plan);
         s.f0 = frames.size();
         for (FramePlan &f : frames_for(s.plan)) frames.push_back(std::move(f));
-        for (size_t i = 0; i < n_planes; i++) {
+        for (size_t i = 0; i < cw.size(); i++) {
             const int f = s.plan.frame[i];
             if (f >= 0)
-                frames[s.f0 + (size_t)f].rect.push_back(tc::PlaneRect{s.io[i].src, s.io[i].dst, (long)(s.io[i].src_stride / 4), (long)(s.io[i].dst_stride / 4),
-                                                                      s.w[i], s.h[i], s.plan.x0[i], s.plan.y0[i], 0});
+                frames[s.f0 + (size_t)f].rect.push_back(tc::PlaneRect{cio[i].src, cio[i].dst, (long)(cio[i].src_stride / 4), (long)(cio[i].dst_stride / 4),
+                                                                      cw[i], ch[i], s.plan.x0[i], s.plan.y0[i], 0});
         }
         rc = reserve_frames(ctx, frames, s.f0, frames.size(), max_channels(s.m));
         if (rc) return rc;
     }
-    return frames.empty() ? W2X_OK : upload_frames(ctx, frames, fd);
+    if (frames.empty() && tta.empty()) return W2X_OK;
+    const TtaPlane *tab = nullptr;
+    int rc = upload_frames(ctx, frames, fd, tta, &tab);
+    for (size_t k = 0; k <= last && !rc; k++)
+        if (steps[k].tta) {
+            steps[k].vtab = tab + tab0[k];
+            steps[k].mtab = tab + tab0[k] + n_planes;
+        }
+    return rc;
 }
 
 // A unit of work of one step: one packed frame (n + 1 launches for all its planes), or one plane converted alone by convert_device
-// (too large to pack, or a step that does not pack).  A step's units: its frames, then its other planes, each in order.
+// (too large to pack, or a step that does not pack).  A step's units: its frames, then its other planes, each in order.  The planes
+// are the ones the model converts: a TTA step's variants.
 struct PlanesUnit { int frame; std::vector<int> planes; };
 std::vector<PlanesUnit> units_of(const Step &s) {
     std::vector<PlanesUnit> units;
-    const int n_planes = (int)s.w.size();
+    const int n_planes = (int)s.cw().size();
     if (s.packed) {
         units.resize((size_t)s.plan.n_frames);
         for (int f = 0; f < s.plan.n_frames; f++) units[(size_t)f].frame = f;
@@ -1196,15 +1271,34 @@ std::vector<PlanesUnit> units_of(const Step &s) {
 
 int run_unit(w2x_ctx *ctx, const Step &s, const std::vector<FrameDev> &fd, const PlanesUnit &u, int block_splitting) {
     if (u.frame < 0) {
-        const int i = u.planes[0];
-        const PlaneIO &p = s.io[(size_t)i];
-        return convert_device(ctx, s.m, p.src, s.w[(size_t)i], s.h[(size_t)i], p.src_stride, 0, 0, p.dst, p.dst_stride, block_splitting, s.up);
+        const size_t i = (size_t)u.planes[0];
+        const PlaneIO &p = s.cio()[i];
+        return convert_device(ctx, s.m, p.src, s.cw()[i], s.ch()[i], p.src_stride, 0, 0, p.dst, p.dst_stride, block_splitting, s.up);
     }
     const size_t f = s.f0 + (size_t)u.frame;
     int rc = run_packed_frame(ctx, s.m, s.dm, fd[f], s.up);
     if (rc || f + 1 < fd.size()) return rc;
     CU_CHECK(cudaEventRecord(ctx->plan_ev, ctx->stream));   // the last kernel reading the frame tables is queued
     ctx->plan_ev_live = true;
+    return W2X_OK;
+}
+
+// The launches of one prepared step, after its progress lines: its units, for a TTA step between the variants kernel and the mean
+// kernel (which reads the tables last).
+int run_step(w2x_ctx *ctx, const Step &s, const std::vector<FrameDev> &fd, int block_splitting) {
+    const int n_planes = (int)s.w.size();
+    if (s.tta) {
+        CU_CHECK(launch_tta_variants(s.vtab, n_planes, s.vtiles, ctx->stream));
+        ctx->launches++;
+    }
+    for (const PlanesUnit &u : units_of(s))
+        if (int rc = run_unit(ctx, s, fd, u, block_splitting)) return rc;
+    if (s.tta) {
+        CU_CHECK(launch_tta_mean(s.mtab, n_planes, s.mtiles, ctx->stream));
+        ctx->launches++;
+        CU_CHECK(cudaEventRecord(ctx->plan_ev, ctx->stream));
+        ctx->plan_ev_live = true;
+    }
     return W2X_OK;
 }
 
@@ -1221,8 +1315,7 @@ int run_steps(w2x_ctx *ctx, const std::vector<Step> &steps, const std::vector<Fr
               w2x_step_fn on_step, void *user, bool host) {
     for (size_t k = k0; k < k1; k++) {
         begin_step(ctx, steps, k, block_splitting, on_step, user, host);
-        for (const PlanesUnit &u : units_of(steps[k]))
-            if (int rc = run_unit(ctx, steps[k], fd, u, block_splitting)) return rc;
+        if (int rc = run_step(ctx, steps[k], fd, block_splitting)) return rc;
     }
     return W2X_OK;
 }
@@ -1240,7 +1333,8 @@ int planes_device(w2x_ctx *ctx, std::vector<Step> &steps, const float *const *d_
 
 // Host planes, checked: dense device staging, inputs in io_buf[0] and outputs in io_buf[1], and ONE run of the copy pipeline.  Each
 // unit of step 0 is a group carrying its planes' uploads, each step between the first and the last one compute-only group, each unit
-// of the last step a group carrying its planes' downloads: uploads overlap the first step and downloads the last.
+// of the last step a group carrying its planes' downloads: uploads overlap the first step and downloads the last.  A TTA step at
+// either end is one group.
 int planes_host(w2x_ctx *ctx, std::vector<Step> &steps, const float *const *in, const int *widths, const int *heights,
                 const size_t *in_strides, float *const *out, const size_t *out_strides, w2x_step_fn on_step, void *user) {
     const Step &L = steps.back();
@@ -1266,7 +1360,12 @@ int planes_host(w2x_ctx *ctx, std::vector<Step> &steps, const float *const *in, 
             groups.back().compute = [&, k] { return run_steps(ctx, steps, fd, k, k + 1, 0, on_step, user, true); };
             continue;
         }
-        const std::vector<PlanesUnit> units = units_of(steps[k]);
+        // a TTA step's variants kernel reads every plane and its mean kernel writes every output: the step is one group
+        std::vector<PlanesUnit> units(1, PlanesUnit{-1, {}});
+        if (steps[k].tta)
+            for (size_t i = 0; i < n_planes; i++) units[0].planes.push_back((int)i);
+        else
+            units = units_of(steps[k]);
         for (size_t j = 0; j < units.size(); j++) {
             HostGroup G;
             for (int i : units[j].planes) {
@@ -1276,7 +1375,7 @@ int planes_host(w2x_ctx *ctx, std::vector<Step> &steps, const float *const *in, 
             }
             G.compute = [&, k, j, u = units[j]] {
                 if (j == 0) begin_step(ctx, steps, k, 0, on_step, user, true);
-                return run_unit(ctx, steps[k], fd, u, 0);
+                return steps[k].tta ? run_step(ctx, steps[k], fd, 0) : run_unit(ctx, steps[k], fd, u, 0);
             };
             groups.push_back(std::move(G));
         }
@@ -1439,7 +1538,7 @@ int check_chain(const char *fn, w2x_ctx *ctx, int n_steps, const w2x_model *cons
             return fail(W2X_ERR_ARG, "%s: step 0: the input row stride must be a multiple of 4 bytes and >= width*4", fn);
         long w = width, h = height;
         for (int k = 0; k < n_steps; k++)
-            if (kinds[k] == W2X_STEP_UPSCALE2X) {
+            if (kinds[k] & W2X_STEP_UPSCALE2X) {
                 w *= 2;
                 h *= 2;
                 if (w > INT_MAX || h > INT_MAX) return fail(W2X_ERR_ARG, "%s: step %d: the output size %ld x %ld overflows int", fn, k, w, h);
@@ -1460,7 +1559,7 @@ int check_chain(const char *fn, w2x_ctx *ctx, int n_steps, const w2x_model *cons
 // Host plane, staged densely in io_buf[0] (input) and io_buf[1] (output): one upload and steps 0 ... n - 2 on the context's stream,
 // then the last step as groups of the copy pipeline: the row bands of w2x_convert_plane's when it would cut that plane, so that the
 // download of band i overlaps the layers of band i + 1, else one.  An upscaling step's bands start on even 2x rows (the source row of
-// a band's first row is then whole).
+// a band's first row is then whole).  A TTA last step is one group: its download waits for the mean kernel.
 int chain_host(w2x_ctx *ctx, std::vector<Step> &steps, const float *in, int width, int height, size_t in_stride_bytes, float *out,
                size_t out_stride_bytes, int block_splitting, w2x_step_fn on_step, void *user) {
     const size_t last = steps.size() - 1;
@@ -1481,6 +1580,12 @@ int chain_host(w2x_ctx *ctx, std::vector<Step> &steps, const float *in, int widt
     }
     const PlaneIO io = steps[last].io[0];
     begin_step(ctx, steps, last, block_splitting, on_step, user, true);
+    if (steps[last].tta) {   // the download follows the mean kernel, which needs every variant's whole output
+        std::vector<HostGroup> one(1);
+        one[0].compute = [&] { return run_step(ctx, steps[last], fd, block_splitting); };
+        one[0].down = {{out, out_stride_bytes, io.dst, io.dst_stride, io.dst_stride, (size_t)h}};
+        return run_host_groups(ctx, one);
+    }
     const int nb = host_copy_bands(ctx, n, w, h, block_splitting);
     auto band_y = [&](int i) { return (int)((long)h * i / nb) & (up ? ~1 : ~0); };
     std::vector<HostGroup> groups((size_t)nb);

@@ -65,6 +65,8 @@ struct w2x_ctx {
     size_t io_bytes[2] = {0, 0};
     float *chain_buf[2] = {nullptr, nullptr};   // the planes between the steps of w2x_convert_chain*
     size_t chain_bytes[2] = {0, 0};
+    float *tta_buf[2] = {nullptr, nullptr};     // a W2X_STEP_TTA step's 8 variants per plane (0) and their conversions (1)
+    size_t tta_bytes[2] = {0, 0};
     bool tc_ready = false;
     cudaStream_t copy_in = nullptr, copy_out = nullptr;   // host<->device copies of run_host_groups overlap the compute stream
     cudaEvent_t ev_in[8] = {}, ev_done[8] = {};

@@ -39,6 +39,23 @@ cudaError_t launch_copy2d(const float *in, long in_stride_floats, float *out, lo
                           cudaStream_t s);
 cudaError_t launch_conv3x3_fp32(const float *in, float *out, const float *wgt, const float *bias, int Cin, int Cout,
                                 int W, int H, cudaStream_t s);
+// Test-time augmentation (chain steps with W2X_STEP_TTA), both engines.  Variant j = 0..7 of a w x h plane X, with t = bit 2,
+// fy = bit 1 and fx = bit 0 of j, is W' x H' = (t ? h : w) x (t ? w : h) and V_j[y][x] = X[r][c], x' = fx ? W'-1-x : x,
+// y' = fy ? H'-1-y : y, (r, c) = t ? (x', y') : (y', x').  A DEVICE table of TtaPlane lists the planes of one call; each kernel
+// tiles every plane into 32 x 32 tiles, plane i owning tiles [blk0_i, blk0_i + ceil(w/32) * ceil(h/32)).
+struct TtaPlane {
+    const float *src;    // tta_variants: the plane X, row stride src_stride floats
+    float *var;          // the 8 variants (tta_variants) or their conversions (tta_mean), dense: j at var + j * w * h, W' wide
+    float *dst;          // tta_mean: the output plane, row stride dst_stride floats
+    long src_stride, dst_stride;
+    int w, h;            // X's size (tta_variants) or the output's (tta_mean)
+    int blk0;
+};
+// V_0 .. V_7 of every plane of the table.  One launch of n_tiles blocks.
+cudaError_t launch_tta_variants(const TtaPlane *tab, int n_planes, int n_tiles, cudaStream_t s);
+// dst[r][c] = (((O_0 + O_1) + O_2) + ... + O_7) * 0.125f in fp32, O_j = the variant output j at the pixel V_j maps (r, c) to.  One
+// launch of n_tiles blocks.
+cudaError_t launch_tta_mean(const TtaPlane *tab, int n_planes, int n_tiles, cudaStream_t s);
 
 // ---- kernels_tc.cu ----------------------------------------------------------------------------
 namespace tc {

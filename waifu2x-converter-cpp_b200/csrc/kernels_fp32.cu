@@ -80,6 +80,83 @@ __global__ void copy2d_kernel(const float *__restrict__ in, long in_stride, floa
     }
 }
 
+// ---- test-time augmentation: the 8 flips / transposes of a plane and the mean of their conversions ---------------------------
+// One block of 32 x 8 threads per 32 x 32 tile; both kernels stage the tile in shared memory so that the transposed variants
+// (t = 1) are read and written along rows too.  The row pitch of 33 floats keeps the column walks free of bank conflicts.
+constexpr int TTA_TILE = 32;
+
+__device__ __forceinline__ int tta_plane_of(const TtaPlane *__restrict__ tab, int n_planes, int b) {
+    int p = 0, p1 = n_planes - 1;                // the plane owning tile b
+    while (p < p1) {
+        const int mid = (p + p1 + 1) >> 1;
+        if (__ldg(&tab[mid].blk0) <= b) p = mid;
+        else p1 = mid - 1;
+    }
+    return p;
+}
+
+// Tile (r0, c0) of X: pixel (r, c) goes to V_j[fy ? h-1-r : r][fx ? w-1-c : c] (t = 0, w wide) or V_j[fy ? w-1-c : c][fx ? h-1-r : r]
+// (t = 1, h wide); a warp writes 32 consecutive columns of one variant row either way.
+__global__ void __launch_bounds__(256) tta_variants_kernel(const TtaPlane *__restrict__ tab, int n_planes) {
+    __shared__ float s[TTA_TILE][TTA_TILE + 1];
+    const TtaPlane R = tab[tta_plane_of(tab, n_planes, (int)blockIdx.x)];
+    const int lb = (int)blockIdx.x - R.blk0, tiles_x = (R.w + TTA_TILE - 1) / TTA_TILE;
+    const int r0 = lb / tiles_x * TTA_TILE, c0 = lb % tiles_x * TTA_TILE;
+    const int l = threadIdx.x & 31, q0 = threadIdx.x >> 5;
+    for (int q = q0; q < TTA_TILE; q += 8)
+        if (r0 + q < R.h && c0 + l < R.w) s[q][l] = __ldg(R.src + (long)(r0 + q) * R.src_stride + c0 + l);
+    __syncthreads();
+    const size_t plane = (size_t)R.w * R.h;
+#pragma unroll
+    for (int j = 0; j < 8; j++) {
+        const bool t = j & 4, fy = j & 2, fx = j & 1;
+        float *V = R.var + (size_t)j * plane;
+        for (int q = q0; q < TTA_TILE; q += 8) {
+            if (!t) {
+                const int r = r0 + q, c = c0 + l;
+                if (r < R.h && c < R.w) V[(size_t)(fy ? R.h - 1 - r : r) * R.w + (fx ? R.w - 1 - c : c)] = s[q][l];
+            } else {
+                const int r = r0 + l, c = c0 + q;
+                if (r < R.h && c < R.w) V[(size_t)(fy ? R.w - 1 - c : c) * R.h + (fx ? R.h - 1 - r : r)] = s[l][q];
+            }
+        }
+    }
+}
+
+// Tile (r0, c0) of the output: all 8 variant outputs' values for it are staged (each read along variant rows), then every pixel sums
+// them in the order j = 0..7 with round-to-nearest adds and scales by 0.125f (exact: a power of two).
+__global__ void __launch_bounds__(256) tta_mean_kernel(const TtaPlane *__restrict__ tab, int n_planes) {
+    __shared__ float s[8][TTA_TILE][TTA_TILE + 1];
+    const TtaPlane R = tab[tta_plane_of(tab, n_planes, (int)blockIdx.x)];
+    const int lb = (int)blockIdx.x - R.blk0, tiles_x = (R.w + TTA_TILE - 1) / TTA_TILE;
+    const int r0 = lb / tiles_x * TTA_TILE, c0 = lb % tiles_x * TTA_TILE;
+    const int l = threadIdx.x & 31, q0 = threadIdx.x >> 5;
+    const size_t plane = (size_t)R.w * R.h;
+#pragma unroll
+    for (int j = 0; j < 8; j++) {
+        const bool t = j & 4, fy = j & 2, fx = j & 1;
+        const float *O = R.var + (size_t)j * plane;
+        for (int q = q0; q < TTA_TILE; q += 8) {
+            if (!t) {
+                const int r = r0 + q, c = c0 + l;
+                if (r < R.h && c < R.w) s[j][q][l] = __ldg(O + (size_t)(fy ? R.h - 1 - r : r) * R.w + (fx ? R.w - 1 - c : c));
+            } else {
+                const int r = r0 + l, c = c0 + q;
+                if (r < R.h && c < R.w) s[j][l][q] = __ldg(O + (size_t)(fy ? R.w - 1 - c : c) * R.h + (fx ? R.h - 1 - r : r));
+            }
+        }
+    }
+    __syncthreads();
+    for (int q = q0; q < TTA_TILE; q += 8) {
+        const int r = r0 + q, c = c0 + l;
+        if (r >= R.h || c >= R.w) continue;
+        float acc = s[0][q][l];
+#pragma unroll
+        for (int j = 1; j < 8; j++) acc = __fadd_rn(acc, s[j][q][l]);
+        R.dst[(long)r * R.dst_stride + c] = __fmul_rn(acc, 0.125f);
+    }
+}
+
 // ---- the fp32 layer kernel --------------------------------------------------------------------
 constexpr int TX = 32, TY = 8;   // pixels per block (one per thread)
 constexpr int CK = 8;            // input planes staged per step
@@ -265,6 +342,18 @@ cudaError_t launch_copy2d(const float *in, long in_stride_floats, float *out, lo
                           cudaStream_t s) {
     dim3 b(32, 8);
     copy2d_kernel<<<grid2d(w, h, b), b, 0, s>>>(in, in_stride_floats, out, out_stride_floats, w, h);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_tta_variants(const TtaPlane *tab, int n_planes, int n_tiles, cudaStream_t s) {
+    if (n_planes < 1 || n_tiles < 1) return cudaErrorInvalidValue;
+    tta_variants_kernel<<<n_tiles, 256, 0, s>>>(tab, n_planes);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_tta_mean(const TtaPlane *tab, int n_planes, int n_tiles, cudaStream_t s) {
+    if (n_planes < 1 || n_tiles < 1) return cudaErrorInvalidValue;
+    tta_mean_kernel<<<n_tiles, 256, 0, s>>>(tab, n_planes);
     return cudaGetLastError();
 }
 

@@ -142,7 +142,19 @@ int main(int argc, char **argv) {
     // the sibling of -j for this implementation (src/main.cpp:58-60 is where the reference declares -j): planes are cut into
     // this many row bands, one per GPU, halo rows exchanged between the GPUs after every layer; W2X_GPUS does the same
     cmd.add("", "gpus", "number of GPUs the conversion is spread over", false, "1", "integer").hidden = true;
+    // test-time augmentation (the -tta / --tta switch of later waifu2x front ends): every pass is the mean of its conversions of the
+    // Y plane's 8 flips and transposes, at 8x the GPU work; stdout and output naming stay as without it
+    cmd.add("", "tta", "average every pass over the 8 flips and transposes of the plane", false, "0", "integer", {"0", "1"}).hidden = true;
     cmd.parse(argc, argv);
+    const bool tta = cmd.get("tta") == "1";
+    {
+        const char *ng = std::getenv("W2X_GPUS");
+        const int gpus = std::atoi(cmd.get("gpus").c_str()) > 1 ? std::atoi(cmd.get("gpus").c_str()) : ng ? std::atoi(ng) : 1;
+        if (tta && gpus > 1) {   // the passes run as one w2x_convert_chain call, which has no multi-GPU form
+            std::cerr << "Error : --tta 1 runs on one GPU; it cannot be combined with " << gpus << " GPUs (--gpus / W2X_GPUS)." << std::endl;
+            std::exit(1);
+        }
+    }
     if (std::atoi(cmd.get("gpus").c_str()) > 1) w2xc::gpuRuntime::setNumberOfGpus(std::atoi(cmd.get("gpus").c_str()));
     // CUDA context creation (~0.2 s) overlaps image decoding, colour conversion and model parsing; joined before the first conversion
     std::thread gpu_warmup([] { w2xc::gpuRuntime::warmup(); });
@@ -192,12 +204,14 @@ int main(int argc, char **argv) {
     // bicubic Y channel is overwritten at :148-154, U and V never feed back into Y).  So on one GPU the noise pass and every 2x
     // iteration run as ONE chain that keeps Y on the device, while the bicubic iterations of U and V run here on the host.
     // -m noise, --gpus n > 1 (w2x_multi_convert_plane), no usable device and a scale model that does not load keep the per-pass path below.
-    bool chained = false;
+    // With --tta 1 every pass is a TTA step of the chain (-m noise a one-step chain); without a device the chain call reports it.
+    bool chained = false;                          // the 2x iterations run in the chain
     if (scalePhase && iterTimesTwiceScaling >= 1 && w2xc::modelUtility::tryGenerateModelFromJSON(modelDir + "/scale2.0x_model.json", scaleModels)) {
         wait_for_gpu();
-        chained = w2xc::gpuRuntime::context() != nullptr && w2xc::gpuRuntime::multi() == nullptr;
+        chained = tta || (w2xc::gpuRuntime::context() != nullptr && w2xc::gpuRuntime::multi() == nullptr);
     }
-    if (chained) {
+    const bool noiseChained = noisePhase && (chained || tta);
+    if (chained || noiseChained) {
         struct Progress {
             bool noise;
             int failedStep = -1;
@@ -210,13 +224,15 @@ int main(int argc, char **argv) {
             }
         } progress{noisePhase};
         std::vector<w2xc::ChainStep> steps;
-        if (noisePhase) steps.push_back({&noiseModels, false});
-        for (int i = 0; i < iterTimesTwiceScaling; i++) steps.push_back({&scaleModels, true});
+        if (noisePhase) steps.push_back({&noiseModels, false, tta});
+        const int chainedIterations = chained ? iterTimesTwiceScaling : 0;
+        for (int i = 0; i < chainedIterations; i++) steps.push_back({&scaleModels, true, tta});
         w2xc::Plane imageY = plane_of(image, 0), out;
+        wait_for_gpu();
         // the bicubic iterations (:144) of U and V: w2ximg::resize computes every channel from that channel alone, so U and V do not
         // depend on the Y values they are resized along with
         std::thread colour([&] {
-            for (int i = 0; i < iterTimesTwiceScaling; i++) image = w2ximg::resize(image, image.width * 2, image.height * 2, w2ximg::CUBIC);
+            for (int i = 0; i < chainedIterations; i++) image = w2ximg::resize(image, image.width * 2, image.height * 2, w2ximg::CUBIC);
         });
         const double t0 = now();
         const bool ok = w2xc::convertChainWithModels(imageY, out, steps, &Progress::step, &progress);
@@ -231,7 +247,7 @@ int main(int argc, char **argv) {
     }
 
     // ===== Noise Reduction Phase ===== (:82-100)
-    if (noisePhase && !chained) {
+    if (noisePhase && !noiseChained) {
         std::vector<std::unique_ptr<w2xc::Model>> &models = noiseModels;
         w2xc::Plane imageY = plane_of(image, 0), out;
         wait_for_gpu();

@@ -314,9 +314,12 @@ inline const w2x_model *modelFileOf(std::vector<std::unique_ptr<Model>> &models)
 // plane stays on the GPU between the steps and the 2x plane is never built; each step's result is bit-identical to
 // convertWithModels on the previous step's (resized) output.  onStep(k) runs before step k starts, then the step prints its
 // progress lines like convertWithModels.  outputPlane is (re)allocated to the final size.  One GPU only (w2x_convert_chain).
+// tta: the step is the mean of its conversions of the plane's 8 flips and transposes (W2X_STEP_TTA), the -tta switch of later
+// waifu2x front ends.  (No default member initialiser: ChainStep stays an aggregate under C++11.)
 struct ChainStep {
     std::vector<std::unique_ptr<Model>> *models;
     bool upscale2x;
+    bool tta;
 };
 inline bool convertChainWithModels(Plane &inputPlane, Plane &outputPlane, const std::vector<ChainStep> &steps,
                                    void (*onStep)(int step, void *user), void *user, bool blockSplitting = true) {
@@ -329,7 +332,7 @@ inline bool convertChainWithModels(Plane &inputPlane, Plane &outputPlane, const 
         const w2x_model *f = s.models ? modelFileOf(*s.models) : nullptr;
         if (!f) return false;
         files.push_back(f);
-        kinds.push_back(s.upscale2x ? W2X_STEP_UPSCALE2X : W2X_STEP_SAME);
+        kinds.push_back((s.upscale2x ? W2X_STEP_UPSCALE2X : W2X_STEP_SAME) | (s.tta ? W2X_STEP_TTA : 0));
         if (s.upscale2x) { w *= 2; h *= 2; }
     }
     if (outputPlane.data == inputPlane.data || outputPlane.width != w || outputPlane.height != h) outputPlane.create(w, h);
