@@ -31,18 +31,16 @@ using namespace w2x;
 namespace w2x {
 namespace eng {
 
-int ensure(void **p, size_t *have, size_t need) {
-    if (*have >= need) return W2X_OK;
-    if (*p) cudaFree(*p);
-    *p = nullptr;
-    *have = 0;
-    cudaError_t e = cudaMalloc(p, need);
-    if (e != cudaSuccess) {
-        cudaGetLastError();
-        return fail(W2X_ERR_NOMEM, "cudaMalloc of %zu bytes failed (%s)", need, cudaGetErrorString(e));
-    }
-    *have = need;
-    return W2X_OK;
+int max_channels(const w2x_model *m) {
+    int maxc = 1;
+    for (auto &L : m->layers) maxc = std::max(maxc, std::max(L.n_in, L.n_out));
+    return maxc;
+}
+
+// The two staging buffers of a host-buffer entry point: its inputs in io_buf[0], its outputs in io_buf[1].
+int reserve_io(w2x_ctx *ctx, size_t in_bytes, size_t out_bytes) {
+    int rc = ctx->io_buf[0].reserve(in_bytes);
+    return rc ? rc : ctx->io_buf[1].reserve(out_bytes);
 }
 
 int get_dev_model(w2x_ctx *ctx, const w2x_model *m, DevModel **out) {
@@ -53,28 +51,28 @@ int get_dev_model(w2x_ctx *ctx, const w2x_model *m, DevModel **out) {
     }
     DevModel dm;
     const size_t n = m->layers.size();
-    dm.w.assign(n, nullptr);
-    dm.b.assign(n, nullptr);
-    dm.pack.assign(n, nullptr);
-    dm.pack8.assign(n, nullptr);
+    dm.w.resize(n);
+    dm.b.resize(n);
+    dm.pack.resize(n);
+    dm.pack8.resize(n);
     dm.out_scale.assign(n, 1.f);
     for (size_t i = 0; i < n; i++) {
         const Layer &L = m->layers[i];
-        CU_CHECK(cudaMalloc(&dm.w[i], L.w.size() * sizeof(float)));
-        CU_CHECK(cudaMemcpyAsync(dm.w[i], L.w.data(), L.w.size() * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+        CU_CHECK(dm.w[i].grow(L.w.size() * sizeof(float)));
+        CU_CHECK(cudaMemcpyAsync(dm.w[i].get(), L.w.data(), L.w.size() * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
         std::vector<float> bf(L.b.size());
         for (size_t k = 0; k < bf.size(); k++) bf[k] = static_cast<float>(L.b[k]);
         dm.b_host.push_back(bf);
-        CU_CHECK(cudaMalloc(&dm.b[i], bf.size() * sizeof(float)));
-        CU_CHECK(cudaMemcpyAsync(dm.b[i], bf.data(), bf.size() * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+        CU_CHECK(dm.b[i].grow(bf.size() * sizeof(float)));
+        CU_CHECK(cudaMemcpyAsync(dm.b[i].get(), bf.data(), bf.size() * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
         CU_CHECK(cudaStreamSynchronize(ctx->stream));   // bf goes out of scope
         const TcPack &P = m->tc[i];
         if (!P.bytes.empty()) {
-            CU_CHECK(cudaMalloc(&dm.pack[i], P.bytes.size() * 2));
-            CU_CHECK(cudaMemcpyAsync(dm.pack[i], P.bytes.data(), P.bytes.size() * 2, cudaMemcpyHostToDevice, ctx->stream));
+            CU_CHECK(dm.pack[i].grow(P.bytes.size() * 2));
+            CU_CHECK(cudaMemcpyAsync(dm.pack[i].get(), P.bytes.data(), P.bytes.size() * 2, cudaMemcpyHostToDevice, ctx->stream));
             dm.out_scale[i] = 1.0f / (P.wscale * tc::ACT_SCALE);
-            CU_CHECK(cudaMalloc(&dm.pack8[i], P.bytes8.size()));
-            CU_CHECK(cudaMemcpyAsync(dm.pack8[i], P.bytes8.data(), P.bytes8.size(), cudaMemcpyHostToDevice, ctx->stream));
+            CU_CHECK(dm.pack8[i].grow(P.bytes8.size()));
+            CU_CHECK(cudaMemcpyAsync(dm.pack8[i].get(), P.bytes8.data(), P.bytes8.size(), cudaMemcpyHostToDevice, ctx->stream));
         }
     }
     if (m->tc_eligible) {
@@ -156,10 +154,10 @@ int launch_layer_tc(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int li, cons
     const int f8 = ctx->precision == W2X_PRECISION_F16_F8X2 ? 1 : 0;
     {
         LayerTimer t(ctx, li);
-        CU_CHECK(tc::launch_tc_layer(in, f8 ? (const void *)dm->pack8[(size_t)li] : (const void *)dm->pack[(size_t)li],
+        CU_CHECK(tc::launch_tc_layer(in, f8 ? (const void *)dm->pack8[(size_t)li].get() : (const void *)dm->pack[(size_t)li].get(),
                                      dm->b_host[(size_t)li].data(), out, L.n_in, L.n_out, pw, ph, dm->out_scale[(size_t)li], ctx->precision,
                                      ctx->num_sms, ctx->stream,
-                                     profile && ctx->prof_buf ? ctx->prof_buf + (size_t)li * tc::PROF_MAX_CTAS * tc::PROF_WORDS : nullptr,
+                                     profile && ctx->prof_buf.get() ? ctx->prof_buf.get() + (size_t)li * tc::PROF_MAX_CTAS * tc::PROF_WORDS : nullptr,
                                      fused ? dm->last_w_t.data() : nullptr, fused ? reinterpret_cast<float *>(out) : nullptr, out_y0, out_rows));
     }
     static const char *const names[3][2] = {{"wgmma_f16x3", "wgmma_f16x3+last"}, {"wgmma_f16+f8x2", "wgmma_f16+f8x2+last"}, {"wgmma_f16", "wgmma_f16+last"}};
@@ -181,22 +179,21 @@ int run_basic(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int engine, const 
               int ph, float *dst, long dst_stride, const PackedGather *packed = nullptr, const tc::FirstSource *direct = nullptr) {
     const int n = (int)m->layers.size();
     if (pw - 2 * n < 1 || ph - 2 * n < 1) return fail(W2X_ERR_ARG, "plane smaller than the model's receptive ring");
-    int maxc = 1;
-    for (auto &L : m->layers) maxc = std::max(maxc, std::max(L.n_in, L.n_out));
+    const int maxc = max_channels(m);
     if (engine == W2X_ENGINE_FP32) {
         const size_t need = (size_t)maxc * pw * ph * sizeof(float);
         for (int i = 0; i < 2; i++) {
-            int rc = ensure(&ctx->buf[i], &ctx->buf_bytes[i], need);
+            int rc = ctx->buf[i].reserve(need);
             if (rc) return rc;
         }
-        float *cur = static_cast<float *>(ctx->buf[0]), *nxt = static_cast<float *>(ctx->buf[1]);
+        float *cur = static_cast<float *>(ctx->buf[0].get()), *nxt = static_cast<float *>(ctx->buf[1].get());
         CU_CHECK(launch_copy2d(src, src_stride, cur, pw, pw, ph, ctx->stream));   // ROI -> dense plane
         ctx->launches++;
         for (int li = 0; li < n; li++) {
             const Layer &L = m->layers[(size_t)li];
             {
                 LayerTimer t(ctx, li);
-                CU_CHECK(launch_conv3x3_fp32(cur, nxt, dm->w[(size_t)li], dm->b[(size_t)li], L.n_in, L.n_out, pw, ph,
+                CU_CHECK(launch_conv3x3_fp32(cur, nxt, dm->w[(size_t)li].get(), dm->b[(size_t)li].get(), L.n_in, L.n_out, pw, ph,
                                              ctx->stream));
             }
             note_kernel(ctx, li, "fp32_direct");
@@ -213,10 +210,10 @@ int run_basic(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int engine, const 
     if (rc) return rc;
     const size_t need = tc::act_bytes(maxc, pw, ph);
     for (int i = 0; i < 2; i++) {
-        rc = ensure(&ctx->buf[i], &ctx->buf_bytes[i], need);
+        rc = ctx->buf[i].reserve(need);
         if (rc) return rc;
     }
-    __half *cur = static_cast<__half *>(ctx->buf[0]), *nxt = static_cast<__half *>(ctx->buf[1]);
+    __half *cur = static_cast<__half *>(ctx->buf[0].get()), *nxt = static_cast<__half *>(ctx->buf[1].get());
     {
         const Layer &L = m->layers[0];
         LayerTimer t(ctx, 0);
@@ -243,23 +240,13 @@ int run_basic(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int engine, const 
             note_kernel(ctx, n - 1, "last_gather");
         } else {
             if (packed) return fail(W2X_ERR_UNSUPPORTED, "packed frames need the fused last layer");
-            CU_CHECK(tc::launch_last(cur, L.n_in, pw, ph, dm->w[(size_t)n - 1], static_cast<float>(L.b[0]), n, dst,
+            CU_CHECK(tc::launch_last(cur, L.n_in, pw, ph, dm->w[(size_t)n - 1].get(), static_cast<float>(L.b[0]), n, dst,
                                      dst_stride, ctx->stream, f8));
             note_kernel(ctx, n - 1, "last_Nx1");
         }
         ctx->launches++;
     }
     return W2X_OK;
-}
-
-// Whole plane (or row band) already available as a padded plane: cut it into horizontal bands that
-// respect the scratch limit, each band re-reads n rows of context above and below.
-// direct_in != nullptr (tensor-core engine): no padded plane exists; the first layer reads d_in (rows_above / rows_below real rows
-// beyond the plane) with the padding folded into its loads.
-int max_channels(const w2x_model *m) {
-    int maxc = 1;
-    for (auto &L : m->layers) maxc = std::max(maxc, std::max(L.n_in, L.n_out));
-    return maxc;
 }
 
 // rows per band of run_padded_plane for a plane w wide: the band's frame (band + 2n rows) fits the scratch limit and has at most
@@ -272,6 +259,10 @@ int scratch_band_rows(const w2x_ctx *ctx, const w2x_model *m, int w, int h) {
     return (int)std::min<long>(h, max_rows);
 }
 
+// Whole plane (or row band) already available as a padded plane: cut it into horizontal bands that
+// respect the scratch limit, each band re-reads n rows of context above and below.
+// direct_in != nullptr (tensor-core engine): no padded plane exists; the first layer reads d_in (rows_above / rows_below real rows
+// beyond the plane) with the padding folded into its loads.
 // up2x (direct_in only): the plane is the nearest-neighbour 2x resize of direct_in, w x h its 2x size (see convert_device).
 int run_padded_plane(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int engine, const float *padp, int w, int h,
                      float *dst, long dst_stride, const float *direct_in = nullptr, long in_stride = 0, int rows_above = 0, int rows_below = 0,
@@ -438,27 +429,28 @@ int convert_device(w2x_ctx *ctx, const w2x_model *m, const float *d_in, int w, i
         return run_padded_plane(ctx, m, dm, engine, nullptr, w, h, d_out, ostride, d_in, (long)(in_stride_bytes / 4), rows_above, rows_below,
                                 up2x);
     }
-    rc = ensure(reinterpret_cast<void **>(&ctx->pad_buf), &ctx->pad_bytes, (size_t)pw * ph * sizeof(float));
+    rc = ctx->pad_buf.reserve((size_t)pw * ph * sizeof(float));
     if (rc) return rc;
+    float *const pad = ctx->pad_buf.get();
     // cv::copyMakeBorder(in, temp, n, n, n, n, BORDER_REPLICATE)   (src/convertRoutine.cpp:35, :96)
     if (up2x)
         CU_CHECK(launch_pad_upsample2x(d_in, w, h, (long)(in_stride_bytes / 4), n, std::min(rows_above, n), std::min(rows_below, n),
-                                       ctx->pad_buf, ctx->stream));
+                                       pad, ctx->stream));
     else
         CU_CHECK(launch_pad_replicate(d_in, w, h, (long)(in_stride_bytes / 4), n, std::min(rows_above, n),
-                                      std::min(rows_below, n), ctx->pad_buf, ctx->stream));
+                                      std::min(rows_below, n), pad, ctx->stream));
     ctx->launches++;
     if (literal) {   // check_blocks has seen every block fit
         const std::vector<int> tab = blocks_of(w, h, n);
         for (size_t i = 0; i < tab.size(); i += 8) {
             const int *t = &tab[i];
-            rc = run_basic(ctx, m, dm, engine, ctx->pad_buf + (long)t[2] * pw + t[4], pw, t[5] - t[4], t[3] - t[2],
+            rc = run_basic(ctx, m, dm, engine, pad + (long)t[2] * pw + t[4], pw, t[5] - t[4], t[3] - t[2],
                            d_out + (long)t[6] * ostride + t[7], ostride);
             if (rc) return rc;
         }
         return W2X_OK;
     }
-    return run_padded_plane(ctx, m, dm, engine, ctx->pad_buf, w, h, d_out, ostride);
+    return run_padded_plane(ctx, m, dm, engine, pad, w, h, d_out, ostride);
 }
 
 }  // namespace eng
@@ -487,12 +479,12 @@ int w2x_ctx_create(int device, w2x_ctx **out_ctx) {
     if (prop.major != 9 || prop.minor != 0)
         return fail(W2X_ERR_NO_DEVICE, "device %d (%s) is sm_%d%d; this build carries sm_90a code only", device,
                     prop.name, prop.major, prop.minor);
+    DeviceGuard g(device);   // before the context: it is still current when an early return destroys what has been created
     auto ctx = std::make_unique<w2x_ctx>();
     ctx->device = device;
     ctx->num_sms = prop.multiProcessorCount;
     ctx->cc_major = prop.major;
     ctx->cc_minor = prop.minor;
-    DeviceGuard g(device);
     CU_CHECK(cudaStreamCreateWithFlags(&ctx->own_stream, cudaStreamNonBlocking));
     ctx->stream = ctx->own_stream;
     if (const char *pe = std::getenv("W2X_PRECISION")) {
@@ -511,13 +503,6 @@ int w2x_ctx_create(int device, w2x_ctx **out_ctx) {
     return W2X_OK;
 }
 
-static void free_dev_model(DevModel &dm) {
-    for (auto p : dm.w) cudaFree(p);
-    for (auto p : dm.b) cudaFree(p);
-    for (auto p : dm.pack) cudaFree(p);
-    for (auto p : dm.pack8) cudaFree(p);
-}
-
 // Drops the context's device copies of a model (weights, packed operands); call it before w2x_model_free in a long-lived
 // context that cycles through many models.  The next conversion with the same model uploads it again.  Refused while band
 // sessions (w2x_band_*, the sub-bands of w2x_slab_*, the cached plan of w2x_multi_*) hold the copies: their passes launch
@@ -532,7 +517,6 @@ int w2x_ctx_forget_model(w2x_ctx *ctx, const w2x_model *model) {
                     it->second.band_sessions);
     DeviceGuard g(ctx->device);
     CU_CHECK(cudaStreamSynchronize(ctx->stream));
-    free_dev_model(it->second);
     ctx->models.erase(it);
     return W2X_OK;
 }
@@ -541,26 +525,6 @@ void w2x_ctx_destroy(w2x_ctx *ctx) {
     if (!ctx) return;
     DeviceGuard g(ctx->device);
     cudaStreamSynchronize(ctx->stream);
-    for (auto &kv : ctx->models) free_dev_model(kv.second);
-    for (int i = 0; i < 2; i++) {
-        cudaFree(ctx->buf[i]);
-        cudaFree(ctx->io_buf[i]);
-        cudaFree(ctx->chain_buf[i]);
-        cudaFree(ctx->tta_buf[i]);
-    }
-    cudaFree(ctx->pad_buf);
-    cudaFree(ctx->plan_buf);
-    cudaFree(ctx->prof_buf);
-    if (ctx->plan_ev) cudaEventDestroy(ctx->plan_ev);
-    for (auto &s : ctx->spans) { cudaEventDestroy(s.e0); cudaEventDestroy(s.e1); }
-    for (auto e : ctx->event_pool) cudaEventDestroy(e);
-    for (int i = 0; i < 8; i++) {
-        if (ctx->ev_in[i]) cudaEventDestroy(ctx->ev_in[i]);
-        if (ctx->ev_done[i]) cudaEventDestroy(ctx->ev_done[i]);
-    }
-    if (ctx->copy_in) cudaStreamDestroy(ctx->copy_in);
-    if (ctx->copy_out) cudaStreamDestroy(ctx->copy_out);
-    if (ctx->own_stream) cudaStreamDestroy(ctx->own_stream);
     delete ctx;
 }
 
@@ -619,23 +583,22 @@ W2X_API int w2x_debug_tc_profile_enable(w2x_ctx *ctx, int on) {
     DeviceGuard g(ctx->device);
     const size_t bytes = (size_t)16 * tc::PROF_MAX_CTAS * tc::PROF_WORDS * sizeof(unsigned long long);
     if (on) {
-        if (!ctx->prof_buf) CU_CHECK(cudaMalloc(&ctx->prof_buf, bytes));
-        CU_CHECK(cudaMemsetAsync(ctx->prof_buf, 0, bytes, ctx->stream));
-    } else if (ctx->prof_buf) {
+        CU_CHECK(ctx->prof_buf.grow(bytes));
+        CU_CHECK(cudaMemsetAsync(ctx->prof_buf.get(), 0, bytes, ctx->stream));
+    } else if (ctx->prof_buf.get()) {
         CU_CHECK(cudaStreamSynchronize(ctx->stream));
-        cudaFree(ctx->prof_buf);
-        ctx->prof_buf = nullptr;
+        ctx->prof_buf.release();
     }
     return W2X_OK;
 }
 // out[PROF_WORDS]: counters of `layer` summed over CTAs; *n_ctas = CTAs that ran.
 W2X_API int w2x_debug_tc_profile_read(w2x_ctx *ctx, int layer, unsigned long long *out, int *n_ctas) {
     if (check_ctx(ctx)) return W2X_ERR_ARG;
-    if (!ctx->prof_buf || layer < 0 || layer >= 16 || !out) return fail(W2X_ERR_ARG, "profile not enabled or bad layer");
+    if (!ctx->prof_buf.get() || layer < 0 || layer >= 16 || !out) return fail(W2X_ERR_ARG, "profile not enabled or bad layer");
     DeviceGuard g(ctx->device);
     std::vector<unsigned long long> h((size_t)tc::PROF_MAX_CTAS * tc::PROF_WORDS);
     CU_CHECK(cudaStreamSynchronize(ctx->stream));
-    CU_CHECK(cudaMemcpy(h.data(), ctx->prof_buf + (size_t)layer * h.size(), h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    CU_CHECK(cudaMemcpy(h.data(), ctx->prof_buf.get() + (size_t)layer * h.size(), h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
     int n = 0;
     for (int w = 0; w < tc::PROF_WORDS; w++) out[w] = 0;
     for (int c = 0; c < tc::PROF_MAX_CTAS; c++) {
@@ -706,9 +669,9 @@ int w2x_convert_plane(w2x_ctx *ctx, const w2x_model *model, const float *in, int
     if (rc) return rc;
     emit_plane_progress(ctx, model, width, height, block_splitting, true);
     DeviceGuard g(ctx->device);
-    for (int i = 0; i < 2 && !rc; i++) rc = ensure(reinterpret_cast<void **>(&ctx->io_buf[i]), &ctx->io_bytes[i], bytes);
+    rc = reserve_io(ctx, bytes, bytes);
     if (rc) return rc;
-    float *din = ctx->io_buf[0], *dout = ctx->io_buf[1];
+    float *din = ctx->io_buf[0].get(), *dout = ctx->io_buf[1].get();
     // Large planes are cut into row bands so that the upload of band i+1 and the download of band i-1 overlap the
     // layers of band i (copy engines + compute run concurrently); each band re-reads n real rows of context from its
     // neighbours, which keeps the result bit-identical to the single-pass path.
@@ -750,11 +713,11 @@ int w2x_filter_layer_device(w2x_ctx *ctx, const w2x_model *model, int layer, con
         // Model::filter semantics (same size, BORDER_REPLICATE): stage a frame with a replicated ring
         // of one pixel, run the same-size tensor-core layer on it, return the interior.
         const int pw = width + 2, ph = height + 2;
-        rc = ensure(&ctx->buf[0], &ctx->buf_bytes[0], tc::act_bytes(L.n_in, pw, ph));
+        rc = ctx->buf[0].reserve(tc::act_bytes(L.n_in, pw, ph));
         if (rc) return rc;
-        rc = ensure(&ctx->buf[1], &ctx->buf_bytes[1], tc::act_bytes(L.n_out, pw, ph));
+        rc = ctx->buf[1].reserve(tc::act_bytes(L.n_out, pw, ph));
         if (rc) return rc;
-        __half *fin = static_cast<__half *>(ctx->buf[0]), *fout = static_cast<__half *>(ctx->buf[1]);
+        __half *fin = static_cast<__half *>(ctx->buf[0].get()), *fout = static_cast<__half *>(ctx->buf[1].get());
         const int f8 = ctx->precision == W2X_PRECISION_F16_F8X2 ? 1 : 0;
         CU_CHECK(tc::launch_planar_to_nhwc(d_in, L.n_in, width, height, fin, ctx->stream, f8));
         rc = launch_layer_tc(ctx, model, dm, layer, fin, fout, pw, ph, false, false);
@@ -765,7 +728,7 @@ int w2x_filter_layer_device(w2x_ctx *ctx, const w2x_model *model, int layer, con
     }
     {
         LayerTimer t(ctx, layer);
-        CU_CHECK(launch_conv3x3_fp32(d_in, d_out, dm->w[(size_t)layer], dm->b[(size_t)layer], L.n_in, L.n_out, width, height,
+        CU_CHECK(launch_conv3x3_fp32(d_in, d_out, dm->w[(size_t)layer].get(), dm->b[(size_t)layer].get(), L.n_in, L.n_out, width, height,
                                      ctx->stream));
     }
     note_kernel(ctx, layer, "fp32_direct");
@@ -792,11 +755,9 @@ int w2x_filter_layer(w2x_ctx *ctx, const w2x_model *model, int layer, const floa
         if (!out_planes[i]) return fail(W2X_ERR_ARG, "w2x_filter_layer: NULL output plane %d", i);
     DeviceGuard g(ctx->device);
     const size_t plane = (size_t)width * height, row = (size_t)width * 4;
-    int rc = ensure(reinterpret_cast<void **>(&ctx->io_buf[0]), &ctx->io_bytes[0], plane * sizeof(float) * (size_t)L.n_in);
+    int rc = reserve_io(ctx, plane * sizeof(float) * (size_t)L.n_in, plane * sizeof(float) * (size_t)L.n_out);
     if (rc) return rc;
-    rc = ensure(reinterpret_cast<void **>(&ctx->io_buf[1]), &ctx->io_bytes[1], plane * sizeof(float) * (size_t)L.n_out);
-    if (rc) return rc;
-    float *din = ctx->io_buf[0], *dout = ctx->io_buf[1];
+    float *din = ctx->io_buf[0].get(), *dout = ctx->io_buf[1].get();
     std::vector<HostGroup> groups(1);
     for (int i = 0; i < L.n_in; i++) groups[0].up.push_back({din + plane * (size_t)i, row, in_planes[i], in_stride_bytes, row, (size_t)height});
     groups[0].compute = [=] { return w2x_filter_layer_device(ctx, model, layer, din, dout, width, height); };
@@ -919,10 +880,10 @@ int upload_frames(w2x_ctx *ctx, std::vector<FramePlan> &frames, std::vector<Fram
         std::memcpy(blob.data() + off_tta, tta.data(), tta.size() * sizeof(TtaPlane));
     }
     if (ctx->plan_ev_live) CU_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->plan_ev, 0));
-    int rc = ensure(&ctx->plan_buf, &ctx->plan_bytes, blob.size());
+    int rc = ctx->plan_buf.reserve(blob.size());
     if (rc) return rc;
-    CU_CHECK(cudaMemcpyAsync(ctx->plan_buf, blob.data(), blob.size(), cudaMemcpyHostToDevice, ctx->stream));
-    const char *base = static_cast<const char *>(ctx->plan_buf);
+    const char *base = ctx->plan_buf.get();
+    CU_CHECK(cudaMemcpyAsync(ctx->plan_buf.get(), blob.data(), blob.size(), cudaMemcpyHostToDevice, ctx->stream));
     if (tta_dev) *tta_dev = reinterpret_cast<const TtaPlane *>(base + off_tta);
     for (size_t f = 0; f < frames.size(); f++) {
         FrameDev &d = (*out)[f];
@@ -938,8 +899,8 @@ int upload_frames(w2x_ctx *ctx, std::vector<FramePlan> &frames, std::vector<Fram
 int reserve_frames(w2x_ctx *ctx, const std::vector<FramePlan> &frames, size_t f0, size_t f1, int maxc) {
     size_t px = 0;
     for (size_t f = f0; f < f1; f++) px = std::max(px, (size_t)frames[f].fw * frames[f].fh);
-    int rc = ensure(reinterpret_cast<void **>(&ctx->pad_buf), &ctx->pad_bytes, px * sizeof(float));
-    for (int i = 0; i < 2 && !rc; i++) rc = ensure(&ctx->buf[i], &ctx->buf_bytes[i], px * (size_t)maxc * 4);
+    int rc = ctx->pad_buf.reserve(px * sizeof(float));
+    for (int i = 0; i < 2 && !rc; i++) rc = ctx->buf[i].reserve(px * (size_t)maxc * 4);
     return rc;
 }
 
@@ -947,12 +908,12 @@ int reserve_frames(w2x_ctx *ctx, const std::vector<FramePlan> &frames, size_t f0
 // frame's planes are the nearest-neighbour 2x resizes of their sources (tc::launch_pack_planes).
 int run_packed_frame(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, const FrameDev &f, bool up2x = false) {
     const int n = (int)m->layers.size();
-    int rc = ensure(reinterpret_cast<void **>(&ctx->pad_buf), &ctx->pad_bytes, (size_t)f.fw * f.fh * sizeof(float));
+    int rc = ctx->pad_buf.reserve((size_t)f.fw * f.fh * sizeof(float));
     if (rc) return rc;
-    CU_CHECK(tc::launch_pack_planes(f.rect, f.shelf_y0, f.shelf_first, f.n_shelf, n, f.fw, f.fh, up2x, ctx->pad_buf, ctx->stream));
+    CU_CHECK(tc::launch_pack_planes(f.rect, f.shelf_y0, f.shelf_first, f.n_shelf, n, f.fw, f.fh, up2x, ctx->pad_buf.get(), ctx->stream));
     ctx->launches++;
     const PackedGather g{f.rect, f.n_rect, f.n_blocks};
-    return run_basic(ctx, m, dm, W2X_ENGINE_TC, ctx->pad_buf, f.fw, f.fw, f.fh, nullptr, 0, &g);
+    return run_basic(ctx, m, dm, W2X_ENGINE_TC, ctx->pad_buf.get(), f.fw, f.fw, f.fh, nullptr, 0, &g);
 }
 
 int run_packed_frames(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, std::vector<FramePlan> &frames) {
@@ -999,12 +960,12 @@ int convert_tiles_dev(w2x_ctx *ctx, const w2x_model *m, const float *d_in, float
         }
         return run_packed_frames(ctx, m, dm, frames);
     }
-    rc = ensure(reinterpret_cast<void **>(&ctx->pad_buf), &ctx->pad_bytes, (size_t)pw * ph * sizeof(float));
+    rc = ctx->pad_buf.reserve((size_t)pw * ph * sizeof(float));
     if (rc) return rc;
     for (int t = 0; t < n_tiles; t++) {   // cv::copyMakeBorder per tile (src/convertRoutine.cpp:35)
-        CU_CHECK(launch_pad_replicate(d_in + (size_t)t * w * h, w, h, w, n, 0, 0, ctx->pad_buf, ctx->stream));
+        CU_CHECK(launch_pad_replicate(d_in + (size_t)t * w * h, w, h, w, n, 0, 0, ctx->pad_buf.get(), ctx->stream));
         ctx->launches++;
-        rc = run_basic(ctx, m, dm, engine, ctx->pad_buf, pw, pw, ph, d_out + (size_t)t * w * h, w);
+        rc = run_basic(ctx, m, dm, engine, ctx->pad_buf.get(), pw, pw, ph, d_out + (size_t)t * w * h, w);
         if (rc) return rc;
     }
     return W2X_OK;
@@ -1176,16 +1137,17 @@ int prepare_planes(w2x_ctx *ctx, std::vector<Step> &steps, const std::vector<Pla
     }
     for (int i = 0; i < 2; i++) {
         if (!need[i]) continue;
-        int rc = ensure(reinterpret_cast<void **>(&ctx->chain_buf[i]), &ctx->chain_bytes[i], need[i]);
+        int rc = ctx->chain_buf[i].reserve(need[i]);
         if (rc) return rc;
     }
     for (int i = 0; i < 2; i++) {
         if (!tta_need[i]) continue;
-        int rc = ensure(reinterpret_cast<void **>(&ctx->tta_buf[i]), &ctx->tta_bytes[i], tta_need[i]);
+        int rc = ctx->tta_buf[i].reserve(tta_need[i]);
         if (rc) return rc;
     }
     std::vector<FramePlan> frames;
     std::vector<TtaPlane> tta;
+    float *const tta_in = ctx->tta_buf[0].get(), *const tta_out = ctx->tta_buf[1].get();
     std::vector<size_t> tab0(steps.size());   // a TTA step's variants table at tta[tab0], its mean table right after it
     for (size_t k = 0; k <= last; k++) {
         Step &s = steps[k];
@@ -1198,7 +1160,7 @@ int prepare_planes(w2x_ctx *ctx, std::vector<Step> &steps, const std::vector<Pla
             PlaneIO &p = s.io[i];
             p.src = k == 0 ? ends[i].src : steps[k - 1].io[i].dst;
             p.src_stride = k == 0 ? ends[i].src_stride : steps[k - 1].io[i].dst_stride;
-            p.dst = k == last ? ends[i].dst : ctx->chain_buf[k & 1] + off;
+            p.dst = k == last ? ends[i].dst : ctx->chain_buf[k & 1].get() + off;
             p.dst_stride = k == last ? ends[i].dst_stride : (size_t)s.w[i] * sizeof(float);
             off += (size_t)s.w[i] * s.h[i];
         }
@@ -1210,17 +1172,17 @@ int prepare_planes(w2x_ctx *ctx, std::vector<Step> &steps, const std::vector<Pla
             for (size_t i = 0; i < n_planes; i++) {   // the variants kernel: plane -> its 8 variants
                 const int sw = s.up ? s.w[i] / 2 : s.w[i], sh = s.up ? s.h[i] / 2 : s.h[i];
                 const size_t in_px = (size_t)sw * sh, out_px = (size_t)s.w[i] * s.h[i];
-                tta.push_back(TtaPlane{s.io[i].src, ctx->tta_buf[0] + in_off, nullptr, (long)(s.io[i].src_stride / 4), 0, sw, sh, s.vtiles});
+                tta.push_back(TtaPlane{s.io[i].src, tta_in + in_off, nullptr, (long)(s.io[i].src_stride / 4), 0, sw, sh, s.vtiles});
                 s.vtiles += tiles(sw, sh);
                 for (int j = 0; j < 8; j++)
-                    s.vio[8 * i + j] = PlaneIO{ctx->tta_buf[0] + in_off + j * in_px, (size_t)(j & 4 ? sh : sw) * sizeof(float),
-                                               ctx->tta_buf[1] + out_off + j * out_px, (size_t)s.vw[8 * i + j] * sizeof(float)};
+                    s.vio[8 * i + j] = PlaneIO{tta_in + in_off + j * in_px, (size_t)(j & 4 ? sh : sw) * sizeof(float),
+                                               tta_out + out_off + j * out_px, (size_t)s.vw[8 * i + j] * sizeof(float)};
                 in_off += 8 * in_px;
                 out_off += 8 * out_px;
             }
             out_off = 0;
             for (size_t i = 0; i < n_planes; i++) {   // the mean kernel: 8 variant outputs -> the step's output
-                tta.push_back(TtaPlane{nullptr, ctx->tta_buf[1] + out_off, s.io[i].dst, 0, (long)(s.io[i].dst_stride / 4), s.w[i], s.h[i], s.mtiles});
+                tta.push_back(TtaPlane{nullptr, tta_out + out_off, s.io[i].dst, 0, (long)(s.io[i].dst_stride / 4), s.w[i], s.h[i], s.mtiles});
                 s.mtiles += tiles(s.w[i], s.h[i]);
                 out_off += 8 * (size_t)s.w[i] * s.h[i];
             }
@@ -1344,10 +1306,9 @@ int planes_host(w2x_ctx *ctx, std::vector<Step> &steps, const float *const *in, 
         in_off[i + 1] = in_off[i] + (size_t)widths[i] * heights[i];
         out_off[i + 1] = out_off[i] + (size_t)L.w[i] * L.h[i];
     }
-    int rc = ensure(reinterpret_cast<void **>(&ctx->io_buf[0]), &ctx->io_bytes[0], in_off.back() * sizeof(float));
-    if (!rc) rc = ensure(reinterpret_cast<void **>(&ctx->io_buf[1]), &ctx->io_bytes[1], out_off.back() * sizeof(float));
+    int rc = reserve_io(ctx, in_off.back() * sizeof(float), out_off.back() * sizeof(float));
     if (rc) return rc;
-    float *din = ctx->io_buf[0], *dout = ctx->io_buf[1];
+    float *din = ctx->io_buf[0].get(), *dout = ctx->io_buf[1].get();
     std::vector<PlaneIO> ends(n_planes);
     for (size_t i = 0; i < n_planes; i++) ends[i] = PlaneIO{din + in_off[i], (size_t)widths[i] * 4, dout + out_off[i], (size_t)L.w[i] * 4};
     std::vector<FrameDev> fd;
@@ -1407,21 +1368,19 @@ int tiles_enqueue_compute(w2x_ctx *ctx, const w2x_model *model, const float *con
     if (rc) return rc;
     DeviceGuard g(ctx->device);
     const size_t tile_bytes = (size_t)width * height * sizeof(float);
-    for (int i = 0; i < 2; i++) {
-        rc = ensure(reinterpret_cast<void **>(&ctx->io_buf[i]), &ctx->io_bytes[i], tile_bytes * (size_t)n_tiles);
-        if (rc) return rc;
-    }
+    rc = reserve_io(ctx, tile_bytes * (size_t)n_tiles, tile_bytes * (size_t)n_tiles);
+    if (rc) return rc;
     for (int t = 0; t < n_tiles; t++)
-        CU_CHECK(cudaMemcpy2DAsync(reinterpret_cast<char *>(ctx->io_buf[0]) + tile_bytes * (size_t)t, (size_t)width * 4, in_tiles[t], in_stride_bytes,
+        CU_CHECK(cudaMemcpy2DAsync(reinterpret_cast<char *>(ctx->io_buf[0].get()) + tile_bytes * (size_t)t, (size_t)width * 4, in_tiles[t], in_stride_bytes,
                                    (size_t)width * 4, (size_t)height, cudaMemcpyHostToDevice, ctx->stream));
-    return convert_tiles_dev(ctx, model, ctx->io_buf[0], ctx->io_buf[1], n_tiles, width, height);
+    return convert_tiles_dev(ctx, model, ctx->io_buf[0].get(), ctx->io_buf[1].get(), n_tiles, width, height);
 }
 
 int tiles_enqueue_download(w2x_ctx *ctx, float *const *out_tiles, int n_tiles, int width, int height, size_t out_stride_bytes) {
     DeviceGuard g(ctx->device);
     const size_t tile_bytes = (size_t)width * height * sizeof(float);
     for (int t = 0; t < n_tiles; t++)
-        CU_CHECK(cudaMemcpy2DAsync(out_tiles[t], out_stride_bytes, reinterpret_cast<char *>(ctx->io_buf[1]) + tile_bytes * (size_t)t, (size_t)width * 4,
+        CU_CHECK(cudaMemcpy2DAsync(out_tiles[t], out_stride_bytes, reinterpret_cast<char *>(ctx->io_buf[1].get()) + tile_bytes * (size_t)t, (size_t)width * 4,
                                    (size_t)width * 4, (size_t)height, cudaMemcpyDeviceToHost, ctx->stream));
     return W2X_OK;
 }
@@ -1448,11 +1407,9 @@ int w2x_convert_tiles(w2x_ctx *ctx, const w2x_model *model, const float *const *
     if (rc) return rc;
     DeviceGuard g(ctx->device);
     const size_t tile_px = (size_t)width * height, row = (size_t)width * 4;
-    for (int i = 0; i < 2; i++) {
-        rc = ensure(reinterpret_cast<void **>(&ctx->io_buf[i]), &ctx->io_bytes[i], tile_px * sizeof(float) * (size_t)n_tiles);
-        if (rc) return rc;
-    }
-    float *din = ctx->io_buf[0], *dout = ctx->io_buf[1];
+    rc = reserve_io(ctx, tile_px * sizeof(float) * (size_t)n_tiles, tile_px * sizeof(float) * (size_t)n_tiles);
+    if (rc) return rc;
+    float *din = ctx->io_buf[0].get(), *dout = ctx->io_buf[1].get();
     // Larger batches run as up to four groups: the uploads of group g+1 and the downloads of group g-1 overlap the layers of
     // group g (copy engines + compute), as the row bands of w2x_convert_plane do.  Tiles are independent, so the grouping
     // does not change a bit of any of them.
@@ -1567,12 +1524,11 @@ int chain_host(w2x_ctx *ctx, std::vector<Step> &steps, const float *in, int widt
     const bool up = steps[last].up;
     const int n = (int)m->layers.size(), w = steps[last].w[0], h = steps[last].h[0];
     const size_t in_dense = (size_t)width * 4;
-    int rc = ensure(reinterpret_cast<void **>(&ctx->io_buf[0]), &ctx->io_bytes[0], (size_t)width * height * sizeof(float));
-    if (!rc) rc = ensure(reinterpret_cast<void **>(&ctx->io_buf[1]), &ctx->io_bytes[1], (size_t)w * h * sizeof(float));
+    int rc = reserve_io(ctx, (size_t)width * height * sizeof(float), (size_t)w * h * sizeof(float));
     std::vector<FrameDev> fd;
-    if (!rc) rc = prepare_planes(ctx, steps, {PlaneIO{ctx->io_buf[0], in_dense, ctx->io_buf[1], (size_t)w * 4}}, false, &fd);
+    if (!rc) rc = prepare_planes(ctx, steps, {PlaneIO{ctx->io_buf[0].get(), in_dense, ctx->io_buf[1].get(), (size_t)w * 4}}, false, &fd);
     if (rc) return rc;
-    CU_CHECK(cudaMemcpy2DAsync(ctx->io_buf[0], in_dense, in, in_stride_bytes, in_dense, (size_t)height, cudaMemcpyHostToDevice, ctx->stream));
+    CU_CHECK(cudaMemcpy2DAsync(ctx->io_buf[0].get(), in_dense, in, in_stride_bytes, in_dense, (size_t)height, cudaMemcpyHostToDevice, ctx->stream));
     rc = run_steps(ctx, steps, fd, 0, last, block_splitting, on_step, user, true);
     if (rc) {   // the upload may still read the caller's plane
         cudaStreamSynchronize(ctx->stream);

@@ -93,6 +93,7 @@ int w2x_band_create(w2x_ctx *ctx, const w2x_model *model, int width, int band_ro
     b->model = model;
     rc = get_dev_model(ctx, model, &b->dm);
     if (rc) return rc;
+    b->dm->band_sessions++;        // w2x_ctx_forget_model refuses until the session goes
     b->n = (int)model->layers.size();
     b->width = width;
     b->rows = band_rows;
@@ -104,49 +105,28 @@ int w2x_band_create(w2x_ctx *ctx, const w2x_model *model, int width, int band_ro
     b->pb = b->down ? 1 : b->n;
     b->pw = width + 2 * b->n;
     b->hf = band_rows + b->pt + b->pb;
-    int maxc = 1;
-    for (auto &L : model->layers) maxc = std::max(maxc, std::max(L.n_in, L.n_out));
-    b->act_bytes = tc::act_bytes(maxc, b->pw, b->hf);
-    auto cleanup = [&](cudaError_t e) {
-        cudaFree(b->pad);
-        cudaFree(b->act[0]);
-        cudaFree(b->act[1]);
-        cudaFree(b->flags);
+    b->act_bytes = tc::act_bytes(max_channels(model), b->pw, b->hf);
+    auto nomem = [](cudaError_t e) {
         cudaGetLastError();
         return fail(W2X_ERR_NOMEM, "w2x_band_create: cudaMalloc failed (%s)", cudaGetErrorString(e));
     };
     cudaError_t e;
-    if ((e = cudaMalloc(&b->pad, (size_t)b->pw * b->hf * sizeof(float))) != cudaSuccess) return cleanup(e);
+    if ((e = b->pad.grow((size_t)b->pw * b->hf * sizeof(float))) != cudaSuccess) return nomem(e);
     for (int i = 0; i < 2; i++)
-        if ((e = cudaMalloc(&b->act[i], b->act_bytes)) != cudaSuccess) return cleanup(e);
-    if ((e = cudaMalloc(&b->flags, 64)) != cudaSuccess) return cleanup(e);
-    if ((e = cudaMemset(b->flags, 0, 64)) != cudaSuccess) return cleanup(e);
-    if ((e = cudaDeviceSynchronize()) != cudaSuccess) return cleanup(e);       // the flag words are zero before a neighbour can write them
-    b->dm->band_sessions++;                                                    // w2x_ctx_forget_model refuses until w2x_band_destroy
+        if ((e = b->act[i].grow(b->act_bytes)) != cudaSuccess) return nomem(e);
+    if ((e = b->flags.grow(64)) != cudaSuccess) return nomem(e);
+    if ((e = cudaMemset(b->flags.get(), 0, 64)) != cudaSuccess) return nomem(e);
+    if ((e = cudaDeviceSynchronize()) != cudaSuccess) return nomem(e);         // the flag words are zero before a neighbour can write them
     *out_band = b.release();
     return W2X_OK;
 }
 
 void w2x_band_destroy(w2x_band *band) {
     if (!band) return;
-    if (band->ctx) {
-        DeviceGuard g(band->ctx->device);
-        cudaStreamSynchronize(band->ctx->stream);
-        for (auto &p : band->peer) {
-            if (!p.ipc) continue;
-            if (p.pad) cudaIpcCloseMemHandle(p.pad);
-            if (p.act[0]) cudaIpcCloseMemHandle(p.act[0]);
-            if (p.act[1]) cudaIpcCloseMemHandle(p.act[1]);
-            if (p.flags) cudaIpcCloseMemHandle(p.flags);
-        }
-        cudaFree(band->pad);
-        cudaFree(band->act[0]);
-        cudaFree(band->act[1]);
-        cudaFree(band->flags);
-        cudaGetLastError();
-    }
-    if (band->dm) band->dm->band_sessions--;
+    DeviceGuard g(band->ctx->device);
+    cudaStreamSynchronize(band->ctx->stream);
     delete band;
+    cudaGetLastError();
 }
 
 // d_in: the band's rows PLUS one real row per neighbour side (the caller fetched them); every frame row is written.
@@ -159,7 +139,7 @@ int w2x_band_load(w2x_band *band, const float *d_in, size_t in_stride_bytes) {
     const long stride = (long)(in_stride_bytes / 4);
     const float *band0 = d_in + (band->up ? stride : 0);
     CU_CHECK(launch_pad_replicate_xy(band0, band->width, band->rows, stride, band->n, band->pt, band->pb, band->up ? 1 : 0,
-                                     band->down ? 1 : 0, band->pad, ctx->stream));
+                                     band->down ? 1 : 0, band->pad.get(), ctx->stream));
     ctx->launches++;
     band->last_step = -1;
     band->cur = 0;
@@ -174,7 +154,7 @@ int w2x_band_load_rows(w2x_band *band, const float *d_in, size_t in_stride_bytes
     w2x_ctx *ctx = band->ctx;
     DeviceGuard g(ctx->device);
     CU_CHECK(launch_pad_replicate_xy(d_in, band->width, band->rows, (long)(in_stride_bytes / 4), band->n, band->pt, band->pb,
-                                     band->ov_up ? band->n : 0, band->ov_down ? band->n : 0, band->pad, ctx->stream, band->up ? 1 : 0,
+                                     band->ov_up ? band->n : 0, band->ov_down ? band->n : 0, band->pad.get(), ctx->stream, band->up ? 1 : 0,
                                      band->down ? 1 : 0));
     ctx->launches++;
     band->last_step = -1;
@@ -196,13 +176,13 @@ int w2x_band_step(w2x_band *band, int step) {
     const int y0 = band->up ? 1 : 0, rows = band->hf - y0 - (band->down ? 1 : 0);
     if (step == 0) {
         LayerTimer t(ctx, 0);
-        const tc::FirstSource fsrc{band->pad, band->pw, band->pw, band->hf, 0, 0, 0, 0};       // the session's padded input frame (halo rows come from the neighbours)
-        CU_CHECK(tc::launch_first(fsrc, band->pw, band->hf, L.w.data(), dm->b_host[0].data(), L.n_out, band->act[0], ctx->stream, f8, y0, rows));
+        const tc::FirstSource fsrc{band->pad.get(), band->pw, band->pw, band->hf, 0, 0, 0, 0};       // the session's padded input frame (halo rows come from the neighbours)
+        CU_CHECK(tc::launch_first(fsrc, band->pw, band->hf, L.w.data(), dm->b_host[0].data(), L.n_out, band->act[0].get(), ctx->stream, f8, y0, rows));
         band->cur = 0;
         note_kernel(ctx, 0, "first_1xN");
         ctx->launches++;
     } else {
-        int rc = launch_layer_tc(ctx, m, dm, step, band->act[band->cur], band->act[band->cur ^ 1], band->pw, band->hf, step == band->n - 2, false, y0, rows);
+        int rc = launch_layer_tc(ctx, m, dm, step, band->act[band->cur].get(), band->act[band->cur ^ 1].get(), band->pw, band->hf, step == band->n - 2, false, y0, rows);
         if (rc) return rc;
         band->cur ^= 1;
     }
@@ -215,7 +195,7 @@ int w2x_band_halo(w2x_band *band, int step, int *n_segments, void **send_up, voi
     if (band_check(band)) return W2X_ERR_ARG;
     if (step != band->last_step || step < 0 || !n_segments || !send_up || !recv_up || !send_down || !recv_down || !seg_bytes)
         return fail(W2X_ERR_ARG, "w2x_band_halo: call it for the step that was queued last");
-    char *base = reinterpret_cast<char *>(band->act[band->cur]);
+    char *base = reinterpret_cast<char *>(band->act[band->cur].get());
     RowSeg seg[4];
     size_t bytes, px;
     const int nseg = row_segments(band, step, seg, &bytes, &px);
@@ -240,7 +220,7 @@ int w2x_band_finish(w2x_band *band, float *d_out, size_t out_stride_bytes) {
     const Layer &L = band->model->layers.back();
     {
         LayerTimer t(ctx, band->n - 1);
-        CU_CHECK(tc::launch_last_gather_xy(reinterpret_cast<const float *>(band->act[band->cur]), band->pw, band->hf,
+        CU_CHECK(tc::launch_last_gather_xy(reinterpret_cast<const float *>(band->act[band->cur].get()), band->pw, band->hf,
                                            static_cast<float>(L.b[0]), band->n, band->pt, band->pb, d_out,
                                            (long)(out_stride_bytes / 4), ctx->stream));
     }
@@ -262,10 +242,10 @@ int w2x_band_export(w2x_band *band, void *blob) {
     bl.n = band->n;
     bl.precision = band->ctx->precision;
     bl.act_bytes = band->act_bytes;
-    CU_CHECK(cudaIpcGetMemHandle(&bl.pad, band->pad));
-    CU_CHECK(cudaIpcGetMemHandle(&bl.act0, band->act[0]));
-    CU_CHECK(cudaIpcGetMemHandle(&bl.act1, band->act[1]));
-    CU_CHECK(cudaIpcGetMemHandle(&bl.flags, band->flags));
+    CU_CHECK(cudaIpcGetMemHandle(&bl.pad, band->pad.get()));
+    CU_CHECK(cudaIpcGetMemHandle(&bl.act0, band->act[0].get()));
+    CU_CHECK(cudaIpcGetMemHandle(&bl.act1, band->act[1].get()));
+    CU_CHECK(cudaIpcGetMemHandle(&bl.flags, band->flags.get()));
     std::memset(blob, 0, W2X_BAND_BLOB_BYTES);
     std::memcpy(blob, &bl, sizeof bl);
     return W2X_OK;
@@ -317,10 +297,10 @@ int w2x_band_connect_local(w2x_band *band, w2x_band *up, w2x_band *down) {
             cudaGetLastError();
         }
         w2x_band::Peer &p = band->peer[side];
-        p.pad = o->pad;
-        p.act[0] = reinterpret_cast<char *>(o->act[0]);
-        p.act[1] = reinterpret_cast<char *>(o->act[1]);
-        p.flags = o->flags;
+        p.pad = o->pad.get();
+        p.act[0] = reinterpret_cast<char *>(o->act[0].get());
+        p.act[1] = reinterpret_cast<char *>(o->act[1].get());
+        p.flags = o->flags.get();
         p.hf = o->hf;
         p.ipc = false;
     }
@@ -340,7 +320,7 @@ int w2x_band_exchange(w2x_band *band, int step) {
     RowSeg seg[4];
     size_t bytes, px;
     const int nseg = row_segments(band, step, seg, &bytes, &px);
-    char *mine = step < 0 ? reinterpret_cast<char *>(band->pad) : reinterpret_cast<char *>(band->act[band->cur]);
+    char *mine = step < 0 ? reinterpret_cast<char *>(band->pad.get()) : reinterpret_cast<char *>(band->act[band->cur].get());
     HaloXArgs a{};
     for (int s = 0; s < nseg; s++) {
         if (band->up) {      // my first owned row -> the up neighbour's halo row below (its last frame row)
@@ -359,13 +339,14 @@ int w2x_band_exchange(w2x_band *band, int step) {
         }
     }
     a.bytes = bytes;
-    a.counter = band->flags + 4;
+    unsigned *const flags = band->flags.get();
+    a.counter = flags + 4;
     a.value = ++band->seq;
     // I am the DOWN neighbour of my up peer (its flag 1) and the UP neighbour of my down peer (its flag 0)
     a.peer_flag[0] = band->up ? band->peer[0].flags + 1 : nullptr;
     a.peer_flag[1] = band->down ? band->peer[1].flags + 0 : nullptr;
-    a.my_flag[0] = band->up ? band->flags + 0 : nullptr;
-    a.my_flag[1] = band->down ? band->flags + 1 : nullptr;
+    a.my_flag[0] = band->up ? flags + 0 : nullptr;
+    a.my_flag[1] = band->down ? flags + 1 : nullptr;
     NvtxRange nvtx("w2x halo exchange");
     CU_CHECK(launch_halo_exchange(a, ctx->stream));
     ctx->launches++;
@@ -401,26 +382,26 @@ struct w2x_slab {
     bool up = false, down = false;
     std::vector<w2x_band *> sub;
     std::vector<int> r0;                         // sub-band s owns slab rows [r0[s], r0[s+1])
-    float *d_in = nullptr, *d_out = nullptr;     // [rows][width]
+    DevBuf<float> d_in, d_out;                   // [rows][width]
     std::vector<cudaEvent_t> ev_in, ev_done;
     cudaEvent_t ev_drained = nullptr;            // the previous pass's downloads have left d_out
+
+    // The sub-bands and the events; d_in and d_out go after this body.  The caller has made the context's device current.
+    ~w2x_slab() {
+        for (auto b : sub) w2x_band_destroy(b);
+        for (auto e : ev_in) cudaEventDestroy(e);
+        for (auto e : ev_done) cudaEventDestroy(e);
+        if (ev_drained) cudaEventDestroy(ev_drained);
+    }
 };
 
 extern "C" {
 
 void w2x_slab_destroy(w2x_slab *s) {
     if (!s) return;
-    for (auto b : s->sub) w2x_band_destroy(b);
-    if (s->ctx) {
-        DeviceGuard g(s->ctx->device);
-        cudaFree(s->d_in);
-        cudaFree(s->d_out);
-        for (auto e : s->ev_in) cudaEventDestroy(e);
-        for (auto e : s->ev_done) cudaEventDestroy(e);
-        if (s->ev_drained) cudaEventDestroy(s->ev_drained);
-        cudaGetLastError();
-    }
+    DeviceGuard g(s->ctx->device);
     delete s;
+    cudaGetLastError();
 }
 
 int w2x_slab_create(w2x_ctx *ctx, const w2x_model *model, int width, int rows, int has_up, int has_down, int order, int n_sub, w2x_slab **out) {
@@ -433,7 +414,8 @@ int w2x_slab_create(w2x_ctx *ctx, const w2x_model *model, int width, int rows, i
     // ... and as many as it takes for every sub-band's frame (its rows + at most n above and below) to stay within MAX_FRAME_ROWS
     const long sub_max = MAX_FRAME_ROWS - 2 * n;
     n_sub = std::max(n_sub, (int)((rows + sub_max - 1) / sub_max));
-    auto s = std::unique_ptr<w2x_slab, void (*)(w2x_slab *)>(new w2x_slab(), w2x_slab_destroy);
+    DeviceGuard g(ctx->device);   // before the slab: it is still current when an early return destroys what has been created
+    auto s = std::make_unique<w2x_slab>();
     s->ctx = ctx;
     s->model = model;
     s->width = width;
@@ -442,7 +424,6 @@ int w2x_slab_create(w2x_ctx *ctx, const w2x_model *model, int width, int rows, i
     s->up = has_up != 0;
     s->down = has_down != 0;
     for (int i = 0; i <= n_sub; i++) s->r0.push_back((int)((long)rows * i / n_sub));
-    DeviceGuard g(ctx->device);
     for (int i = 0; i < n_sub; i++) {
         w2x_band *b = nullptr;
         const int ue = i == 0 ? (s->up ? W2X_EDGE_NEIGHBOUR : W2X_EDGE_BORDER) : W2X_EDGE_OVERLAP;
@@ -451,8 +432,8 @@ int w2x_slab_create(w2x_ctx *ctx, const w2x_model *model, int width, int rows, i
         if (rc) return rc;
         s->sub.push_back(b);
     }
-    CU_CHECK(cudaMalloc(&s->d_in, (size_t)rows * width * 4));
-    CU_CHECK(cudaMalloc(&s->d_out, (size_t)rows * width * 4));
+    CU_CHECK(s->d_in.grow((size_t)rows * width * 4));
+    CU_CHECK(s->d_out.grow((size_t)rows * width * 4));
     for (int i = 0; i < n_sub; i++) {
         cudaEvent_t e;
         CU_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
@@ -514,14 +495,14 @@ int slab_enqueue_compute(w2x_slab *s, const float *in, size_t in_stride_bytes) {
         int ya, yb;
         if (!s->order) { ya = s->r0[(size_t)i] + (t == 0 ? 0 : n); yb = s->r0[(size_t)i + 1] + (t == K - 1 ? 0 : n); }
         else { ya = s->r0[(size_t)i] - (t == K - 1 ? 0 : n); yb = s->r0[(size_t)i + 1] - (t == 0 ? 0 : n); }
-        CU_CHECK(cudaMemcpy2DAsync(s->d_in + (size_t)ya * s->width, rowb, reinterpret_cast<const char *>(in) + (size_t)ya * in_stride_bytes, in_stride_bytes, rowb,
+        CU_CHECK(cudaMemcpy2DAsync(s->d_in.get() + (size_t)ya * s->width, rowb, reinterpret_cast<const char *>(in) + (size_t)ya * in_stride_bytes, in_stride_bytes, rowb,
                                    (size_t)(yb - ya), cudaMemcpyHostToDevice, ctx->copy_in));
         CU_CHECK(cudaEventRecord(s->ev_in[(size_t)i], ctx->copy_in));
     }
     for (int t = 0; t < K; t++) {
         const int i = at(t), y = s->r0[(size_t)i];
         CU_CHECK(cudaStreamWaitEvent(ctx->stream, s->ev_in[(size_t)i], 0));   // own rows + the overlap rows (earlier uploads are ordered before it)
-        int rc = w2x_band_run(s->sub[(size_t)i], s->d_in + (size_t)y * s->width, rowb, s->d_out + (size_t)y * s->width, rowb);
+        int rc = w2x_band_run(s->sub[(size_t)i], s->d_in.get() + (size_t)y * s->width, rowb, s->d_out.get() + (size_t)y * s->width, rowb);
         if (rc) {
             cudaStreamSynchronize(ctx->copy_in);
             cudaStreamSynchronize(ctx->stream);
@@ -543,7 +524,7 @@ int slab_enqueue_download(w2x_slab *s, float *out, size_t out_stride_bytes) {
     for (int t = 0; t < K; t++) {
         const int i = s->order ? K - 1 - t : t, y = s->r0[(size_t)i], rows = s->r0[(size_t)i + 1] - y;
         CU_CHECK(cudaStreamWaitEvent(ctx->copy_out, s->ev_done[(size_t)i], 0));
-        CU_CHECK(cudaMemcpy2DAsync(reinterpret_cast<char *>(out) + (size_t)y * out_stride_bytes, out_stride_bytes, s->d_out + (size_t)y * s->width, rowb, rowb,
+        CU_CHECK(cudaMemcpy2DAsync(reinterpret_cast<char *>(out) + (size_t)y * out_stride_bytes, out_stride_bytes, s->d_out.get() + (size_t)y * s->width, rowb, rowb,
                                    (size_t)rows, cudaMemcpyDeviceToHost, ctx->copy_out));
     }
     CU_CHECK(cudaEventRecord(s->ev_drained, ctx->copy_out));

@@ -21,12 +21,51 @@
 namespace w2x {
 namespace eng {
 
+// One cudaMalloc block and its owner: freed by the destructor, move-only.  It only ever grows, and a grow keeps no contents.  The
+// device that allocated it must be current whenever it grows or goes (DeviceGuard in the caller).
+struct DevMem {
+    void *p = nullptr;
+    size_t bytes = 0;
+    DevMem() = default;
+    DevMem(DevMem &&o) noexcept : p(o.p), bytes(o.bytes) { o.p = nullptr; o.bytes = 0; }
+    DevMem &operator=(DevMem &&o) noexcept {   // o takes this block away and frees it when it goes
+        std::swap(p, o.p);
+        std::swap(bytes, o.bytes);
+        return *this;
+    }
+    ~DevMem() { release(); }
+    void release() {
+        if (p) cudaFree(p);
+        p = nullptr;
+        bytes = 0;
+    }
+    // At least `need` bytes: nothing happens when they are there; else the old block is freed first (cudaFree also orders the free
+    // after the kernels that still read it) and a failed cudaMalloc leaves the buffer empty and no sticky error behind.
+    cudaError_t grow(size_t need) {
+        if (bytes >= need) return cudaSuccess;
+        release();
+        cudaError_t e = cudaMalloc(&p, need);
+        if (e == cudaSuccess) bytes = need;
+        else cudaGetLastError();
+        return e;
+    }
+    int reserve(size_t need) {   // grow() for scratch: running out of device memory is W2X_ERR_NOMEM
+        cudaError_t e = grow(need);
+        if (e != cudaSuccess) return fail(W2X_ERR_NOMEM, "cudaMalloc of %zu bytes failed (%s)", need, cudaGetErrorString(e));
+        return W2X_OK;
+    }
+};
+template <class T>
+struct DevBuf : DevMem {
+    T *get() const { return static_cast<T *>(p); }
+};
+
 struct DevModel {                       // device-resident copy of one model
-    std::vector<float *> w;             // per layer [Cout][Cin][9] fp32
-    std::vector<float *> b;             // per layer [Cout] fp32  ((float)bias, src/modelHandler.cpp:147)
+    std::vector<DevBuf<float>> w;       // per layer [Cout][Cin][9] fp32
+    std::vector<DevBuf<float>> b;       // per layer [Cout] fp32  ((float)bias, src/modelHandler.cpp:147)
     std::vector<std::vector<float>> b_host;   // the same on the host (the tensor-core kernels take them as kernel parameters)
-    std::vector<uint16_t *> pack;       // per layer tensor-core operand image (nullptr if not eligible)
-    std::vector<uint8_t *> pack8;       // same for the "f8" flavour (fp16 main product + e4m3 corrections)
+    std::vector<DevBuf<uint16_t>> pack; // per layer tensor-core operand image (empty if not eligible)
+    std::vector<DevBuf<uint8_t>> pack8; // same for the "f8" flavour (fp16 main product + e4m3 corrections)
     std::vector<float> out_scale;       // 1 / (wscale * ACT_SCALE)
     std::vector<float> last_w_t;        // HOST: last layer's weights transposed to [9][Cin] (fused last layer, passed as kernel parameters)
     int band_sessions = 0;              // live w2x_band sessions that launch with these copies (w2x_ctx_forget_model refuses while > 0)
@@ -57,25 +96,32 @@ struct w2x_ctx {
     std::vector<std::string> layer_kernel;
     std::map<uint64_t, w2x::eng::DevModel> models;
     // scratch
-    void *buf[2] = {nullptr, nullptr};
-    size_t buf_bytes[2] = {0, 0};
-    float *pad_buf = nullptr;
-    size_t pad_bytes = 0;
-    float *io_buf[2] = {nullptr, nullptr};   // device staging for the host-buffer entry points
-    size_t io_bytes[2] = {0, 0};
-    float *chain_buf[2] = {nullptr, nullptr};   // the planes between the steps of w2x_convert_chain*
-    size_t chain_bytes[2] = {0, 0};
-    float *tta_buf[2] = {nullptr, nullptr};     // a W2X_STEP_TTA step's 8 variants per plane (0) and their conversions (1)
-    size_t tta_bytes[2] = {0, 0};
+    w2x::eng::DevBuf<void> buf[2];
+    w2x::eng::DevBuf<float> pad_buf;
+    w2x::eng::DevBuf<float> io_buf[2];      // device staging for the host-buffer entry points
+    w2x::eng::DevBuf<float> chain_buf[2];   // the planes between the steps of w2x_convert_chain*
+    w2x::eng::DevBuf<float> tta_buf[2];     // a W2X_STEP_TTA step's 8 variants per plane (0) and their conversions (1)
     bool tc_ready = false;
     cudaStream_t copy_in = nullptr, copy_out = nullptr;   // host<->device copies of run_host_groups overlap the compute stream
     cudaEvent_t ev_in[8] = {}, ev_done[8] = {};
     int host_bands = 0;                                   // 0 = automatic (up to 4 bands of >= 512 rows), 1 = no pipelining
-    void *plan_buf = nullptr;                             // device tables of the packed frames (w2x_convert_planes, w2x_convert_tiles)
-    size_t plan_bytes = 0;
+    w2x::eng::DevBuf<char> plan_buf;                      // device tables of the packed frames (w2x_convert_planes, w2x_convert_tiles)
     cudaEvent_t plan_ev = nullptr;                        // recorded after the last kernel that reads plan_buf
     bool plan_ev_live = false;
-    unsigned long long *prof_buf = nullptr;   // [16 layers][PROF_MAX_CTAS][PROF_WORDS], debug profile
+    w2x::eng::DevBuf<unsigned long long> prof_buf;   // [16 layers][PROF_MAX_CTAS][PROF_WORDS], debug profile
+
+    // The streams and events (those w2x_ctx_create got as far as creating); the buffers and the models free themselves after this
+    // body.  The caller has made `device` current and keeps it so until the delete returns (w2x_ctx_destroy).
+    ~w2x_ctx() {
+        auto drop = [](cudaEvent_t e) { if (e) cudaEventDestroy(e); };
+        drop(plan_ev);
+        for (auto &s : spans) { drop(s.e0); drop(s.e1); }
+        for (auto e : event_pool) drop(e);
+        for (int i = 0; i < 8; i++) { drop(ev_in[i]); drop(ev_done[i]); }
+        if (copy_in) cudaStreamDestroy(copy_in);
+        if (copy_out) cudaStreamDestroy(copy_out);
+        if (own_stream) cudaStreamDestroy(own_stream);
+    }
 };
 
 // One rank's rows of a plane (w2x_band_*): every intermediate activation keeps only the band's rows plus one halo row per
@@ -83,27 +129,38 @@ struct w2x_ctx {
 struct w2x_band {
     w2x_ctx *ctx = nullptr;
     const w2x_model *model = nullptr;
-    w2x::eng::DevModel *dm = nullptr;
+    w2x::eng::DevModel *dm = nullptr;   // set together with its band_sessions count
     int width = 0, rows = 0, n = 0;
     bool up = false, down = false; // a neighbour GPU owns the rows above / below: one halo row, exchanged after every layer
     bool ov_up = false, ov_down = false;   // the n rows above / below are REAL input rows supplied with the band (recomputed overlap, no exchange)
     int pt = 0, pb = 0;            // frame rows above / below the band: 1 (neighbour halo) or n (image border: replicated; overlap: real rows)
     int pw = 0, hf = 0;            // frame width / height
-    float *pad = nullptr;          // padded fp32 input frame
-    __half *act[2] = {nullptr, nullptr};
+    w2x::eng::DevBuf<float> pad;   // padded fp32 input frame
+    w2x::eng::DevBuf<__half> act[2];
     size_t act_bytes = 0;
     int cur = 0;                   // act[cur] holds the output of the last queued step
     int last_step = -1;
     // peer-memory exchange (w2x_band_connect* / w2x_band_exchange)
-    unsigned *flags = nullptr;     // [0] "rows from the up neighbour have landed", [1] same from down, [4] block counter
+    w2x::eng::DevBuf<unsigned> flags;   // [0] "rows from the up neighbour have landed", [1] same from down, [4] block counter
     unsigned seq = 0;              // exchanges issued so far: the value the next one publishes / waits for is seq + 1
     struct Peer {
         float *pad = nullptr;
         char *act[2] = {nullptr, nullptr};
         unsigned *flags = nullptr;
         int hf = 0;
-        bool ipc = false;          // mapped with cudaIpcOpenMemHandle (closed in w2x_band_destroy)
+        bool ipc = false;          // mapped with cudaIpcOpenMemHandle (closed with the session); else the neighbour's own pointers
     } peer[2];                     // 0 = up, 1 = down
+
+    // Unmaps the neighbours' memory before the session's own buffers go (after this body), and gives the model's device copies
+    // back to w2x_ctx_forget_model.  The caller has made the context's device current (w2x_band_create, w2x_band_destroy).
+    ~w2x_band() {
+        for (auto &p : peer) {
+            if (!p.ipc) continue;
+            for (void *q : {(void *)p.pad, (void *)p.act[0], (void *)p.act[1], (void *)p.flags})
+                if (q) cudaIpcCloseMemHandle(q);
+        }
+        if (dm) dm->band_sessions--;
+    }
 };
 
 namespace w2x {
@@ -130,7 +187,7 @@ struct DeviceGuard {
 };
 
 // ---- helpers defined in engine.cu --------------------------------------------------------------------------------------
-int ensure(void **p, size_t *have, size_t need);
+int max_channels(const w2x_model *m);   // the widest activation of the model, in channels
 int get_dev_model(w2x_ctx *ctx, const w2x_model *m, DevModel **out);
 cudaEvent_t take_event(w2x_ctx *ctx);
 void note_kernel(w2x_ctx *ctx, int layer, const char *name);
