@@ -301,7 +301,8 @@ W2X_API int w2x_convert_planes_device(w2x_ctx *ctx, const w2x_model *model, int 
  * whole sequence can run in one call that keeps the plane on the device between steps and never builds the 2x plane.
  * Step k computes P_{k+1} = convertWithModels(models[k], U_k(P_k)), P_0 = in, U_k = identity (W2X_STEP_SAME) or the nearest 2x
  * resize (W2X_STEP_UPSCALE2X); every P_{k+1} is bit-identical to w2x_convert_plane(ctx, models[k], U_k(P_k), ..., block_splitting)
- * on the same context settings.  The output is (width << u) x (height << u), u = the number of upscaling steps.
+ * on the same context settings.  The output is (width << u) x (height << u), u = the number of upscaling steps.  With n_steps == 1
+ * and W2X_STEP_SAME this is w2x_convert_plane (w2x_convert_plane_device): same bits, same progress lines, same launches.
  * Before step k is queued, on_step(k, user) is called (if not NULL); then the step logs the progress lines w2x_convert_plane
  * (host entry) or w2x_convert_plane_device (device entry) logs for its plane, block lines included.
  * Every argument is checked before anything is queued; W2X_ERR_ARG names the step: n_steps < 1, a NULL models / kinds array or

@@ -166,17 +166,19 @@ int launch_layer_tc(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int li, cons
     return W2X_OK;
 }
 
-// ---- convertWithModelsBasic on an already padded ROI ------------------------------------------
-// src: pw x ph fp32 region (row stride src_stride floats) that already contains the n-pixel ring.
+// A pw x ph fp32 region (row stride `stride` floats) that already contains the n-pixel ring, as the first layer's source.
+tc::FirstSource padded(const float *p, long stride, int pw, int ph) { return tc::FirstSource{p, stride, pw, ph, 0, 0, 0, 0}; }
+
+// ---- convertWithModelsBasic on a pw x ph frame ------------------------------------------------
+// src: what the first layer reads: a padded region (padded()), or (tensor-core engine only) an unpadded plane with the replicate
+// padding folded into the loads.  The fp32 engine copies src.in / src.stride_floats, which is then always a padded region.
 // dst: receives the (pw-2n) x (ph-2n) interior.
 // packed (tensor-core engine with the fused last layer only): src is a packed frame of pw x ph holding many padded planes (see
 // tc::PlaneRect); the layers run ONCE on it -- the seams pollute only the rings that are cropped anyway -- and one gather writes
 // every plane's interior to its own destination; dst / dst_stride are then unused.
-// direct (tensor-core engine, one plane): the first layer reads the UNPADDED plane it describes and folds the replicate padding into
-// its loads; src / src_stride are then unused.
 struct PackedGather { const tc::PlaneRect *rect; int n_rect, n_blocks; };
-int run_basic(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int engine, const float *src, long src_stride, int pw,
-              int ph, float *dst, long dst_stride, const PackedGather *packed = nullptr, const tc::FirstSource *direct = nullptr) {
+int run_basic(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int engine, const tc::FirstSource &src, int pw, int ph, float *dst,
+              long dst_stride, const PackedGather *packed = nullptr) {
     const int n = (int)m->layers.size();
     if (pw - 2 * n < 1 || ph - 2 * n < 1) return fail(W2X_ERR_ARG, "plane smaller than the model's receptive ring");
     const int maxc = max_channels(m);
@@ -187,7 +189,7 @@ int run_basic(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int engine, const 
             if (rc) return rc;
         }
         float *cur = static_cast<float *>(ctx->buf[0].get()), *nxt = static_cast<float *>(ctx->buf[1].get());
-        CU_CHECK(launch_copy2d(src, src_stride, cur, pw, pw, ph, ctx->stream));   // ROI -> dense plane
+        CU_CHECK(launch_copy2d(src.in, src.stride_floats, cur, pw, pw, ph, ctx->stream));   // ROI -> dense plane
         ctx->launches++;
         for (int li = 0; li < n; li++) {
             const Layer &L = m->layers[(size_t)li];
@@ -217,9 +219,8 @@ int run_basic(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int engine, const 
     {
         const Layer &L = m->layers[0];
         LayerTimer t(ctx, 0);
-        const tc::FirstSource padded{src, src_stride, pw, ph, 0, 0, 0, 0};
-        CU_CHECK(tc::launch_first(direct ? *direct : padded, pw, ph, L.w.data(), dm->b_host[0].data(), L.n_out, cur, ctx->stream, f8));
-        note_kernel(ctx, 0, direct && direct->up2x ? "first_1xN+up2x" : "first_1xN");
+        CU_CHECK(tc::launch_first(src, pw, ph, L.w.data(), dm->b_host[0].data(), L.n_out, cur, ctx->stream, f8));
+        note_kernel(ctx, 0, src.up2x ? "first_1xN+up2x" : "first_1xN");
         ctx->launches++;
     }
     const bool fuse = ctx->fuse_last && n >= 3 && !dm->last_w_t.empty();
@@ -249,46 +250,14 @@ int run_basic(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int engine, const 
     return W2X_OK;
 }
 
-// rows per band of run_padded_plane for a plane w wide: the band's frame (band + 2n rows) fits the scratch limit and has at most
-// MAX_FRAME_ROWS rows
+// rows per scratch band of convert_device for a plane w wide: the band's frame (band + 2n rows) fits the scratch limit and has at
+// most MAX_FRAME_ROWS rows
 int scratch_band_rows(const w2x_ctx *ctx, const w2x_model *m, int w, int h) {
     const int n = (int)m->layers.size();
     const size_t per_row = (size_t)max_channels(m) * (w + 2 * n) * 4;   // both engines: 4 bytes per activation element
     long max_rows = std::min((long)(ctx->scratch_limit / per_row), MAX_FRAME_ROWS) - 2 * n;
     if (max_rows < 16) max_rows = 16;
     return (int)std::min<long>(h, max_rows);
-}
-
-// Whole plane (or row band) already available as a padded plane: cut it into horizontal bands that
-// respect the scratch limit, each band re-reads n rows of context above and below.
-// direct_in != nullptr (tensor-core engine): no padded plane exists; the first layer reads d_in (rows_above / rows_below real rows
-// beyond the plane) with the padding folded into its loads.
-// up2x (direct_in only): the plane is the nearest-neighbour 2x resize of direct_in, w x h its 2x size (see convert_device).
-int run_padded_plane(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int engine, const float *padp, int w, int h,
-                     float *dst, long dst_stride, const float *direct_in = nullptr, long in_stride = 0, int rows_above = 0, int rows_below = 0,
-                     bool up2x = false) {
-    const int n = (int)m->layers.size();
-    const int pw = w + 2 * n;
-    const int band = scratch_band_rows(ctx, m, w, h);
-    for (int y0 = 0; y0 < h; y0 += band) {
-        const int bh = std::min(band, h - y0);
-        int rc;
-        if (direct_in && up2x) {
-            // the band's 2x rows [y0, y0 + bh) seen from source row y0 >> 1: on an odd y0 the band is 2x row 1 of that source row
-            const int p = y0 & 1;
-            tc::FirstSource fs{direct_in + (long)(y0 >> 1) * in_stride, in_stride, w, bh + p, n, n - p, std::min(n, y0 + rows_above) - p,
-                               std::min(n, h - y0 - bh + rows_below)};
-            fs.up2x = true;
-            rc = run_basic(ctx, m, dm, engine, nullptr, 0, pw, bh + 2 * n, dst + (long)y0 * dst_stride, dst_stride, nullptr, &fs);
-        } else if (direct_in) {
-            const tc::FirstSource fs{direct_in + (long)y0 * in_stride, in_stride, w, bh, n, n, std::min(n, y0 + rows_above), std::min(n, h - y0 - bh + rows_below)};
-            rc = run_basic(ctx, m, dm, engine, nullptr, 0, pw, bh + 2 * n, dst + (long)y0 * dst_stride, dst_stride, nullptr, &fs);
-        } else {
-            rc = run_basic(ctx, m, dm, engine, padp + (long)y0 * pw, pw, pw, bh + 2 * n, dst + (long)y0 * dst_stride, dst_stride);
-        }
-        if (rc) return rc;
-    }
-    return W2X_OK;
 }
 
 int check_ctx(w2x_ctx *ctx) {
@@ -301,7 +270,7 @@ bool literal_walk(const w2x_ctx *ctx, int w, int h, int block_splitting) {
     return block_splitting && ctx->walk == W2X_WALK_BLOCKS && w2x_requires_splitting(w, h);
 }
 
-// Row bands of w2x_convert_plane's host copy pipeline for a plane of width x height (1 = no pipeline: one upload, one pass,
+// Row bands of a host plane's copy pipeline (chain_host) for a plane of width x height (1 = no pipeline: one upload, one pass,
 // one download).  The literal block walk keeps its own order, and a band needs 2n rows of its own.
 int host_copy_bands(const w2x_ctx *ctx, int n_model, int width, int height, int block_splitting) {
     int nb = ctx->host_bands > 0 ? ctx->host_bands : std::min(4, height / 512);
@@ -399,7 +368,7 @@ int check_plane(w2x_ctx *ctx, const w2x_model *m, const float *d_in, int w, int 
 
 // The progress lines of one convertWithModels-equivalent plane of w x h (host: through w2x_convert_plane's copy pipeline).  A
 // plane the reference splits gets the reference's block sequence, whichever walk runs it; any other the layers' lines once when
-// the copy pipeline cuts it into bands, else once per scratch band of run_padded_plane.
+// the copy pipeline cuts it into bands, else once per scratch band of convert_device.
 void emit_plane_progress(w2x_ctx *ctx, const w2x_model *m, int w, int h, int block_splitting, bool host) {
     if (!ctx->log) return;
     const int n = (int)m->layers.size();
@@ -422,35 +391,45 @@ int convert_device(w2x_ctx *ctx, const w2x_model *m, const float *d_in, int w, i
     if (rc) return rc;
     const int n = (int)m->layers.size();
     const int pw = w + 2 * n, ph = h + 2 * n;
-    const long ostride = (long)(out_stride_bytes / 4);
+    const long istride = (long)(in_stride_bytes / 4), ostride = (long)(out_stride_bytes / 4);
     const bool literal = literal_walk(ctx, w, h, block_splitting);
-    if (engine == W2X_ENGINE_TC && !literal) {
-        // cv::copyMakeBorder (src/convertRoutine.cpp:35, :96) is folded into the first layer's loads: no padded copy of the plane
-        return run_padded_plane(ctx, m, dm, engine, nullptr, w, h, d_out, ostride, d_in, (long)(in_stride_bytes / 4), rows_above, rows_below,
-                                up2x);
+    // cv::copyMakeBorder(in, temp, n, n, n, n, BORDER_REPLICATE)   (src/convertRoutine.cpp:35, :96): the tensor-core engine folds it
+    // into the first layer's loads and reads d_in directly, except on the literal walk, whose blocks are regions of the padded plane
+    const bool direct = engine == W2X_ENGINE_TC && !literal;
+    float *pad = nullptr;
+    if (!direct) {
+        rc = ctx->pad_buf.reserve((size_t)pw * ph * sizeof(float));
+        if (rc) return rc;
+        pad = ctx->pad_buf.get();
+        if (up2x)
+            CU_CHECK(launch_pad_upsample2x(d_in, w, h, istride, n, std::min(rows_above, n), std::min(rows_below, n), pad, ctx->stream));
+        else
+            CU_CHECK(launch_pad_replicate(d_in, w, h, istride, n, std::min(rows_above, n), std::min(rows_below, n), pad, ctx->stream));
+        ctx->launches++;
     }
-    rc = ctx->pad_buf.reserve((size_t)pw * ph * sizeof(float));
-    if (rc) return rc;
-    float *const pad = ctx->pad_buf.get();
-    // cv::copyMakeBorder(in, temp, n, n, n, n, BORDER_REPLICATE)   (src/convertRoutine.cpp:35, :96)
-    if (up2x)
-        CU_CHECK(launch_pad_upsample2x(d_in, w, h, (long)(in_stride_bytes / 4), n, std::min(rows_above, n), std::min(rows_below, n),
-                                       pad, ctx->stream));
-    else
-        CU_CHECK(launch_pad_replicate(d_in, w, h, (long)(in_stride_bytes / 4), n, std::min(rows_above, n),
-                                      std::min(rows_below, n), pad, ctx->stream));
-    ctx->launches++;
     if (literal) {   // check_blocks has seen every block fit
         const std::vector<int> tab = blocks_of(w, h, n);
         for (size_t i = 0; i < tab.size(); i += 8) {
             const int *t = &tab[i];
-            rc = run_basic(ctx, m, dm, engine, pad + (long)t[2] * pw + t[4], pw, t[5] - t[4], t[3] - t[2],
+            rc = run_basic(ctx, m, dm, engine, padded(pad + (long)t[2] * pw + t[4], pw, t[5] - t[4], t[3] - t[2]), t[5] - t[4], t[3] - t[2],
                            d_out + (long)t[6] * ostride + t[7], ostride);
             if (rc) return rc;
         }
         return W2X_OK;
     }
-    return run_padded_plane(ctx, m, dm, engine, pad, w, h, d_out, ostride);
+    // horizontal bands that respect the scratch limit, each re-reading n rows of context above and below
+    const int band = scratch_band_rows(ctx, m, w, h);
+    for (int y0 = 0; y0 < h; y0 += band) {
+        const int bh = std::min(band, h - y0);
+        // up2x: the band's 2x rows [y0, y0 + bh) seen from source row y0 >> 1; on an odd y0 the band is 2x row 1 of that source row
+        const int p = up2x ? y0 & 1 : 0;
+        const tc::FirstSource src = direct ? tc::FirstSource{d_in + (long)(up2x ? y0 >> 1 : y0) * istride, istride, w, bh + p, n, n - p,
+                                                             std::min(n, y0 + rows_above) - p, std::min(n, h - y0 - bh + rows_below), up2x}
+                                           : padded(pad + (long)y0 * pw, pw, pw, bh + 2 * n);
+        rc = run_basic(ctx, m, dm, engine, src, pw, bh + 2 * n, d_out + (long)y0 * ostride, ostride);
+        if (rc) return rc;
+    }
+    return W2X_OK;
 }
 
 }  // namespace eng
@@ -633,15 +612,6 @@ W2X_API int w2x_debug_set_fuse_last(w2x_ctx *ctx, int on) {
     return W2X_OK;
 }
 
-int w2x_convert_plane_device(w2x_ctx *ctx, const w2x_model *model, const float *d_in, int width, int height,
-                             size_t in_stride_bytes, float *d_out, size_t out_stride_bytes, int block_splitting) {
-    if (check_ctx(ctx)) return W2X_ERR_ARG;
-    int rc = check_plane(ctx, model, d_in, width, height, in_stride_bytes, d_out, out_stride_bytes, block_splitting);
-    if (rc) return rc;
-    emit_plane_progress(ctx, model, width, height, block_splitting, false);
-    return convert_device(ctx, model, d_in, width, height, in_stride_bytes, 0, 0, d_out, out_stride_bytes, block_splitting);
-}
-
 int w2x_convert_band_device(w2x_ctx *ctx, const w2x_model *model, const float *d_in, int width, int band_height,
                             int rows_above, int rows_below, size_t in_stride_bytes, float *d_out, size_t out_stride_bytes) {
     if (check_ctx(ctx)) return W2X_ERR_ARG;
@@ -656,42 +626,6 @@ int w2x_convert_band_device(w2x_ctx *ctx, const w2x_model *model, const float *d
     emit_plane_progress(ctx, model, width, band_height, 0, false);
     return convert_device(ctx, model, band0, width, band_height, in_stride_bytes, rows_above, rows_below, d_out,
                           out_stride_bytes, 0);
-}
-
-int w2x_convert_plane(w2x_ctx *ctx, const w2x_model *model, const float *in, int width, int height, size_t in_stride_bytes,
-                      float *out, size_t out_stride_bytes, int block_splitting) {
-    if (check_ctx(ctx)) return W2X_ERR_ARG;
-    if (!model || !in || !out || width < 1 || height < 1) return fail(W2X_ERR_ARG, "w2x_convert_plane: bad argument");
-    if (in_stride_bytes < (size_t)width * 4 || out_stride_bytes < (size_t)width * 4)
-        return fail(W2X_ERR_ARG, "w2x_convert_plane: row stride smaller than a row");
-    const size_t bytes = (size_t)width * height * sizeof(float), row = (size_t)width * 4;
-    int rc = check_plane(ctx, model, in, width, height, row, out, row, block_splitting);   // the rest, on the dense staged planes
-    if (rc) return rc;
-    emit_plane_progress(ctx, model, width, height, block_splitting, true);
-    DeviceGuard g(ctx->device);
-    rc = reserve_io(ctx, bytes, bytes);
-    if (rc) return rc;
-    float *din = ctx->io_buf[0].get(), *dout = ctx->io_buf[1].get();
-    // Large planes are cut into row bands so that the upload of band i+1 and the download of band i-1 overlap the
-    // layers of band i (copy engines + compute run concurrently); each band re-reads n real rows of context from its
-    // neighbours, which keeps the result bit-identical to the single-pass path.
-    const int n_model = (int)model->layers.size();
-    const int nb = host_copy_bands(ctx, n_model, width, height, block_splitting);
-    std::vector<HostGroup> groups((size_t)nb);
-    for (int i = 0; i < nb; i++) {
-        const int y = (int)((long)height * i / nb), y_end = (int)((long)height * (i + 1) / nb);
-        // upload i carries band i plus the n rows of context band i needs from band i+1, so that band i waits for ITS upload only
-        const int u = i == 0 ? 0 : y + n_model, u_end = i + 1 < nb ? y_end + n_model : height;
-        groups[(size_t)i].up = {{din + (size_t)u * width, row, reinterpret_cast<const char *>(in) + (size_t)u * in_stride_bytes, in_stride_bytes,
-                                 row, (size_t)(u_end - u)}};
-        groups[(size_t)i].compute = [=] {
-            return convert_device(ctx, model, din + (size_t)y * width, width, y_end - y, row, i > 0 ? n_model : 0, i + 1 < nb ? n_model : 0,
-                                  dout + (size_t)y * width, row, nb > 1 ? 0 : block_splitting);
-        };
-        groups[(size_t)i].down = {{reinterpret_cast<char *>(out) + (size_t)y * out_stride_bytes, out_stride_bytes, dout + (size_t)y * width, row,
-                                   row, (size_t)(y_end - y)}};
-    }
-    return run_host_groups(ctx, groups);
 }
 
 int w2x_filter_layer_device(w2x_ctx *ctx, const w2x_model *model, int layer, const float *d_in, float *d_out, int width,
@@ -913,7 +847,7 @@ int run_packed_frame(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, const Frame
     CU_CHECK(tc::launch_pack_planes(f.rect, f.shelf_y0, f.shelf_first, f.n_shelf, n, f.fw, f.fh, up2x, ctx->pad_buf.get(), ctx->stream));
     ctx->launches++;
     const PackedGather g{f.rect, f.n_rect, f.n_blocks};
-    return run_basic(ctx, m, dm, W2X_ENGINE_TC, ctx->pad_buf.get(), f.fw, f.fw, f.fh, nullptr, 0, &g);
+    return run_basic(ctx, m, dm, W2X_ENGINE_TC, padded(ctx->pad_buf.get(), f.fw, f.fw, f.fh), f.fw, f.fh, nullptr, 0, &g);
 }
 
 int run_packed_frames(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, std::vector<FramePlan> &frames) {
@@ -965,7 +899,7 @@ int convert_tiles_dev(w2x_ctx *ctx, const w2x_model *m, const float *d_in, float
     for (int t = 0; t < n_tiles; t++) {   // cv::copyMakeBorder per tile (src/convertRoutine.cpp:35)
         CU_CHECK(launch_pad_replicate(d_in + (size_t)t * w * h, w, h, w, n, 0, 0, ctx->pad_buf.get(), ctx->stream));
         ctx->launches++;
-        rc = run_basic(ctx, m, dm, engine, ctx->pad_buf.get(), pw, pw, ph, d_out + (size_t)t * w * h, w);
+        rc = run_basic(ctx, m, dm, engine, padded(ctx->pad_buf.get(), pw, pw, ph), pw, ph, d_out + (size_t)t * w * h, w);
         if (rc) return rc;
     }
     return W2X_OK;
@@ -1513,22 +1447,25 @@ int check_chain(const char *fn, w2x_ctx *ctx, int n_steps, const w2x_model *cons
     }, steps);
 }
 
-// Host plane, staged densely in io_buf[0] (input) and io_buf[1] (output): one upload and steps 0 ... n - 2 on the context's stream,
-// then the last step as groups of the copy pipeline: the row bands of w2x_convert_plane's when it would cut that plane, so that the
-// download of band i overlaps the layers of band i + 1, else one.  An upscaling step's bands start on even 2x rows (the source row of
-// a band's first row is then whole).  A TTA last step is one group: its download waits for the mean kernel.
+// Host plane, staged densely in io_buf[0] (input) and io_buf[1] (output).  The last step runs as groups of the copy pipeline: the
+// row bands of host_copy_bands when it cuts the plane, so that the download of band i overlaps the layers of band i + 1, else one.
+// An upscaling step's bands start on even 2x rows (the source row of a band's first row is then whole).  When the last step is
+// step 0, group i also uploads the input rows that band i is the first to read, so that uploads overlap the layers as well;
+// otherwise one upload and steps 0 ... n - 2 go first on the context's stream.  A TTA last step is one group: its download waits for
+// the mean kernel.
 int chain_host(w2x_ctx *ctx, std::vector<Step> &steps, const float *in, int width, int height, size_t in_stride_bytes, float *out,
                size_t out_stride_bytes, int block_splitting, w2x_step_fn on_step, void *user) {
     const size_t last = steps.size() - 1;
     const w2x_model *m = steps[last].m;
-    const bool up = steps[last].up;
+    const bool up = steps[last].up, band_uploads = last == 0 && !steps[last].tta;
     const int n = (int)m->layers.size(), w = steps[last].w[0], h = steps[last].h[0];
     const size_t in_dense = (size_t)width * 4;
     int rc = reserve_io(ctx, (size_t)width * height * sizeof(float), (size_t)w * h * sizeof(float));
     std::vector<FrameDev> fd;
     if (!rc) rc = prepare_planes(ctx, steps, {PlaneIO{ctx->io_buf[0].get(), in_dense, ctx->io_buf[1].get(), (size_t)w * 4}}, false, &fd);
     if (rc) return rc;
-    CU_CHECK(cudaMemcpy2DAsync(ctx->io_buf[0].get(), in_dense, in, in_stride_bytes, in_dense, (size_t)height, cudaMemcpyHostToDevice, ctx->stream));
+    if (!band_uploads)
+        CU_CHECK(cudaMemcpy2DAsync(ctx->io_buf[0].get(), in_dense, in, in_stride_bytes, in_dense, (size_t)height, cudaMemcpyHostToDevice, ctx->stream));
     rc = run_steps(ctx, steps, fd, 0, last, block_splitting, on_step, user, true);
     if (rc) {   // the upload may still read the caller's plane
         cudaStreamSynchronize(ctx->stream);
@@ -1544,11 +1481,17 @@ int chain_host(w2x_ctx *ctx, std::vector<Step> &steps, const float *in, int widt
     }
     const int nb = host_copy_bands(ctx, n, w, h, block_splitting);
     auto band_y = [&](int i) { return (int)((long)h * i / nb) & (up ? ~1 : ~0); };
+    // band_uploads: upload i carries input rows [u(i), u(i + 1)); band i reads source rows up to (band_y(i + 1) + n - 1) >> up, its n
+    // rows of context below included, so that it waits for its own upload only
+    auto u = [&](int i) { return i == 0 ? 0 : i == nb ? height : std::min(height, ((band_y(i) + n - 1) >> (up ? 1 : 0)) + 1); };
     std::vector<HostGroup> groups((size_t)nb);
     for (int i = 0; i < nb; i++) {
         const int y = band_y(i), rows = band_y(i + 1) - y;
         const float *band_src = reinterpret_cast<const float *>(reinterpret_cast<const char *>(io.src) + (size_t)(up ? y / 2 : y) * io.src_stride);
         float *band_dst = io.dst + (size_t)y * w;
+        if (band_uploads)
+            groups[(size_t)i].up = {{ctx->io_buf[0].get() + (size_t)u(i) * width, in_dense, reinterpret_cast<const char *>(in) + (size_t)u(i) * in_stride_bytes,
+                                     in_stride_bytes, in_dense, (size_t)(u(i + 1) - u(i))}};
         groups[(size_t)i].compute = [=] {
             return convert_device(ctx, m, band_src, w, rows, io.src_stride, i > 0 ? n : 0, i + 1 < nb ? n : 0, band_dst, io.dst_stride,
                                   nb > 1 ? 0 : block_splitting, up);
@@ -1561,6 +1504,31 @@ int chain_host(w2x_ctx *ctx, std::vector<Step> &steps, const float *in, int widt
 }  // namespace
 
 extern "C" {
+
+// The plane entry points: a one-step W2X_STEP_SAME w2x_convert_chain_device / w2x_convert_chain behind their own argument checks.
+int w2x_convert_plane_device(w2x_ctx *ctx, const w2x_model *model, const float *d_in, int width, int height,
+                             size_t in_stride_bytes, float *d_out, size_t out_stride_bytes, int block_splitting) {
+    if (check_ctx(ctx)) return W2X_ERR_ARG;
+    int rc = check_plane(ctx, model, d_in, width, height, in_stride_bytes, d_out, out_stride_bytes, block_splitting);
+    if (rc) return rc;
+    DeviceGuard g(ctx->device);
+    std::vector<Step> steps = one_step(model, 1, &width, &height);
+    return planes_device(ctx, steps, &d_in, &in_stride_bytes, &d_out, &out_stride_bytes, false, block_splitting, nullptr, nullptr);
+}
+
+int w2x_convert_plane(w2x_ctx *ctx, const w2x_model *model, const float *in, int width, int height, size_t in_stride_bytes,
+                      float *out, size_t out_stride_bytes, int block_splitting) {
+    if (check_ctx(ctx)) return W2X_ERR_ARG;
+    if (!model || !in || !out || width < 1 || height < 1) return fail(W2X_ERR_ARG, "w2x_convert_plane: bad argument");
+    if (in_stride_bytes < (size_t)width * 4 || out_stride_bytes < (size_t)width * 4)
+        return fail(W2X_ERR_ARG, "w2x_convert_plane: row stride smaller than a row");
+    const size_t row = (size_t)width * 4;
+    int rc = check_plane(ctx, model, in, width, height, row, out, row, block_splitting);   // the rest, on the dense staged planes
+    if (rc) return rc;
+    DeviceGuard g(ctx->device);
+    std::vector<Step> steps = one_step(model, 1, &width, &height);
+    return chain_host(ctx, steps, in, width, height, in_stride_bytes, out, out_stride_bytes, block_splitting, nullptr, nullptr);
+}
 
 int w2x_convert_chain_device(w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, const float *d_in, int width,
                              int height, size_t in_stride_bytes, float *d_out, size_t out_stride_bytes, int block_splitting,
