@@ -102,7 +102,8 @@ W2X_API void w2x_ctx_destroy(w2x_ctx *ctx);
 /* A context caches device copies of every model it has converted with; this drops one model's copies
  * (call before w2x_model_free when a long-lived context cycles through many models).  Returns W2X_ERR_ARG, and keeps
  * the copies, while band sessions on this context use the model: w2x_band_* sessions, the sub-bands of w2x_slab_*
- * and the plan w2x_multi_convert_plane keeps for its last (model, width, height).  Destroy those first. */
+ * and the plans w2x_multi_convert_plane and w2x_multi_convert_chain keep for their last (models, width, height).  Destroy those
+ * first. */
 W2X_API int w2x_ctx_forget_model(w2x_ctx *ctx, const w2x_model *model);
 W2X_API int w2x_ctx_set_engine(w2x_ctx *ctx, int engine);
 W2X_API int w2x_ctx_get_engine(const w2x_ctx *ctx);
@@ -383,6 +384,32 @@ W2X_API int w2x_multi_convert_plane(w2x_multi *multi, const w2x_model *model, co
 W2X_API int w2x_multi_convert_tiles(w2x_multi *multi, const w2x_model *model, const float *const *in_tiles,
                                     float *const *out_tiles, int n_tiles, int width, int height,
                                     size_t in_stride_bytes, size_t out_stride_bytes);
+/* w2x_convert_chain on N GPUs: the noise pass and the 2x steps of one plane in one call, the plane's row bands staying on their GPUs
+ * between the steps.  A nearest 2x resize maps the rows [a, b) a GPU owns onto [2a, 2b), so the cut of step 0 holds at every step
+ * and no row changes GPU: step 0 uploads, every later step reads the previous step's rows where its GPU left them (an upscaling
+ * step through the resize, into the band's padded input frame; the 2x plane is never built), only the last step downloads, and
+ * the host sees no intermediate plane.  Between GPUs a step trades the halo row of its input frame and one row per layer.
+ * Every step's plane, and so the output, is bit-identical to w2x_convert_chain on one context with the same precision and the
+ * same arguments.
+ * Arguments are checked as by w2x_convert_chain, before anything is printed, allocated or queued, W2X_ERR_ARG (or, for a model
+ * the engine refuses, W2X_ERR_UNSUPPORTED) naming the step.  A step with W2X_STEP_TTA is refused with W2X_ERR_ARG naming the step:
+ * it has no multi-GPU form (the transposed variants would turn row bands into column bands).
+ * Before step k is queued on any GPU, on_step(k, user) is called (if not NULL); then the step logs, through the first context's log
+ * function (w2x_multi_set_log), the lines w2x_convert_chain logs for it.
+ * GPUs used: min(n_devices, height / (4 * the largest n_layers of the steps)), decided on the INPUT height (later steps only get
+ * taller).  Fewer than 2, a model without a tensor-core form, or W2X_ENGINE_FP32 on the first context: the whole call is
+ * w2x_convert_chain on the first context.  With n_steps == 1 and W2X_STEP_SAME the call is w2x_multi_convert_plane: same bits,
+ * same lines, same launches.
+ * Device memory: every step keeps sessions of its own (a neighbour may deliver a halo row of step k + 1 while this GPU still reads
+ * step k), about 1 KiB per frame pixel a GPU owns per step (two activation frames of up to 128 channels at 4 bytes per element):
+ * 1920 x 1080 noise + 2x on 2 GPUs is about 1 + 4.3 GB per GPU.  It is kept, like w2x_multi_convert_plane's plan and beside it,
+ * for the next call with the same models, kinds, size and precision, and freed by any other chain call or w2x_multi_destroy.  All of
+ * it is reserved before the first copy or launch: W2X_ERR_NOMEM leaves nothing queued and no plan behind.
+ * HOST buffers, synchronous. */
+W2X_API int w2x_multi_convert_chain(w2x_multi *multi, int n_steps, const w2x_model *const *models, const int *kinds,
+                                    const float *in, int width, int height, size_t in_stride_bytes,
+                                    float *out, size_t out_stride_bytes, int block_splitting,
+                                    w2x_step_fn on_step, void *user);
 
 /* ---- instrumentation ---------------------------------------------------------------------- */
 /* Number of kernels of THIS library launched by the context so far. */

@@ -41,7 +41,7 @@ ABI_SYMBOLS = (
     "w2x_host_alloc", "w2x_host_free", "w2x_ctx_forget_model", "w2x_slab_create", "w2x_slab_destroy", "w2x_slab_export",
     "w2x_slab_connect", "w2x_slab_connect_local", "w2x_slab_convert", "w2x_slab_convert_async", "w2x_slab_synchronize",
     "w2x_convert_planes", "w2x_convert_planes_device", "w2x_convert_chain", "w2x_convert_chain_device",
-    "w2x_convert_planes_chain", "w2x_convert_planes_chain_device",
+    "w2x_convert_planes_chain", "w2x_convert_planes_chain_device", "w2x_multi_convert_chain",
 )
 BAND_BLOB_BYTES = 320
 
@@ -159,6 +159,8 @@ def lib():
     L.w2x_multi_set_log.argtypes = [vp, LOG_FN, vp]
     L.w2x_multi_convert_plane.argtypes = [vp, vp, vp, ci, ci, cs, vp, cs, ci]
     L.w2x_multi_convert_tiles.argtypes = [vp, vp, C.POINTER(vp), C.POINTER(vp), ci, ci, ci, cs, cs]
+    L.w2x_multi_convert_chain.argtypes = [vp, ci, C.POINTER(vp), pi, vp, ci, ci, cs, vp, cs, ci, STEP_FN, vp]
+    L.w2x_debug_pad_upsample2x_xy.argtypes = [vp, vp, ci, ci, C.c_long, ci, ci, ci, ci, ci, ci, ci, ci, ci, vp]
     L.w2x_debug_set_host_bands.argtypes = [vp, ci]
     L.w2x_debug_set_fuse_last.argtypes = [vp, ci]
     L.w2x_debug_set_num_sms.argtypes = [vp, ci]
@@ -344,6 +346,14 @@ class Context:
     def debug_set_fuse_last(self, on): _check(lib().w2x_debug_set_fuse_last(self._h, int(on)))
     def debug_set_num_sms(self, n): _check(lib().w2x_debug_set_num_sms(self._h, int(n)))
     def debug_tc_profile_enable(self, on=True): _check(lib().w2x_debug_tc_profile_enable(self._h, int(on)))
+
+    def debug_pad_upsample2x_xy(self, src, row0, w2, h2, pad_x, pad_top, pad_bottom, rows_above, rows_below, skip_top, skip_bottom, out):
+        """launch_pad_upsample2x_xy alone: src is the half-resolution plane (2-D float32, row-strided views pass as they are), its row
+        row0 holds 2x row 0 of the band; the frame is written into `out` (dense), whose skipped rows stay as they are."""
+        _check(lib().w2x_debug_pad_upsample2x_xy(self._h, C.c_void_p(src.ctypes.data), src.shape[0], row0, src.strides[0] // 4, w2, h2, pad_x,
+                                                 pad_top, pad_bottom, rows_above, rows_below, skip_top, skip_bottom,
+                                                 C.c_void_p(out.ctypes.data)))
+        return out
 
     def debug_tc_profile_read(self, layer):
         """per-role cycle counters of the tensor-core kernel of `layer`, averaged per CTA (dict)."""
@@ -652,6 +662,32 @@ class Multi:
         _check(lib().w2x_multi_convert_plane(self._h, model._h, C.c_void_p(x.ctypes.data), w, h, x.strides[0],
                                              C.c_void_p(out.ctypes.data), out.strides[0], int(bool(block_splitting))))
         return out
+
+    def convert_chain(self, steps, plane, out=None, block_splitting=True, on_step=None):
+        """Context.convert_chain with the plane's row bands on this handle's GPUs (w2x_multi_convert_chain): same arguments, same bits."""
+        x = np.asarray(plane, np.float32)
+        if x.ndim != 2:
+            raise ValueError("plane must be 2-D")
+        if x.strides[1] != 4 or x.strides[0] % 4 or x.strides[0] < x.shape[1] * 4:
+            x = np.ascontiguousarray(x)
+        h, w = x.shape
+        n, models, kinds, cb, ups = Context._chain_args(steps, on_step)
+        if out is None:
+            out = np.empty((h << ups, w << ups), np.float32)
+        if out.ndim != 2 or out.dtype != np.float32 or out.strides[1] != 4 or out.shape != (h << ups, w << ups):
+            raise ValueError(f"out must be a float32 array of shape {(h << ups, w << ups)} with unit column stride")
+        _check(lib().w2x_multi_convert_chain(self._h, n, models, kinds, C.c_void_p(x.ctypes.data), w, h, x.strides[0],
+                                             C.c_void_p(out.ctypes.data), out.strides[0], int(bool(block_splitting)), cb, None))
+        return out
+
+    def launch_counts(self):
+        """w2x_ctx_launch_count of every device's context"""
+        counts = []
+        for i in range(lib().w2x_multi_device_count(self._h)):
+            n = C.c_uint64()
+            _check(lib().w2x_ctx_launch_count(lib().w2x_multi_ctx(self._h, i), C.byref(n)))
+            counts.append(n.value)
+        return counts
 
     def convert_tiles(self, model: Model, tiles, out=None):
         x = np.ascontiguousarray(tiles, np.float32)

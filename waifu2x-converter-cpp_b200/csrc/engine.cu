@@ -1503,6 +1503,16 @@ int chain_host(w2x_ctx *ctx, std::vector<Step> &steps, const float *in, int widt
 }
 }  // namespace
 
+namespace w2x {
+namespace eng {
+int check_chain_host(const char *fn, w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, const float *in, int width,
+                     int height, size_t in_stride_bytes, const float *out, size_t out_stride_bytes, int block_splitting) {
+    std::vector<Step> steps;
+    return check_chain(fn, ctx, n_steps, models, kinds, in, width, height, in_stride_bytes, out, out_stride_bytes, block_splitting, true, &steps);
+}
+}  // namespace eng
+}  // namespace w2x
+
 extern "C" {
 
 // The plane entry points: a one-step W2X_STEP_SAME w2x_convert_chain_device / w2x_convert_chain behind their own argument checks.

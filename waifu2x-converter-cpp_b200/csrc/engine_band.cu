@@ -56,6 +56,23 @@ inline char *seg_at(char *base, int frame_rows, size_t px, const RowSeg &s, int 
     return base + s.plane_mul * px * (size_t)frame_rows + s.pitch * (size_t)row + s.in_row;
 }
 
+// w2x_band_load_rows, also through the nearest 2x resize: with up2x the band's rows are 2x rows of a half-resolution plane, the band
+// starts on an even one, and d_in points at the source row holding it; an overlap edge then reads the ceil(n / 2) source rows beyond.
+int band_load_rows_from(w2x_band *band, const float *d_in, size_t in_stride_bytes, bool up2x) {
+    if (band_check(band)) return W2X_ERR_ARG;
+    if (!d_in || in_stride_bytes % 4 || in_stride_bytes < (size_t)(up2x ? (band->width + 1) / 2 : band->width) * 4)
+        return fail(W2X_ERR_ARG, "w2x_band_load_rows: bad input");
+    w2x_ctx *ctx = band->ctx;
+    DeviceGuard g(ctx->device);
+    const auto pad = up2x ? launch_pad_upsample2x_xy : launch_pad_replicate_xy;
+    CU_CHECK(pad(d_in, band->width, band->rows, (long)(in_stride_bytes / 4), band->n, band->pt, band->pb, band->ov_up ? band->n : 0,
+                 band->ov_down ? band->n : 0, band->pad.get(), ctx->stream, band->up ? 1 : 0, band->down ? 1 : 0));
+    ctx->launches++;
+    band->last_step = -1;
+    band->cur = 0;
+    return W2X_OK;
+}
+
 constexpr uint32_t BLOB_MAGIC = 0x77327862u;   // "w2xb"
 struct BandBlob {                              // what w2x_band_export hands to the neighbour ranks
     uint32_t magic;
@@ -65,6 +82,8 @@ struct BandBlob {                              // what w2x_band_export hands to 
     cudaIpcMemHandle_t pad, act0, act1, flags;
 };
 static_assert(sizeof(BandBlob) <= W2X_BAND_BLOB_BYTES, "blob does not fit W2X_BAND_BLOB_BYTES");
+
+int band_run_from(w2x_band *band, const float *d_in, size_t in_stride_bytes, bool up2x, float *d_out, size_t out_stride_bytes);
 
 }  // namespace
 
@@ -148,19 +167,7 @@ int w2x_band_load(w2x_band *band, const float *d_in, size_t in_stride_bytes) {
 
 // d_in: the band's OWN rows; the halo rows of the input frame are left to the neighbours (w2x_band_exchange(band, -1)).  On an
 // overlap edge (W2X_EDGE_OVERLAP) the n input rows beyond the band must be readable at d_in - n rows / d_in + rows.
-int w2x_band_load_rows(w2x_band *band, const float *d_in, size_t in_stride_bytes) {
-    if (band_check(band)) return W2X_ERR_ARG;
-    if (!d_in || in_stride_bytes % 4 || in_stride_bytes < (size_t)band->width * 4) return fail(W2X_ERR_ARG, "w2x_band_load_rows: bad input");
-    w2x_ctx *ctx = band->ctx;
-    DeviceGuard g(ctx->device);
-    CU_CHECK(launch_pad_replicate_xy(d_in, band->width, band->rows, (long)(in_stride_bytes / 4), band->n, band->pt, band->pb,
-                                     band->ov_up ? band->n : 0, band->ov_down ? band->n : 0, band->pad.get(), ctx->stream, band->up ? 1 : 0,
-                                     band->down ? 1 : 0));
-    ctx->launches++;
-    band->last_step = -1;
-    band->cur = 0;
-    return W2X_OK;
-}
+int w2x_band_load_rows(w2x_band *band, const float *d_in, size_t in_stride_bytes) { return band_load_rows_from(band, d_in, in_stride_bytes, false); }
 
 int w2x_band_step(w2x_band *band, int step) {
     if (band_check(band)) return W2X_ERR_ARG;
@@ -355,7 +362,15 @@ int w2x_band_exchange(w2x_band *band, int step) {
 
 // One whole pass of a connected band: own rows in, own rows out; everything is queued on the context's stream.
 int w2x_band_run(w2x_band *band, const float *d_in, size_t in_stride_bytes, float *d_out, size_t out_stride_bytes) {
-    int rc = w2x_band_load_rows(band, d_in, in_stride_bytes);
+    return band_run_from(band, d_in, in_stride_bytes, false, d_out, out_stride_bytes);
+}
+
+}  // extern "C"
+
+namespace {
+// w2x_band_run from a row source that may be a half-resolution plane (band_load_rows_from)
+int band_run_from(w2x_band *band, const float *d_in, size_t in_stride_bytes, bool up2x, float *d_out, size_t out_stride_bytes) {
+    int rc = band_load_rows_from(band, d_in, in_stride_bytes, up2x);
     if (rc) return rc;
     if ((rc = w2x_band_exchange(band, -1))) return rc;
     for (int k = 0; k <= band->n - 2; k++) {
@@ -364,8 +379,7 @@ int w2x_band_run(w2x_band *band, const float *d_in, size_t in_stride_bytes, floa
     }
     return w2x_band_finish(band, d_out, out_stride_bytes);
 }
-
-}  // extern "C"
+}  // namespace
 
 // =========================================================================================================================
 // One GPU's slab of a multi-GPU plane with HOST buffers: upload, layers and download pipelined over sub-bands
@@ -380,6 +394,7 @@ struct w2x_slab {
     const w2x_model *model = nullptr;
     int width = 0, rows = 0, order = 0;
     bool up = false, down = false;
+    bool half_in = false;                        // d_in holds the rows at half resolution: [rows / 2][width / 2], read through the 2x resize
     std::vector<w2x_band *> sub;
     std::vector<int> r0;                         // sub-band s owns slab rows [r0[s], r0[s+1])
     DevBuf<float> d_in, d_out;                   // [rows][width]
@@ -395,16 +410,12 @@ struct w2x_slab {
     }
 };
 
-extern "C" {
-
-void w2x_slab_destroy(w2x_slab *s) {
-    if (!s) return;
-    DeviceGuard g(s->ctx->device);
-    delete s;
-    cudaGetLastError();
-}
-
-int w2x_slab_create(w2x_ctx *ctx, const w2x_model *model, int width, int rows, int has_up, int has_down, int order, int n_sub, w2x_slab **out) {
+namespace {
+// w2x_slab_create for a step of w2x_multi_convert_chain: without d_in when the slab's rows come from another slab's d_out; up2x: the
+// slab's rows are read through the nearest 2x resize, so every sub-band starts on an even row (the first copy of a source row) and
+// d_in, if any, holds the half-resolution rows.
+int slab_create(w2x_ctx *ctx, const w2x_model *model, int width, int rows, int has_up, int has_down, int order, int n_sub, bool with_d_in,
+                bool up2x, w2x_slab **out) {
     if (check_ctx(ctx)) return W2X_ERR_ARG;
     if (!model || !out || width < 1 || rows < 1) return fail(W2X_ERR_ARG, "w2x_slab_create: bad argument");
     *out = nullptr;
@@ -423,7 +434,7 @@ int w2x_slab_create(w2x_ctx *ctx, const w2x_model *model, int width, int rows, i
     s->order = order ? 1 : 0;
     s->up = has_up != 0;
     s->down = has_down != 0;
-    for (int i = 0; i <= n_sub; i++) s->r0.push_back((int)((long)rows * i / n_sub));
+    for (int i = 0; i <= n_sub; i++) s->r0.push_back(i == n_sub ? rows : (int)((long)rows * i / n_sub) & (up2x ? ~1 : ~0));
     for (int i = 0; i < n_sub; i++) {
         w2x_band *b = nullptr;
         const int ue = i == 0 ? (s->up ? W2X_EDGE_NEIGHBOUR : W2X_EDGE_BORDER) : W2X_EDGE_OVERLAP;
@@ -432,8 +443,10 @@ int w2x_slab_create(w2x_ctx *ctx, const w2x_model *model, int width, int rows, i
         if (rc) return rc;
         s->sub.push_back(b);
     }
-    CU_CHECK(s->d_in.grow((size_t)rows * width * 4));
-    CU_CHECK(s->d_out.grow((size_t)rows * width * 4));
+    s->half_in = with_d_in && up2x;
+    int rc = with_d_in ? s->d_in.reserve(s->half_in ? (size_t)(rows / 2) * (width / 2) * 4 : (size_t)rows * width * 4) : W2X_OK;
+    if (!rc) rc = s->d_out.reserve((size_t)rows * width * 4);
+    if (rc) return rc;
     for (int i = 0; i < n_sub; i++) {
         cudaEvent_t e;
         CU_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
@@ -444,6 +457,20 @@ int w2x_slab_create(w2x_ctx *ctx, const w2x_model *model, int width, int rows, i
     CU_CHECK(cudaEventCreateWithFlags(&s->ev_drained, cudaEventDisableTiming));
     *out = s.release();
     return W2X_OK;
+}
+}  // namespace
+
+extern "C" {
+
+void w2x_slab_destroy(w2x_slab *s) {
+    if (!s) return;
+    DeviceGuard g(s->ctx->device);
+    delete s;
+    cudaGetLastError();
+}
+
+int w2x_slab_create(w2x_ctx *ctx, const w2x_model *model, int width, int rows, int has_up, int has_down, int order, int n_sub, w2x_slab **out) {
+    return slab_create(ctx, model, width, rows, has_up, has_down, order, n_sub, true, false, out);
 }
 
 // blob = [top sub-band's session | bottom sub-band's session]
@@ -478,15 +505,20 @@ int w2x_slab_connect_local(w2x_slab *s, w2x_slab *up, w2x_slab *down) {
 }  // extern "C"
 
 namespace {
-// Phase 1 of a pass: uploads and the layer loops of every sub-band (nothing here can block the host on another GPU's progress).
-int slab_enqueue_compute(w2x_slab *s, const float *in, size_t in_stride_bytes) {
+// Phase 1 of a pass, first half: the slab's rows from the host into d_in, one upload per sub-band.
+int slab_enqueue_upload(w2x_slab *s, const float *in, size_t in_stride_bytes) {
     w2x_ctx *ctx = s->ctx;
     DeviceGuard g(ctx->device);
     const int K = (int)s->sub.size();
     const size_t rowb = (size_t)s->width * 4;
     auto at = [&](int t) { return s->order ? K - 1 - t : t; };      // t-th sub-band in processing order
     CU_CHECK(cudaStreamWaitEvent(ctx->copy_in, s->ev_done[(size_t)at(K - 1)], 0));   // the previous pass has finished reading d_in
-    CU_CHECK(cudaStreamWaitEvent(ctx->stream, s->ev_drained, 0));                    // ... and its downloads have left d_out
+    if (s->half_in) {   // a quarter of the slab's pixels: one upload, which every sub-band waits for
+        const size_t half_rowb = (size_t)(s->width / 2) * 4;
+        CU_CHECK(cudaMemcpy2DAsync(s->d_in.get(), half_rowb, in, in_stride_bytes, half_rowb, (size_t)(s->rows / 2), cudaMemcpyHostToDevice, ctx->copy_in));
+        for (auto e : s->ev_in) CU_CHECK(cudaEventRecord(e, ctx->copy_in));
+        return W2X_OK;
+    }
     // Upload t carries the t-th sub-band's rows shifted by n towards the sub-band processed next: its own rows minus the n the previous
     // upload already brought, plus the n rows of overlap context it reads from the next one -- so a sub-band waits for ITS upload only.
     const int n = (int)s->model->layers.size();
@@ -499,10 +531,25 @@ int slab_enqueue_compute(w2x_slab *s, const float *in, size_t in_stride_bytes) {
                                    (size_t)(yb - ya), cudaMemcpyHostToDevice, ctx->copy_in));
         CU_CHECK(cudaEventRecord(s->ev_in[(size_t)i], ctx->copy_in));
     }
+    return W2X_OK;
+}
+
+// Second half: the layer loops of every sub-band from a device row source (nothing here can block the host on another GPU's
+// progress).  `src` holds the slab's rows: d_in after slab_enqueue_upload (uploaded: each sub-band waits for its upload), or, in a
+// chain, the d_out of the previous step's slab on this GPU, as it is or (up2x) at half resolution.  An overlap edge of an upscaling
+// sub-band reads ceil(n / 2) source rows of the NEIGHBOURING sub-band's output of the previous step; all of that step's sub-bands
+// were queued on this stream before any of this step's, so stream order alone has them written.
+int slab_enqueue_run(w2x_slab *s, const float *src, size_t src_stride_bytes, bool up2x, bool uploaded) {
+    w2x_ctx *ctx = s->ctx;
+    DeviceGuard g(ctx->device);
+    const int K = (int)s->sub.size();
+    const size_t rowb = (size_t)s->width * 4;
+    CU_CHECK(cudaStreamWaitEvent(ctx->stream, s->ev_drained, 0));                    // the previous pass's downloads have left d_out
     for (int t = 0; t < K; t++) {
-        const int i = at(t), y = s->r0[(size_t)i];
-        CU_CHECK(cudaStreamWaitEvent(ctx->stream, s->ev_in[(size_t)i], 0));   // own rows + the overlap rows (earlier uploads are ordered before it)
-        int rc = w2x_band_run(s->sub[(size_t)i], s->d_in.get() + (size_t)y * s->width, rowb, s->d_out.get() + (size_t)y * s->width, rowb);
+        const int i = s->order ? K - 1 - t : t, y = s->r0[(size_t)i];
+        if (uploaded) CU_CHECK(cudaStreamWaitEvent(ctx->stream, s->ev_in[(size_t)i], 0));   // own rows + the overlap rows (earlier uploads are ordered before it)
+        const float *rows = reinterpret_cast<const float *>(reinterpret_cast<const char *>(src) + (size_t)(up2x ? y / 2 : y) * src_stride_bytes);
+        int rc = band_run_from(s->sub[(size_t)i], rows, src_stride_bytes, up2x, s->d_out.get() + (size_t)y * s->width, rowb);
         if (rc) {
             cudaStreamSynchronize(ctx->copy_in);
             cudaStreamSynchronize(ctx->stream);
@@ -511,6 +558,12 @@ int slab_enqueue_compute(w2x_slab *s, const float *in, size_t in_stride_bytes) {
         CU_CHECK(cudaEventRecord(s->ev_done[(size_t)i], ctx->stream));
     }
     return W2X_OK;
+}
+
+int slab_enqueue_compute(w2x_slab *s, const float *in, size_t in_stride_bytes) {
+    int rc = slab_enqueue_upload(s, in, in_stride_bytes);
+    if (rc) return rc;
+    return slab_enqueue_run(s, s->d_in.get(), (size_t)(s->half_in ? s->width / 2 : s->width) * 4, s->half_in, true);
 }
 
 // Phase 2: every sub-band's rows go home as soon as its layers are done.  (A download into PAGEABLE memory blocks the host
@@ -569,6 +622,14 @@ struct w2x_multi {
     int plan_w = 0, plan_h = 0, plan_precision = -1;
     std::vector<w2x_slab *> slabs;
     std::vector<int> r0;                       // first row of every slab (+ the plane height at the end)
+    // w2x_multi_convert_chain's plan, beside the one above: the slabs of the last (models, kinds, width, height), one per step and GPU
+    struct Chain {
+        std::vector<uint64_t> uids;
+        std::vector<int> kinds;
+        int w = 0, h = 0, precision = -1;
+        std::vector<std::vector<w2x_slab *>> slabs;   // [step][GPU]; GPU i owns rows [r0[i] << u, r0[i + 1] << u) of a step after u upscales
+        std::vector<int> r0;                          // in input rows
+    } chain;
 };
 
 namespace {
@@ -577,6 +638,12 @@ void multi_drop_plan(w2x_multi *m) {
     for (auto b : m->slabs) w2x_slab_destroy(b);
     m->slabs.clear();
     m->plan_uid = 0;
+}
+
+void multi_drop_chain(w2x_multi *m) {
+    for (auto &step : m->chain.slabs)
+        for (auto b : step) w2x_slab_destroy(b);
+    m->chain = w2x_multi::Chain();
 }
 
 // pinned view of a caller buffer for the duration of one call (pageable memory makes every async copy a staged, blocking one)
@@ -618,6 +685,7 @@ int w2x_multi_create(const int *devices, int n_devices, w2x_multi **out) {
 void w2x_multi_destroy(w2x_multi *m) {
     if (!m) return;
     multi_drop_plan(m);
+    multi_drop_chain(m);
     for (auto c : m->ctx) w2x_ctx_destroy(c);
     delete m;
 }
@@ -673,6 +741,102 @@ int w2x_multi_convert_plane(w2x_multi *m, const w2x_model *model, const float *i
     return rc;
 }
 
+// w2x_convert_chain over row bands.  A nearest 2x step maps the rows [a, b) a GPU owns onto [2a, 2b), so the cut of step 0 stays a
+// valid cut at every later step and no row ever changes GPU: the rows a GPU's slab of step k leaves in its d_out are, on that GPU,
+// the (half-resolution) source of its slab of step k + 1.  Only step 0 uploads and only the last step downloads; the one cross-GPU
+// traffic a step adds is the halo row of its input frame, which w2x_band_exchange(band, -1) already moves.  Every step has sessions
+// (frames, flags) of its own: a neighbour may deliver a halo row of step k + 1 while this GPU still reads step k.
+int w2x_multi_convert_chain(w2x_multi *m, int n_steps, const w2x_model *const *models, const int *kinds, const float *in, int width,
+                            int height, size_t in_stride_bytes, float *out, size_t out_stride_bytes, int block_splitting,
+                            w2x_step_fn on_step, void *user) {
+    const char *fn = "w2x_multi_convert_chain";
+    if (!m || m->ctx.empty()) return fail(W2X_ERR_ARG, "%s: NULL handle", fn);
+    w2x_ctx *ctx0 = m->ctx[0];
+    int rc = check_chain_host(fn, ctx0, n_steps, models, kinds, in, width, height, in_stride_bytes, out, out_stride_bytes, block_splitting);
+    if (rc) return rc;
+    for (int k = 0; k < n_steps; k++)
+        if (kinds[k] & W2X_STEP_TTA)
+            return fail(W2X_ERR_ARG, "%s: step %d: W2X_STEP_TTA has no multi-GPU form (its transposed variants would turn row bands into column bands)", fn, k);
+    if (n_steps == 1 && kinds[0] == W2X_STEP_SAME) {
+        if (on_step) on_step(0, user);
+        return w2x_multi_convert_plane(m, models[0], in, width, height, in_stride_bytes, out, out_stride_bytes, block_splitting);
+    }
+    int n_max = 0;
+    bool tc = ctx0->engine != W2X_ENGINE_FP32;
+    for (int k = 0; k < n_steps; k++) {
+        n_max = std::max(n_max, (int)models[k]->layers.size());
+        tc = tc && models[k]->tc_eligible;
+    }
+    // decided on the input height with the deepest model: later steps only get taller
+    const int nd = std::min((int)m->ctx.size(), height / (4 * n_max));
+    if (nd < 2 || !tc)
+        return w2x_convert_chain(ctx0, n_steps, models, kinds, in, width, height, in_stride_bytes, out, out_stride_bytes, block_splitting, on_step, user);
+    // ---- plan: per step one slab per GPU, neighbours of a step wired through peer memory; all device memory is reserved here ----
+    w2x_multi::Chain &c = m->chain;
+    std::vector<uint64_t> uids;
+    for (int k = 0; k < n_steps; k++) uids.push_back(models[k]->uid);
+    const std::vector<int> kv(kinds, kinds + n_steps);
+    if (c.uids != uids || c.kinds != kv || c.w != width || c.h != height || c.precision != ctx0->precision || c.slabs.empty() ||
+        (int)c.slabs[0].size() != nd) {
+        multi_drop_chain(m);
+        for (int i = 0; i <= nd; i++) c.r0.push_back((int)((long)height * i / nd));
+        c.slabs.resize((size_t)n_steps);
+        int u = 0;
+        for (int k = 0; k < n_steps && !rc; k++) {
+            const bool up = (kinds[k] & W2X_STEP_UPSCALE2X) != 0;
+            u += up;
+            for (int i = 0; i < nd && !rc; i++) {
+                m->ctx[(size_t)i]->precision = ctx0->precision;
+                w2x_slab *sl = nullptr;
+                rc = slab_create(m->ctx[(size_t)i], models[k], width << u, (c.r0[(size_t)i + 1] - c.r0[(size_t)i]) << u, i > 0, i + 1 < nd, i & 1, 0,
+                                 k == 0, up, &sl);
+                if (!rc) c.slabs[(size_t)k].push_back(sl);
+            }
+            for (int i = 0; i < nd && !rc; i++)
+                rc = w2x_slab_connect_local(c.slabs[(size_t)k][(size_t)i], i > 0 ? c.slabs[(size_t)k][(size_t)i - 1] : nullptr,
+                                            i + 1 < nd ? c.slabs[(size_t)k][(size_t)i + 1] : nullptr);
+        }
+        if (rc) { multi_drop_chain(m); return rc; }
+        c.uids = uids;
+        c.kinds = kv;
+        c.w = width;
+        c.h = height;
+        c.precision = ctx0->precision;
+    }
+    const size_t last = (size_t)n_steps - 1;
+    int u_last = 0;
+    for (int k = 0; k < n_steps; k++) u_last += (kinds[k] & W2X_STEP_UPSCALE2X) != 0;
+    const int ow = width << u_last;
+    HostPin pin_in(in, in_stride_bytes * (size_t)(height - 1) + (size_t)width * 4),
+        pin_out(out, out_stride_bytes * (size_t)(((size_t)height << u_last) - 1) + (size_t)ow * 4);
+    // ---- queue step-major, every GPU from this one thread: on_step(k) and step k's lines come before step k is queued anywhere, and a
+    // GPU's step k + 1 follows its own step k in stream order.  Nothing queued here can block this thread on a GPU's progress. ----
+    int w = width, h = height;
+    for (size_t k = 0; k <= last && rc == W2X_OK; k++) {
+        const bool up = (kinds[k] & W2X_STEP_UPSCALE2X) != 0;
+        if (up) w *= 2, h *= 2;
+        if (on_step) on_step((int)k, user);
+        emit_plane_progress(ctx0, models[k], w, h, block_splitting, true);
+        for (int i = 0; i < nd && rc == W2X_OK; i++) {
+            w2x_slab *sl = c.slabs[k][(size_t)i];
+            if (k == 0) {
+                rc = slab_enqueue_compute(sl, reinterpret_cast<const float *>(reinterpret_cast<const char *>(in) + (size_t)c.r0[(size_t)i] * in_stride_bytes), in_stride_bytes);
+            } else {
+                const w2x_slab *prev = c.slabs[k - 1][(size_t)i];
+                rc = slab_enqueue_run(sl, prev->d_out.get(), (size_t)prev->width * 4, up, false);
+            }
+        }
+    }
+    for (int i = 0; i < nd && rc == W2X_OK; i++)      // every GPU's layers are queued: a download may block this thread now
+        rc = slab_enqueue_download(c.slabs[last][(size_t)i], reinterpret_cast<float *>(reinterpret_cast<char *>(out) + ((size_t)c.r0[(size_t)i] << u_last) * out_stride_bytes),
+                                   out_stride_bytes);
+    for (int i = 0; i < nd; i++) {
+        int r2 = w2x_slab_synchronize(c.slabs[last][(size_t)i]);
+        if (rc == W2X_OK) rc = r2;
+    }
+    return rc;
+}
+
 // Independent planes of one shape (the reference's block loop, src/convertRoutine.cpp:114-165, and BASELINE config 5):
 // tile t goes to GPU t mod N, every GPU runs its tiles as ONE batched pass; no exchange.
 int w2x_multi_convert_tiles(w2x_multi *m, const w2x_model *model, const float *const *in_tiles, float *const *out_tiles, int n_tiles,
@@ -711,6 +875,31 @@ int w2x_multi_set_precision(w2x_multi *m, int precision) {
 int w2x_multi_set_log(w2x_multi *m, w2x_log_fn fn, void *user) {
     if (!m) return fail(W2X_ERR_ARG, "NULL handle");
     return w2x_ctx_set_log(m->ctx[0], fn, user);
+}
+
+// Test hook: launch_pad_upsample2x_xy alone on HOST arrays.  `in` is in_rows x in_stride_floats, its row in_row0 holds 2x row 0 of the
+// band; `out` is the dense frame and comes back with the rows the kernel skipped as the caller left them.
+W2X_API int w2x_debug_pad_upsample2x_xy(w2x_ctx *ctx, const float *in, int in_rows, int in_row0, long in_stride_floats, int w2, int h2, int pad_x,
+                                        int pad_top, int pad_bottom, int rows_above, int rows_below, int skip_top, int skip_bottom, float *out) {
+    if (check_ctx(ctx)) return W2X_ERR_ARG;
+    if (!in || !out || w2 < 1 || h2 < 1 || in_rows < 1 || pad_x < 0 || pad_top < 0 || pad_bottom < 0 || rows_above < 0 || rows_below < 0 ||
+        skip_top < 0 || skip_bottom < 0 || in_stride_floats < (w2 + 1) / 2 || in_row0 + ((-rows_above) >> 1) < 0 ||
+        in_row0 + ((h2 - 1 + rows_below) >> 1) >= in_rows)
+        return fail(W2X_ERR_ARG, "w2x_debug_pad_upsample2x_xy: bad argument");
+    DeviceGuard g(ctx->device);
+    const size_t in_bytes = (size_t)in_rows * in_stride_floats * 4, out_bytes = (size_t)(w2 + 2 * pad_x) * (h2 + pad_top + pad_bottom) * 4;
+    DevBuf<float> d_in, d_out;
+    int rc = d_in.reserve(in_bytes);
+    if (!rc) rc = d_out.reserve(out_bytes);
+    if (rc) return rc;
+    CU_CHECK(cudaMemcpyAsync(d_in.get(), in, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
+    CU_CHECK(cudaMemcpyAsync(d_out.get(), out, out_bytes, cudaMemcpyHostToDevice, ctx->stream));
+    CU_CHECK(launch_pad_upsample2x_xy(d_in.get() + (size_t)in_row0 * in_stride_floats, w2, h2, in_stride_floats, pad_x, pad_top, pad_bottom, rows_above,
+                                      rows_below, d_out.get(), ctx->stream, skip_top, skip_bottom));
+    ctx->launches++;
+    CU_CHECK(cudaMemcpyAsync(out, d_out.get(), out_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    CU_CHECK(cudaStreamSynchronize(ctx->stream));
+    return W2X_OK;
 }
 
 }  // extern "C"

@@ -195,6 +195,12 @@ int ensure_tc(w2x_ctx *ctx);
 int check_ctx(w2x_ctx *ctx);
 int pick_engine(w2x_ctx *ctx, const w2x_model *m);
 void emit_reference_progress(w2x_ctx *ctx, int w, int h, int n_layers, bool split);   // the reference's stdout lines of one convertWithModels call
+// The lines of one plane of w x h through w2x_convert_plane (host) / w2x_convert_plane_device: a step of w2x_convert_chain*
+void emit_plane_progress(w2x_ctx *ctx, const w2x_model *m, int w, int h, int block_splitting, bool host);
+// Every argument of w2x_convert_chain (HOST planes), before anything is printed, allocated or queued: W2X_ERR_ARG /
+// W2X_ERR_UNSUPPORTED naming `fn` and the step.
+int check_chain_host(const char *fn, w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, const float *in, int width,
+                     int height, size_t in_stride_bytes, const float *out, size_t out_stride_bytes, int block_splitting);
 // One tensor-core layer `li` on frames of pw x ph: in -> out (or, fused with the last layer, -> per-pixel tap partials in `out`).
 // Only frame rows [out_y0, out_y0 + out_rows) are stored (out_rows < 0: the whole frame).
 int launch_layer_tc(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int li, const __half *in, __half *out, int pw, int ph,

@@ -20,6 +20,13 @@ cudaError_t launch_pad_replicate_xy(const float *in, int w, int h, long in_strid
 // rows_below count real 2x rows beyond it.  Writes the dense (w2 + 2 pad) x (h2 + 2 pad) plane.
 cudaError_t launch_pad_upsample2x(const float *in, int w2, int h2, long in_stride_floats, int pad, int rows_above, int rows_below,
                                   float *out, cudaStream_t s);
+// The row-band form of launch_pad_upsample2x, with launch_pad_replicate_xy's frame: pixel (fy, fx) of the (w2 + 2 pad_x) x
+// (h2 + pad_top + pad_bottom) frame = in[clamp(fy - pad_top, -rows_above, h2 - 1 + rows_below) >> 1][clamp(fx - pad_x, 0, w2 - 1) >> 1]
+// (>> floors, so with an odd rows_above the first real row above is the SECOND 2x row of its source row).  `in` points at the source
+// row holding 2x row 0 of the band, which is an even 2x row of the plane; rows_above / rows_below count real 2x rows beyond the band;
+// the top skip_top / bottom skip_bottom frame rows are not written (a neighbour GPU stores them).
+cudaError_t launch_pad_upsample2x_xy(const float *in, int w2, int h2, long in_stride_floats, int pad_x, int pad_top, int pad_bottom,
+                                     int rows_above, int rows_below, float *out, cudaStream_t s, int skip_top = 0, int skip_bottom = 0);
 // Peer-memory halo exchange (engine_band.cu): ONE kernel copies up to 8 row segments into the neighbour GPUs' frames,
 // publishes `value` in their flag words once every byte is visible system-wide, then waits until the neighbours have
 // published the same value here.  Flag values only grow, so nothing is ever reset.

@@ -58,6 +58,52 @@ __global__ void pad_upsample2x_kernel(const float *__restrict__ in, int w2, int 
     }
 }
 
+// The band-frame form of pad_upsample2x_kernel (pad_replicate_kernel's frame, read through the resize): separate top / bottom pads
+// and frame rows left to a neighbour GPU.  A thread owns 4 frame columns of one 2x row PAIR (2q, 2q + 1): clamping either row to
+// [-rows_above, h2 - 1 + rows_below] and halving gives the same source row (a clamp bound inside the pair pulls the other row onto
+// its partner), so the at most 3 source floats behind the 4 columns are read once, through the read-only path, and stored to both
+// rows -- as one 16-byte store each when VEC (frame rows of a multiple of 4 floats in a 16-byte aligned frame).
+template <bool VEC>
+__global__ void __launch_bounds__(256) pad_upsample2x_xy_kernel(const float *__restrict__ in, int w2, int h2, long in_stride, int pad_x,
+                                                                int pad_top, int pad_bottom, int rows_above, int rows_below,
+                                                                float *__restrict__ out, int skip_top, int skip_bottom) {
+    const int W = w2 + 2 * pad_x, H = h2 + pad_top + pad_bottom;
+    const int x0 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
+    if (x0 >= W) return;
+    const int q0 = -((pad_top + 1) >> 1);                  // the pair holding frame row 0 (2x row -pad_top)
+    const int pairs = ((h2 + pad_bottom - 1) >> 1) - q0 + 1;
+    int sx[4];
+#pragma unroll
+    for (int j = 0; j < 4; j++) sx[j] = min(max(x0 + j - pad_x, 0), w2 - 1) >> 1;
+    for (int by = blockIdx.y; by < row_blocks(pairs, blockDim.y); by += gridDim.y) {
+        const int p = by * blockDim.y + threadIdx.y;
+        if (p >= pairs) continue;
+        const int y = 2 * (q0 + p);                        // the pair's first 2x row; frame rows y + pad_top and y + pad_top + 1
+        const int fy = y + pad_top;
+        const bool st0 = fy >= skip_top && fy < H - skip_bottom, st1 = fy + 1 >= skip_top && fy + 1 < H - skip_bottom;
+        if (!st0 && !st1) continue;
+        const int sy = min(max(y, -rows_above), h2 - 1 + rows_below) >> 1;   // arithmetic shift: floor, also above the band
+        const float *row = in + (long)sy * in_stride;
+        float v[4];
+        v[0] = __ldg(row + sx[0]);
+#pragma unroll
+        for (int j = 1; j < 4; j++) v[j] = sx[j] == sx[j - 1] ? v[j - 1] : __ldg(row + sx[j]);
+        float *o = out + (long)fy * W + x0;
+        if (VEC) {
+            const float4 v4 = make_float4(v[0], v[1], v[2], v[3]);
+            if (st0) *reinterpret_cast<float4 *>(o) = v4;
+            if (st1) *reinterpret_cast<float4 *>(o + W) = v4;
+        } else {
+#pragma unroll
+            for (int j = 0; j < 4; j++) {
+                if (x0 + j >= W) break;
+                if (st0) o[j] = v[j];
+                if (st1) o[W + j] = v[j];
+            }
+        }
+    }
+}
+
 // crop [pad, pad+h) x [pad, pad+w) of a dense (h+2pad) x (w+2pad) plane (src/convertRoutine.cpp:40-46)
 __global__ void crop_kernel(const float *__restrict__ in, int w, int h, int pad,
                             float *__restrict__ out, long out_stride) {
@@ -274,6 +320,23 @@ cudaError_t launch_pad_upsample2x(const float *in, int w2, int h2, long in_strid
     dim3 b(32, 8);
     pad_upsample2x_kernel<<<grid2d(w2 + 2 * pad, h2 + 2 * pad, b), b, 0, s>>>(in, w2, h2, in_stride_floats, pad, rows_above,
                                                                                rows_below, out);
+    return cudaGetLastError();
+}
+
+// A row band's padded 2x input frame, materialised.  Folding the resize into the band's first-layer loads (the first_1xN+up2x form
+// of the one-GPU chain) is deliberately not done: the frame is 4 bytes per pixel beside 512 bytes per pixel of activations, and the
+// fold would need the halo exchange to deliver half-resolution rows into a side buffer instead of a row of the frame.
+cudaError_t launch_pad_upsample2x_xy(const float *in, int w2, int h2, long in_stride_floats, int pad_x, int pad_top, int pad_bottom,
+                                     int rows_above, int rows_below, float *out, cudaStream_t s, int skip_top, int skip_bottom) {
+    const int W = w2 + 2 * pad_x, pairs = ((h2 + pad_bottom - 1) >> 1) + ((pad_top + 1) >> 1) + 1;
+    dim3 b(32, 8);
+    const dim3 g = grid2d((W + 3) / 4, pairs, b);
+    if (W % 4 == 0 && reinterpret_cast<uintptr_t>(out) % 16 == 0)
+        pad_upsample2x_xy_kernel<true><<<g, b, 0, s>>>(in, w2, h2, in_stride_floats, pad_x, pad_top, pad_bottom, rows_above, rows_below, out,
+                                                       skip_top, skip_bottom);
+    else
+        pad_upsample2x_xy_kernel<false><<<g, b, 0, s>>>(in, w2, h2, in_stride_floats, pad_x, pad_top, pad_bottom, rows_above, rows_below, out,
+                                                        skip_top, skip_bottom);
     return cudaGetLastError();
 }
 

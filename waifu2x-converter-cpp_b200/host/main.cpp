@@ -148,10 +148,9 @@ int main(int argc, char **argv) {
     cmd.parse(argc, argv);
     const bool tta = cmd.get("tta") == "1";
     {
-        const char *ng = std::getenv("W2X_GPUS");
-        const int gpus = std::atoi(cmd.get("gpus").c_str()) > 1 ? std::atoi(cmd.get("gpus").c_str()) : ng ? std::atoi(ng) : 1;
-        if (tta && gpus > 1) {   // the passes run as one w2x_convert_chain call, which has no multi-GPU form
-            std::cerr << "Error : --tta 1 runs on one GPU; it cannot be combined with " << gpus << " GPUs (--gpus / W2X_GPUS)." << std::endl;
+        const int gpus = w2xc::gpuRuntime::plannedNumberOfGpus(std::atoi(cmd.get("gpus").c_str()));
+        if (tta && gpus > 1) {   // a TTA step has no multi-GPU form (w2x_multi_convert_chain refuses it)
+            std::cerr << "Error : --tta 1 runs on one GPU; it cannot be combined with " << gpus << " GPUs (--gpus / W2X_GPUS / W2X_DEVICES)." << std::endl;
             std::exit(1);
         }
     }
@@ -201,14 +200,14 @@ int main(int argc, char **argv) {
     if (noisePhase && !w2xc::modelUtility::generateModelFromJSON(modelDir + "/noise" + std::to_string(nrLevel) + "_model.json", noiseModels))
         leave(-1);                                                                          // :88-89
     // The Y plane after each pass depends only on the Y plane before it (split / merge / an exact 2x nearest resize copy values, the
-    // bicubic Y channel is overwritten at :148-154, U and V never feed back into Y).  So on one GPU the noise pass and every 2x
-    // iteration run as ONE chain that keeps Y on the device, while the bicubic iterations of U and V run here on the host.
-    // -m noise, --gpus n > 1 (w2x_multi_convert_plane), no usable device and a scale model that does not load keep the per-pass path below.
+    // bicubic Y channel is overwritten at :148-154, U and V never feed back into Y).  So the noise pass and every 2x iteration run as
+    // ONE chain that keeps Y on the device (with --gpus n > 1: its row bands, each on its GPU), while the bicubic iterations of U and
+    // V run here on the host.  -m noise, no usable device and a scale model that does not load keep the per-pass path below.
     // With --tta 1 every pass is a TTA step of the chain (-m noise a one-step chain); without a device the chain call reports it.
     bool chained = false;                          // the 2x iterations run in the chain
     if (scalePhase && iterTimesTwiceScaling >= 1 && w2xc::modelUtility::tryGenerateModelFromJSON(modelDir + "/scale2.0x_model.json", scaleModels)) {
         wait_for_gpu();
-        chained = tta || (w2xc::gpuRuntime::context() != nullptr && w2xc::gpuRuntime::multi() == nullptr);
+        chained = tta || w2xc::gpuRuntime::context() != nullptr;
     }
     const bool noiseChained = noisePhase && (chained || tta);
     if (chained || noiseChained) {

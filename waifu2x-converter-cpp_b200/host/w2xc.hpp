@@ -71,13 +71,37 @@ struct Plane {
 // Process-wide GPU runtime shared by Model::filter and convertWithModels (the reference keeps its process-wide state in
 // the modelUtility singleton as well).  The number of GPUs is the sibling of the reference's -j (src/main.cpp:58-60):
 // gpuRuntime::setNumberOfGpus(n) before the first conversion, or W2X_GPUS=n in the environment; planes are then cut into n
-// row bands with a per-layer halo exchange between the GPUs (bit-identical to one GPU).  W2X_DEVICE picks the first device.
+// row bands with a per-layer halo exchange between the GPUs (bit-identical to one GPU).  W2X_DEVICE picks the first device of n
+// consecutive ones; W2X_DEVICES=a,b,c names the devices one by one instead (GPUs that are not adjacent on a shared machine; a device
+// may be named more than once) and overrides W2X_DEVICE and W2X_GPUS -- a number set with setNumberOfGpus must then equal its length.
 class gpuRuntime {
 public:
     static bool setNumberOfGpus(int n) {
         if (n < 1 || created()) return false;
         requested() = n;
         return true;
+    }
+    // "a,b,c" -> {a, b, c}: 1 to 64 decimal device numbers, nothing else (no signs, blanks or empty fields)
+    static bool parseDeviceList(const char *list, std::vector<int> &ids) {
+        ids.clear();
+        if (!list || !*list) return false;
+        for (const char *p = list;; p++) {
+            if (*p < '0' || *p > '9') return false;
+            long v = 0;
+            for (; *p >= '0' && *p <= '9'; p++)
+                if ((v = v * 10 + (*p - '0')) > 1000000) return false;
+            ids.push_back((int)v);
+            if (!*p) return ids.size() <= 64;
+            if (*p != ',') return false;
+        }
+    }
+    // the number of GPUs a run with `requestedGpus` (0 = not given) will use, before the runtime exists: W2X_DEVICES, else the
+    // request, else W2X_GPUS, else 1
+    static int plannedNumberOfGpus(int requestedGpus) {
+        std::vector<int> ids;
+        if (parseDeviceList(std::getenv("W2X_DEVICES"), ids)) return (int)ids.size();
+        const char *ng = std::getenv("W2X_GPUS");
+        return requestedGpus > 1 ? requestedGpus : ng && std::atoi(ng) > 1 ? std::atoi(ng) : 1;
     }
     // nullptr if the runtime could not be created; the reason is printed ONCE, by the first caller that needs the context (not by
     // whichever thread happened to construct the runtime: a front end may create it in the background, see host/main.cpp)
@@ -101,11 +125,24 @@ private:
     gpuRuntime() {
         created() = true;
         const char *dev = std::getenv("W2X_DEVICE"), *ng = std::getenv("W2X_GPUS");
-        const int first = dev ? std::atoi(dev) : 0;
+        int first = dev ? std::atoi(dev) : 0;
         int n = requested() > 0 ? requested() : (ng ? std::atoi(ng) : 1);
-        if (n > 1) {
-            std::vector<int> ids;
+        std::vector<int> ids;
+        if (const char *list = std::getenv("W2X_DEVICES")) {
+            if (!parseDeviceList(list, ids)) {
+                error_ = std::string("W2X_DEVICES must be a comma-separated list of 1 to 64 device numbers (got \"") + list + "\")";
+                return;
+            }
+            if (requested() > 0 && requested() != (int)ids.size()) {
+                error_ = "W2X_DEVICES names " + std::to_string(ids.size()) + " device(s) but " + std::to_string(requested()) + " GPUs were asked for";
+                return;
+            }
+            n = (int)ids.size();
+            first = ids[0];
+        } else {
             for (int i = 0; i < n; i++) ids.push_back(first + i);
+        }
+        if (n > 1) {
             if (w2x_multi_create(ids.data(), n, &multi_) != W2X_OK) {
                 error_ = w2x_last_error();
                 multi_ = nullptr;
@@ -313,7 +350,8 @@ inline const w2x_model *modelFileOf(std::vector<std::unique_ptr<Model>> &models)
 // file, as for convertWithModels) and whether the plane is first resized to 2w x 2h by cv::resize INTER_NEAREST (:132-140).  The
 // plane stays on the GPU between the steps and the 2x plane is never built; each step's result is bit-identical to
 // convertWithModels on the previous step's (resized) output.  onStep(k) runs before step k starts, then the step prints its
-// progress lines like convertWithModels.  outputPlane is (re)allocated to the final size.  One GPU only (w2x_convert_chain).
+// progress lines like convertWithModels.  outputPlane is (re)allocated to the final size.  With several GPUs the plane's row bands stay
+// on their GPUs between the steps (w2x_multi_convert_chain, which has no form of a tta step), else w2x_convert_chain.
 // tta: the step is the mean of its conversions of the plane's 8 flips and transposes (W2X_STEP_TTA), the -tta switch of later
 // waifu2x front ends.  (No default member initialiser: ChainStep stays an aggregate under C++11.)
 struct ChainStep {
@@ -341,7 +379,12 @@ inline bool convertChainWithModels(Plane &inputPlane, Plane &outputPlane, const 
     } printer;
     (void)printer;
     w2x_ctx_set_log(ctx, &Printer::line, nullptr);
-    int rc = w2x_convert_chain(ctx, (int)steps.size(), files.data(), kinds.data(), inputPlane.data, inputPlane.width, inputPlane.height,
+    int rc;
+    if (w2x_multi *mg = gpuRuntime::multi())   // its lines go through the first context's log function, set above
+        rc = w2x_multi_convert_chain(mg, (int)steps.size(), files.data(), kinds.data(), inputPlane.data, inputPlane.width, inputPlane.height,
+                                     inputPlane.stride_bytes, outputPlane.data, outputPlane.stride_bytes, blockSplitting ? 1 : 0, onStep, user);
+    else
+        rc = w2x_convert_chain(ctx, (int)steps.size(), files.data(), kinds.data(), inputPlane.data, inputPlane.width, inputPlane.height,
                                inputPlane.stride_bytes, outputPlane.data, outputPlane.stride_bytes, blockSplitting ? 1 : 0, onStep, user);
     if (rc != W2X_OK) {
         std::cerr << w2x_last_error() << std::endl;
