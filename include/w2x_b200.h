@@ -120,7 +120,18 @@ W2X_API int w2x_ctx_get_engine(const w2x_ctx *ctx);
  *                           fp32 engine on sampled rows of a 4096x4096 white-noise scale2.0x pass (2.1 % of the 8-bit
  *                           values change, by 1); 566 Mpix/s on that pass against the default's 309 in the same run,
  *                           H100 80GB HBM3 at a 400 W power limit
- * The environment variable W2X_PRECISION=f16x3|f8|f16 sets the initial value of new contexts. */
+ * Activation range (a = the largest |activation| entering any tensor-core layer; relative error = max-abs error /
+ * max(1, max |reference|); the shipped models reach a = 1 on planes in [0, 1] and grow about linearly with the input's
+ * scale, so a plane in 0..255 reaches a = 100 to 300).  Asserted by tests/test_activation_range.py:
+ *   W2X_PRECISION_F16X3     <= 1e-6 relative to float64 arithmetic (2e-5 to the reference's own fp32 path) for
+ *                           a < 4094 (16 a < 65520, the fp16 limit of the activation records)
+ *   W2X_PRECISION_F16_F8X2  <= 6e-5 relative for a < 56 (16 a < 896).  From a = 56 the e4m3 copies saturate
+ *                           (xh8 = e4m3(16 a / 2) at 448, from a = 64 also xl8) and the corrections are capped:
+ *                           <= 1e-3 relative for a < 4094 (about 1e-4 at a = 150 to 300)
+ *   W2X_PRECISION_F16       <= 4e-3 relative for a < 4094
+ * Beyond a = 4094 every precision saturates its records at +-65504 (fp16 hi and lo): outputs stay finite, with no
+ * accuracy bound (they no longer follow the reference).  The fp32 engine has no such limit. */
+/* The environment variable W2X_PRECISION=f16x3|f8|f16 sets the initial value of new contexts. */
 #define W2X_PRECISION_F16X3 0
 #define W2X_PRECISION_F16_F8X2 1
 #define W2X_PRECISION_F16 2

@@ -12,19 +12,28 @@ pattern the kernel may produce:
   emulate_last_separate last_layer_kernel on the record frame
 """
 import numpy as np
+import torch
 
 F32 = np.float32
 F8_A, F8_C = 10, 1                 # xl8 = e4m3(xl * 2^F8_A), xh8 = e4m3(xh * 2^-F8_C)   (csrc/tc_config.cuh)
 ACT_SCALE = F32(16)
 
 
+F16_MAX = 65504.0
+
+
 def f16(x):
-    """round to fp16 (nearest, ties to even) and back to float32"""
-    return np.asarray(x, F32).astype(np.float16).astype(F32)
+    """round to fp16 (nearest, ties to even), saturating at +-65504 as the kernels' cvt.rn.satfinite.f16 does (NaN stays
+    NaN), and back to float32.  Below 65520 in magnitude this is the plain rounding; clipping first cannot move a value
+    that rounds to 65504 anyway."""
+    return np.clip(np.asarray(x, F32), -F16_MAX, F16_MAX).astype(np.float16).astype(F32)
 
 
 def e4m3(x):
-    """nearest e4m3fn value (ties to even, saturating at +-448: cvt.rn.satfinite.e4m3), as float64"""
+    """nearest e4m3fn value (ties to even, saturating at +-448: cvt.rn.satfinite.e4m3), as float64 (a float64 tensor for a
+    tensor).  torch's float8_e4m3fn cast is no model of the kernels: it returns NaN above 448."""
+    if isinstance(x, torch.Tensor):
+        return torch.from_numpy(e4m3(x.detach().to(torch.float64).numpy()))
     x = np.asarray(x, np.float64)
     a = np.abs(x)
     _, e = np.frexp(np.maximum(a, 2.0 ** -6))            # a = m 2^e, m in [0.5, 1): the binade's quantum is 2^(e - 4)

@@ -13,9 +13,14 @@ import torch.nn.functional as F
 ACT_SCALE = 16.0
 
 
+def half_sat(x):
+    """fp16 rounding saturating at +-65504, as the kernels' records convert (a plain .half() gives inf above 65519)"""
+    return x.clamp(-65504.0, 65504.0).to(torch.float16)
+
+
 def split16(x):
-    hi = x.to(torch.float16)
-    lo = (x - hi.to(x.dtype)).to(torch.float16)
+    hi = half_sat(x)
+    lo = half_sat(x - hi.to(x.dtype))
     return hi, lo
 
 

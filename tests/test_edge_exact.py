@@ -138,18 +138,21 @@ def selection_terms(x16r, w, f8):
     return (xh * col(wh), xl * col(wh_c), xh_c * col(wl_c)), ws, (wh, wl, wh_c, wl_c)
 
 
-def selection_acc(terms, f8):
-    """the float32 accumulator: f16x3 the exact sum; f16+f8x2 the main product plus the correction buffer (one add)"""
+def selection_acc(terms, f8, xh_only=False):
+    """the float32 accumulator: f16x3 the exact sum; f16+f8x2 the main product plus the correction buffer (one add); f16
+    (xh_only) the main product alone"""
     main, c1, c2 = terms
+    if xh_only:
+        return main.astype(F32)
     if f8:
         return add32(main.astype(F32), (c1 + c2).astype(F32))
     return (main + c1 + c2).astype(F32)
 
 
-def emulate_selection(x16r, w, b, f8):
+def emulate_selection(x16r, w, b, f8, xh_only=False):
     """a selection layer on the tensor-core engine: activations * 16 out ([Cout, H, W])"""
     terms, ws, _ = selection_terms(x16r, w, f8)
-    return tc_activation(selection_acc(terms, f8), ws, b)
+    return tc_activation(selection_acc(terms, f8, xh_only), ws, b)
 
 
 def _units(arrs):
@@ -194,7 +197,8 @@ def selection_report(x16r, w, b, f8):
     x = np.asarray(x16r, F32)
     d = x - f16(x)
     up, down = (np.asarray(x, np.float64) * (1 + s * 2.0 ** -20) for s in (1, -1))
-    rep["fp16 ties"] = int(np.sum((d != 0) & (up.astype(np.float16) != down.astype(np.float16))))
+    with np.errstate(over="ignore"):                                  # values past the fp16 range are no ties
+        rep["fp16 ties"] = int(np.sum((d != 0) & (up.astype(np.float16) != down.astype(np.float16))))
     xl8 = e4m3(d.astype(np.float64) * 2.0 ** F8_A)
     rep["subnormal xl8"] = int(np.sum((xl8 != 0) & (np.abs(xl8) < 2.0 ** -6)))
     rep["zeros"] = int(np.sum(x == 0))
@@ -210,16 +214,16 @@ def assert_selection(rep):
     assert rep["v_max"] < 448, rep                                  # xh8 = e4m3(v / 2) and xl8 stay below saturation
 
 
-def emulate_tc_model(plane, layers, f8, fused):
-    """Context.convert_plane of 1 -> C1 -> selection layers -> 1 on the tensor-core engine; also returns the middle layers'
-    inputs (with their zero ring) for selection_report"""
+def emulate_tc_model(plane, layers, f8, fused, xh_only=False):
+    """Context.convert_plane of 1 -> C1 -> selection layers -> 1 on the tensor-core engine (xh_only: W2X_PRECISION_F16,
+    f16x3 records); also returns the middle layers' inputs (with their zero ring) for selection_report"""
     n = len(layers)
     x16 = emulate_first_layer(np.pad(np.asarray(plane, F32), n, mode="edge"), *layers[0])
     inputs = []
     for w, b in layers[1:-1]:
         xr = np.pad(x16, ((0, 0), (1, 1), (1, 1)))                     # the TMA loads zero-fill outside the frame
         inputs.append((xr, w, b))
-        x16 = emulate_selection(xr, w, b, f8)
+        x16 = emulate_selection(xr, w, b, f8, xh_only)
     w2, b2 = layers[-1]
     out = emulate_last_fused(x16, w2, b2, n) if fused else emulate_last_separate(x16, w2, b2, n, f8)
     return out, inputs
@@ -624,3 +628,180 @@ def test_geometry_entry_points_are_bit_exact(w2x, tc_ctxs, prec):
         for band in bands:
             band.close()
     assert not fails, "\n".join(fails)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# the saturating range: x16 and v past 448, past 1024 and around 65504
+# ---------------------------------------------------------------------------------------------------------------------
+# (plane exponent s: planes = ordinary planes * 2^s plus fixed values around the fp16 limit; weight exponent t: the
+# selection weights * 2^-t, so wscale = 2^(11 + t), or the 2^14 clamp for t >= 4.  At the clamp a third of the outputs
+# get w = +-2^-(13 - t) (wh = 2, wh8 = e4m3(2^-9): the smallest e4m3 subnormal) and a third w = +-2^-(12 - t) (1 - 2^-12)
+# (wl = -2^-10, wl8 = e4m3(-2^-9)): with wscale 2^13 those copies would round to zero and drop a correction product, so
+# the bits depend on the packer clamping at 2^14 (test_the_clamp_cases_depend_on_the_2_14_clamp).)
+SAT_CASES = [(6, -11), (9, -6), (11, 2), (12, 4), (12, 5)]
+SAT_SPECIAL = np.array([65504, 65519, 65520, 65535, 70000, 98304, 131072, 1e6, 896, 960, 1023.75, 1024, 1500.5]) / 16
+
+
+def sat_planes(c, h, w, s, seed):
+    x = ordinary_planes(c, h, w, seed) * F32(2.0 ** s)
+    rng = np.random.default_rng(seed + 1)
+    pick = rng.random((c, h, w)) < 0.15
+    x[pick] = (rng.choice(SAT_SPECIAL, int(pick.sum())) * rng.choice([-1.0, 1.0], int(pick.sum()))).astype(F32)
+    return x.astype(F32)
+
+
+def sat_selection_layer(cin, cout, case, seed, t):
+    w, b = selection_layer(cin, cout, case, seed)
+    if t >= 4:                                                        # the clamp: wh8 or wl8 on the smallest e4m3 subnormal
+        o = np.arange(cout)
+        i, ky, kx = _selection(w)
+        sign = np.sign(w[o, i, ky, kx]).astype(np.float64)
+        edge = np.where(o % 3 == 1, sign * 2.0 ** -(13 - t), sign * 2.0 ** -(12 - t) * (1 - 2.0 ** -12))
+        w[o, i, ky, kx] = np.where(o % 3 == 0, w[o, i, ky, kx], edge)
+    return (w * F32(2.0 ** -t)).astype(F32), b
+
+
+def _sat_filter_cases():
+    for k, (cin, cout) in enumerate(SHAPES):
+        for c, (s, t) in enumerate(SAT_CASES):
+            w, b = sat_selection_layer(cin, cout, k, 500 + k, t)
+            yield (cin, cout), (s, t), w, b, sat_planes(cin, 9 + c, 17 + 2 * c, s, seed=100 * k + c)
+
+
+def _sat_counts(x16):
+    x = np.asarray(x16, F32)
+    xh = f16(x)
+    d = (x - xh).astype(np.float64)
+    return np.array([np.sum(np.abs(xh) > 928), np.sum(np.abs(d) * 2.0 ** F8_A > 464), np.sum(np.abs(x) >= 65520),
+                     np.sum((np.abs(x) >= 65504) & (np.abs(x) < 65520))])
+
+
+def assert_selection_exact(rep):
+    """assert_selection without its small-input range: exact weight copies, float32-exact partial sums, correction groups
+    within GROUP_SPAN_MAX bits"""
+    assert rep["splits exact"] and rep["partial sums fit float32"] and rep.get("group_span", 0) <= GROUP_SPAN_MAX, rep
+
+
+def test_the_clamp_cases_depend_on_the_2_14_clamp(w2x, monkeypatch):
+    """The packer clamps wscale at 2^14 for every clamp case, and the cases have teeth: emulated with a clamp at 2^13 they
+    change bits in f16+f8x2 (the e4m3 subnormal copies round to zero).  f16x3 and f16 keep every bit (the fp16 copies
+    only scale), so the packer assertion is what pins the clamp for them."""
+    cases = [c for c in _sat_filter_cases() if c[1][1] >= 4]
+    assert cases
+    for _, _, w, b, _ in cases:
+        assert w2x.Model.from_arrays([w], [b]).debug_tc_pack(0)[3] == 2.0 ** 14
+    want = [readback(emulate_selection(mul32(np.pad(x, ((0, 0), (1, 1), (1, 1)), mode="edge"), F32(16)), w, b, True), True)
+            for _, _, w, b, x in cases]
+    clamp = T.wscale_of
+    monkeypatch.setattr(T, "wscale_of", lambda w_: min(clamp(w_), 2.0 ** 13))
+    changed = 0
+    for (_, _, w, b, x), y in zip(cases, want):
+        got = readback(emulate_selection(mul32(np.pad(x, ((0, 0), (1, 1), (1, 1)), mode="edge"), F32(16)), w, b, True), True)
+        changed += not np.array_equal(got, y)
+    assert changed == len(cases), (changed, len(cases))
+
+
+@pytest.mark.parametrize("prec", ["f16x3", "f16+f8x2", "f16"])
+def test_saturating_selection_conditions_hold(prec):
+    """the selection conditions (but v, which now may saturate) on every saturating case; across them the inputs (planar_to_nhwc)
+    and the outputs (the epilogue) reach xh8 and xl8 saturation, hi saturation and the last values below it"""
+    f8 = prec == "f16+f8x2"
+    ins, outs, wscales = np.zeros(4, int), np.zeros(4, int), set()
+    for _, (s, t), w, b, x in _sat_filter_cases():
+        xr = mul32(np.pad(x, ((0, 0), (1, 1), (1, 1)), mode="edge"), F32(16))
+        rep = selection_report(xr, w, b, f8)
+        assert rep["wscale"] == 2.0 ** min(11 + t, 14), rep
+        assert_selection_exact(rep)
+        ins += _sat_counts(xr)
+        outs += _sat_counts(emulate_selection(xr, w, b, f8, prec == "f16"))
+        wscales.add(rep["wscale"])
+    print(prec, "inputs", ins, "outputs", outs)
+    assert (ins > 0).all() and (outs[:3] > 0).all(), (ins, outs)
+    assert wscales == {2.0 ** 0, 2.0 ** 5, 2.0 ** 13, 2.0 ** 14}
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("prec", ["f16x3", "f16+f8x2", "f16"])
+def test_saturating_filter_layer_selection_is_bit_exact(w2x, prec):
+    """planar_to_nhwc on planes with x16 past 896, 1024 and 65504 (hi, lo, xh8, xl8 saturated), one selection layer at
+    wscale 2^0 .. the 2^14 clamp, nhwc_to_planar of saturated records, at every, one and three SMs: finite and bit-exact"""
+    f8, xh_only = prec == "f16+f8x2", prec == "f16"
+    ctx = w2x.Context(0, engine=w2x.ENGINE_TC)
+    ctx.set_precision({"f16x3": w2x.PRECISION_F16X3, "f16+f8x2": w2x.PRECISION_F16_F8X2, "f16": w2x.PRECISION_F16}[prec])
+    fails = []
+    try:
+        for (cin, cout), case, w, b, x in _sat_filter_cases():
+            model = w2x.Model.from_arrays([w], [b])
+            xr = mul32(np.pad(x, ((0, 0), (1, 1), (1, 1)), mode="edge"), F32(16))
+            want = readback(emulate_selection(xr, w, b, f8, xh_only), f8)
+            assert np.isfinite(want).all()
+            for sms in NUM_SMS:
+                ctx.debug_set_num_sms(sms)
+                got = ctx.filter_layer(model, 0, x)
+                if not np.array_equal(got, want):
+                    fails.append(f"{cin}->{cout} case={case} sms={sms}: {_mismatch(got, want)}")
+    finally:
+        ctx.close()
+    assert not fails, "\n".join(fails[:20])
+
+
+# (widths, first-layer weight exponent g): one selection layer, or two in a row, the second reading the first's epilogue
+# records (hi / lo or hi / xh8 / xl8) in the saturating range
+SAT_MODELS = [((32, 64), 8), ((32, 64), 12), ((64, 32), 12), ((128, 128), 8), ((32, 64, 128), 12), ((128, 32, 64), 10)]
+
+
+def _sat_model(k, widths, g):
+    layers = sel_model(widths, k, 77 + k)
+    layers[0] = ((layers[0][0] * F32(2.0 ** g)).astype(F32), layers[0][1] * 2.0 ** g)
+    return layers, plane_for(13 + k, 21, k)
+
+
+@pytest.mark.parametrize("prec", ["f16x3", "f16+f8x2", "f16"])
+def test_saturating_model_conditions_hold(prec):
+    """selection_report on the middle layers' inputs of every case below (both the plane and its 2x resize); the first
+    layer's records saturate hi where g = 12, and the second selection layer of each chain reads epilogue records whose
+    xh8 and xl8 saturate"""
+    f8, xh_only = prec == "f16+f8x2", prec == "f16"
+    for k, (widths, g) in enumerate(SAT_MODELS):
+        layers, x = _sat_model(k, widths, g)
+        for plane in (x, np.repeat(np.repeat(x, 2, axis=0), 2, axis=1)):
+            inputs = emulate_tc_model(plane, layers, f8, True, xh_only)[1]
+            for xr, w, b in inputs:
+                assert_selection_exact(selection_report(xr, w, b, f8))
+            first = _sat_counts(inputs[0][0])
+            assert first[0] > 0 and (g != 12 or first[2] > 0), (widths, g, first)
+            if len(inputs) > 1:
+                assert (_sat_counts(inputs[1][0])[:2] > 0).all(), (widths, g, _sat_counts(inputs[1][0]))
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("prec", ["f16x3", "f16+f8x2", "f16"])
+def test_saturating_first_layer_is_bit_exact(w2x, prec):
+    """first_layer_kernel with weights * 2^8 .. 2^12 (its records past 896, 1024 and 65504) in both variants: the plane
+    itself (convert_plane) and its nearest-neighbour 2x resize read in place (a chain's upscale step, UP2X); one selection
+    layer, or two with the second reading saturated epilogue records; the last layer fused and separate"""
+    f8, xh_only = prec == "f16+f8x2", prec == "f16"
+    ctx = w2x.Context(0, engine=w2x.ENGINE_TC)
+    ctx.set_precision({"f16x3": w2x.PRECISION_F16X3, "f16+f8x2": w2x.PRECISION_F16_F8X2, "f16": w2x.PRECISION_F16}[prec])
+    fails = []
+    try:
+        for k, (widths, g) in enumerate(SAT_MODELS):
+            layers, x = _sat_model(k, widths, g)
+            model = _model(w2x, layers)
+            up = np.repeat(np.repeat(x, 2, axis=0), 2, axis=1)
+            for fused in (True, False):
+                ctx.debug_set_fuse_last(fused)
+                for name, got, plane in (("plane", lambda: ctx.convert_plane(model, x), x),
+                                         ("up2x", lambda: ctx.convert_chain([(model, True)], x), up)):
+                    want, inputs = emulate_tc_model(plane, layers, f8, fused, xh_only)
+                    for xr, w, b in inputs:
+                        assert_selection_exact(selection_report(xr, w, b, f8))
+                    assert np.isfinite(want).all()
+                    for sms in NUM_SMS:
+                        ctx.debug_set_num_sms(sms)
+                        r = got()
+                        if not np.array_equal(r, want):
+                            fails.append(f"{widths} 2^{g} {name} fused={fused} sms={sms}: {_mismatch(r, want)}")
+    finally:
+        ctx.close()
+    assert not fails, "\n".join(fails[:20])

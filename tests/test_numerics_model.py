@@ -5,6 +5,7 @@ import numpy as np
 import pytest
 
 import tc_numerics_model as T
+from exact_arith import e4m3
 
 
 @pytest.mark.parametrize("name", ["scale2.0x", "noise1", "noise2"])
@@ -37,13 +38,10 @@ def test_single_pass_fp16_would_fail_the_gate(oracle_mod, oracle_models, ncpu):
 
 def test_fp16_plus_two_e4m3_corrections_is_inside_the_gate(oracle_mod, oracle_models, ncpu):
     """W2X_PRECISION_F16_F8X2: xh*wh in fp16, xl*wh and xh*wl on e4m3 copies (scale exponents F8_A = 10, F8_C = 1).
-    Emulated with torch.float8_e4m3fn: ~2e-5 on white noise, 4x inside the 1e-4 gate."""
+    Emulated with the kernels' saturating e4m3 rounding (exact_arith.e4m3): ~2e-5 on white noise, 4x inside the 1e-4 gate."""
     import torch
     import torch.nn.functional as F
     A, Cc = 10, 1
-
-    def e4m3(t):
-        return t.to(torch.float8_e4m3fn).to(torch.float64)
 
     worst = 0.0
     for name in ("scale2.0x", "noise1"):
@@ -59,7 +57,7 @@ def test_fp16_plus_two_e4m3_corrections_is_inside_the_gate(oracle_mod, oracle_mo
             w = torch.from_numpy(om.weights[li]) * ws
             wh = w.half().float()
             xs = act * 16.0
-            xh = xs.half().float()
+            xh = T.half_sat(xs).float()
             acc = (F.conv2d(xh.double(), wh.double(), padding=1) +
                    F.conv2d(e4m3((xs - xh) * 2.0 ** A), e4m3(wh * 2.0 ** -A), padding=1) +
                    F.conv2d(e4m3(xh * 2.0 ** -Cc), e4m3((w - wh) * 2.0 ** Cc), padding=1))
@@ -69,13 +67,31 @@ def test_fp16_plus_two_e4m3_corrections_is_inside_the_gate(oracle_mod, oracle_mo
     assert worst <= 4e-5, worst
 
 
+def test_the_emulators_saturate_where_torchs_casts_do_not():
+    """The kernels convert with cvt.rn.satfinite: e4m3 clamps at +-448 and fp16 at +-65504.  torch's float8_e4m3fn cast
+    gives NaN once a value rounds past 448 and .half() gives inf from 65520, so neither models the kernels there; the
+    emulators go through exact_arith.e4m3 and half_sat.  Below the thresholds all of them agree."""
+    import torch
+    from exact_arith import f16
+    p = torch.tensor([416.0, 448.0, 460.0, 464.0, 465.0, 480.0, 896.0, 1e4, 3e38, -470.0, -1e4])
+    torch_cast = p.to(torch.float8_e4m3fn).to(torch.float64)
+    ours = e4m3(p)
+    assert ours.dtype == torch.float64
+    assert ours.tolist() == [416.0, 448.0, 448.0, 448.0, 448.0, 448.0, 448.0, 448.0, 448.0, -448.0, -448.0]
+    assert torch.equal(torch_cast[:4], ours[:4]) and torch.isnan(torch_cast[4:]).all()
+    h = torch.tensor([65504.0, 65519.0, 65520.0, 7e4, -1e9, float("nan")])
+    assert T.half_sat(h).float()[:5].tolist() == [65504.0, 65504.0, 65504.0, 65504.0, -65504.0]
+    assert torch.isnan(T.half_sat(h)[5])
+    assert torch.isinf(h.half()[2:5]).all()
+    assert np.array_equal(f16(h.numpy()), T.half_sat(h).float().numpy(), equal_nan=True)
+
+
 def _f8_emulated(om, x, drop_xl=(), drop_wl=()):
     """the default precision's arithmetic (see the test above) for one plane, wide accumulation; drop_xl / drop_wl: layers
     whose xl*wh / xh*wl correction pass is left out (what-if experiments, not a shipped mode)"""
     import torch
     import torch.nn.functional as F
     A, Cc = 10, 1
-    e4m3 = lambda t: t.to(torch.float8_e4m3fn).to(torch.float64)
     n = len(om)
     act = torch.from_numpy(np.pad(x, n, mode="edge"))[None, None]
     act = T.leaky(F.conv2d(F.pad(act, (1, 1, 1, 1), mode="replicate"), torch.from_numpy(om.weights[0])) +
@@ -85,7 +101,7 @@ def _f8_emulated(om, x, drop_xl=(), drop_wl=()):
         w = torch.from_numpy(om.weights[li]) * ws
         wh = w.half().float()
         xs = act * 16.0
-        xh = xs.half().float()
+        xh = T.half_sat(xs).float()
         acc = F.conv2d(xh.double(), wh.double(), padding=1)
         if li not in drop_xl:
             acc = acc + F.conv2d(e4m3((xs - xh) * 2.0 ** A), e4m3(wh * 2.0 ** -A), padding=1)
@@ -149,17 +165,16 @@ def test_winograd_f2x2_3x3_in_the_split_arithmetic_would_stay_inside_the_gate(or
     import torch
     import torch.nn.functional as F
     A, Cc = 10, 1
-    e4m3 = lambda t: t.to(torch.float8_e4m3fn).to(torch.float64)
     Bt = torch.tensor([[1, 0, -1, 0], [0, 1, 1, 0], [0, -1, 1, 0], [0, 1, 0, -1]], dtype=torch.float64)
     G = torch.tensor([[1, 0, 0], [.5, .5, .5], [.5, -.5, .5], [0, 0, 1]], dtype=torch.float64)
     At = torch.tensor([[1, 1, 1, 0], [0, 1, -1, -1]], dtype=torch.float64)
 
     def split_mm(V, U):     # [P, Cin] x [Cout, Cin]^T in the GPU's arithmetic
-        Vh, Uh = V.float().half().double(), U.float().half().double()
+        Vh, Uh = T.half_sat(V.float()).double(), U.float().half().double()
         return Vh @ Uh.T + e4m3((V - Vh) * 2.0 ** A) @ e4m3(Uh * 2.0 ** -A).T + e4m3(Vh * 2.0 ** -Cc) @ e4m3((U - Uh) * 2.0 ** Cc).T
 
     def conv_direct(xs, w):
-        wh, xh = w.float().half().double(), xs.float().half().double()
+        wh, xh = w.float().half().double(), T.half_sat(xs.float()).double()
         return (F.conv2d(xh, wh, padding=1) + F.conv2d(e4m3((xs - xh) * 2.0 ** A), e4m3(wh * 2.0 ** -A), padding=1) +
                 F.conv2d(e4m3(xh * 2.0 ** -Cc), e4m3((w - wh) * 2.0 ** Cc), padding=1))
 

@@ -48,7 +48,7 @@ LATTICE_WSCALE = 2.0 ** 10
 # ---------------------------------------------------------------------------------------------------------------------
 # emulator
 # ---------------------------------------------------------------------------------------------------------------------
-def operands(x16, w, f8):
+def operands(x16, w, f8, xh_only=False):
     """The three factor pairs a tensor-core layer multiplies, as float64 with the e4m3 copies' power-of-two scales taken
     out (scaling by 2^k commutes with the products): [(xh, wh), (xl, wh), (xh, wl)], and wscale.  x16: activations * 16
     (float32 [C, ...]); w: raw weights [Cout, Cin, 3, 3]."""
@@ -64,6 +64,8 @@ def operands(x16, w, f8):
                  (e4m3(xh * 2.0 ** -F8_C) * 2.0 ** F8_C, e4m3(wl * 2.0 ** F8_C) * 2.0 ** -F8_C)]     # xh8 * wl8
     else:
         pairs = [(xh, wh), (f16(xl), wh), (xh, f16(wl))]
+    if xh_only:                                                      # W2X_PRECISION_F16: the xh * wh product alone
+        pairs = pairs[:1]
     return [(np.asarray(a, np.float64), np.asarray(b, np.float64)) for a, b in pairs], ws
 
 
@@ -127,22 +129,22 @@ def accumulate(pairs, exact=True):
 
 
 
-def emulate_filter_layer(planes, w, b, f8, exact=True):
+def emulate_filter_layer(planes, w, b, f8, exact=True, xh_only=False):
     """Context.filter_layer on the tensor-core engine: planar_to_nhwc (replicate ring, x16, split) -> layer -> nhwc_to_planar"""
     x16 = mul32(np.pad(planes, ((0, 0), (1, 1), (1, 1)), mode="edge"), F32(16))
-    pairs, ws = operands(x16, w, f8)
+    pairs, ws = operands(x16, w, f8, xh_only)
     return readback(tc_activation(accumulate(pairs, exact), ws, b), f8)
 
 
 
 
-def emulate_model(plane, model, f8, fused):
+def emulate_model(plane, model, f8, fused, xh_only=False):
     """Context.convert_plane of a 1 -> C1 -> C2 -> 1 model on the tensor-core engine"""
     (w0, b0), (w1, b1), (w2, b2) = model
     n = 3
     frame = np.pad(plane, n, mode="edge")
     x16 = emulate_first_layer(frame, w0, b0)
-    pairs, ws = operands(x16, w1, f8)
+    pairs, ws = operands(x16, w1, f8, xh_only)
     zpad = [(np.pad(a, ((0, 0), (1, 1), (1, 1))), b) for a, b in pairs]     # the TMA loads zero-fill outside the frame
     a1 = tc_activation(accumulate(zpad), ws, b1)                      # [C2, ph, pw], activations * 16
     return emulate_last_fused(a1, w2, b2, n) if fused else emulate_last_separate(a1, w2, b2, n, f8)
@@ -240,6 +242,143 @@ def assert_lattice(rep):
     assert rep["group_max_q"] <= GROUP_MAX_Q, rep["group_max_q"]
     assert rep["v_max"] < 1024, rep["v_max"]
     assert rep["wscale"] == LATTICE_WSCALE, rep["wscale"]
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# the lattice scaled into the range where the operand copies saturate
+# ---------------------------------------------------------------------------------------------------------------------
+# Activation regimes: x16 = n 2^a + k 2^l (n in +-NS, k in {-1, 0, 1}), xh = fp16(x16) = n 2^a, xl = k 2^l:
+#   base  x16 in {1, 2}               nothing saturates (the lattice above)
+#   xh8   x16 in [896, 1024)          xh8 = e4m3(xh / 2) saturates at 448 for xh = 960 (480 -> 448); xl8 is exact
+#   xl8   x16 in {2048, 3072} +- 1/2  xh8 saturates (1024, 1536 -> 448) and xl8 = e4m3(1/2 * 2^10) too (512 -> 448)
+# The tensor cores multiply whatever the copies hold: the emulator's saturating split is what the kernel must produce.
+# No regime puts the layer's INPUT just below 65504: there xh / xl8-grain is 2^20 Q, so a handful of products already
+# leaves fp32's 24 bits and the sum would depend on the HGMMA order.  The wgmma reads such records in
+# tests/test_edge_exact.py (selection layers, one product per output: planar_to_nhwc and first-layer records past 65504
+# and up to 10^6); here the layer's OUTPUT crosses 65504 (wexp 0 and 5) and the epilogue's saturated records are read
+# back by nhwc_to_planar and last_layer_kernel.
+# The coarser activations cost partial-sum headroom (main products up to 2^16 Q where the base lattice has 2^14 Q), so
+# fewer weights are nonzero there; lattice_report measures (b) and (c) on the very operands of the precision under test.
+# Weight exponent e: w = (wh + wl) 2^-e, so the packer picks wscale 2^e (2^14 for e > 14: the clamp) and the kernel sees
+# w * wscale = (wh + wl) 2^(e - min(e, 14)); the products keep their bits, the epilogue's v = acc / wscale + 16 b moves by
+# 2^(10 - e) against the base lattice's and crosses the epilogue's own saturation thresholds (v >= 896: xh8, v >= 1024:
+# xl8 may, |v| >= 65520: hi would be inf without the saturating conversion).
+REGIMES = {"base": ((1.0, 2.0), 0, -13, 0.25), "xh8": ((1.75, 1.875), 9, -4, 0.04), "xl8": ((1.0, 1.5), 11, -1, 0.015)}
+# (c) for the regimes: a group reaches 98 Q (7 bits; saturated xl8 * wh = 14 Q, xh8 * wl = 7 Q in the xl8 regime), inside
+# the 13-bit correction groups tests/test_edge_exact.py has the H100's e4m3 accumulator hold exactly
+REGIME_GROUP_MAX_Q = 128
+REGIME_Q = {"base": 2.0 ** -4, "xh8": 2.0 ** 3, "xl8": 2.0 ** 4}    # the quantum of every product, f16x3 or e4m3 copies
+
+
+def regime_planes(c, h, w, seed, regime):
+    """input planes x = (n 2^a + k 2^l) / 16 of an activation regime"""
+    ns, a, l, _ = REGIMES[regime]
+    rng = np.random.default_rng(seed)
+    n = rng.choice([-1.0, 1.0], size=(c, h, w)) * rng.choice(ns, size=(c, h, w)) * 2.0 ** a
+    k = rng.choice([-1, 0, 1], size=(c, h, w), p=[0.25, 0.5, 0.25])
+    return ((n + k * 2.0 ** l) / 16).astype(F32)
+
+
+def regime_layer(cin, cout, seed, regime, wexp):
+    """lattice_layer with the regime's density and weight exponent wexp (wscale = 2^min(wexp, 14))"""
+    rng = np.random.default_rng(seed)
+    shape = (cout, cin, 3, 3)
+    nz = rng.random(shape) < REGIMES[regime][3]
+    wh = np.where(nz, rng.choice([-512.0, 512.0], size=shape), 0.0)
+    wl = np.where(nz, rng.choice([-0.125, 0.0, 0.125], size=shape, p=[0.25, 0.5, 0.25]), 0.0)
+    wh[0, 0, 1, 1], wl[0, 0, 1, 1] = 512.0, 0.125                     # |w| = (512 + 1/8) 2^-wexp: wscale = 2^wexp
+    w = ((wh + wl) * 2.0 ** -wexp).astype(F32)
+    b = rng.integers(-256, 257, cout) * 2.0 ** -10
+    return w, b
+
+
+def regime_model(c1, c2, seed, regime, wexp):
+    """lattice_model in a regime: the first layer's outputs are x16 = n1 2^a or n2 2^a (+ k 2^l), all positive"""
+    (n1, n2), a, l, _ = REGIMES[regime]
+    rng = np.random.default_rng(seed)
+    w0 = np.zeros((c1, 1, 3, 3), F32)
+    tap, sign = rng.integers(0, 9, c1), rng.choice([-1.0, 1.0], c1)
+    w0[np.arange(c1), 0, tap // 3, tap % 3] = sign * (n2 - n1) * 2.0 ** a / 16
+    b0 = (np.where(sign > 0, n1, n2) * 2.0 ** a + rng.integers(-1, 2, c1) * 2.0 ** l) / 16
+    w1, b1 = regime_layer(c1, c2, seed + 1, regime, wexp)
+    w2 = (rng.standard_normal((1, c2, 3, 3)) * 0.05).astype(F32)
+    b2 = np.array([F32(rng.standard_normal() * 0.05)], np.float64)
+    return [(w0, b0), (w1, b1), (w2, b2)]
+
+
+def saturation(x16):
+    """how many of the values x16 (activations * 16, as a record encodes them) saturate which conversion"""
+    x = np.asarray(x16, F32)
+    xh = f16(x)
+    d = (x - xh).astype(np.float64)
+    return {"xh8": int(np.sum(np.abs(xh) * 2.0 ** -F8_C > 464)),          # rounds past 448: e4m3 would need 480
+            "xl8": int(np.sum(np.abs(d) * 2.0 ** F8_A > 464)),
+            "hi": int(np.sum(np.abs(x) >= 65520))}
+
+
+def regime_of(x16):
+    """the activation regime of a layer input, from its fp16 hi values alone"""
+    ax = np.abs(f16(x16).astype(np.float64))
+    ax = ax[ax != 0]
+    if ax.max() < 3:
+        return "base"
+    if ax.min() >= 896 and ax.max() < 1024:
+        return "xh8"
+    if ax.min() >= 1024 and ax.max() < 65504:
+        return "xl8"
+    return "mixed"
+
+
+def regime_report(x16_ring, w, b, prec):
+    """(b), (c), the quantum and the no-lone-wl rule on the operands the precision multiplies (the emulator's saturating
+    split), the input's regime, the wscale, and which saturations the layer's input and its epilogue exercise"""
+    f8, xh_only = prec == "f16+f8x2", prec == "f16"
+    pairs, ws = operands(np.asarray(x16_ring, F32), w, f8, xh_only)
+    units, q = accumulate_units(pairs)
+    mag, q_mag = accumulate_units([(np.abs(a), np.abs(b_)) for a, b_ in pairs])
+    assert q_mag == q
+    rep = {"q": q, "sum_max_q": float(max((mag + units).max(), (mag - units).max())) / 2, "wscale": ws}
+    wsc = (w * F32(ws)).astype(F32)
+    rep["no lone wl"] = bool(np.all((wsc == f16(wsc)) | (f16(wsc) != 0)))
+    g = 0.0
+    if f8:                                                            # (c) on the e4m3 copies the wgmma multiplies
+        (_, _), (xl8, wh8), (xh8, wl8) = pairs
+        h, wd = xl8.shape[1] - 2, xl8.shape[2] - 2
+        for c in range(xl8.shape[0] // 32):
+            cs = slice(32 * c, 32 * c + 32)
+            for ky in range(3):
+                for kx in range(3):
+                    s = (np.einsum("oi,ihw->ohw", np.abs(wh8[:, cs, ky, kx]), np.abs(xl8[cs, ky:ky + h, kx:kx + wd])) +
+                         np.einsum("oi,ihw->ohw", np.abs(wl8[:, cs, ky, kx]), np.abs(xh8[cs, ky:ky + h, kx:kx + wd])))
+                    g = max(g, float(s.max()))
+    rep["group_max_q"] = g / q
+    rep["regime"] = regime_of(x16_ring)
+    rep["in"] = saturation(x16_ring)
+    v = tc_activation((units.astype(np.float64) * q).astype(F32), ws, b)
+    rep["out"] = saturation(v)
+    rep["v_max"] = float(np.abs(v).max())
+    return rep
+
+
+def assert_regime(rep, regime, wexp):
+    assert rep["regime"] == regime, rep
+    assert rep["wscale"] == 2.0 ** min(wexp, 14), rep
+    assert rep["no lone wl"], rep
+    assert rep["sum_max_q"] <= SUM_MAX_Q, rep
+    assert rep["group_max_q"] <= REGIME_GROUP_MAX_Q, rep
+    assert rep["q"] >= REGIME_Q[regime] * 2.0 ** (min(wexp, 14) - wexp), rep
+    if regime == "base":                                              # what each regime is there for
+        assert not any(rep["in"].values()), rep
+    elif regime == "xh8":
+        assert rep["in"]["xh8"] > 0 and rep["in"]["xl8"] == 0 and rep["in"]["hi"] == 0, rep
+    else:
+        assert rep["in"]["xh8"] > 0 and rep["in"]["xl8"] > 0 and rep["in"]["hi"] == 0, rep
+
+
+# (activation regime, weight exponent): wscale 2^0, 2^5, 2^10, 2^13 and the 2^14 clamp (wexp 16); the epilogue's v then
+# reaches every saturation threshold of the record encodings (checked by test_regime_conditions_hold)
+REGIME_CASES = [("base", 0), ("base", 5), ("xh8", 10), ("xh8", 0), ("xl8", 13), ("xl8", 16), ("xl8", 5)]
+ALL_PRECISIONS = ["f16x3", "f16+f8x2", "f16"]
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -487,3 +626,126 @@ def test_output_does_not_depend_on_the_grid(w2x, tc_ctxs, oracle_mod, oracle_mod
         ctx.debug_set_num_sms(0)
         ctx.debug_set_fuse_last(True)
     assert not fails, "\n".join(fails)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# the saturating range: activation regimes and weight exponents
+# ---------------------------------------------------------------------------------------------------------------------
+REGIME_LAYER_SIZES = [(14, 15), (29, 23)]
+REGIME_MODEL_SIZES = [(11, 18), (25, 27)]
+
+
+def _regime_id(case):
+    return f"{case[0]}-wexp{case[1]}"
+
+
+def _regime_layer_inputs(case, cin, cout, i, wd, h):
+    regime, wexp = case
+    w, b = regime_layer(cin, cout, seed=100 * cin + cout + wexp, regime=regime, wexp=wexp)
+    x = regime_planes(cin, h, wd, seed=1000 * i + cin + cout, regime=regime)
+    return w, b, x
+
+
+@pytest.mark.parametrize("prec", ALL_PRECISIONS)
+def test_regime_conditions_hold(prec):
+    """(b), (c), the input regime and the wscale on every single-layer and whole-model input of the GPU tests below; and
+    across them the epilogue's output reaches each saturation: v past 896 (xh8), an xl8 past 448, |v| >= 65520 (hi)"""
+    out = {"xh8": 0, "xl8": 0, "hi": 0}
+    for case in REGIME_CASES:
+        for cin, cout in SHAPES:
+            for i, (wd, h) in enumerate(REGIME_LAYER_SIZES):
+                w, b, x = _regime_layer_inputs(case, cin, cout, i, wd, h)
+                rep = regime_report(mul32(np.pad(x, ((0, 0), (1, 1), (1, 1)), mode="edge"), F32(16)), w, b, prec)
+                assert_regime(rep, *case)
+                out = {k: out[k] + rep["out"][k] for k in out}
+            m = regime_model(cin, cout, 10 * cin + cout, *case)
+            for i, (wd, h) in enumerate(REGIME_MODEL_SIZES):
+                x16 = emulate_first_layer(np.pad(binary_plane(h, wd, i), 3, mode="edge"), *m[0])
+                rep = regime_report(np.pad(x16, ((0, 0), (1, 1), (1, 1))), *m[1], prec)
+                assert_regime(rep, *case)
+                out = {k: out[k] + rep["out"][k] for k in out}
+    print(prec, "epilogue saturations", out)
+    assert all(v > 0 for v in out.values()), out
+
+
+def test_the_lattice_catches_a_dropped_saturation():
+    """The regimes' emulation differs from the unsaturated arithmetic: with xh8, xl8 and the epilogue's hi computed without
+    the clamps, the emulated layers change (so a kernel that did not saturate could not match)"""
+    w, b, x = _regime_layer_inputs(("xl8", 5), 32, 32, 0, *REGIME_LAYER_SIZES[0])
+    x16 = mul32(np.pad(x, ((0, 0), (1, 1), (1, 1)), mode="edge"), F32(16))
+    pairs, _ = operands(x16, w, True)
+    xh = f16(x16).astype(np.float64)
+    assert not np.array_equal(pairs[2][0], xh) and not np.array_equal(pairs[1][0], x16 - xh)
+    v = emulate_filter_layer(x, w, b, f8=False)
+    assert np.isfinite(v).all() and np.abs(v).max() >= 2 * 65504 / 16 - 1     # hi and lo both saturated somewhere
+
+
+def _prec_ctx(w2x, prec):
+    ctx = w2x.Context(0, engine=w2x.ENGINE_TC)
+    ctx.set_precision({"f16x3": w2x.PRECISION_F16X3, "f16+f8x2": w2x.PRECISION_F16_F8X2, "f16": w2x.PRECISION_F16}[prec])
+    return ctx
+
+
+@pytest.fixture(scope="module")
+def all_ctxs(w2x):
+    c = {p: _prec_ctx(w2x, p) for p in ALL_PRECISIONS}
+    yield c
+    for v in c.values():
+        v.close()
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("case", REGIME_CASES, ids=_regime_id)
+@pytest.mark.parametrize("prec", ALL_PRECISIONS)
+def test_single_layer_in_saturating_regimes_is_bit_exact(w2x, all_ctxs, case, prec):
+    """planar_to_nhwc -> tc_conv3x3_kernel<Cin, Cout> -> nhwc_to_planar on activations whose e4m3 copies saturate, at
+    wscale 2^0 .. the 2^14 clamp, every shape, on every SM, one SM and three SMs.  The epilogue's records saturate too
+    (v up to 10^6: hi = 65504 and lo saturated); every output must be finite and bit-exact."""
+    ctx, f8, xh_only = all_ctxs[prec], prec == "f16+f8x2", prec == "f16"
+    fails = []
+    try:
+        for cin, cout in SHAPES:
+            for i, (wd, h) in enumerate(REGIME_LAYER_SIZES):
+                w, b, x = _regime_layer_inputs(case, cin, cout, i, wd, h)
+                assert_regime(regime_report(mul32(np.pad(x, ((0, 0), (1, 1), (1, 1)), mode="edge"), F32(16)), w, b, prec), *case)
+                model = w2x.Model.from_arrays([w], [b])
+                want = emulate_filter_layer(x, w, b, f8, xh_only=xh_only)
+                assert np.isfinite(want).all()
+                for sms in NUM_SMS:
+                    ctx.debug_set_num_sms(sms)
+                    got = ctx.filter_layer(model, 0, x)
+                    if not np.array_equal(got, want):
+                        fails.append(f"{cin}->{cout} {wd}x{h} num_sms={sms}: {_mismatch(got, want)}")
+    finally:
+        ctx.debug_set_num_sms(0)
+    assert not fails, "\n".join(fails[:20])
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("case", REGIME_CASES, ids=_regime_id)
+@pytest.mark.parametrize("prec", ALL_PRECISIONS)
+def test_whole_model_in_saturating_regimes_is_bit_exact(w2x, all_ctxs, case, prec):
+    """1 -> C1 -> C2 -> 1 through convert_plane with the first layer's records in a saturating regime (first_layer_kernel's
+    hi / lo / xh8 / xl8), the middle layer at the case's wscale, the last layer fused and separate (last_layer_kernel
+    reads the middle layer's saturated records)"""
+    ctx, f8, xh_only = all_ctxs[prec], prec == "f16+f8x2", prec == "f16"
+    fails = []
+    try:
+        for c1, c2 in SHAPES:
+            m = regime_model(c1, c2, 10 * c1 + c2, *case)
+            model = w2x.Model.from_arrays([t[0] for t in m], [t[1] for t in m])
+            for i, (wd, h) in enumerate(REGIME_MODEL_SIZES):
+                x = binary_plane(h, wd, i)
+                for fused in (True, False):
+                    want = emulate_model(x, m, f8, fused, xh_only)
+                    assert np.isfinite(want).all()
+                    ctx.debug_set_fuse_last(fused)
+                    for sms in NUM_SMS:
+                        ctx.debug_set_num_sms(sms)
+                        got = ctx.convert_plane(model, x)
+                        if not np.array_equal(got, want):
+                            fails.append(f"{c1}-{c2} {wd}x{h} fused={fused} num_sms={sms}: {_mismatch(got, want)}")
+    finally:
+        ctx.debug_set_num_sms(0)
+        ctx.debug_set_fuse_last(True)
+    assert not fails, "\n".join(fails[:20])

@@ -81,7 +81,7 @@ first_layer_kernel(const FirstSrc src, int pw, int ph, int out_y0, const __grid_
                 const float2 rr = f32x2_add(t, prm.b[pr]);               // (0 + t) + (float)bias
                 const float2 sc = f32x2_mul(rr, make_float2(0.1f, 0.1f));
                 const float a0 = fmaxf(rr.x, sc.x), a1 = fmaxf(rr.y, sc.y);     // leaky-ReLU 0.1, already x ACT_SCALE
-                __half2 h = __floats2half2_rn(a0, a1);
+                __half2 h = f32x2_to_f16x2_sat(a0, a1);
                 float2 hf = __half22float2(h);
                 hi[i] = *reinterpret_cast<uint32_t *>(&h);
                 if constexpr (F8) {
@@ -93,7 +93,7 @@ first_layer_kernel(const FirstSrc src, int pw, int ph, int out_y0, const __grid_
                     if (i & 1) { lo[i >> 1] |= h8 << 16; lo[2 + (i >> 1)] |= l8 << 16; }     // lo[0..1] = xh8 (8 bytes), lo[2..3] = xl8
                     else { lo[i >> 1] = h8; lo[2 + (i >> 1)] = l8; }
                 } else {
-                    __half2 l = __floats2half2_rn(a0 - hf.x, a1 - hf.y);
+                    __half2 l = f32x2_to_f16x2_sat(a0 - hf.x, a1 - hf.y);
                     lo[i] = *reinterpret_cast<uint32_t *>(&l);
                 }
             }
@@ -262,7 +262,7 @@ __global__ void planar_to_nhwc_kernel(const float *__restrict__ in, int C, int w
     int x = (int)(pix % pw), y = (int)(pix / pw);
     int sx = min(max(x - 1, 0), w - 1), sy = min(max(y - 1, 0), h - 1);
     float a = in[((long)c * h + sy) * w + sx] * ACT_SCALE;
-    __half hh = __float2half_rn(a);
+    __half hh = f32_to_f16_sat(a);
     // RECORD frame: [pixel][C/32][128 B] = {fp16 x32 | xh8 x32 | xl8 x32} or {hi x32 | lo x32}
     uint8_t *recp = reinterpret_cast<uint8_t *>(out) + (pix * (C / 32) + c / 32) * 128;
     const int k = c % 32;
@@ -272,7 +272,7 @@ __global__ void planar_to_nhwc_kernel(const float *__restrict__ in, int C, int w
         recp[64 + k] = (uint8_t)__nv_cvt_float_to_fp8(hf * (1.0f / (float)(1 << F8_C)), __NV_SATFINITE, __NV_E4M3);
         recp[96 + k] = (uint8_t)__nv_cvt_float_to_fp8((a - hf) * (float)(1 << F8_A), __NV_SATFINITE, __NV_E4M3);
     } else {
-        reinterpret_cast<__half *>(recp + 64)[k] = __float2half_rn(a - hf);
+        reinterpret_cast<__half *>(recp + 64)[k] = f32_to_f16_sat(a - hf);
     }
 }
 

@@ -34,7 +34,7 @@ __device__ __forceinline__ void epilogue_store(const TcParams &p, const float *b
                     const int jj = cb * 4 + j, ch = 8 * jj + 2 * q;
                     const float v0 = activate(acc[h][4 * jj + 2 * e], p.out_scale, bias[ch]);
                     const float v1 = activate(acc[h][4 * jj + 2 * e + 1], p.out_scale, bias[ch + 1]);
-                    const __half2 hh = __floats2half2_rn(v0, v1);
+                    const __half2 hh = f32x2_to_f16x2_sat(v0, v1);
                     const float2 hf = __half22float2(hh);
                     asm volatile("st.shared.b32 [%0], %1;" ::"r"(rowaddr + (((uint32_t)j ^ sw) << 4) + 4u * q), "r"(*reinterpret_cast<const uint32_t *>(&hh)) : "memory");
                     if constexpr (F8) {
@@ -46,7 +46,7 @@ __device__ __forceinline__ void epilogue_store(const TcParams &p, const float *b
                         asm volatile("st.shared.b16 [%0], %1;" ::"r"(rowaddr + (((uint32_t)(4 + (j >> 1)) ^ sw) << 4) + in_unit), "h"(h8) : "memory");
                         asm volatile("st.shared.b16 [%0], %1;" ::"r"(rowaddr + (((uint32_t)(6 + (j >> 1)) ^ sw) << 4) + in_unit), "h"(l8) : "memory");
                     } else {
-                        const __half2 lo = __floats2half2_rn(v0 - hf.x, v1 - hf.y);
+                        const __half2 lo = f32x2_to_f16x2_sat(v0 - hf.x, v1 - hf.y);
                         asm volatile("st.shared.b32 [%0], %1;" ::"r"(rowaddr + (((uint32_t)(4 + j) ^ sw) << 4) + 4u * q), "r"(*reinterpret_cast<const uint32_t *>(&lo)) : "memory");
                     }
                 }

@@ -8,6 +8,20 @@
 // ================================================================================================
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
+// fp32 -> fp16, round to nearest even, saturating: a value that would round to +-inf becomes +-65504 (NaN stays NaN), every
+// other value converts to the bits __float2half_rn gives.  The record encodings use these, so an activation beyond the fp16
+// range leaves a finite record (hi = +-65504, lo = v - hi saturated the same way) instead of hi = inf, lo = -inf.
+__device__ __forceinline__ __half2 f32x2_to_f16x2_sat(float a, float b) {     // low half a, high half b (= __floats2half2_rn)
+    uint32_t r;
+    asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(b), "f"(a));
+    return *reinterpret_cast<__half2 *>(&r);
+}
+__device__ __forceinline__ __half f32_to_f16_sat(float a) {
+    uint16_t r;
+    asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(r) : "f"(a));
+    return *reinterpret_cast<__half *>(&r);
+}
+
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
 }
