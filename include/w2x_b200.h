@@ -138,7 +138,10 @@ W2X_API int w2x_ctx_get_engine(const w2x_ctx *ctx);
 W2X_API int w2x_ctx_set_precision(w2x_ctx *ctx, int precision);
 W2X_API int w2x_ctx_get_precision(const w2x_ctx *ctx);
 /* Run on a caller-owned CUDA stream (cudaStream_t passed as void*); NULL = the ctx's own stream.
- * A host-buffer entry point starts its copies only after the work already queued on the context's stream. */
+ * A host-buffer entry point starts its copies only after the work already queued on the context's stream.
+ * Work queued after a switch starts after everything the context queued before it, on any stream: the new
+ * stream waits for the previous one (one event, no host wait; setting the current stream again does nothing).
+ * The previous stream must still be valid when it is replaced. */
 W2X_API int w2x_ctx_set_stream(w2x_ctx *ctx, void *cuda_stream);
 /* Block until everything queued by this context has finished. */
 W2X_API int w2x_ctx_synchronize(w2x_ctx *ctx);
@@ -427,7 +430,7 @@ W2X_API int w2x_multi_convert_chain(w2x_multi *multi, int n_steps, const w2x_mod
 W2X_API int w2x_ctx_launch_count(const w2x_ctx *ctx, uint64_t *n_launches);
 /* When enabled, every layer kernel launched by convert_* is bracketed by CUDA events on the
  * launching stream; w2x_ctx_layer_times returns, per layer, the summed milliseconds and launch
- * count since the last reset (synchronises the stream). */
+ * count since the last reset (synchronises the stream; W2X_ERR_CUDA when a timed span cannot be read). */
 W2X_API int w2x_ctx_set_timing(w2x_ctx *ctx, int enabled);
 W2X_API int w2x_ctx_layer_times(w2x_ctx *ctx, int max_layers, float *ms, int *launches,
                                 int *n_layers_out, int reset);

@@ -478,6 +478,7 @@ int w2x_ctx_create(int device, w2x_ctx **out_ctx) {
         CU_CHECK(cudaEventCreateWithFlags(&ctx->ev_done[i], cudaEventDisableTiming));
     }
     CU_CHECK(cudaEventCreateWithFlags(&ctx->plan_ev, cudaEventDisableTiming));
+    CU_CHECK(cudaEventCreateWithFlags(&ctx->switch_ev, cudaEventDisableTiming));
     *out_ctx = ctx.release();
     return W2X_OK;
 }
@@ -523,9 +524,18 @@ int w2x_ctx_set_precision(w2x_ctx *ctx, int precision) {
 }
 int w2x_ctx_get_precision(const w2x_ctx *ctx) { return ctx ? ctx->precision : -1; }
 
+// Every call on the context shares its scratch, and only the order of one stream keeps two calls apart.  So a switch makes the new
+// stream wait for everything queued on the old one: the calls after it never overlap the calls before it, and whatever waits for the
+// current stream (w2x_ctx_synchronize, w2x_ctx_layer_times, w2x_ctx_forget_model, w2x_ctx_destroy, the first upload of
+// run_host_groups) waits for those too.
 int w2x_ctx_set_stream(w2x_ctx *ctx, void *cuda_stream) {
     if (check_ctx(ctx)) return W2X_ERR_ARG;
-    ctx->stream = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->own_stream;
+    cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->own_stream;
+    if (s == ctx->stream) return W2X_OK;
+    DeviceGuard g(ctx->device);
+    CU_CHECK(cudaEventRecord(ctx->switch_ev, ctx->stream));
+    CU_CHECK(cudaStreamWaitEvent(s, ctx->switch_ev, 0));
+    ctx->stream = s;
     return W2X_OK;
 }
 
@@ -733,7 +743,7 @@ int w2x_ctx_layer_times(w2x_ctx *ctx, int max_layers, float *ms, int *launches, 
     int top = 0;
     for (auto &s : ctx->spans) {
         float t = 0.f;
-        cudaEventElapsedTime(&t, s.e0, s.e1);
+        CU_CHECK(cudaEventElapsedTime(&t, s.e0, s.e1));
         if (s.layer >= 0 && s.layer < max_layers) { ms[s.layer] += t; launches[s.layer]++; }
         top = std::max(top, s.layer + 1);
     }

@@ -86,6 +86,7 @@ struct w2x_ctx {
     int precision = W2X_PRECISION_F16_F8X2;   // default; W2X_PRECISION=f16x3|f16 in the environment or w2x_ctx_set_precision() selects another scheme
     cudaStream_t own_stream = nullptr;
     cudaStream_t stream = nullptr;
+    cudaEvent_t switch_ev = nullptr;   // w2x_ctx_set_stream: recorded on the old stream, waited for by the new one
     size_t scratch_limit = (size_t)16 << 30;
     w2x_log_fn log = nullptr;
     void *log_user = nullptr;
@@ -115,6 +116,7 @@ struct w2x_ctx {
     ~w2x_ctx() {
         auto drop = [](cudaEvent_t e) { if (e) cudaEventDestroy(e); };
         drop(plan_ev);
+        drop(switch_ev);
         for (auto &s : spans) { drop(s.e0); drop(s.e1); }
         for (auto e : event_pool) drop(e);
         for (int i = 0; i < 8; i++) { drop(ev_in[i]); drop(ev_done[i]); }
