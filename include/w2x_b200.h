@@ -407,7 +407,8 @@ W2X_API int w2x_multi_convert_tiles(w2x_multi *multi, const w2x_model *model, co
  * same arguments.
  * Arguments are checked as by w2x_convert_chain, before anything is printed, allocated or queued, W2X_ERR_ARG (or, for a model
  * the engine refuses, W2X_ERR_UNSUPPORTED) naming the step.  A step with W2X_STEP_TTA is refused with W2X_ERR_ARG naming the step:
- * it has no multi-GPU form (the transposed variants would turn row bands into column bands).
+ * it has no row-band form (the transposed variants would turn row bands into column bands).  w2x_multi_convert_planes_chain runs TTA
+ * steps across GPUs, a plane's variants on different GPUs; call it with the one plane.
  * Before step k is queued on any GPU, on_step(k, user) is called (if not NULL); then the step logs, through the first context's log
  * function (w2x_multi_set_log), the lines w2x_convert_chain logs for it.
  * GPUs used: min(n_devices, height / (4 * the largest n_layers of the steps)), decided on the INPUT height (later steps only get
@@ -424,6 +425,41 @@ W2X_API int w2x_multi_convert_chain(w2x_multi *multi, int n_steps, const w2x_mod
                                     const float *in, int width, int height, size_t in_stride_bytes,
                                     float *out, size_t out_stride_bytes, int block_splitting,
                                     w2x_step_fn on_step, void *user);
+
+/* w2x_convert_planes_chain on N GPUs: a collection of planes of any sizes, each plane on one GPU, and each W2X_STEP_TTA step's 8
+ * variants of a plane spread over the GPUs.  A TTA step is 8 independent conversions and an ordered mean, so its variants split across
+ * GPUs with no per-layer exchange: one large image's TTA step spreads as evenly as a collection's.  w2x_multi_convert_planes is the
+ * one-step W2X_STEP_SAME case (w2x_convert_planes on N GPUs).
+ * Every output is bit-identical to w2x_convert_planes_chain on the first context with the same kinds, precision and engine, W2X_STEP_TTA
+ * steps included: every context the call uses takes the first context's precision and engine.
+ * Arguments are checked exactly as w2x_convert_planes_chain checks them, with the same messages naming the step or the plane, before
+ * anything is printed, allocated or queued on any context.
+ * Before step k is queued on any GPU, on_step(k, user) is called (if not NULL); then, through the first context's log function
+ * (w2x_multi_set_log), the lines w2x_convert_planes_chain logs for step k, in plane order.
+ * Placement (a pure function of the sizes, kinds, models and N): the work of a plane at a step is its output pixels times the step
+ * model's multiply-adds per pixel (9 Cin Cout summed over its layers), a TTA step counting 8 times.  Every plane has one owner GPU for
+ * the whole call, which holds its input, its intermediate planes and its output and runs its plain steps.  In a TTA step, variant j of
+ * plane i is converted on GPU (owner(i) + j) mod nd; the owner builds the variants and writes the mean.  When nd divides 8, every GPU
+ * converts 8 / nd variants of every plane.  Owners are chosen greedily: planes in decreasing order of total work (ties: the lower
+ * index), each taking the owner that minimises the largest per-GPU load once its work is added (ties: the owner with the smaller load
+ * before the plane, then the lower GPU index).
+ * GPUs used: nd = min(n_devices, 8 n_planes) when a step has W2X_STEP_TTA, else min(n_devices, n_planes).  With nd == 1 the call is
+ * w2x_convert_planes_chain on the first context: same bits, same lines, same launches.
+ * A TTA step needs peer access between every two distinct devices it uses (contexts of one device always qualify); without it the call
+ * returns W2X_ERR_UNSUPPORTED naming the pair, before anything is queued.
+ * Device memory: each GPU holds the staging of the planes it owns, the two chain buffers of its planes, the TTA buffers of the variants
+ * it converts and its frame scratch.  All of it is reserved on every GPU before the first copy or launch anywhere: W2X_ERR_NOMEM leaves
+ * nothing queued on any context.
+ * Every dependency between GPUs is a CUDA event (a converting GPU waits for the owner's variants kernel, the owner's mean for every
+ * converting GPU); no kernel waits on a flag, so contexts of one device cannot hold each other up.
+ * HOST buffers, synchronous; pageable buffers are pinned for the call.  Every GPU's work is queued before any is waited for. */
+W2X_API int w2x_multi_convert_planes(w2x_multi *multi, const w2x_model *model, int n_planes, const float *const *in,
+                                     const int *widths, const int *heights, const size_t *in_strides,
+                                     float *const *out, const size_t *out_strides);
+W2X_API int w2x_multi_convert_planes_chain(w2x_multi *multi, int n_steps, const w2x_model *const *models, const int *kinds,
+                                           int n_planes, const float *const *in, const int *widths, const int *heights,
+                                           const size_t *in_strides, float *const *out, const size_t *out_strides,
+                                           w2x_step_fn on_step, void *user);
 
 /* ---- instrumentation ---------------------------------------------------------------------- */
 /* Number of kernels of THIS library launched by the context so far. */

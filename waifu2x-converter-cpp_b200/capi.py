@@ -42,6 +42,7 @@ ABI_SYMBOLS = (
     "w2x_slab_connect", "w2x_slab_connect_local", "w2x_slab_convert", "w2x_slab_convert_async", "w2x_slab_synchronize",
     "w2x_convert_planes", "w2x_convert_planes_device", "w2x_convert_chain", "w2x_convert_chain_device",
     "w2x_convert_planes_chain", "w2x_convert_planes_chain_device", "w2x_multi_convert_chain",
+    "w2x_multi_convert_planes", "w2x_multi_convert_planes_chain",
 )
 BAND_BLOB_BYTES = 320
 
@@ -160,6 +161,9 @@ def lib():
     L.w2x_multi_convert_plane.argtypes = [vp, vp, vp, ci, ci, cs, vp, cs, ci]
     L.w2x_multi_convert_tiles.argtypes = [vp, vp, C.POINTER(vp), C.POINTER(vp), ci, ci, ci, cs, cs]
     L.w2x_multi_convert_chain.argtypes = [vp, ci, C.POINTER(vp), pi, vp, ci, ci, cs, vp, cs, ci, STEP_FN, vp]
+    L.w2x_multi_convert_planes.argtypes = [vp, vp, ci, C.POINTER(vp), pi, pi, ps, C.POINTER(vp), ps]
+    L.w2x_multi_convert_planes_chain.argtypes = [vp, ci, C.POINTER(vp), pi, ci, C.POINTER(vp), pi, pi, ps, C.POINTER(vp), ps, STEP_FN, vp]
+    L.w2x_debug_plan_multi_planes.argtypes = [ci, ci, C.POINTER(vp), pi, ci, pi, pi, pi, C.POINTER(C.c_longlong)]
     L.w2x_debug_pad_upsample2x_xy.argtypes = [vp, vp, ci, ci, C.c_long, ci, ci, ci, ci, ci, ci, ci, ci, ci, vp]
     L.w2x_debug_set_host_bands.argtypes = [vp, ci]
     L.w2x_debug_set_fuse_last.argtypes = [vp, ci]
@@ -228,6 +232,23 @@ def debug_plan_planes(widths, heights, n_layers=7, max_channels=128, scratch_lim
     dims = np.zeros((max(nf, 1), 2), np.int32)
     lib().w2x_debug_plan_planes(n, *args, dims.ctypes.data_as(pi), nf)
     return frame, x0, y0, dims[:nf]
+
+
+def debug_plan_multi_planes(n_devices, steps, widths, heights):
+    """The placement of w2x_multi_convert_planes_chain on n_devices GPUs (no device needed); steps as in Context.convert_planes_chain
+    -> (nd, owner [n], load [nd]): the GPUs used, every plane's owner and the planned work (multiply-adds) per GPU."""
+    n, models, kinds, _, _ = Context._chain_args(steps, None)
+    k = len(widths)
+    w = np.ascontiguousarray(widths, np.int32)
+    h = np.ascontiguousarray(heights, np.int32)
+    owner = np.zeros(k, np.int32)
+    load = np.zeros(max(n_devices, 1), np.int64)
+    pi = C.POINTER(C.c_int)
+    nd = lib().w2x_debug_plan_multi_planes(n_devices, n, models, kinds, k, w.ctypes.data_as(pi), h.ctypes.data_as(pi),
+                                           owner.ctypes.data_as(pi), load.ctypes.data_as(C.POINTER(C.c_longlong)))
+    if nd < 0:
+        raise W2xError(-nd, lib().w2x_last_error().decode())
+    return nd, owner, load[:nd]
 
 
 def _plane_arrays(planes, fix):
@@ -678,6 +699,20 @@ class Multi:
             raise ValueError(f"out must be a float32 array of shape {(h << ups, w << ups)} with unit column stride")
         _check(lib().w2x_multi_convert_chain(self._h, n, models, kinds, C.c_void_p(x.ctypes.data), w, h, x.strides[0],
                                              C.c_void_p(out.ctypes.data), out.strides[0], int(bool(block_splitting)), cb, None))
+        return out
+
+    def convert_planes(self, model: Model, planes, out=None):
+        """Context.convert_planes with each plane on one of this handle's GPUs (w2x_multi_convert_planes): same arguments, same bits."""
+        xs, ip, ws, hs, ist, out, op, ost = Context._planes_args(planes, out, 0)
+        _check(lib().w2x_multi_convert_planes(self._h, model._h, len(xs), ip, ws, hs, ist, op, ost))
+        return out
+
+    def convert_planes_chain(self, steps, planes, out=None, on_step=None):
+        """Context.convert_planes_chain across this handle's GPUs (w2x_multi_convert_planes_chain): each plane on one GPU, a TTA step's
+        8 variants of a plane spread over them.  Same arguments, same bits."""
+        n, models, kinds, cb, ups = Context._chain_args(steps, on_step)
+        xs, ip, ws, hs, ist, out, op, ost = Context._planes_args(planes, out, ups)
+        _check(lib().w2x_multi_convert_planes_chain(self._h, n, models, kinds, len(xs), ip, ws, hs, ist, op, ost, cb, None))
         return out
 
     def launch_counts(self):

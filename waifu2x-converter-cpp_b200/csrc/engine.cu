@@ -288,56 +288,80 @@ struct HostGroup {
     std::vector<Copy> down;
 };
 
-// Runs the groups in order and returns once every download has landed.  One group runs on the context's stream alone.  With more,
-// uploads go on copy_in up to 8 groups ahead (ev_in / ev_done are 8 deep) and downloads on copy_out, so that the uploads of later
-// groups and the downloads of earlier ones overlap the compute of the current one.  The first upload waits for the work already
-// queued on the context's stream, which may still read the staging buffers.  On an error every stream is drained before returning:
-// queued copies still touch the caller's buffers and the staging.
-int run_host_groups(w2x_ctx *ctx, const std::vector<HostGroup> &groups) {
-    const int ng = (int)groups.size();
-    auto copy = [](const HostGroup::Copy &c, cudaMemcpyKind kind, cudaStream_t s) {
+// Queues the groups in order (start, then queue(g1) for successive ends g1; several contexts' pipes may be interleaved so), then
+// finish() returns once every download has landed.  One group runs on the context's stream alone.  With more, uploads go on copy_in
+// up to 8 groups ahead (ev_in / ev_done are 8 deep) and downloads on copy_out, so that the uploads of later groups and the downloads
+// of earlier ones overlap the compute of the current one.  The first upload waits for the work already queued on the context's
+// stream, which may still read the staging buffers.  On an error every stream is drained before returning: queued copies still touch
+// the caller's buffers and the staging.
+struct HostPipe {
+    w2x_ctx *ctx;
+    const std::vector<HostGroup> &groups;
+    int next = 0;
+
+    static cudaError_t copy(const HostGroup::Copy &c, cudaMemcpyKind kind, cudaStream_t s) {
         return cudaMemcpy2DAsync(c.dst, c.dst_pitch, c.src, c.src_pitch, c.row_bytes, c.rows, kind, s);
-    };
-    auto upload = [&](int gi) -> int {
+    }
+    int ng() const { return (int)groups.size(); }
+    int upload(int gi) {
         if (groups[(size_t)gi].up.empty()) return W2X_OK;
         for (auto &c : groups[(size_t)gi].up) CU_CHECK(copy(c, cudaMemcpyHostToDevice, ctx->copy_in));
         CU_CHECK(cudaEventRecord(ctx->ev_in[gi % 8], ctx->copy_in));
         return W2X_OK;
-    };
-    auto queue = [&]() -> int {
-        if (ng == 1) {
-            for (auto &c : groups[0].up) CU_CHECK(copy(c, cudaMemcpyHostToDevice, ctx->stream));
-            int rc = groups[0].compute();
-            if (rc) return rc;
-            for (auto &c : groups[0].down) CU_CHECK(copy(c, cudaMemcpyDeviceToHost, ctx->stream));
-            return W2X_OK;
-        }
+    }
+    int start() {
+        if (ng() <= 1) return W2X_OK;
+        DeviceGuard g(ctx->device);
         CU_CHECK(cudaEventRecord(ctx->ev_done[0], ctx->stream));   // not recorded again before group 0's compute is queued
         CU_CHECK(cudaStreamWaitEvent(ctx->copy_in, ctx->ev_done[0], 0));
         int rc = W2X_OK;
-        for (int gi = 0; gi < std::min(8, ng) && !rc; gi++) rc = upload(gi);
-        for (int gi = 0; gi < ng && !rc; gi++) {
-            const HostGroup &G = groups[(size_t)gi];
+        for (int gi = 0; gi < std::min(8, ng()) && !rc; gi++) rc = upload(gi);
+        return rc;
+    }
+    int queue(int g1) {   // groups [next, g1)
+        DeviceGuard g(ctx->device);
+        for (; next < g1; next++) {
+            const HostGroup &G = groups[(size_t)next];
+            if (ng() == 1) {
+                for (auto &c : G.up) CU_CHECK(copy(c, cudaMemcpyHostToDevice, ctx->stream));
+                int rc = G.compute();
+                if (rc) return rc;
+                for (auto &c : G.down) CU_CHECK(copy(c, cudaMemcpyDeviceToHost, ctx->stream));
+                continue;
+            }
+            const int gi = next;
             if (!G.up.empty()) CU_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->ev_in[gi % 8], 0));
-            rc = G.compute();
-            if (rc) break;
+            int rc = G.compute();
+            if (rc) return rc;
             CU_CHECK(cudaEventRecord(ctx->ev_done[gi % 8], ctx->stream));
             CU_CHECK(cudaStreamWaitEvent(ctx->copy_out, ctx->ev_done[gi % 8], 0));
             for (auto &c : G.down) CU_CHECK(copy(c, cudaMemcpyDeviceToHost, ctx->copy_out));
-            if (gi + 8 < ng) rc = upload(gi + 8);   // ev_in[gi % 8]'s previous record has been waited for above
+            if (gi + 8 < ng()) {   // ev_in[gi % 8]'s previous record has been waited for above
+                rc = upload(gi + 8);
+                if (rc) return rc;
+            }
         }
-        return rc;
-    };
-    int rc = queue();
-    if (rc) {
-        cudaStreamSynchronize(ctx->copy_in);
-        cudaStreamSynchronize(ctx->stream);
-        cudaStreamSynchronize(ctx->copy_out);
-        return rc;
+        return W2X_OK;
     }
-    if (ng > 1) CU_CHECK(cudaStreamSynchronize(ctx->copy_out));
-    CU_CHECK(cudaStreamSynchronize(ctx->stream));
-    return W2X_OK;
+    int finish(int rc) {
+        DeviceGuard g(ctx->device);
+        if (rc) {
+            cudaStreamSynchronize(ctx->copy_in);
+            cudaStreamSynchronize(ctx->stream);
+            cudaStreamSynchronize(ctx->copy_out);
+            return rc;
+        }
+        if (ng() > 1) CU_CHECK(cudaStreamSynchronize(ctx->copy_out));
+        CU_CHECK(cudaStreamSynchronize(ctx->stream));
+        return W2X_OK;
+    }
+};
+
+int run_host_groups(w2x_ctx *ctx, const std::vector<HostGroup> &groups) {
+    HostPipe p{ctx, groups};
+    int rc = p.start();
+    if (!rc) rc = p.queue(p.ng());
+    return p.finish(rc);
 }
 
 // The literal walk needs every block inside the plane; block_table places columns by the block height, as the reference does, so
@@ -479,6 +503,7 @@ int w2x_ctx_create(int device, w2x_ctx **out_ctx) {
     }
     CU_CHECK(cudaEventCreateWithFlags(&ctx->plan_ev, cudaEventDisableTiming));
     CU_CHECK(cudaEventCreateWithFlags(&ctx->switch_ev, cudaEventDisableTiming));
+    for (auto &e : ctx->tta_ev) CU_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     *out_ctx = ctx.release();
     return W2X_OK;
 }
@@ -780,15 +805,19 @@ struct FrameDev {                   // the same frame with its table in ctx->pla
     const int *shelf_y0, *shelf_first;
 };
 
-// Puts each frame's rectangles in shelf order, numbers their gather blocks and uploads all tables in ONE copy on the context's
-// stream, `tta` (the tables of the TTA kernels, at *tta_dev) after them.  The copy waits for the kernels of an earlier call that still
-// read the buffer (plan_ev), and its source is pageable memory, so it is staged before cudaMemcpyAsync returns and the host vectors
-// may go at once.
-int upload_frames(w2x_ctx *ctx, std::vector<FramePlan> &frames, std::vector<FrameDev> *out, const std::vector<TtaPlane> &tta = {},
-                  const TtaPlane **tta_dev = nullptr) {
-    auto align = [](size_t b) { return (b + 15) & ~(size_t)15; };
+// The device tables of a call's frames, then those of its TTA kernels, as one blob for plan_buf.
+struct Tables {
     std::vector<char> blob;
     std::vector<size_t> off_rect, off_shelf;
+    size_t off_tta = 0;
+    size_t bytes(size_t n_tta) const { return off_tta + n_tta * sizeof(TtaPlane); }
+};
+
+// Puts each frame's rectangles in shelf order, numbers their gather blocks and lays their tables out in t (*out gets the sizes).
+void frame_tables(std::vector<FramePlan> &frames, std::vector<FrameDev> *out, Tables *t) {
+    auto align = [](size_t b) { return (b + 15) & ~(size_t)15; };
+    std::vector<char> &blob = t->blob;
+    std::vector<size_t> &off_rect = t->off_rect, &off_shelf = t->off_shelf;
     out->assign(frames.size(), FrameDev{});
     for (size_t f = 0; f < frames.size(); f++) {
         auto &R = frames[f].rect;
@@ -818,24 +847,34 @@ int upload_frames(w2x_ctx *ctx, std::vector<FramePlan> &frames, std::vector<Fram
         std::memcpy(blob.data() + off_shelf.back(), sy.data(), sy.size() * sizeof(int));
         std::memcpy(blob.data() + off_shelf.back() + sy.size() * sizeof(int), sf.data(), sf.size() * sizeof(int));
     }
-    const size_t off_tta = align(blob.size());
-    if (!tta.empty()) {
-        blob.resize(off_tta + tta.size() * sizeof(TtaPlane));
-        std::memcpy(blob.data() + off_tta, tta.data(), tta.size() * sizeof(TtaPlane));
-    }
+    t->off_tta = align(blob.size());
+}
+
+// Uploads t's frame tables and `tta` (the tables of the TTA kernels, at *tta_dev) in ONE copy on the context's stream, into plan_buf
+// as reserved for them.  The copy waits for the kernels of an earlier call that still read the buffer (plan_ev), and its source is
+// pageable memory, so it is staged before cudaMemcpyAsync returns and the host vectors may go at once.
+int upload_tables(w2x_ctx *ctx, Tables &t, std::vector<FrameDev> *out, const std::vector<TtaPlane> &tta = {}, const TtaPlane **tta_dev = nullptr) {
+    std::vector<char> &blob = t.blob;
+    blob.resize(t.bytes(tta.size()));
+    if (!tta.empty()) std::memcpy(blob.data() + t.off_tta, tta.data(), tta.size() * sizeof(TtaPlane));
     if (ctx->plan_ev_live) CU_CHECK(cudaStreamWaitEvent(ctx->stream, ctx->plan_ev, 0));
-    int rc = ctx->plan_buf.reserve(blob.size());
-    if (rc) return rc;
     const char *base = ctx->plan_buf.get();
     CU_CHECK(cudaMemcpyAsync(ctx->plan_buf.get(), blob.data(), blob.size(), cudaMemcpyHostToDevice, ctx->stream));
-    if (tta_dev) *tta_dev = reinterpret_cast<const TtaPlane *>(base + off_tta);
-    for (size_t f = 0; f < frames.size(); f++) {
+    if (tta_dev) *tta_dev = reinterpret_cast<const TtaPlane *>(base + t.off_tta);
+    for (size_t f = 0; f < out->size(); f++) {
         FrameDev &d = (*out)[f];
-        d.rect = reinterpret_cast<const tc::PlaneRect *>(base + off_rect[f]);
-        d.shelf_y0 = reinterpret_cast<const int *>(base + off_shelf[f]);
+        d.rect = reinterpret_cast<const tc::PlaneRect *>(base + t.off_rect[f]);
+        d.shelf_y0 = reinterpret_cast<const int *>(base + t.off_shelf[f]);
         d.shelf_first = d.shelf_y0 + d.n_shelf;
     }
     return W2X_OK;
+}
+
+int upload_frames(w2x_ctx *ctx, std::vector<FramePlan> &frames, std::vector<FrameDev> *out) {
+    Tables t;
+    frame_tables(frames, out, &t);
+    int rc = ctx->plan_buf.reserve(t.bytes(0));
+    return rc ? rc : upload_tables(ctx, t, out);
 }
 
 // Sizes the scratch for the largest of frames [f0, f1) of a model of maxc channels once, so that no buffer is reallocated between
@@ -976,9 +1015,10 @@ struct Step {
     PlanesPlan plan;                    // packed: each converted plane's frame (-1: converted alone) and place
     size_t f0 = 0;                      // packed: index of its frame 0 in the call's frame table
     std::vector<PlaneIO> io;            // each plane's source and destination at this step
-    // tta: the 8n planes the model converts -- variant j of plane i at 8 i + j, its output vw x vh -- with their sources in
-    // ctx->tta_buf[0] and outputs in ctx->tta_buf[1], and the tables of the variants and the mean kernel (tiles: their blocks)
-    std::vector<int> vw, vh;
+    // tta: the variant planes the model converts on this context -- vof lists them as 8 i + j, variant j of plane i in the call's
+    // numbering; every one of the 8n on one context -- their outputs vw x vh, with their sources in ctx->tta_buf[0] and outputs in
+    // ctx->tta_buf[1], and the tables of the variants and the mean kernel of the planes (w, h) the context owns (tiles: their blocks)
+    std::vector<int> vof, vw, vh;
     std::vector<PlaneIO> vio;
     const TtaPlane *vtab = nullptr, *mtab = nullptr;
     int vtiles = 0, mtiles = 0;
@@ -1003,6 +1043,7 @@ std::vector<Step> step_table(int n_steps, const w2x_model *const *models, const 
         s.h = h;
         for (int i = 0; i < n_planes && s.tta; i++)
             for (int j = 0; j < 8; j++) {
+                s.vof.push_back(8 * i + j);
                 s.vw.push_back(j & 4 ? h[(size_t)i] : w[(size_t)i]);
                 s.vh.push_back(j & 4 ? w[(size_t)i] : h[(size_t)i]);
             }
@@ -1059,25 +1100,65 @@ int check_planes_chain(const char *fn, w2x_ctx *ctx, int n_steps, const w2x_mode
     }, steps);
 }
 
-// Everything before the first copy or launch: the models on the device; where each plane comes from and goes to at each step (step
-// 0 reads ends[i].src, the last step writes ends[i].dst, step k < last writes its outputs densely into chain_buf[k & 1]); with
-// `pack`, each step that packs_frames allows is planned into frames on its OUTPUT sizes, so that a plane may pack at one step and be
-// converted alone after a 2x step (without, every plane is converted alone); the intermediate buffers and the frame scratch; then ONE
-// upload of every step's frame tables, so that no step waits for the host.
-// A TTA step converts the 8n variant planes instead (variant j of plane i: 8 i + j), dense in tta_buf[0] (an upscaling step's
-// variants are those of its half-resolution sources: the nearest 2x resize commutes with every flip and transpose) with their outputs
-// dense in tta_buf[1]; with `pack` those are what its frames are planned on.  Its kernel tables go up with the frame tables.
-int prepare_planes(w2x_ctx *ctx, std::vector<Step> &steps, const std::vector<PlaneIO> &ends, bool pack, std::vector<FrameDev> *fd) {
-    const size_t n_planes = ends.size(), last = steps.size() - 1;
+// What one context does in a call: the steps on the planes it owns (own: their numbers in the call; Step::w, h and io are theirs), of
+// a TTA step the variants it converts (Step::vof), where its planes come from and go to (ends), and its frame tables (fd).  A call on
+// one context has one part owning every plane and converting every variant.
+struct Part {
+    w2x_ctx *ctx;
+    std::vector<int> own;
+    std::vector<Step> steps;
+    std::vector<PlaneIO> ends;
+    std::vector<FrameDev> fd;
+    std::vector<FramePlan> frames;   // prepare_parts' working state
+    Tables tables;
+    size_t n_tta = 0;
+};
+
+// Part p's steps: the call's steps on its planes, a TTA step's variants restricted to vof[k] (8 i + j each, ascending).
+std::vector<Step> part_steps(const std::vector<Step> &all, const std::vector<int> &own, const std::vector<std::vector<int>> &vof) {
+    std::vector<Step> steps(all.size());
+    for (size_t k = 0; k < all.size(); k++) {
+        const Step &a = all[k];
+        Step &s = steps[k];
+        s.m = a.m;
+        s.up = a.up;
+        s.tta = a.tta;
+        for (int i : own) {
+            s.w.push_back(a.w[(size_t)i]);
+            s.h.push_back(a.h[(size_t)i]);
+        }
+        for (int v : vof[k]) {
+            s.vof.push_back(v);
+            s.vw.push_back(a.vw[(size_t)v]);
+            s.vh.push_back(a.vh[(size_t)v]);
+        }
+    }
+    return steps;
+}
+
+// The first half of prepare_parts on one part: every device buffer and the model copies, where each plane and variant lives.  Its
+// planes come from and go to: step 0 reads ends[i].src, the last step writes ends[i].dst, step k < last writes its outputs densely into
+// chain_buf[k & 1]; a TTA step's variants (an upscaling step's are those of its half-resolution sources: the nearest 2x resize
+// commutes with every flip and transpose) lie dense in tta_buf[0] in vof order, their outputs dense in tta_buf[1].  With `pack`, each
+// step that packs_frames allows is planned into frames on its OUTPUT sizes, so that a plane may pack at one step and be converted
+// alone after a 2x step (without, every plane is converted alone); a TTA step's frames are planned on the variants it converts.
+int reserve_part(Part &P, bool pack) {
+    w2x_ctx *ctx = P.ctx;
+    DeviceGuard g(ctx->device);
+    std::vector<Step> &steps = P.steps;
+    const size_t n_planes = P.own.size(), last = steps.size() - 1;
     size_t need[2] = {0, 0}, tta_need[2] = {0, 0};
     for (size_t k = 0; k <= last; k++) {
-        size_t px = 0;
-        for (size_t i = 0; i < n_planes; i++) px += (size_t)steps[k].w[i] * steps[k].h[i];
-        if (k < last) need[k & 1] = std::max(need[k & 1], px * sizeof(float));
-        if (steps[k].tta) {
-            tta_need[0] = std::max(tta_need[0], 8 * (steps[k].up ? px / 4 : px) * sizeof(float));
-            tta_need[1] = std::max(tta_need[1], 8 * px * sizeof(float));
+        const Step &s = steps[k];
+        size_t px = 0, vin = 0, vout = 0;
+        for (size_t i = 0; i < n_planes; i++) px += (size_t)s.w[i] * s.h[i];
+        for (size_t v = 0; v < s.vw.size(); v++) {
+            vout += (size_t)s.vw[v] * s.vh[v];
+            vin += (size_t)s.vw[v] * s.vh[v] / (s.up ? 4 : 1);
         }
+        if (k < last) need[k & 1] = std::max(need[k & 1], px * sizeof(float));
+        tta_need[0] = std::max(tta_need[0], vin * sizeof(float));
+        tta_need[1] = std::max(tta_need[1], vout * sizeof(float));
     }
     for (int i = 0; i < 2; i++) {
         if (!need[i]) continue;
@@ -1089,72 +1170,114 @@ int prepare_planes(w2x_ctx *ctx, std::vector<Step> &steps, const std::vector<Pla
         int rc = ctx->tta_buf[i].reserve(tta_need[i]);
         if (rc) return rc;
     }
-    std::vector<FramePlan> frames;
-    std::vector<TtaPlane> tta;
-    float *const tta_in = ctx->tta_buf[0].get(), *const tta_out = ctx->tta_buf[1].get();
-    std::vector<size_t> tab0(steps.size());   // a TTA step's variants table at tta[tab0], its mean table right after it
+    P.frames.clear();
+    P.n_tta = 0;
     for (size_t k = 0; k <= last; k++) {
         Step &s = steps[k];
         int rc = get_dev_model(ctx, s.m, &s.dm);
         if (rc) return rc;
-        s.packed = pack && packs_frames(ctx, s.m, s.dm, pick_engine(ctx, s.m));
+        s.packed = pack && !s.cw().empty() && packs_frames(ctx, s.m, s.dm, pick_engine(ctx, s.m));
         s.io.resize(n_planes);
         size_t off = 0;
         for (size_t i = 0; i < n_planes; i++) {
             PlaneIO &p = s.io[i];
-            p.src = k == 0 ? ends[i].src : steps[k - 1].io[i].dst;
-            p.src_stride = k == 0 ? ends[i].src_stride : steps[k - 1].io[i].dst_stride;
-            p.dst = k == last ? ends[i].dst : ctx->chain_buf[k & 1].get() + off;
-            p.dst_stride = k == last ? ends[i].dst_stride : (size_t)s.w[i] * sizeof(float);
+            p.src = k == 0 ? P.ends[i].src : steps[k - 1].io[i].dst;
+            p.src_stride = k == 0 ? P.ends[i].src_stride : steps[k - 1].io[i].dst_stride;
+            p.dst = k == last ? P.ends[i].dst : ctx->chain_buf[k & 1].get() + off;
+            p.dst_stride = k == last ? P.ends[i].dst_stride : (size_t)s.w[i] * sizeof(float);
             off += (size_t)s.w[i] * s.h[i];
         }
         if (s.tta) {
-            auto tiles = [](int w, int h) { return ((w + 31) / 32) * ((h + 31) / 32); };
-            s.vio.resize(8 * n_planes);
-            tab0[k] = tta.size();
+            s.vio.resize(s.vof.size());
             size_t in_off = 0, out_off = 0;
-            for (size_t i = 0; i < n_planes; i++) {   // the variants kernel: plane -> its 8 variants
-                const int sw = s.up ? s.w[i] / 2 : s.w[i], sh = s.up ? s.h[i] / 2 : s.h[i];
-                const size_t in_px = (size_t)sw * sh, out_px = (size_t)s.w[i] * s.h[i];
-                tta.push_back(TtaPlane{s.io[i].src, tta_in + in_off, nullptr, (long)(s.io[i].src_stride / 4), 0, sw, sh, s.vtiles});
-                s.vtiles += tiles(sw, sh);
-                for (int j = 0; j < 8; j++)
-                    s.vio[8 * i + j] = PlaneIO{tta_in + in_off + j * in_px, (size_t)(j & 4 ? sh : sw) * sizeof(float),
-                                               tta_out + out_off + j * out_px, (size_t)s.vw[8 * i + j] * sizeof(float)};
-                in_off += 8 * in_px;
-                out_off += 8 * out_px;
+            for (size_t v = 0; v < s.vof.size(); v++) {
+                const int sw = s.up ? s.vw[v] / 2 : s.vw[v], sh = s.up ? s.vh[v] / 2 : s.vh[v];
+                s.vio[v] = PlaneIO{ctx->tta_buf[0].get() + in_off, (size_t)sw * sizeof(float), ctx->tta_buf[1].get() + out_off,
+                                   (size_t)s.vw[v] * sizeof(float)};
+                in_off += (size_t)sw * sh;
+                out_off += (size_t)s.vw[v] * s.vh[v];
             }
-            out_off = 0;
-            for (size_t i = 0; i < n_planes; i++) {   // the mean kernel: 8 variant outputs -> the step's output
-                tta.push_back(TtaPlane{nullptr, tta_out + out_off, s.io[i].dst, 0, (long)(s.io[i].dst_stride / 4), s.w[i], s.h[i], s.mtiles});
-                s.mtiles += tiles(s.w[i], s.h[i]);
-                out_off += 8 * (size_t)s.w[i] * s.h[i];
-            }
+            P.n_tta += 2 * n_planes;   // the variants and the mean kernel's rows of the planes it owns
         }
         if (!s.packed) continue;
         const std::vector<int> &cw = s.cw(), &ch = s.ch();
         const std::vector<PlaneIO> &cio = s.cio();
         plan_for(ctx, s.m, (int)cw.size(), cw.data(), ch.data(), &s.plan);
-        s.f0 = frames.size();
-        for (FramePlan &f : frames_for(s.plan)) frames.push_back(std::move(f));
+        s.f0 = P.frames.size();
+        for (FramePlan &f : frames_for(s.plan)) P.frames.push_back(std::move(f));
         for (size_t i = 0; i < cw.size(); i++) {
             const int f = s.plan.frame[i];
             if (f >= 0)
-                frames[s.f0 + (size_t)f].rect.push_back(tc::PlaneRect{cio[i].src, cio[i].dst, (long)(cio[i].src_stride / 4), (long)(cio[i].dst_stride / 4),
-                                                                      cw[i], ch[i], s.plan.x0[i], s.plan.y0[i], 0});
+                P.frames[s.f0 + (size_t)f].rect.push_back(tc::PlaneRect{cio[i].src, cio[i].dst, (long)(cio[i].src_stride / 4), (long)(cio[i].dst_stride / 4),
+                                                                        cw[i], ch[i], s.plan.x0[i], s.plan.y0[i], 0});
         }
-        rc = reserve_frames(ctx, frames, s.f0, frames.size(), max_channels(s.m));
+        rc = reserve_frames(ctx, P.frames, s.f0, P.frames.size(), max_channels(s.m));
         if (rc) return rc;
     }
-    if (frames.empty() && tta.empty()) return W2X_OK;
-    const TtaPlane *tab = nullptr;
-    int rc = upload_frames(ctx, frames, fd, tta, &tab);
-    for (size_t k = 0; k <= last && !rc; k++)
-        if (steps[k].tta) {
-            steps[k].vtab = tab + tab0[k];
-            steps[k].mtab = tab + tab0[k] + n_planes;
+    P.tables = Tables();
+    frame_tables(P.frames, &P.fd, &P.tables);
+    if (P.frames.empty() && !P.n_tta) return W2X_OK;
+    return ctx->plan_buf.reserve(P.tables.bytes(P.n_tta));
+}
+
+// Everything before the first launch of a call, on every part: first every buffer of every part (reserve_part), so that W2X_ERR_NOMEM
+// leaves nothing queued on any context; then on each part ONE upload of every step's frame tables and TTA kernel tables, so that no
+// step waits for the host.  A TTA step's variants kernel on the part owning plane i writes variant j wherever the part converting it
+// keeps it, and the mean kernel reads its output there.
+int prepare_parts(std::vector<Part> &parts, bool pack) {
+    for (Part &P : parts)
+        if (int rc = reserve_part(P, pack)) return rc;
+    const size_t n_steps = parts[0].steps.size();
+    std::vector<std::vector<const PlaneIO *>> var_at(n_steps);   // [k][8 i + j]: where variant j of plane i lives at TTA step k
+    for (const Part &P : parts)
+        for (size_t k = 0; k < n_steps; k++) {
+            const Step &s = P.steps[k];
+            for (size_t v = 0; v < s.vof.size(); v++) {
+                if (var_at[k].size() <= (size_t)s.vof[v]) var_at[k].resize((size_t)s.vof[v] + 1);
+                var_at[k][(size_t)s.vof[v]] = &s.vio[v];
+            }
         }
-    return rc;
+    auto tiles = [](int w, int h) { return ((w + 31) / 32) * ((h + 31) / 32); };
+    for (Part &P : parts) {
+        if (P.frames.empty() && !P.n_tta) continue;
+        DeviceGuard g(P.ctx->device);
+        std::vector<TtaPlane> tta;
+        std::vector<size_t> tab0(n_steps);   // a TTA step's variants table at tta[tab0], its mean table right after it
+        for (size_t k = 0; k < n_steps; k++) {
+            Step &s = P.steps[k];
+            if (!s.tta) continue;
+            tab0[k] = tta.size();
+            for (size_t i = 0; i < P.own.size(); i++) {   // the variants kernel: plane -> its 8 variants
+                const int sw = s.up ? s.w[i] / 2 : s.w[i], sh = s.up ? s.h[i] / 2 : s.h[i];
+                TtaPlane t{s.io[i].src, {}, nullptr, (long)(s.io[i].src_stride / 4), 0, sw, sh, s.vtiles};
+                for (int j = 0; j < 8; j++) t.var[j] = const_cast<float *>(var_at[k][(size_t)(8 * P.own[i] + j)]->src);
+                tta.push_back(t);
+                s.vtiles += tiles(sw, sh);
+            }
+            for (size_t i = 0; i < P.own.size(); i++) {   // the mean kernel: 8 variant outputs -> the step's output
+                TtaPlane t{nullptr, {}, s.io[i].dst, 0, (long)(s.io[i].dst_stride / 4), s.w[i], s.h[i], s.mtiles};
+                for (int j = 0; j < 8; j++) t.var[j] = var_at[k][(size_t)(8 * P.own[i] + j)]->dst;
+                tta.push_back(t);
+                s.mtiles += tiles(s.w[i], s.h[i]);
+            }
+        }
+        const TtaPlane *tab = nullptr;
+        int rc = upload_tables(P.ctx, P.tables, &P.fd, tta, &tab);
+        if (rc) return rc;
+        for (size_t k = 0; k < n_steps; k++)
+            if (P.steps[k].tta) {
+                P.steps[k].vtab = tab + tab0[k];
+                P.steps[k].mtab = tab + tab0[k] + P.own.size();
+            }
+    }
+    return W2X_OK;
+}
+
+// The one-context call: one part owning every plane (its ends still to be set).
+Part one_part(w2x_ctx *ctx, std::vector<Step> &steps) {
+    Part P{ctx, std::vector<int>(steps[0].w.size()), std::move(steps), {}, {}, {}, {}, 0};
+    for (size_t i = 0; i < P.own.size(); i++) P.own[i] = (int)i;
+    return P;
 }
 
 // A unit of work of one step: one packed frame (n + 1 launches for all its planes), or one plane converted alone by convert_device
@@ -1189,23 +1312,35 @@ int run_unit(w2x_ctx *ctx, const Step &s, const std::vector<FrameDev> &fd, const
     return W2X_OK;
 }
 
-// The launches of one prepared step, after its progress lines: its units, for a TTA step between the variants kernel and the mean
-// kernel (which reads the tables last).
-int run_step(w2x_ctx *ctx, const Step &s, const std::vector<FrameDev> &fd, int block_splitting) {
-    const int n_planes = (int)s.w.size();
-    if (s.tta) {
-        CU_CHECK(launch_tta_variants(s.vtab, n_planes, s.vtiles, ctx->stream));
-        ctx->launches++;
-    }
+// The three launches of a TTA step around its units, on the context's stream: the variants kernel of the planes the context owns,
+// the units of the variants it converts, the mean kernel of its planes (which reads the tables last).
+int tta_variants(w2x_ctx *ctx, const Step &s) {
+    CU_CHECK(launch_tta_variants(s.vtab, (int)s.w.size(), s.vtiles, ctx->stream));
+    ctx->launches++;
+    return W2X_OK;
+}
+
+int run_units(w2x_ctx *ctx, const Step &s, const std::vector<FrameDev> &fd, int block_splitting) {
     for (const PlanesUnit &u : units_of(s))
         if (int rc = run_unit(ctx, s, fd, u, block_splitting)) return rc;
-    if (s.tta) {
-        CU_CHECK(launch_tta_mean(s.mtab, n_planes, s.mtiles, ctx->stream));
-        ctx->launches++;
-        CU_CHECK(cudaEventRecord(ctx->plan_ev, ctx->stream));
-        ctx->plan_ev_live = true;
-    }
     return W2X_OK;
+}
+
+int tta_mean(w2x_ctx *ctx, const Step &s) {
+    CU_CHECK(launch_tta_mean(s.mtab, (int)s.w.size(), s.mtiles, ctx->stream));
+    ctx->launches++;
+    CU_CHECK(cudaEventRecord(ctx->plan_ev, ctx->stream));
+    ctx->plan_ev_live = true;
+    return W2X_OK;
+}
+
+// The launches of one prepared step, after its progress lines: its units, for a TTA step between the variants kernel and the mean
+// kernel.
+int run_step(w2x_ctx *ctx, const Step &s, const std::vector<FrameDev> &fd, int block_splitting) {
+    int rc = s.tta ? tta_variants(ctx, s) : W2X_OK;
+    if (!rc) rc = run_units(ctx, s, fd, block_splitting);
+    if (!rc && s.tta) rc = tta_mean(ctx, s);
+    return rc;
 }
 
 // on_step(k), then the step's (resized) planes' lines, plane by plane, as the single-plane entry point prints them.  A packed
@@ -1226,68 +1361,265 @@ int run_steps(w2x_ctx *ctx, const std::vector<Step> &steps, const std::vector<Fr
     return W2X_OK;
 }
 
-// Device planes, checked: the steps in order on the context's stream (pack: see prepare_planes).
+// Device planes, checked: the steps in order on the context's stream (pack: see reserve_part).
 int planes_device(w2x_ctx *ctx, std::vector<Step> &steps, const float *const *d_in, const size_t *in_strides, float *const *d_out,
                   const size_t *out_strides, bool pack, int block_splitting, w2x_step_fn on_step, void *user) {
-    std::vector<PlaneIO> ends(steps[0].w.size());
-    for (size_t i = 0; i < ends.size(); i++) ends[i] = PlaneIO{d_in[i], in_strides[i], d_out[i], out_strides[i]};
-    std::vector<FrameDev> fd;
-    int rc = prepare_planes(ctx, steps, ends, pack, &fd);
+    std::vector<Part> parts{one_part(ctx, steps)};
+    Part &P = parts[0];
+    P.ends.resize(P.own.size());
+    for (size_t i = 0; i < P.ends.size(); i++) P.ends[i] = PlaneIO{d_in[i], in_strides[i], d_out[i], out_strides[i]};
+    int rc = prepare_parts(parts, pack);
     if (rc) return rc;
-    return run_steps(ctx, steps, fd, 0, steps.size(), block_splitting, on_step, user, false);
+    return run_steps(ctx, P.steps, P.fd, 0, P.steps.size(), block_splitting, on_step, user, false);
 }
 
-// Host planes, checked: dense device staging, inputs in io_buf[0] and outputs in io_buf[1], and ONE run of the copy pipeline.  Each
-// unit of step 0 is a group carrying its planes' uploads, each step between the first and the last one compute-only group, each unit
-// of the last step a group carrying its planes' downloads: uploads overlap the first step and downloads the last.  A TTA step at
-// either end is one group.
+// Host planes, checked, on parts (one per context) of the call's step table `all`, staged densely on each part's context, inputs in
+// io_buf[0] and outputs in io_buf[1], and ONE run of a copy pipeline per part.  Each unit of step 0 is a group carrying its planes'
+// uploads, each step between the first and the last one compute-only group, each unit of the last step a group carrying its planes'
+// downloads: uploads overlap the first step and downloads the last.  A TTA step is three groups: the variants kernel (carrying the
+// uploads at step 0), the units of the variants, the mean kernel (carrying the downloads at the last step).  Every part's groups are
+// queued before any part is waited for, phase by phase (a plain step is one phase, a TTA step three), and on_step(k) and step k's lines
+// (through `log`) come before its first phase.  Between parts, the units of a TTA step wait for every other part's variants kernel
+// (tta_ev[0]) and a mean kernel for every other part's units (tta_ev[1]): every record is queued before the waits that name it.
+int planes_host(w2x_ctx *log, const std::vector<Step> &all, std::vector<Part> &parts, const float *const *in, const int *widths,
+                const int *heights, const size_t *in_strides, float *const *out, const size_t *out_strides, w2x_step_fn on_step, void *user) {
+    const size_t np = parts.size(), last = all.size() - 1;
+    std::vector<std::vector<size_t>> in_off(np), out_off(np);
+    for (size_t p = 0; p < np; p++) {
+        Part &P = parts[p];
+        const Step &L = P.steps.back();
+        const size_t n = P.own.size();
+        in_off[p].assign(n + 1, 0);
+        out_off[p].assign(n + 1, 0);
+        for (size_t i = 0; i < n; i++) {
+            const int g = P.own[i];
+            in_off[p][i + 1] = in_off[p][i] + (size_t)widths[g] * heights[g];
+            out_off[p][i + 1] = out_off[p][i] + (size_t)L.w[i] * L.h[i];
+        }
+        DeviceGuard dg(P.ctx->device);
+        int rc = reserve_io(P.ctx, in_off[p].back() * sizeof(float), out_off[p].back() * sizeof(float));
+        if (rc) return rc;
+        P.ends.resize(n);
+        for (size_t i = 0; i < n; i++)
+            P.ends[i] = PlaneIO{P.ctx->io_buf[0].get() + in_off[p][i], (size_t)widths[P.own[i]] * 4, P.ctx->io_buf[1].get() + out_off[p][i], (size_t)L.w[i] * 4};
+    }
+    int rc = prepare_parts(parts, true);
+    if (rc) return rc;
+    std::vector<std::vector<HostGroup>> groups(np);
+    std::vector<std::vector<int>> upto(np);   // [part][phase]: how many of the part's groups are queued by the end of the phase
+    for (size_t p = 0; p < np; p++) {
+        Part &P = parts[p];
+        w2x_ctx *ctx = P.ctx;
+        std::vector<HostGroup> &G = groups[p];
+        auto copies = [&, p](HostGroup &g, const std::vector<int> &planes, bool up, bool down) {
+            const Step &L = P.steps.back();
+            for (int i : planes) {
+                const int gi = P.own[(size_t)i];
+                const size_t row = (size_t)widths[gi] * 4, out_row = (size_t)L.w[(size_t)i] * 4;
+                if (up) g.up.push_back({P.ctx->io_buf[0].get() + in_off[p][(size_t)i], row, in[gi], in_strides[gi], row, (size_t)heights[gi]});
+                if (down)
+                    g.down.push_back({out[gi], out_strides[gi], P.ctx->io_buf[1].get() + out_off[p][(size_t)i], out_row, out_row, (size_t)L.h[(size_t)i]});
+            }
+        };
+        std::vector<int> mine(P.own.size());
+        for (size_t i = 0; i < mine.size(); i++) mine[i] = (int)i;
+        auto add = [&](HostGroup &&g) { G.push_back(std::move(g)); };
+        for (size_t k = 0; k <= last; k++) {
+            const Step &s = P.steps[k];
+            if (s.tta) {
+                if (!mine.empty()) {
+                    HostGroup g;
+                    copies(g, mine, k == 0, false);
+                    g.compute = [ctx, &s] {
+                        int rc = tta_variants(ctx, s);
+                        if (!rc) CU_CHECK(cudaEventRecord(ctx->tta_ev[0], ctx->stream));
+                        return rc;
+                    };
+                    add(std::move(g));
+                }
+                upto[p].push_back((int)G.size());
+                if (!s.vof.empty()) {
+                    HostGroup g;
+                    g.compute = [&parts, &P, &s, k] {
+                        for (const Part &Q : parts)
+                            if (&Q != &P && !Q.own.empty()) CU_CHECK(cudaStreamWaitEvent(P.ctx->stream, Q.ctx->tta_ev[0], 0));
+                        int rc = run_units(P.ctx, s, P.fd, 0);
+                        if (!rc) CU_CHECK(cudaEventRecord(P.ctx->tta_ev[1], P.ctx->stream));
+                        return rc;
+                    };
+                    add(std::move(g));
+                }
+                upto[p].push_back((int)G.size());
+                if (!mine.empty()) {
+                    HostGroup g;
+                    copies(g, mine, false, k == last);
+                    g.compute = [&parts, &P, &s, k] {
+                        for (const Part &Q : parts)
+                            if (&Q != &P && !Q.steps[k].vof.empty()) CU_CHECK(cudaStreamWaitEvent(P.ctx->stream, Q.ctx->tta_ev[1], 0));
+                        return tta_mean(P.ctx, s);
+                    };
+                    add(std::move(g));
+                }
+            } else if (k > 0 && k < last) {
+                if (!mine.empty()) {
+                    HostGroup g;
+                    g.compute = [&P, &s] { return run_step(P.ctx, s, P.fd, 0); };
+                    add(std::move(g));
+                }
+            } else {
+                for (const PlanesUnit &u : units_of(s)) {
+                    HostGroup g;
+                    copies(g, u.planes, k == 0, k == last);
+                    g.compute = [&P, &s, u] { return run_unit(P.ctx, s, P.fd, u, 0); };
+                    add(std::move(g));
+                }
+            }
+            upto[p].push_back((int)G.size());
+        }
+    }
+    std::vector<HostPipe> pipes;
+    for (size_t p = 0; p < np; p++) pipes.push_back(HostPipe{parts[p].ctx, groups[p]});
+    for (size_t p = 0; p < np && !rc; p++) rc = pipes[p].start();
+    for (size_t k = 0, ph = 0; k <= last && !rc; k++) {
+        begin_step(log, all, k, 0, on_step, user, true);
+        for (int t = 0; t < (all[k].tta ? 3 : 1) && !rc; t++, ph++)
+            for (size_t p = 0; p < np && !rc; p++) rc = pipes[p].queue(upto[p][ph]);
+    }
+    for (HostPipe &pp : pipes) {
+        const int r2 = pp.finish(rc);
+        if (!rc) rc = r2;
+    }
+    return rc;
+}
+
+// The one-context host call.
 int planes_host(w2x_ctx *ctx, std::vector<Step> &steps, const float *const *in, const int *widths, const int *heights,
                 const size_t *in_strides, float *const *out, const size_t *out_strides, w2x_step_fn on_step, void *user) {
-    const Step &L = steps.back();
-    const size_t n_planes = L.w.size(), last = steps.size() - 1;
-    std::vector<size_t> in_off(n_planes + 1, 0), out_off(n_planes + 1, 0);
-    for (size_t i = 0; i < n_planes; i++) {
-        in_off[i + 1] = in_off[i] + (size_t)widths[i] * heights[i];
-        out_off[i + 1] = out_off[i] + (size_t)L.w[i] * L.h[i];
+    std::vector<Part> parts{one_part(ctx, steps)};
+    return planes_host(ctx, parts[0].steps, parts, in, widths, heights, in_strides, out, out_strides, on_step, user);
+}
+
+// ---- a collection across the GPUs of a w2x_multi (w2x_multi_convert_planes*) ----------------------------------------------------
+// The work of a model per output pixel: 9 Cin Cout multiply-adds summed over its layers.
+long long macs_per_pixel(const w2x_model *m) {
+    long long s = 0;
+    for (const Layer &L : m->layers) s += 9LL * L.n_in * L.n_out;
+    return s;
+}
+
+// The placement of w2x_multi_convert_planes_chain on n_dev GPUs (include/w2x_b200.h): returns nd, the GPUs used, with owner[i] in
+// [0, nd) and the planned work per GPU in load[0 .. nd).  A plane's plain steps run on its owner and variant j of its TTA steps on
+// (owner + j) mod nd; planes are placed greedily in decreasing order of total work (ties: the lower index), each on the owner that
+// keeps the largest load after it smallest (ties: the owner with the smaller load before it, then the lower index).
+int plan_multi(int n_dev, const std::vector<Step> &steps, std::vector<int> *owner, std::vector<long long> *load) {
+    const size_t n = steps[0].w.size();
+    bool tta = false;
+    for (const Step &s : steps) tta = tta || s.tta;
+    const int nd = (int)std::min<long long>(n_dev, (tta ? 8LL : 1LL) * (long long)n);
+    std::vector<long long> plain(n, 0), var(n, 0);   // a plane's work on its owner, and per variant of its TTA steps
+    for (const Step &s : steps) {
+        const long long macs = macs_per_pixel(s.m);
+        for (size_t i = 0; i < n; i++) (s.tta ? var : plain)[i] += (long long)s.w[i] * s.h[i] * macs;
     }
-    int rc = reserve_io(ctx, in_off.back() * sizeof(float), out_off.back() * sizeof(float));
-    if (rc) return rc;
-    float *din = ctx->io_buf[0].get(), *dout = ctx->io_buf[1].get();
-    std::vector<PlaneIO> ends(n_planes);
-    for (size_t i = 0; i < n_planes; i++) ends[i] = PlaneIO{din + in_off[i], (size_t)widths[i] * 4, dout + out_off[i], (size_t)L.w[i] * 4};
-    std::vector<FrameDev> fd;
-    rc = prepare_planes(ctx, steps, ends, true, &fd);
-    if (rc) return rc;
-    std::vector<HostGroup> groups;
-    for (size_t k = 0; k <= last; k++) {
-        if (k > 0 && k < last) {
-            groups.emplace_back();
-            groups.back().compute = [&, k] { return run_steps(ctx, steps, fd, k, k + 1, 0, on_step, user, true); };
-            continue;
-        }
-        // a TTA step's variants kernel reads every plane and its mean kernel writes every output: the step is one group
-        std::vector<PlanesUnit> units(1, PlanesUnit{-1, {}});
-        if (steps[k].tta)
-            for (size_t i = 0; i < n_planes; i++) units[0].planes.push_back((int)i);
-        else
-            units = units_of(steps[k]);
-        for (size_t j = 0; j < units.size(); j++) {
-            HostGroup G;
-            for (int i : units[j].planes) {
-                const size_t row = (size_t)widths[i] * 4, out_row = (size_t)L.w[(size_t)i] * 4;
-                if (k == 0) G.up.push_back({din + in_off[(size_t)i], row, in[i], in_strides[i], row, (size_t)heights[i]});
-                if (k == last) G.down.push_back({out[i], out_strides[i], dout + out_off[(size_t)i], out_row, out_row, (size_t)L.h[(size_t)i]});
+    std::vector<int> order(n);
+    for (size_t i = 0; i < n; i++) order[i] = (int)i;
+    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return plain[(size_t)a] + 8 * var[(size_t)a] > plain[(size_t)b] + 8 * var[(size_t)b]; });
+    owner->assign(n, 0);
+    load->assign((size_t)nd, 0);
+    std::vector<long long> &L = *load, with(L);
+    for (int i : order) {
+        int best = -1;
+        long long best_max = 0;
+        for (int o = 0; o < nd; o++) {
+            with = L;
+            with[(size_t)o] += plain[(size_t)i];
+            for (int j = 0; j < 8 && tta; j++) with[(size_t)((o + j) % nd)] += var[(size_t)i];
+            const long long mx = *std::max_element(with.begin(), with.end());
+            if (best < 0 || mx < best_max || (mx == best_max && L[(size_t)o] < L[(size_t)best])) {
+                best = o;
+                best_max = mx;
             }
-            G.compute = [&, k, j, u = units[j]] {
-                if (j == 0) begin_step(ctx, steps, k, 0, on_step, user, true);
-                return steps[k].tta ? run_step(ctx, steps[k], fd, 0) : run_unit(ctx, steps[k], fd, u, 0);
-            };
-            groups.push_back(std::move(G));
         }
+        (*owner)[(size_t)i] = best;
+        L[(size_t)best] += plain[(size_t)i];
+        for (int j = 0; j < 8 && tta; j++) L[(size_t)((best + j) % nd)] += var[(size_t)i];
     }
-    return run_host_groups(ctx, groups);
+    return nd;
 }
 }  // namespace
+
+namespace w2x {
+namespace eng {
+int multi_planes_chain(const char *fn, const std::vector<w2x_ctx *> &ctxs, int n_steps, const w2x_model *const *models, const int *kinds,
+                       int n_planes, const float *const *in, const int *widths, const int *heights, const size_t *in_strides,
+                       float *const *out, const size_t *out_strides, w2x_step_fn on_step, void *user) {
+    w2x_ctx *ctx0 = ctxs[0];
+    std::vector<Step> all;
+    int rc = check_planes_chain(fn, ctx0, n_steps, models, kinds, n_planes, in, widths, heights, in_strides, out, out_strides, &all);
+    if (rc) return rc;
+    std::vector<int> owner;
+    std::vector<long long> load;
+    const int nd = plan_multi((int)ctxs.size(), all, &owner, &load);
+    if (nd == 1) return w2x_convert_planes_chain(ctx0, n_steps, models, kinds, n_planes, in, widths, heights, in_strides, out, out_strides, on_step, user);
+    bool tta = false;
+    for (const Step &s : all) tta = tta || s.tta;
+    for (int a = 0; a < nd && tta; a++)   // a TTA step's kernels on one GPU store to and load from the others' buffers
+        for (int b = 0; b < nd; b++) {
+            const int da = ctxs[(size_t)a]->device, db = ctxs[(size_t)b]->device;
+            if (da == db) continue;
+            int can = 0;
+            CU_CHECK(cudaDeviceCanAccessPeer(&can, da, db));
+            if (!can) return fail(W2X_ERR_UNSUPPORTED, "%s: device %d cannot map the memory of device %d (no peer access)", fn, da, db);
+            DeviceGuard g(da);
+            cudaError_t e = cudaDeviceEnablePeerAccess(db, 0);
+            if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) CU_CHECK(e);
+            cudaGetLastError();
+        }
+    std::vector<Part> parts((size_t)nd);
+    for (int i = 0; i < n_planes; i++) parts[(size_t)owner[(size_t)i]].own.push_back(i);
+    for (int d = 0; d < nd; d++) {
+        Part &P = parts[(size_t)d];
+        P.ctx = ctxs[(size_t)d];
+        P.ctx->precision = ctx0->precision;
+        P.ctx->engine = ctx0->engine;
+        std::vector<std::vector<int>> vof(all.size());
+        for (size_t k = 0; k < all.size(); k++)
+            for (int i = 0; i < n_planes && all[k].tta; i++)
+                for (int j = 0; j < 8; j++)
+                    if ((owner[(size_t)i] + j) % nd == d) vof[k].push_back(8 * i + j);
+        P.steps = part_steps(all, P.own, vof);
+    }
+    NvtxRange nvtx("w2x multi convert planes chain");
+    const Step &L = all.back();
+    std::vector<std::unique_ptr<HostPin>> pins;
+    for (int i = 0; i < n_planes; i++) {
+        pins.push_back(std::make_unique<HostPin>(in[i], in_strides[i] * (size_t)(heights[i] - 1) + (size_t)widths[i] * 4));
+        pins.push_back(std::make_unique<HostPin>(out[i], out_strides[i] * (size_t)(L.h[(size_t)i] - 1) + (size_t)L.w[(size_t)i] * 4));
+    }
+    return planes_host(ctx0, all, parts, in, widths, heights, in_strides, out, out_strides, on_step, user);
+}
+}  // namespace eng
+}  // namespace w2x
+
+extern "C" {
+// Test hook (not part of the stable ABI): the placement of w2x_multi_convert_planes_chain on n_devices GPUs, without a device.  owner
+// gets every plane's GPU, load (n_devices entries) the planned work per GPU used.  Returns the number of GPUs used, or -W2X_ERR_ARG.
+W2X_API int w2x_debug_plan_multi_planes(int n_devices, int n_steps, const w2x_model *const *models, const int *kinds, int n_planes,
+                                        const int *widths, const int *heights, int *owner, long long *load) {
+    if (n_devices < 1 || n_steps < 1 || !models || !kinds || n_planes < 1 || !widths || !heights || !owner || !load)
+        return -fail(W2X_ERR_ARG, "w2x_debug_plan_multi_planes: bad argument");
+    for (int k = 0; k < n_steps; k++)
+        if (!models[k] || kinds[k] & ~(W2X_STEP_UPSCALE2X | W2X_STEP_TTA)) return -fail(W2X_ERR_ARG, "w2x_debug_plan_multi_planes: step %d", k);
+    for (int i = 0; i < n_planes; i++)
+        if (widths[i] < 1 || heights[i] < 1) return -fail(W2X_ERR_ARG, "w2x_debug_plan_multi_planes: plane %d has no pixels", i);
+    std::vector<int> own;
+    std::vector<long long> ld;
+    const int nd = plan_multi(n_devices, step_table(n_steps, models, kinds, n_planes, widths, heights), &own, &ld);
+    std::copy(own.begin(), own.end(), owner);
+    std::copy(ld.begin(), ld.end(), load);
+    return nd;
+}
+}  // extern "C"
 
 namespace w2x {
 namespace eng {
@@ -1463,16 +1795,19 @@ int check_chain(const char *fn, w2x_ctx *ctx, int n_steps, const w2x_model *cons
 // step 0, group i also uploads the input rows that band i is the first to read, so that uploads overlap the layers as well;
 // otherwise one upload and steps 0 ... n - 2 go first on the context's stream.  A TTA last step is one group: its download waits for
 // the mean kernel.
-int chain_host(w2x_ctx *ctx, std::vector<Step> &steps, const float *in, int width, int height, size_t in_stride_bytes, float *out,
+int chain_host(w2x_ctx *ctx, std::vector<Step> &table, const float *in, int width, int height, size_t in_stride_bytes, float *out,
                size_t out_stride_bytes, int block_splitting, w2x_step_fn on_step, void *user) {
+    std::vector<Part> parts{one_part(ctx, table)};
+    std::vector<Step> &steps = parts[0].steps;
+    std::vector<FrameDev> &fd = parts[0].fd;
     const size_t last = steps.size() - 1;
     const w2x_model *m = steps[last].m;
     const bool up = steps[last].up, band_uploads = last == 0 && !steps[last].tta;
     const int n = (int)m->layers.size(), w = steps[last].w[0], h = steps[last].h[0];
     const size_t in_dense = (size_t)width * 4;
     int rc = reserve_io(ctx, (size_t)width * height * sizeof(float), (size_t)w * h * sizeof(float));
-    std::vector<FrameDev> fd;
-    if (!rc) rc = prepare_planes(ctx, steps, {PlaneIO{ctx->io_buf[0].get(), in_dense, ctx->io_buf[1].get(), (size_t)w * 4}}, false, &fd);
+    parts[0].ends = {PlaneIO{ctx->io_buf[0].get(), in_dense, ctx->io_buf[1].get(), (size_t)w * 4}};
+    if (!rc) rc = prepare_parts(parts, false);
     if (rc) return rc;
     if (!band_uploads)
         CU_CHECK(cudaMemcpy2DAsync(ctx->io_buf[0].get(), in_dense, in, in_stride_bytes, in_dense, (size_t)height, cudaMemcpyHostToDevice, ctx->stream));

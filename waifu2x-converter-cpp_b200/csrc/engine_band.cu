@@ -646,21 +646,6 @@ void multi_drop_chain(w2x_multi *m) {
     m->chain = w2x_multi::Chain();
 }
 
-// pinned view of a caller buffer for the duration of one call (pageable memory makes every async copy a staged, blocking one)
-struct HostPin {
-    void *p = nullptr;
-    HostPin(const void *ptr, size_t bytes) {
-        cudaPointerAttributes at{};
-        if (cudaPointerGetAttributes(&at, ptr) == cudaSuccess && at.type != cudaMemoryTypeUnregistered) return;   // already pinned (w2x_host_alloc, cudaHostAlloc, ...)
-        cudaGetLastError();
-        if (bytes >= ((size_t)4 << 20) && cudaHostRegister(const_cast<void *>(ptr), bytes, cudaHostRegisterPortable) == cudaSuccess) p = const_cast<void *>(ptr);
-        else cudaGetLastError();
-    }
-    ~HostPin() {
-        if (p) cudaHostUnregister(p);
-    }
-};
-
 }  // namespace
 
 extern "C" {
@@ -835,6 +820,22 @@ int w2x_multi_convert_chain(w2x_multi *m, int n_steps, const w2x_model *const *m
         if (rc == W2X_OK) rc = r2;
     }
     return rc;
+}
+
+int w2x_multi_convert_planes_chain(w2x_multi *m, int n_steps, const w2x_model *const *models, const int *kinds, int n_planes,
+                                   const float *const *in, const int *widths, const int *heights, const size_t *in_strides, float *const *out,
+                                   const size_t *out_strides, w2x_step_fn on_step, void *user) {
+    if (!m || m->ctx.empty()) return fail(W2X_ERR_ARG, "w2x_multi_convert_planes_chain: NULL handle");
+    return multi_planes_chain("w2x_multi_convert_planes_chain", m->ctx, n_steps, models, kinds, n_planes, in, widths, heights, in_strides,
+                              out, out_strides, on_step, user);
+}
+
+int w2x_multi_convert_planes(w2x_multi *m, const w2x_model *model, int n_planes, const float *const *in, const int *widths,
+                             const int *heights, const size_t *in_strides, float *const *out, const size_t *out_strides) {
+    if (!m || m->ctx.empty()) return fail(W2X_ERR_ARG, "w2x_multi_convert_planes: NULL handle");
+    const int same = W2X_STEP_SAME;
+    return multi_planes_chain("w2x_multi_convert_planes", m->ctx, 1, &model, &same, n_planes, in, widths, heights, in_strides, out,
+                              out_strides, nullptr, nullptr);
 }
 
 // Independent planes of one shape (the reference's block loop, src/convertRoutine.cpp:114-165, and BASELINE config 5):

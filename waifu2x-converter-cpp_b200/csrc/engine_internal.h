@@ -102,6 +102,7 @@ struct w2x_ctx {
     w2x::eng::DevBuf<float> io_buf[2];      // device staging for the host-buffer entry points
     w2x::eng::DevBuf<float> chain_buf[2];   // the planes between the steps of w2x_convert_chain*
     w2x::eng::DevBuf<float> tta_buf[2];     // a W2X_STEP_TTA step's 8 variants per plane (0) and their conversions (1)
+    cudaEvent_t tta_ev[2] = {};             // w2x_multi_convert_planes_chain: after a TTA step's variants kernel (0), after its units (1)
     bool tc_ready = false;
     cudaStream_t copy_in = nullptr, copy_out = nullptr;   // host<->device copies of run_host_groups overlap the compute stream
     cudaEvent_t ev_in[8] = {}, ev_done[8] = {};
@@ -117,6 +118,8 @@ struct w2x_ctx {
         auto drop = [](cudaEvent_t e) { if (e) cudaEventDestroy(e); };
         drop(plan_ev);
         drop(switch_ev);
+        drop(tta_ev[0]);
+        drop(tta_ev[1]);
         for (auto &s : spans) { drop(s.e0); drop(s.e1); }
         for (auto e : event_pool) drop(e);
         for (int i = 0; i < 8; i++) { drop(ev_in[i]); drop(ev_done[i]); }
@@ -208,8 +211,30 @@ int check_chain_host(const char *fn, w2x_ctx *ctx, int n_steps, const w2x_model 
 int launch_layer_tc(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int li, const __half *in, __half *out, int pw, int ph,
                     bool fused, bool profile, int out_y0 = 0, int out_rows = -1);
 
+// w2x_multi_convert_planes_chain on the contexts of a w2x_multi (engine.cu): `fn` names the entry point in messages.
+int multi_planes_chain(const char *fn, const std::vector<w2x_ctx *> &ctxs, int n_steps, const w2x_model *const *models, const int *kinds,
+                       int n_planes, const float *const *in, const int *widths, const int *heights, const size_t *in_strides,
+                       float *const *out, const size_t *out_strides, w2x_step_fn on_step, void *user);
+
 int tiles_enqueue_compute(w2x_ctx *ctx, const w2x_model *model, const float *const *in_tiles, float *const *out_tiles, int n_tiles, int width, int height, size_t in_stride_bytes, size_t out_stride_bytes);
 int tiles_enqueue_download(w2x_ctx *ctx, float *const *out_tiles, int n_tiles, int width, int height, size_t out_stride_bytes);
+
+// pinned view of a caller buffer for the duration of one call (pageable memory makes every async copy a staged, blocking one)
+struct HostPin {
+    void *p = nullptr;
+    HostPin(const void *ptr, size_t bytes) {
+        cudaPointerAttributes at{};
+        if (cudaPointerGetAttributes(&at, ptr) == cudaSuccess && at.type != cudaMemoryTypeUnregistered) return;   // already pinned (w2x_host_alloc, cudaHostAlloc, ...)
+        cudaGetLastError();
+        if (bytes >= ((size_t)4 << 20) && cudaHostRegister(const_cast<void *>(ptr), bytes, cudaHostRegisterPortable) == cudaSuccess) p = const_cast<void *>(ptr);
+        else cudaGetLastError();
+    }
+    HostPin(const HostPin &) = delete;
+    HostPin &operator=(const HostPin &) = delete;
+    ~HostPin() {
+        if (p) cudaHostUnregister(p);
+    }
+};
 
 struct NvtxRange {    // a named range on the calling thread's timeline (nsys / ncu --nvtx), e.g. "w2x L3", "w2x halo exchange"
     explicit NvtxRange(const char *name) { nvtxRangePushA(name); }

@@ -52,7 +52,8 @@ cudaError_t launch_conv3x3_fp32(const float *in, float *out, const float *wgt, c
 // tiles every plane into 32 x 32 tiles, plane i owning tiles [blk0_i, blk0_i + ceil(w/32) * ceil(h/32)).
 struct TtaPlane {
     const float *src;    // tta_variants: the plane X, row stride src_stride floats
-    float *var;          // the 8 variants (tta_variants) or their conversions (tta_mean), dense: j at var + j * w * h, W' wide
+    float *var[8];       // variant j (tta_variants) or its conversion (tta_mean), dense and W' wide, on the GPU that converts it
+                         // (a peer address when that is not the launching GPU)
     float *dst;          // tta_mean: the output plane, row stride dst_stride floats
     long src_stride, dst_stride;
     int w, h;            // X's size (tta_variants) or the output's (tta_mean)

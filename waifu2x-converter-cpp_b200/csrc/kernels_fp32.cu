@@ -152,11 +152,10 @@ __global__ void __launch_bounds__(256) tta_variants_kernel(const TtaPlane *__res
     for (int q = q0; q < TTA_TILE; q += 8)
         if (r0 + q < R.h && c0 + l < R.w) s[q][l] = __ldg(R.src + (long)(r0 + q) * R.src_stride + c0 + l);
     __syncthreads();
-    const size_t plane = (size_t)R.w * R.h;
 #pragma unroll
     for (int j = 0; j < 8; j++) {
         const bool t = j & 4, fy = j & 2, fx = j & 1;
-        float *V = R.var + (size_t)j * plane;
+        float *V = R.var[j];
         for (int q = q0; q < TTA_TILE; q += 8) {
             if (!t) {
                 const int r = r0 + q, c = c0 + l;
@@ -177,11 +176,10 @@ __global__ void __launch_bounds__(256) tta_mean_kernel(const TtaPlane *__restric
     const int lb = (int)blockIdx.x - R.blk0, tiles_x = (R.w + TTA_TILE - 1) / TTA_TILE;
     const int r0 = lb / tiles_x * TTA_TILE, c0 = lb % tiles_x * TTA_TILE;
     const int l = threadIdx.x & 31, q0 = threadIdx.x >> 5;
-    const size_t plane = (size_t)R.w * R.h;
 #pragma unroll
     for (int j = 0; j < 8; j++) {
         const bool t = j & 4, fy = j & 2, fx = j & 1;
-        const float *O = R.var + (size_t)j * plane;
+        const float *O = R.var[j];
         for (int q = q0; q < TTA_TILE; q += 8) {
             if (!t) {
                 const int r = r0 + q, c = c0 + l;
