@@ -350,6 +350,37 @@ W2X_API int w2x_convert_chain_device(w2x_ctx *ctx, int n_steps, const w2x_model 
                                      float *d_out, size_t out_stride_bytes, int block_splitting, w2x_step_fn on_step,
                                      void *user);
 
+/* ---- a window of a chain's output ------------------------------------------------------------------- */
+/* Part of a chain's output without converting the rest: the visible part of a large page, the area around an edit patched into a
+ * previous output, or the tiles of a plane too large to hold.  An output pixel of a step depends only on the (2 n + 1)^2
+ * neighbourhood of its input pixel (n = the model's layer count), replicated only at the plane's own border, so a window computed
+ * from real neighbours is the same window of the whole conversion, seams included.  window = {x0, y0, w, h} of the
+ * (width << u) x (height << u) output (u = the number of upscaling steps).  Working back from the last step, a step's input window
+ * is its output window grown by its model's layer count on every side and clamped to the step's input plane, then for an
+ * upscaling step halved (floor at the top-left, ceil at the bottom-right); the first step's input window is the source rectangle.
+ * w2x_chain_region_source writes it to source[4] = {x0, y0, w, h} of the width x height input plane; it needs no device.
+ * W2X_STEP_TTA steps have no window form. */
+W2X_API int w2x_chain_region_source(int n_steps, const w2x_model *const *models, const int *kinds, int width, int height,
+                                    const int *window, int *source);
+/* That window of w2x_convert_chain(..., block_splitting = 0) on the whole width x height plane, bit-identical on the same context
+ * settings (engine, precision).  src points at the source rectangle's top-left pixel, and nothing outside the rectangle is read; out
+ * receives the window (w x h).  Each step converts only its output window, reading real neighbours where the previous window has
+ * them and replicating at the plane's border; intermediate windows stay on the device in the context's chain buffers.  Before
+ * step k is queued, on_step(k, user) is called (if not NULL); then the step logs the lines w2x_convert_plane_device(...,
+ * block_splitting = 0) logs for a plane the size of its output window, and launches the kernels that call launches for it.
+ * Every argument is checked before anything is printed, allocated or queued: W2X_ERR_ARG names the step or the problem (the
+ * checks of w2x_convert_chain, a W2X_STEP_TTA step, a NULL or empty window or one outside the output, NULL planes, row strides
+ * that are not multiples of 4 bytes or shorter than the rectangle's / window's row); W2X_ERR_UNSUPPORTED a model the context's
+ * engine refuses.  Every buffer is reserved before the first copy or launch, so W2X_ERR_NOMEM leaves nothing queued.
+ * HOST buffers, synchronous. */
+W2X_API int w2x_convert_chain_region(w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, int width,
+                                     int height, const int *window, const float *src, size_t src_stride_bytes, float *out,
+                                     size_t out_stride_bytes, w2x_step_fn on_step, void *user);
+/* Same on DEVICE buffers, asynchronous on the context's stream. */
+W2X_API int w2x_convert_chain_region_device(w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, int width,
+                                            int height, const int *window, const float *d_src, size_t src_stride_bytes, float *d_out,
+                                            size_t out_stride_bytes, w2x_step_fn on_step, void *user);
+
 /* ---- a chain of conversions on a collection of planes of any sizes ------------------------------------ */
 /* w2x_convert_chain for every plane of a w2x_convert_planes collection, in one call: the default noise_scale mode of a sprite set,
  * say.  Step k maps every plane P to convertWithModels(models[k], U_k(P)), U_k as in w2x_convert_chain, with block splitting off;

@@ -42,7 +42,8 @@ ABI_SYMBOLS = (
     "w2x_slab_connect", "w2x_slab_connect_local", "w2x_slab_convert", "w2x_slab_convert_async", "w2x_slab_synchronize",
     "w2x_convert_planes", "w2x_convert_planes_device", "w2x_convert_chain", "w2x_convert_chain_device",
     "w2x_convert_planes_chain", "w2x_convert_planes_chain_device", "w2x_multi_convert_chain",
-    "w2x_multi_convert_planes", "w2x_multi_convert_planes_chain",
+    "w2x_multi_convert_planes", "w2x_multi_convert_planes_chain", "w2x_chain_region_source", "w2x_convert_chain_region",
+    "w2x_convert_chain_region_device",
 )
 BAND_BLOB_BYTES = 320
 
@@ -147,6 +148,9 @@ def lib():
     L.w2x_convert_planes_device.argtypes = [vp, vp, ci, C.POINTER(vp), pi, pi, ps, C.POINTER(vp), ps]
     L.w2x_convert_chain.argtypes = [vp, ci, C.POINTER(vp), pi, vp, ci, ci, cs, vp, cs, ci, STEP_FN, vp]
     L.w2x_convert_chain_device.argtypes = [vp, ci, C.POINTER(vp), pi, vp, ci, ci, cs, vp, cs, ci, STEP_FN, vp]
+    L.w2x_chain_region_source.argtypes = [ci, C.POINTER(vp), pi, ci, ci, pi, pi]
+    L.w2x_convert_chain_region.argtypes = [vp, ci, C.POINTER(vp), pi, ci, ci, pi, vp, cs, vp, cs, STEP_FN, vp]
+    L.w2x_convert_chain_region_device.argtypes = [vp, ci, C.POINTER(vp), pi, ci, ci, pi, vp, cs, vp, cs, STEP_FN, vp]
     L.w2x_convert_planes_chain.argtypes = [vp, ci, C.POINTER(vp), pi, ci, C.POINTER(vp), pi, pi, ps, C.POINTER(vp), ps, STEP_FN, vp]
     L.w2x_convert_planes_chain_device.argtypes = [vp, ci, C.POINTER(vp), pi, ci, C.POINTER(vp), pi, pi, ps, C.POINTER(vp), ps, STEP_FN, vp]
     L.w2x_debug_plan_planes.argtypes = [ci, pi, pi, ci, ci, cs, pi, pi, pi, pi, ci]
@@ -232,6 +236,16 @@ def debug_plan_planes(widths, heights, n_layers=7, max_channels=128, scratch_lim
     dims = np.zeros((max(nf, 1), 2), np.int32)
     lib().w2x_debug_plan_planes(n, *args, dims.ctypes.data_as(pi), nf)
     return frame, x0, y0, dims[:nf]
+
+
+def chain_region_source(steps, size, window):
+    """The source rectangle (x0, y0, w, h) of the input plane that window (x0, y0, w, h) of a chain's output reads (no device
+    needed); steps as in Context.convert_chain without TTA, size = the input plane's (width, height)."""
+    n, models, kinds, _, _ = Context._chain_args(steps, None)
+    win = (C.c_int * 4)(*[int(v) for v in window])
+    src = (C.c_int * 4)()
+    _check(lib().w2x_chain_region_source(n, models, kinds, int(size[0]), int(size[1]), win, src))
+    return tuple(src)
 
 
 def debug_plan_multi_planes(n_devices, steps, widths, heights):
@@ -520,6 +534,44 @@ class Context:
         n, models, kinds, cb, _ = self._chain_args(steps, on_step)
         _check(lib().w2x_convert_chain_device(self._h, n, models, kinds, C.c_void_p(d_in), w, h, in_stride_bytes, C.c_void_p(d_out),
                                               out_stride_bytes, int(bool(block_splitting)), cb, None))
+
+    # a window of a chain's output from its source rectangle alone, bit-identical to the window of the whole chain
+    def convert_chain_region(self, steps, source, size, window, out=None, on_step=None):
+        """Window (x0, y0, w, h) of convert_chain(steps, plane, block_splitting=False) on a plane of size = (width, height), from
+        `source` alone: the 2-D float32 source rectangle chain_region_source(steps, size, window) of that plane (a row-strided view,
+        such as a slice of the whole plane, is passed as it is) -> the h x w window; `out` may be such an array (strided views
+        included), written in place.  on_step(k) is called before step k."""
+        x = np.asarray(source, np.float32)
+        if x.ndim != 2:
+            raise ValueError("source must be 2-D")
+        if x.strides[1] != 4 or x.strides[0] % 4 or x.strides[0] < x.shape[1] * 4:
+            x = np.ascontiguousarray(x)
+        try:
+            sx0, sy0, sw, sh = chain_region_source(steps, size, window)
+        except W2xError:                # the call below refuses the same arguments, in its own name
+            sx0, sy0, sw, sh = 0, 0, x.shape[1], x.shape[0]
+        if x.shape != (sh, sw):
+            raise ValueError(f"source must be the source rectangle {(sx0, sy0, sw, sh)}: shape {(sh, sw)}, not {x.shape}")
+        n, models, kinds, cb, _ = self._chain_args(steps, on_step)
+        ww, wh = int(window[2]), int(window[3])
+        if out is None:
+            out = np.empty((wh, ww), np.float32)
+        if out.ndim != 2 or out.dtype != np.float32 or out.strides[1] != 4 or out.strides[0] % 4:
+            raise ValueError("out must be a 2-D float32 array with unit column stride and a row stride that is a multiple of 4 bytes")
+        if out.shape != (wh, ww):
+            raise ValueError(f"out must have shape {(wh, ww)}")
+        win = (C.c_int * 4)(*[int(v) for v in window])
+        _check(lib().w2x_convert_chain_region(self._h, n, models, kinds, int(size[0]), int(size[1]), win, C.c_void_p(x.ctypes.data),
+                                              x.strides[0], C.c_void_p(out.ctypes.data), out.strides[0], cb, None))
+        return out
+
+    def convert_chain_region_device(self, steps, d_src, size, window, src_stride_bytes, d_out, out_stride_bytes, on_step=None):
+        """Device pointers (ints): d_src at the source rectangle's top-left pixel, d_out receiving the window; asynchronous on the
+        context's stream."""
+        n, models, kinds, cb, _ = self._chain_args(steps, on_step)
+        win = (C.c_int * 4)(*[int(v) for v in window])
+        _check(lib().w2x_convert_chain_region_device(self._h, n, models, kinds, int(size[0]), int(size[1]), win, C.c_void_p(d_src),
+                                                     src_stride_bytes, C.c_void_p(d_out), out_stride_bytes, cb, None))
 
     # convert_chain for every plane of a convert_planes collection, each step packing the planes into frames
     def convert_planes_chain(self, steps, planes, out=None, on_step=None):

@@ -402,11 +402,14 @@ void emit_plane_progress(w2x_ctx *ctx, const w2x_model *m, int w, int h, int blo
     for (int p = 0; p < passes; p++) emit_reference_progress(ctx, w, h, n, false);
 }
 
-// convertWithModels on checked device buffers (rows_above / rows_below: real neighbour rows available around the band).  up2x: the
-// plane converted is the nearest-neighbour 2x resize of d_in, never materialised; w x h is its (2x) size, the row counts are 2x
-// rows, and a band of it starts on an even 2x row with d_in pointing at its first source row.
+// convertWithModels on checked device buffers (rows_above / rows_below: real neighbour rows available around the band;
+// cols_left / cols_right: real neighbour columns left and right of it, for a window).  up2x: the plane converted is the
+// nearest-neighbour 2x resize of d_in, never materialised; w x h is its (2x) size, the row and column counts are in 2x pixels, and
+// d_in points at the source pixel holding its first row and column, which are the first copies of that pixel's row and column --
+// or, with phase_y / phase_x = 1 (a window starting on an odd 2x row / column), the second ones.
 int convert_device(w2x_ctx *ctx, const w2x_model *m, const float *d_in, int w, int h, size_t in_stride_bytes,
-                   int rows_above, int rows_below, float *d_out, size_t out_stride_bytes, int block_splitting, bool up2x = false) {
+                   int rows_above, int rows_below, float *d_out, size_t out_stride_bytes, int block_splitting, bool up2x = false,
+                   int cols_left = 0, int cols_right = 0, int phase_x = 0, int phase_y = 0) {
     DeviceGuard g(ctx->device);
     NvtxRange nvtx("w2x convertWithModels");
     const int engine = pick_engine(ctx, m);
@@ -420,15 +423,20 @@ int convert_device(w2x_ctx *ctx, const w2x_model *m, const float *d_in, int w, i
     // cv::copyMakeBorder(in, temp, n, n, n, n, BORDER_REPLICATE)   (src/convertRoutine.cpp:35, :96): the tensor-core engine folds it
     // into the first layer's loads and reads d_in directly, except on the literal walk, whose blocks are regions of the padded plane
     const bool direct = engine == W2X_ENGINE_TC && !literal;
+    const int px = up2x ? phase_x : 0, cl = std::min(cols_left, n) - px, cr = std::min(cols_right, n);
     float *pad = nullptr;
     if (!direct) {
         rc = ctx->pad_buf.reserve((size_t)pw * ph * sizeof(float));
         if (rc) return rc;
         pad = ctx->pad_buf.get();
-        if (up2x)
-            CU_CHECK(launch_pad_upsample2x(d_in, w, h, istride, n, std::min(rows_above, n), std::min(rows_below, n), pad, ctx->stream));
-        else
-            CU_CHECK(launch_pad_replicate(d_in, w, h, istride, n, std::min(rows_above, n), std::min(rows_below, n), pad, ctx->stream));
+        if (up2x) {
+            const int py = phase_y;
+            CU_CHECK(launch_pad_upsample2x(d_in, w + px, h + py, istride, n, std::min(rows_above, n) - py, std::min(rows_below, n), pad,
+                                           ctx->stream, cl, cr, n - px, n - py));
+        } else {
+            CU_CHECK(launch_pad_replicate(d_in, w, h, istride, n, std::min(rows_above, n), std::min(rows_below, n), pad, ctx->stream, cl,
+                                          cr));
+        }
         ctx->launches++;
     }
     if (literal) {   // check_blocks has seen every block fit
@@ -445,10 +453,11 @@ int convert_device(w2x_ctx *ctx, const w2x_model *m, const float *d_in, int w, i
     const int band = scratch_band_rows(ctx, m, w, h);
     for (int y0 = 0; y0 < h; y0 += band) {
         const int bh = std::min(band, h - y0);
-        // up2x: the band's 2x rows [y0, y0 + bh) seen from source row y0 >> 1; on an odd y0 the band is 2x row 1 of that source row
-        const int p = up2x ? y0 & 1 : 0;
-        const tc::FirstSource src = direct ? tc::FirstSource{d_in + (long)(up2x ? y0 >> 1 : y0) * istride, istride, w, bh + p, n, n - p,
-                                                             std::min(n, y0 + rows_above) - p, std::min(n, h - y0 - bh + rows_below), up2x}
+        // up2x: the band's 2x rows [y0, y0 + bh) seen from source row yy >> 1; on an odd yy the band is 2x row 1 of that source row
+        const int yy = y0 + (up2x ? phase_y : 0), p = up2x ? yy & 1 : 0;
+        const tc::FirstSource src = direct ? tc::FirstSource{d_in + (long)(up2x ? yy >> 1 : y0) * istride, istride, w + px, bh + p, n - px,
+                                                             n - p, std::min(n, y0 + rows_above) - p, std::min(n, h - y0 - bh + rows_below),
+                                                             up2x, cl, cr}
                                            : padded(pad + (long)y0 * pw, pw, pw, bh + 2 * n);
         rc = run_basic(ctx, m, dm, engine, src, pw, bh + 2 * n, d_out + (long)y0 * ostride, ostride);
         if (rc) return rc;
@@ -1906,6 +1915,135 @@ int w2x_convert_chain(w2x_ctx *ctx, int n_steps, const w2x_model *const *models,
     DeviceGuard g(ctx->device);
     NvtxRange nvtx("w2x convert chain");
     return chain_host(ctx, steps, in, width, height, in_stride_bytes, out, out_stride_bytes, block_splitting, on_step, user);
+}
+
+}  // extern "C"
+
+// ---- a window of a chain's output (w2x_convert_chain_region*) ----------------------------------------------------------------
+// Step k converts only its output window wins[k + 1], reading its input window wins[k]: the source rectangle at step 0, else the
+// previous step's output window, dense in chain_buf[(k - 1) & 1].  The window is a plane of its own to convert_device, with the real
+// neighbours its input window holds beyond it as row and column context, so that only the plane's own border is replicated.
+namespace {
+struct Region {
+    std::vector<const w2x_model *> m;
+    std::vector<bool> up;
+    std::vector<Rect> wins;   // region_windows
+};
+
+// Every argument of w2x_convert_chain_region*, before anything is printed, allocated or queued.
+int check_region(const char *fn, w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, int width, int height,
+                 const int *window, const void *src, size_t src_stride_bytes, const void *out, size_t out_stride_bytes, Region *r) {
+    if (check_ctx(ctx)) return W2X_ERR_ARG;
+    int rc = region_windows(fn, n_steps, models, kinds, width, height, window, &r->wins);
+    if (rc) return rc;
+    const Rect &s = r->wins.front(), &o = r->wins.back();
+    if (!src) return fail(W2X_ERR_ARG, "%s: NULL source", fn);
+    if (src_stride_bytes % 4 || src_stride_bytes < (size_t)s.w * 4)
+        return fail(W2X_ERR_ARG, "%s: the source row stride must be a multiple of 4 bytes and >= the source rectangle's row (%d bytes)", fn,
+                    s.w * 4);
+    if (!out) return fail(W2X_ERR_ARG, "%s: NULL output", fn);
+    if (out_stride_bytes % 4 || out_stride_bytes < (size_t)o.w * 4)
+        return fail(W2X_ERR_ARG, "%s: the output row stride must be a multiple of 4 bytes and >= the window's row (%d bytes)", fn, o.w * 4);
+    for (int k = 0; k < n_steps; k++) {
+        if (pick_engine(ctx, models[k]) >= 0) continue;
+        const std::string why = w2x_last_error();
+        return fail(W2X_ERR_UNSUPPORTED, "%s: step %d: %s", fn, k, why.c_str());
+    }
+    r->m.assign(models, models + n_steps);
+    for (int k = 0; k < n_steps; k++) r->up.push_back((kinds[k] & W2X_STEP_UPSCALE2X) != 0);
+    return W2X_OK;
+}
+
+// Every buffer of a region's steps: the models, the chain buffers of the intermediate windows, and the scratch that convert_device
+// and run_basic reserve for a plane the size of each output window (its scratch band's activation frames, and the fp32 engine's
+// padded plane), so that W2X_ERR_NOMEM comes before the first copy or launch.
+int reserve_region(w2x_ctx *ctx, const Region &r) {
+    const size_t last = r.m.size() - 1;
+    size_t need[2] = {0, 0}, act = 0, pad = 0;
+    for (size_t k = 0; k <= last; k++) {
+        const w2x_model *m = r.m[k];
+        DevModel *dm = nullptr;
+        int rc = get_dev_model(ctx, m, &dm);
+        if (rc) return rc;
+        const Rect &o = r.wins[k + 1];
+        const int n = (int)m->layers.size(), pw = o.w + 2 * n;
+        if (k < last) need[k & 1] = std::max(need[k & 1], (size_t)o.w * o.h * sizeof(float));
+        // both engines: 4 bytes per activation element (tc::act_bytes)
+        act = std::max(act, (size_t)max_channels(m) * pw * (scratch_band_rows(ctx, m, o.w, o.h) + 2 * n) * 4);
+        if (pick_engine(ctx, m) == W2X_ENGINE_FP32) pad = std::max(pad, (size_t)pw * (o.h + 2 * n) * sizeof(float));
+        else if ((rc = ensure_tc(ctx))) return rc;
+    }
+    for (int i = 0; i < 2; i++) {
+        if (!need[i]) continue;
+        if (int rc = ctx->chain_buf[i].reserve(need[i])) return rc;
+    }
+    for (int i = 0; i < 2; i++)
+        if (int rc = ctx->buf[i].reserve(act)) return rc;
+    return pad ? ctx->pad_buf.reserve(pad) : W2X_OK;
+}
+
+// The steps of a checked, reserved region on the context's stream: src is the source rectangle, out the window.
+int run_region(w2x_ctx *ctx, const Region &r, const float *src, size_t src_stride, float *out, size_t out_stride, w2x_step_fn on_step,
+               void *user) {
+    const size_t last = r.m.size() - 1;
+    for (size_t k = 0; k <= last; k++) {
+        const w2x_model *m = r.m[k];
+        const Rect &i = r.wins[k], &o = r.wins[k + 1];
+        if (on_step) on_step((int)k, user);
+        emit_plane_progress(ctx, m, o.w, o.h, 0, false);
+        // an upscaling step's window is in 2x pixels: it starts at source pixel (o.y0 >> 1, o.x0 >> 1), on the second copy of that
+        // pixel's row / column when o.y0 / o.x0 is odd, and its input window holds s * i of real 2x pixels
+        const int s = r.up[k] ? 2 : 1;
+        const float *in = reinterpret_cast<const float *>(reinterpret_cast<const char *>(src) + (size_t)(o.y0 / s - i.y0) * src_stride) +
+                          (o.x0 / s - i.x0);
+        float *dst = k == last ? out : ctx->chain_buf[k & 1].get();
+        const size_t dst_stride = k == last ? out_stride : (size_t)o.w * sizeof(float);
+        int rc = convert_device(ctx, m, in, o.w, o.h, src_stride, o.y0 - s * i.y0, s * i.y1() - o.y1(), dst, dst_stride, 0, r.up[k],
+                                o.x0 - s * i.x0, s * i.x1() - o.x1(), o.x0 % s, o.y0 % s);
+        if (rc) return rc;
+        src = dst;
+        src_stride = dst_stride;
+    }
+    return W2X_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int w2x_convert_chain_region(w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, int width, int height,
+                             const int *window, const float *src, size_t src_stride_bytes, float *out, size_t out_stride_bytes,
+                             w2x_step_fn on_step, void *user) {
+    Region r;
+    int rc = check_region("w2x_convert_chain_region", ctx, n_steps, models, kinds, width, height, window, src, src_stride_bytes, out,
+                          out_stride_bytes, &r);
+    if (rc) return rc;
+    DeviceGuard g(ctx->device);
+    NvtxRange nvtx("w2x convert chain region");
+    const Rect &s = r.wins.front(), &o = r.wins.back();
+    const size_t srow = (size_t)s.w * sizeof(float), orow = (size_t)o.w * sizeof(float);
+    rc = reserve_io(ctx, srow * s.h, orow * o.h);
+    if (!rc) rc = reserve_region(ctx, r);
+    if (rc) return rc;
+    float *d_src = ctx->io_buf[0].get(), *d_out = ctx->io_buf[1].get();
+    std::vector<HostGroup> one(1);
+    one[0].up = {{d_src, srow, src, src_stride_bytes, srow, (size_t)s.h}};
+    one[0].compute = [&] { return run_region(ctx, r, d_src, srow, d_out, orow, on_step, user); };
+    one[0].down = {{out, out_stride_bytes, d_out, orow, orow, (size_t)o.h}};
+    return run_host_groups(ctx, one);
+}
+
+int w2x_convert_chain_region_device(w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, int width, int height,
+                                    const int *window, const float *d_src, size_t src_stride_bytes, float *d_out, size_t out_stride_bytes,
+                                    w2x_step_fn on_step, void *user) {
+    Region r;
+    int rc = check_region("w2x_convert_chain_region_device", ctx, n_steps, models, kinds, width, height, window, d_src, src_stride_bytes,
+                          d_out, out_stride_bytes, &r);
+    if (rc) return rc;
+    DeviceGuard g(ctx->device);
+    NvtxRange nvtx("w2x convert chain region");
+    rc = reserve_region(ctx, r);
+    if (rc) return rc;
+    return run_region(ctx, r, d_src, src_stride_bytes, d_out, out_stride_bytes, on_step, user);
 }
 
 }  // extern "C"

@@ -66,7 +66,7 @@ int band_load_rows_from(w2x_band *band, const float *d_in, size_t in_stride_byte
     DeviceGuard g(ctx->device);
     const auto pad = up2x ? launch_pad_upsample2x_xy : launch_pad_replicate_xy;
     CU_CHECK(pad(d_in, band->width, band->rows, (long)(in_stride_bytes / 4), band->n, band->pt, band->pb, band->ov_up ? band->n : 0,
-                 band->ov_down ? band->n : 0, band->pad.get(), ctx->stream, band->up ? 1 : 0, band->down ? 1 : 0));
+                 band->ov_down ? band->n : 0, band->pad.get(), ctx->stream, band->up ? 1 : 0, band->down ? 1 : 0, 0, 0, -1));   // a pointer takes no defaults
     ctx->launches++;
     band->last_step = -1;
     band->cur = 0;

@@ -6,6 +6,7 @@
 // (src/convertRoutine.cpp:100-131 for the input ROI, :143-155 for the output ROI), including the
 // float ceil of :100-105 and the use of blockSize.height for the output column offset at :153-154.
 #include <algorithm>
+#include <climits>
 #include <cmath>
 
 #include "w2x_internal.h"
@@ -97,9 +98,64 @@ int plan_planes(int n, const int *widths, const int *heights, int n_layers, int 
     return (int)fw->size();
 }
 
+int region_windows(const char *fn, int n_steps, const w2x_model *const *models, const int *kinds, int width, int height,
+                   const int *window, std::vector<Rect> *wins) {
+    if (n_steps < 1) return fail(W2X_ERR_ARG, "%s: n_steps is %d: at least one step (step 0) is needed", fn, n_steps);
+    if (!models) return fail(W2X_ERR_ARG, "%s: step 0: NULL models array", fn);
+    if (!kinds) return fail(W2X_ERR_ARG, "%s: step 0: NULL kinds array", fn);
+    long W = width, H = height;
+    for (int k = 0; k < n_steps; k++) {
+        const w2x_model *m = models[k];
+        if (!m) return fail(W2X_ERR_ARG, "%s: step %d: NULL model", fn, k);
+        if (kinds[k] & W2X_STEP_TTA) return fail(W2X_ERR_ARG, "%s: step %d: a W2X_STEP_TTA step has no window form", fn, k);
+        if (kinds[k] & ~W2X_STEP_UPSCALE2X)
+            return fail(W2X_ERR_ARG, "%s: step %d: kind %d is neither W2X_STEP_SAME (0) nor W2X_STEP_UPSCALE2X (1)", fn, k, kinds[k]);
+        if (m->layers.front().n_in != 1 || m->layers.back().n_out != 1)
+            return fail(W2X_ERR_ARG, "%s: step %d: model must map 1 plane to 1 plane", fn, k);
+    }
+    if (width < 1 || height < 1) return fail(W2X_ERR_ARG, "%s: step 0: input size %d x %d", fn, width, height);
+    for (int k = 0; k < n_steps; k++)
+        if (kinds[k] & W2X_STEP_UPSCALE2X) {
+            W *= 2;
+            H *= 2;
+            if (W > INT_MAX || H > INT_MAX) return fail(W2X_ERR_ARG, "%s: step %d: the output size %ld x %ld overflows int", fn, k, W, H);
+        }
+    if (!window) return fail(W2X_ERR_ARG, "%s: NULL window", fn);
+    const Rect o{window[0], window[1], window[2], window[3]};
+    if (o.w < 1 || o.h < 1) return fail(W2X_ERR_ARG, "%s: empty window %d x %d", fn, o.w, o.h);
+    if (o.x0 < 0 || o.y0 < 0 || o.x0 > W - o.w || o.y0 > H - o.h)
+        return fail(W2X_ERR_ARG, "%s: window {%d, %d, %d, %d} is not inside the %ld x %ld output", fn, o.x0, o.y0, o.w, o.h, W, H);
+    wins->assign((size_t)n_steps + 1, o);
+    for (int k = n_steps - 1; k >= 0; k--) {   // (W, H): step k's output plane
+        const Rect &r = (*wins)[(size_t)k + 1];
+        const int n = (int)models[k]->layers.size();
+        int x0 = std::max(0, r.x0 - n), y0 = std::max(0, r.y0 - n);
+        int x1 = (int)std::min<long>(W, (long)r.x1() + n), y1 = (int)std::min<long>(H, (long)r.y1() + n);
+        if (kinds[k] & W2X_STEP_UPSCALE2X) {
+            x0 >>= 1, y0 >>= 1, x1 = (x1 + 1) >> 1, y1 = (y1 + 1) >> 1;
+            W /= 2, H /= 2;
+        }
+        (*wins)[(size_t)k] = Rect{x0, y0, x1 - x0, y1 - y0};
+    }
+    return W2X_OK;
+}
+
 }  // namespace w2x
 
 extern "C" {
+
+int w2x_chain_region_source(int n_steps, const w2x_model *const *models, const int *kinds, int width, int height, const int *window,
+                            int *source) {
+    std::vector<w2x::Rect> wins;
+    int rc = w2x::region_windows("w2x_chain_region_source", n_steps, models, kinds, width, height, window, &wins);
+    if (rc) return rc;
+    if (!source) return w2x::fail(W2X_ERR_ARG, "w2x_chain_region_source: NULL source");
+    source[0] = wins[0].x0;
+    source[1] = wins[0].y0;
+    source[2] = wins[0].w;
+    source[3] = wins[0].h;
+    return W2X_OK;
+}
 
 int w2x_set_jobs(int n_job) {
     if (n_job < 1) return w2x::fail(W2X_ERR_ARG, "w2x_set_jobs: number of jobs must be >= 1");

@@ -8,25 +8,33 @@
 namespace w2x {
 
 // ---- kernels_fp32.cu --------------------------------------------------------------------------
+// cols_left / cols_right (all padding launchers): real columns readable left / right of the plane (windows), read instead of
+// replicating its edge columns, as rows_above / rows_below are for rows.
 cudaError_t launch_pad_replicate(const float *in, int w, int h, long in_stride_floats, int pad, int rows_above,
-                                 int rows_below, float *out, cudaStream_t s);
-// general form: horizontal pad pad_x, vertical pads pad_top / pad_bottom (row-band sessions)
+                                 int rows_below, float *out, cudaStream_t s, int cols_left = 0, int cols_right = 0);
+// general form: left pad pad_x, right pad pad_right (-1: pad_x), vertical pads pad_top / pad_bottom (row-band sessions)
 // skip_top / skip_bottom: frame rows at the top / bottom that are NOT written (a neighbour GPU stores them)
 cudaError_t launch_pad_replicate_xy(const float *in, int w, int h, long in_stride_floats, int pad_x, int pad_top,
                                     int pad_bottom, int rows_above, int rows_below, float *out, cudaStream_t s,
-                                    int skip_top = 0, int skip_bottom = 0);
+                                    int skip_top = 0, int skip_bottom = 0, int cols_left = 0, int cols_right = 0,
+                                    int pad_right = -1);
 // launch_pad_replicate of the nearest-neighbour 2x resize of `in` (pixel (y, x) = in[y >> 1][x >> 1]) without materialising it:
 // w2 x h2 is the 2x plane (or a band of it starting on an even 2x row, `in` pointing at its first source row) and rows_above /
 // rows_below count real 2x rows beyond it.  Writes the dense (w2 + 2 pad) x (h2 + 2 pad) plane.
+// pad_left / pad_top >= 0 replace pad on that side (a window starting on an odd 2x column / row: w2 / h2 then include the 2x
+// column / row before it, which is the first copy of in's column / row 0, and the frame is (w2 + pad_left + pad) wide).
 cudaError_t launch_pad_upsample2x(const float *in, int w2, int h2, long in_stride_floats, int pad, int rows_above, int rows_below,
-                                  float *out, cudaStream_t s);
+                                  float *out, cudaStream_t s, int cols_left = 0, int cols_right = 0, int pad_left = -1,
+                                  int pad_top = -1);
 // The row-band form of launch_pad_upsample2x, with launch_pad_replicate_xy's frame: pixel (fy, fx) of the (w2 + 2 pad_x) x
 // (h2 + pad_top + pad_bottom) frame = in[clamp(fy - pad_top, -rows_above, h2 - 1 + rows_below) >> 1][clamp(fx - pad_x, 0, w2 - 1) >> 1]
 // (>> floors, so with an odd rows_above the first real row above is the SECOND 2x row of its source row).  `in` points at the source
 // row holding 2x row 0 of the band, which is an even 2x row of the plane; rows_above / rows_below count real 2x rows beyond the band;
-// the top skip_top / bottom skip_bottom frame rows are not written (a neighbour GPU stores them).
+// the top skip_top / bottom skip_bottom frame rows are not written (a neighbour GPU stores them); the column clamp is
+// [-cols_left, w2 - 1 + cols_right] and the right pad pad_right (-1: pad_x).
 cudaError_t launch_pad_upsample2x_xy(const float *in, int w2, int h2, long in_stride_floats, int pad_x, int pad_top, int pad_bottom,
-                                     int rows_above, int rows_below, float *out, cudaStream_t s, int skip_top = 0, int skip_bottom = 0);
+                                     int rows_above, int rows_below, float *out, cudaStream_t s, int skip_top = 0, int skip_bottom = 0,
+                                     int cols_left = 0, int cols_right = 0, int pad_right = -1);
 // Peer-memory halo exchange (engine_band.cu): ONE kernel copies up to 8 row segments into the neighbour GPUs' frames,
 // publishes `value` in their flag words once every byte is visible system-wide, then waits until the neighbours have
 // published the same value here.  Flag values only grow, so nothing is ever reset.
@@ -82,15 +90,18 @@ cudaError_t init_kernels();
 // First layer (Cin = 1): same-size 3x3 correlation with BORDER_REPLICATE (src/modelHandler.cpp:141-142) on the frame of pw x ph
 // whose pixel (fy, fx) is the source plane's pixel (clamp(fy - pad_top), clamp(fx - pad_x)) -- i.e. cv::copyMakeBorder
 // (src/convertRoutine.cpp:35,96) is folded into the loads; pad_x = pad_top = 0 with w x h = pw x ph reads an already padded ROI.
-// rows_above / rows_below: real rows readable beyond the plane (row bands).  -> RECORD frame.
-// up2x: the source plane is the nearest-neighbour 2x resize of `in` (pixel (y, x) = in[y >> 1][x >> 1]); w, h, pad_top and the
-// row counts are in 2x rows / columns, `in` points at the source row holding 2x row 0 (see first_layer_kernel).
+// rows_above / rows_below: real rows readable beyond the plane (row bands); cols_left / cols_right: real columns readable beyond
+// it (windows), so that frame column fx reads column clamp(fx - pad_x, -cols_left, w - 1 + cols_right).  pad_x is the LEFT pad:
+// the right pad is pw - w - pad_x, as the bottom pad is ph - h - pad_top.  -> RECORD frame.
+// up2x: the source plane is the nearest-neighbour 2x resize of `in` (pixel (y, x) = in[y >> 1][x >> 1]); w, h, the pads and the
+// row and column counts are in 2x rows / columns, `in` points at the source pixel holding 2x pixel (0, 0) (see first_layer_kernel).
 // `wgt` ([C][9]) and `bias` ((float)bias) are HOST pointers: they travel as kernel parameters.
 struct FirstSource {
     const float *in;
     long stride_floats;
     int w, h, pad_x, pad_top, rows_above, rows_below;
     bool up2x = false;
+    int cols_left = 0, cols_right = 0;
 };
 cudaError_t launch_first(const FirstSource &src, int pw, int ph, const float *wgt /*[C][9]*/, const float *bias, int cout, __half *out,
                          cudaStream_t s, int f8 = 0, int out_y0 = 0, int out_rows = -1);

@@ -25,14 +25,16 @@ __device__ __forceinline__ int row_blocks(int rows, unsigned block_rows) { retur
 
 // ---- cv::copyMakeBorder(BORDER_REPLICATE) (src/convertRoutine.cpp:35,96) ----------------------
 // rows_above/rows_below > 0 mean real neighbour rows exist there (row-band mode): the source
-// pointer addresses band row 0 and may be read at rows [-rows_above, h + rows_below).
+// pointer addresses band row 0 and may be read at rows [-rows_above, h + rows_below); likewise cols_left/cols_right for
+// columns (windows).  pad_x is the left pad, pad_right the right one.
 __global__ void pad_replicate_kernel(const float *__restrict__ in, int w, int h, long in_stride,
                                      int pad_x, int pad_top, int pad_bottom, int rows_above, int rows_below,
-                                     float *__restrict__ out, int skip_top, int skip_bottom) {
-    const int W = w + 2 * pad_x, H = h + pad_top + pad_bottom;
+                                     float *__restrict__ out, int skip_top, int skip_bottom, int pad_right, int cols_left,
+                                     int cols_right) {
+    const int W = w + pad_x + pad_right, H = h + pad_top + pad_bottom;
     const int x = blockIdx.x * blockDim.x + threadIdx.x;
     if (x >= W) return;
-    const int sx = min(max(x - pad_x, 0), w - 1);
+    const int sx = min(max(x - pad_x, -cols_left), w - 1 + cols_right);
     for (int by = blockIdx.y; by < row_blocks(H, blockDim.y); by += gridDim.y) {
         const int y = by * blockDim.y + threadIdx.y;
         if (y >= H - skip_bottom || y < skip_top) continue;
@@ -43,17 +45,19 @@ __global__ void pad_replicate_kernel(const float *__restrict__ in, int w, int h,
 
 // The same padding of the nearest-neighbour 2x resize of `in` (cv::resize INTER_NEAREST to exactly twice the size,
 // src/main.cpp:135-139, whose pixel (y, x) is in[y >> 1][x >> 1]): w2 x h2 are the 2x plane's (or band's) size, the rows count
-// in 2x rows, and the band starts on an even 2x row, so that its first row is the first copy of in's row 0.
+// in 2x rows, and the band starts on an even 2x row, so that its first row is the first copy of in's row 0.  The left and top pads
+// may be smaller than pad (a window starting on an odd 2x column / row), and cols_left / cols_right count real 2x columns.
 __global__ void pad_upsample2x_kernel(const float *__restrict__ in, int w2, int h2, long in_stride, int pad, int rows_above,
-                                      int rows_below, float *__restrict__ out) {
-    const int W = w2 + 2 * pad, H = h2 + 2 * pad;
+                                      int rows_below, float *__restrict__ out, int pad_left, int pad_top, int cols_left,
+                                      int cols_right) {
+    const int W = w2 + pad_left + pad, H = h2 + pad_top + pad;
     const int x = blockIdx.x * blockDim.x + threadIdx.x;
     if (x >= W) return;
-    const int sx = min(max(x - pad, 0), w2 - 1) >> 1;
+    const int sx = min(max(x - pad_left, -cols_left), w2 - 1 + cols_right) >> 1;   // arithmetic shift: floor, also left of the window
     for (int by = blockIdx.y; by < row_blocks(H, blockDim.y); by += gridDim.y) {
         const int y = by * blockDim.y + threadIdx.y;
         if (y >= H) continue;
-        const int sy = min(max(y - pad, -rows_above), h2 - 1 + rows_below) >> 1;   // arithmetic shift: floor, also above the band
+        const int sy = min(max(y - pad_top, -rows_above), h2 - 1 + rows_below) >> 1;   // arithmetic shift: floor, also above the band
         out[(long)y * W + x] = in[(long)sy * in_stride + sx];
     }
 }
@@ -66,15 +70,16 @@ __global__ void pad_upsample2x_kernel(const float *__restrict__ in, int w2, int 
 template <bool VEC>
 __global__ void __launch_bounds__(256) pad_upsample2x_xy_kernel(const float *__restrict__ in, int w2, int h2, long in_stride, int pad_x,
                                                                 int pad_top, int pad_bottom, int rows_above, int rows_below,
-                                                                float *__restrict__ out, int skip_top, int skip_bottom) {
-    const int W = w2 + 2 * pad_x, H = h2 + pad_top + pad_bottom;
+                                                                float *__restrict__ out, int skip_top, int skip_bottom, int pad_right,
+                                                                int cols_left, int cols_right) {
+    const int W = w2 + pad_x + pad_right, H = h2 + pad_top + pad_bottom;
     const int x0 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
     if (x0 >= W) return;
     const int q0 = -((pad_top + 1) >> 1);                  // the pair holding frame row 0 (2x row -pad_top)
     const int pairs = ((h2 + pad_bottom - 1) >> 1) - q0 + 1;
     int sx[4];
 #pragma unroll
-    for (int j = 0; j < 4; j++) sx[j] = min(max(x0 + j - pad_x, 0), w2 - 1) >> 1;
+    for (int j = 0; j < 4; j++) sx[j] = min(max(x0 + j - pad_x, -cols_left), w2 - 1 + cols_right) >> 1;
     for (int by = blockIdx.y; by < row_blocks(pairs, blockDim.y); by += gridDim.y) {
         const int p = by * blockDim.y + threadIdx.y;
         if (p >= pairs) continue;
@@ -300,24 +305,29 @@ conv3x3_planar_fp32(const float *__restrict__ in, float *__restrict__ out,
 static inline dim3 grid2d(int w, int h, dim3 b) { return dim3((w + b.x - 1) / b.x, std::min<unsigned>((h + b.y - 1) / b.y, MAX_GRID_Y)); }
 
 cudaError_t launch_pad_replicate(const float *in, int w, int h, long in_stride_floats, int pad,
-                                 int rows_above, int rows_below, float *out, cudaStream_t s) {
-    return launch_pad_replicate_xy(in, w, h, in_stride_floats, pad, pad, pad, rows_above, rows_below, out, s);
+                                 int rows_above, int rows_below, float *out, cudaStream_t s, int cols_left, int cols_right) {
+    return launch_pad_replicate_xy(in, w, h, in_stride_floats, pad, pad, pad, rows_above, rows_below, out, s, 0, 0, cols_left, cols_right);
 }
 
 cudaError_t launch_pad_replicate_xy(const float *in, int w, int h, long in_stride_floats, int pad_x, int pad_top,
                                     int pad_bottom, int rows_above, int rows_below, float *out, cudaStream_t s,
-                                    int skip_top, int skip_bottom) {
+                                    int skip_top, int skip_bottom, int cols_left, int cols_right, int pad_right) {
+    if (pad_right < 0) pad_right = pad_x;
     dim3 b(32, 8);
-    pad_replicate_kernel<<<grid2d(w + 2 * pad_x, h + pad_top + pad_bottom, b), b, 0, s>>>(
-        in, w, h, in_stride_floats, pad_x, pad_top, pad_bottom, rows_above, rows_below, out, skip_top, skip_bottom);
+    pad_replicate_kernel<<<grid2d(w + pad_x + pad_right, h + pad_top + pad_bottom, b), b, 0, s>>>(
+        in, w, h, in_stride_floats, pad_x, pad_top, pad_bottom, rows_above, rows_below, out, skip_top, skip_bottom, pad_right,
+        cols_left, cols_right);
     return cudaGetLastError();
 }
 
 cudaError_t launch_pad_upsample2x(const float *in, int w2, int h2, long in_stride_floats, int pad, int rows_above, int rows_below,
-                                  float *out, cudaStream_t s) {
+                                  float *out, cudaStream_t s, int cols_left, int cols_right, int pad_left, int pad_top) {
+    if (pad_left < 0) pad_left = pad;
+    if (pad_top < 0) pad_top = pad;
     dim3 b(32, 8);
-    pad_upsample2x_kernel<<<grid2d(w2 + 2 * pad, h2 + 2 * pad, b), b, 0, s>>>(in, w2, h2, in_stride_floats, pad, rows_above,
-                                                                               rows_below, out);
+    pad_upsample2x_kernel<<<grid2d(w2 + pad_left + pad, h2 + pad_top + pad, b), b, 0, s>>>(in, w2, h2, in_stride_floats, pad, rows_above,
+                                                                                          rows_below, out, pad_left, pad_top, cols_left,
+                                                                                          cols_right);
     return cudaGetLastError();
 }
 
@@ -325,16 +335,18 @@ cudaError_t launch_pad_upsample2x(const float *in, int w2, int h2, long in_strid
 // of the one-GPU chain) is deliberately not done: the frame is 4 bytes per pixel beside 512 bytes per pixel of activations, and the
 // fold would need the halo exchange to deliver half-resolution rows into a side buffer instead of a row of the frame.
 cudaError_t launch_pad_upsample2x_xy(const float *in, int w2, int h2, long in_stride_floats, int pad_x, int pad_top, int pad_bottom,
-                                     int rows_above, int rows_below, float *out, cudaStream_t s, int skip_top, int skip_bottom) {
-    const int W = w2 + 2 * pad_x, pairs = ((h2 + pad_bottom - 1) >> 1) + ((pad_top + 1) >> 1) + 1;
+                                     int rows_above, int rows_below, float *out, cudaStream_t s, int skip_top, int skip_bottom,
+                                     int cols_left, int cols_right, int pad_right) {
+    if (pad_right < 0) pad_right = pad_x;
+    const int W = w2 + pad_x + pad_right, pairs = ((h2 + pad_bottom - 1) >> 1) + ((pad_top + 1) >> 1) + 1;
     dim3 b(32, 8);
     const dim3 g = grid2d((W + 3) / 4, pairs, b);
     if (W % 4 == 0 && reinterpret_cast<uintptr_t>(out) % 16 == 0)
         pad_upsample2x_xy_kernel<true><<<g, b, 0, s>>>(in, w2, h2, in_stride_floats, pad_x, pad_top, pad_bottom, rows_above, rows_below, out,
-                                                       skip_top, skip_bottom);
+                                                       skip_top, skip_bottom, pad_right, cols_left, cols_right);
     else
         pad_upsample2x_xy_kernel<false><<<g, b, 0, s>>>(in, w2, h2, in_stride_floats, pad_x, pad_top, pad_bottom, rows_above, rows_below, out,
-                                                        skip_top, skip_bottom);
+                                                        skip_top, skip_bottom, pad_right, cols_left, cols_right);
     return cudaGetLastError();
 }
 

@@ -155,7 +155,7 @@ static cudaError_t launch_first_c(const FirstSource &src, int pw, int ph, const 
         for (int k = 0; k < 9; k++) prm.w[p * 9 + k] = make_float2(wgt[(2 * p) * 9 + k] * ACT_SCALE, wgt[(2 * p + 1) * 9 + k] * ACT_SCALE);
         prm.b[p] = make_float2(bias[2 * p] * ACT_SCALE, bias[2 * p + 1] * ACT_SCALE);
     }
-    FirstSrc fs{src.in, src.stride_floats, src.w, src.h, src.pad_x, src.pad_top, src.rows_above, src.rows_below};
+    FirstSrc fs{src.in, src.stride_floats, src.w, src.h, src.pad_x, src.pad_top, src.rows_above, src.rows_below, src.cols_left, src.cols_right};
     CUtensorMap omap;
     dim3 grid((pw + 31) / 32, (out_rows + 7) / 8);   // blocks tile the store window
     if (grid.y > 65535) return cudaErrorInvalidConfiguration;

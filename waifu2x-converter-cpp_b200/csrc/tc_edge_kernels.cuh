@@ -29,17 +29,19 @@ __device__ __forceinline__ float2 f32x2_fma(float2 a, float2 b, float2 c) { retu
 __device__ __forceinline__ float2 f32x2_mul(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 __device__ __forceinline__ float2 f32x2_add(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 
-// in: plane of w x h (row stride in_stride), readable at rows [-rows_above, h + rows_below); frame = (w + 2 pad_x) x (h + pad_top + pad_bottom)
+// in: plane of w x h (row stride in_stride), readable at rows [-rows_above, h + rows_below) and columns [-cols_left, w + cols_right);
+// frame pixel (fy, fx) reads the plane at (fy - pad_top, fx - pad_x) clamped to that readable rectangle
 struct FirstSrc {
     const float *in;
     long in_stride;
-    int w, h, pad_x, pad_top, rows_above, rows_below;
+    int w, h, pad_x, pad_top, rows_above, rows_below, cols_left, cols_right;
 };
 
 // UP2X: the plane of w x h the frame pads is the nearest-neighbour 2x resize of `in` (cv::resize INTER_NEAREST to exactly twice
 // the size, src/main.cpp:135-139), never materialised: its pixel (y, x) is in[y >> 1][x >> 1].  Row 0 of that virtual plane is the
 // first copy of in's row 0, so a band starting on an odd 2x row has pad_top one smaller, rows_above one smaller and h one larger
-// than its even-row neighbour would (tc::FirstSource::up2x, set up by the engine).
+// than its even-row neighbour would (tc::FirstSource::up2x, set up by the engine); a window starting on an odd 2x column likewise
+// has pad_x and cols_left one smaller and w one larger.
 template <int COUT, bool F8, bool UP2X>
 __global__ void __launch_bounds__(256, 4)
 first_layer_kernel(const FirstSrc src, int pw, int ph, int out_y0, const __grid_constant__ CUtensorMap tmap_out,
@@ -56,8 +58,8 @@ first_layer_kernel(const FirstSrc src, int pw, int ph, int out_y0, const __grid_
             // same-size correlation on the padded plane with BORDER_REPLICATE (src/modelHandler.cpp:141-142), the padded plane itself
             // being the replicate-padded input: clamp to the frame, then to the rows / columns that really exist
             const int fy = min(max(y + ky - 1, 0), ph - 1), fx = min(max(x + kx - 1, 0), pw - 1);
-            const int sy = min(max(fy - src.pad_top, -src.rows_above), src.h - 1 + src.rows_below), sx = min(max(fx - src.pad_x, 0), src.w - 1);
-            const int ry = UP2X ? sy >> 1 : sy, rx = UP2X ? sx >> 1 : sx;   // arithmetic shift: floor, also for the rows above
+            const int sy = min(max(fy - src.pad_top, -src.rows_above), src.h - 1 + src.rows_below), sx = min(max(fx - src.pad_x, -src.cols_left), src.w - 1 + src.cols_right);
+            const int ry = UP2X ? sy >> 1 : sy, rx = UP2X ? sx >> 1 : sx;   // arithmetic shift: floor, also above and to the left
             v[ky * 3 + kx] = __ldg(src.in + (long)ry * src.in_stride + rx);
         }
     const uint32_t r = (uint32_t)threadIdx.x;                            // pixel index inside the block = row of the staged image

@@ -74,4 +74,17 @@ int block_table(int w, int h, int bw, int bh, int n_model, int *table, int capac
 // receive the frame sizes.
 int plan_planes(int n, const int *widths, const int *heights, int n_layers, int max_channels, size_t scratch_limit, int *frame,
                 int *x0, int *y0, std::vector<int> *fw, std::vector<int> *fh);
+// A rectangle {x0, y0, w, h} of a plane.
+struct Rect {
+    int x0, y0, w, h;
+    int x1() const { return x0 + w; }
+    int y1() const { return y0 + h; }
+};
+// The windows a chain region reads and writes, after checking every argument that needs no context (W2X_ERR_ARG naming the step
+// or the problem, `fn` first): (*wins)[k + 1] is step k's output window, on that step's output plane, and (*wins)[k] its input
+// window on its input plane -- (*wins)[0] the source rectangle, the last entry `window`.  A step's input window is its output
+// window grown by the model's layer count on every side and clamped to the step's plane, then, for an upscaling step, halved
+// (floor at the top-left, ceil at the bottom-right).
+int region_windows(const char *fn, int n_steps, const w2x_model *const *models, const int *kinds, int width, int height,
+                   const int *window, std::vector<Rect> *wins);
 }  // namespace w2x
