@@ -168,6 +168,10 @@ W2X_API void *w2x_host_alloc(size_t bytes);
 W2X_API void w2x_host_free(void *p);
 
 /* ---- the hot path ------------------------------------------------------------------------- */
+/* Device memory of w2x_convert_plane*, w2x_convert_planes*, w2x_convert_chain*, w2x_convert_planes_chain* and
+ * w2x_convert_chain_region*: every buffer a call uses (the host entries' staging, the planes between steps, TTA variants, packed
+ * frames, activation and padding scratch) is reserved before its first progress line, on_step call, copy or launch, so
+ * W2X_ERR_NOMEM leaves nothing logged, called back or queued.  The context keeps its buffers for later calls. */
 /* Replaces bool w2xc::convertWithModels(cv::Mat& in, cv::Mat& out, models, bool blockSplitting)
  * (src/convertRoutine.hpp:25-28, src/convertRoutine.cpp:21-51): out = crop_n(L_{n-1}(...L_0(
  * replicate_pad_n(in)))) with every layer = 3x3 correlation + bias + leaky-ReLU(0.1).
@@ -337,8 +341,7 @@ W2X_API int w2x_convert_planes_device(w2x_ctx *ctx, const w2x_model *model, int 
  * transforms the half-resolution plane and never builds the 2x one.  w2x_convert_planes_chain* packs the 8n variants of its n
  * planes into frames; w2x_convert_chain* converts each variant alone with the caller's block_splitting.  A TTA step logs the lines
  * of the same step without the flag, and launches what the plain step launches on the 8n variant planes, plus 2 (building the
- * variants, and the mean).  Its buffers (the 8 variants of every plane, their 8 outputs, the frame scratch) are reserved before
- * the first copy or launch, like every other buffer of the call. */
+ * variants, and the mean). */
 #define W2X_STEP_TTA 4
 typedef void (*w2x_step_fn)(int step, void *user);
 W2X_API int w2x_convert_chain(w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds,
@@ -371,7 +374,7 @@ W2X_API int w2x_chain_region_source(int n_steps, const w2x_model *const *models,
  * Every argument is checked before anything is printed, allocated or queued: W2X_ERR_ARG names the step or the problem (the
  * checks of w2x_convert_chain, a W2X_STEP_TTA step, a NULL or empty window or one outside the output, NULL planes, row strides
  * that are not multiples of 4 bytes or shorter than the rectangle's / window's row); W2X_ERR_UNSUPPORTED a model the context's
- * engine refuses.  Every buffer is reserved before the first copy or launch, so W2X_ERR_NOMEM leaves nothing queued.
+ * engine refuses.
  * HOST buffers, synchronous. */
 W2X_API int w2x_convert_chain_region(w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, int width,
                                      int height, const int *window, const float *src, size_t src_stride_bytes, float *out,
@@ -399,7 +402,6 @@ W2X_API int w2x_convert_chain_region_device(w2x_ctx *ctx, int n_steps, const w2x
  * outputs (as in w2x_convert_planes).
  * Device memory: two buffers of the context, each holding one step's outputs for the whole collection (only with 2 steps and
  * more), plus the frame scratch of w2x_convert_planes; the host entry also stages every input and every output plane on the device.
- * All of it is reserved before the first copy or launch: W2X_ERR_NOMEM leaves nothing queued.
  * HOST buffers, synchronous; uploads overlap the first step and downloads the last. */
 W2X_API int w2x_convert_planes_chain(w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, int n_planes,
                                      const float *const *in, const int *widths, const int *heights, const size_t *in_strides,

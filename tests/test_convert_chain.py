@@ -6,7 +6,7 @@ resized with np.repeat(np.repeat(y, 2, 0), 2, 1) first for an upscaling step -- 
 1 -> C1 -> C2 -> 1 models, on sizes from 1 x 1 to planes the reference block-splits, through both entry points with strided planes,
 on the fp32 engine, the literal block walk and the fuse-off probe, with small scratch limits (bands starting on odd and even 2x
 rows), on a plane whose 2x output is taller than one frame, and on a torch stream.  Also: each step against the CPU oracle, launch
-counts and kernel names, the progress lines and callbacks, argument errors, and the CLI (pixels and stdout).
+counts and kernel names, the progress lines and callbacks, argument errors, W2X_ERR_NOMEM, and the CLI (pixels and stdout).
 """
 import ctypes as C
 import os
@@ -21,6 +21,7 @@ from test_gpu_parity import TC_TOL
 pytestmark = pytest.mark.gpu
 
 PRECISIONS = [0, 1, 2]   # f16x3, f16+f8x2, f16
+ERR_NOMEM = 8
 SIZES = [(1, 1), (1, 300), (300, 1), (15, 13), (45, 33), (443, 443), (700, 300)]   # (w, h); 443 x 443 is split once doubled
 PATTERNS = ["U", "SU", "UU", "SUU", "US"]
 CLI = os.path.join(ROOT, "waifu2x-converter-cpp_b200", "w2x-converter")
@@ -338,6 +339,62 @@ def test_argument_errors_name_the_step(w2x, ctx, shipped):
     with pytest.raises(w2x.W2xError) as e:
         ctx.convert_chain_device([(noise, False), (None, True)], 1 << 20, 8, 8, 32, 1 << 21, 64)
     assert e.value.status == 1 and "step 1" in e.value.message
+
+
+def act_bytes(om, w, h):
+    """one activation frame of a w x h plane converted in one band: the model's widest layer x the padded plane x 4 bytes"""
+    n = len(om.weights)
+    return max(max(wt.shape[:2]) for wt in om.weights) * (w + 2 * n) * (h + 2 * n) * 4
+
+
+@pytest.mark.parametrize("case", ["tc", "fp32", "later_step"])
+def test_out_of_memory_leaves_nothing_queued(w2x, shipped, oracle_models, oracle_mod, case):
+    """W2X_ERR_NOMEM comes before any on_step call, progress line, copy or launch: with the device all but full (both engines, both
+    entries), and with room for step 0's activation frames but not for step 1's larger ones (the device entry)"""
+    import torch
+    c = w2x.Context(0, engine=w2x.ENGINE_FP32 if case == "fp32" else w2x.ENGINE_TC)
+    filler = None
+    try:
+        steps = [(shipped["noise1"], False), (shipped["scale2.0x"], True)]
+        c.convert_chain(steps, plane(oracle_mod, 16, 16, 1))      # the models' device copies and small buffers exist
+        w = h = 1024 if case == "later_step" else 2048
+        x = plane(oracle_mod, w, h, 2)
+        out = np.full((2 * h, 2 * w), -3.25, np.float32)
+        d_in = torch.from_numpy(x).cuda()
+        d_out = torch.full((2 * h, 2 * w), -3.25, device="cuda")
+        leave = (w * h + 4 * w * h + w * h) * 4 + (256 << 20)       # the host entry's staging and step 0's output plane
+        if case == "later_step":
+            step0, step1 = act_bytes(oracle_models["noise1"], w, h), act_bytes(oracle_models["scale2.0x"], 2 * w, 2 * h)
+            leave += 2 * step0
+            assert step1 > leave - step0, (step0, step1)             # a frame of step 1 does not fit beside one of step 0
+        torch.cuda.synchronize()
+        free, _ = torch.cuda.mem_get_info()
+        filler = torch.empty(max(free - leave, 0), dtype=torch.uint8, device="cuda")
+        torch.cuda.synchronize()
+        lines, calls = [], []
+        c.set_log(lines.append)
+        n0 = c.launch_count()
+        for entry in ["device"] + (["host"] if case != "later_step" else []):
+            with pytest.raises(w2x.W2xError) as e:
+                if entry == "device":
+                    c.convert_chain_device(steps, d_in.data_ptr(), w, h, w * 4, d_out.data_ptr(), 2 * w * 4, on_step=calls.append)
+                else:
+                    c.convert_chain(steps, x, out=out, on_step=calls.append)
+            assert e.value.status == ERR_NOMEM, (entry, e.value.message)
+            assert c.launch_count() == n0 and not calls and not lines, (entry, c.launch_count() - n0, calls, lines[:2])
+        c.synchronize()
+        del filler
+        filler = None
+        torch.cuda.empty_cache()
+        assert (out == -3.25).all() and (d_out == -3.25).all().item()
+        c.convert_chain_device(steps, d_in.data_ptr(), w, h, w * 4, d_out.data_ptr(), 2 * w * 4)   # with the memory back, it runs
+        c.synchronize()
+        assert not (d_out == -3.25).all().item()
+    finally:
+        c.set_log(None)
+        del filler
+        torch.cuda.empty_cache()
+        c.close()
 
 
 # ---- the CLI ----------------------------------------------------------------------------------------------------------------

@@ -6,7 +6,8 @@ Every output is checked bit for bit (np.array_equal) against the per-plane conve
 per-step loop of convert_planes on the resized planes: in all three precisions, on patterns U, SU, UU, SUU and US, with the shipped
 models and random 1 -> C1 -> C2 -> 1 models of different widths, on collections of 1 to 300 planes with sides from 1 to 160.  Also:
 plans that change between steps, both entry points with strided planes and a torch stream, the fp32 engine and the fuse-off probe,
-the one-step case against convert_planes, launch counts, on_step calls and progress lines, rejected calls, and the CPU oracle.
+the one-step case against convert_planes, launch counts, on_step calls and progress lines, rejected calls, W2X_ERR_NOMEM, and the CPU
+oracle.
 """
 import ctypes as C
 
@@ -24,7 +25,7 @@ PRECISIONS = [0, 1, 2]   # f16x3, f16+f8x2, f16
 PATTERNS = ["U", "SU", "UU", "SUU", "US"]
 EDGES = [(1, 1), (1, 37), (37, 1), (1, 160), (160, 1), (160, 160), (15, 13)]
 COUNTS = {"U": 1, "SU": 7, "UU": 60, "SUU": 300, "US": 25}   # planes per collection
-ERR_ARG, ERR_UNSUPPORTED = 1, 7
+ERR_ARG, ERR_UNSUPPORTED, ERR_NOMEM = 1, 7, 8
 STEP_FN = C.CFUNCTYPE(None, C.c_int, C.c_void_p)
 
 
@@ -341,6 +342,39 @@ def test_rejected_calls(w2x, ctx, shipped):
     assert all((o == sentinel).all() for o in outs)
     assert all(bool((d == float(sentinel)).all()) for d in d_out)
     assert call(True) == 0 and call(False) == 0      # the same arguments, unbroken, go through
+
+
+def test_out_of_memory_leaves_nothing_queued(w2x, shipped, oracle_mod):
+    """with the device all but full, a collection whose frame has its buffers already but whose plane converted alone cannot reserve
+    its scratch returns W2X_ERR_NOMEM before any on_step call, progress line or launch, the frame's included"""
+    c = w2x.Context(0, engine=w2x.ENGINE_TC)
+    filler = None
+    try:
+        steps = [(shipped["noise1"], False)]
+        c.set_scratch_limit(256 << 20)      # frames of at most 256 MiB / (128 channels x 4 bytes) = 512 Ki pixels
+        small, large = planes_for(oracle_mod, [(64, 64), (1024, 1024)], 7)   # padded 78 x 78 packs, 1038 x 1038 does not
+        device_chain(c, steps, [small])     # the model's device copy and the frame's buffers exist
+        d_in = dev([small, large])
+        d_out = [torch.full(x.shape, -3.25, device="cuda") for x in (small, large)]
+        torch.cuda.synchronize()
+        free, _ = torch.cuda.mem_get_info()
+        filler = torch.empty(max(free - (64 << 20), 0), dtype=torch.uint8, device="cuda")
+        torch.cuda.synchronize()
+        lines, calls = [], []
+        c.set_log(lines.append)
+        n0 = c.launch_count()
+        with pytest.raises(w2x.W2xError) as e:
+            c.convert_planes_chain_device(steps, ptrs(d_in), [64, 1024], [64, 1024], [64 * 4, 1024 * 4], ptrs(d_out), [64 * 4, 1024 * 4],
+                                          calls.append)
+        assert e.value.status == ERR_NOMEM, e.value.message
+        assert c.launch_count() == n0 and not calls and not lines
+        c.synchronize()
+        assert all(bool((d == -3.25).all()) for d in d_out)
+    finally:
+        c.set_log(None)
+        del filler
+        torch.cuda.empty_cache()
+        c.close()
 
 
 def test_against_the_oracle(ctx, shipped, oracle_models, oracle_mod):

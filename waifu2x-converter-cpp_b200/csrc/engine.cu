@@ -402,6 +402,25 @@ void emit_plane_progress(w2x_ctx *ctx, const w2x_model *m, int w, int h, int blo
     for (int p = 0; p < passes; p++) emit_reference_progress(ctx, w, h, n, false);
 }
 
+// The scratch of a convert_device call on a w x h plane, reserved: the two activation frames of its largest scratch band (on the
+// literal walk, of its largest reference block), the padded plane unless the first layer reads the plane directly, and the
+// tensor-core kernels.  An upscaling call's plane is its 2x size; the resize changes none of it.
+int reserve_convert(w2x_ctx *ctx, const w2x_model *m, int engine, int w, int h, int block_splitting) {
+    const int n = (int)m->layers.size(), maxc = max_channels(m), pw = w + 2 * n;
+    const bool literal = literal_walk(ctx, w, h, block_splitting);
+    size_t act = 0;   // both engines: 4 bytes per activation element
+    if (literal) {
+        const std::vector<int> tab = blocks_of(w, h, n);
+        for (size_t i = 0; i < tab.size(); i += 8) act = std::max(act, tc::act_bytes(maxc, tab[i + 5] - tab[i + 4], tab[i + 3] - tab[i + 2]));
+    } else {
+        act = tc::act_bytes(maxc, pw, scratch_band_rows(ctx, m, w, h) + 2 * n);
+    }
+    int rc = engine == W2X_ENGINE_TC ? ensure_tc(ctx) : W2X_OK;
+    for (int i = 0; i < 2 && !rc; i++) rc = ctx->buf[i].reserve(act);
+    if (!rc && (engine != W2X_ENGINE_TC || literal)) rc = ctx->pad_buf.reserve((size_t)pw * (h + 2 * n) * sizeof(float));
+    return rc;
+}
+
 // convertWithModels on checked device buffers (rows_above / rows_below: real neighbour rows available around the band;
 // cols_left / cols_right: real neighbour columns left and right of it, for a window).  up2x: the plane converted is the
 // nearest-neighbour 2x resize of d_in, never materialised; w x h is its (2x) size, the row and column counts are in 2x pixels, and
@@ -415,20 +434,18 @@ int convert_device(w2x_ctx *ctx, const w2x_model *m, const float *d_in, int w, i
     const int engine = pick_engine(ctx, m);
     DevModel *dm = nullptr;
     int rc = get_dev_model(ctx, m, &dm);
+    if (!rc) rc = reserve_convert(ctx, m, engine, w, h, block_splitting);
     if (rc) return rc;
     const int n = (int)m->layers.size();
-    const int pw = w + 2 * n, ph = h + 2 * n;
+    const int pw = w + 2 * n;
     const long istride = (long)(in_stride_bytes / 4), ostride = (long)(out_stride_bytes / 4);
     const bool literal = literal_walk(ctx, w, h, block_splitting);
     // cv::copyMakeBorder(in, temp, n, n, n, n, BORDER_REPLICATE)   (src/convertRoutine.cpp:35, :96): the tensor-core engine folds it
     // into the first layer's loads and reads d_in directly, except on the literal walk, whose blocks are regions of the padded plane
     const bool direct = engine == W2X_ENGINE_TC && !literal;
     const int px = up2x ? phase_x : 0, cl = std::min(cols_left, n) - px, cr = std::min(cols_right, n);
-    float *pad = nullptr;
+    float *pad = direct ? nullptr : ctx->pad_buf.get();
     if (!direct) {
-        rc = ctx->pad_buf.reserve((size_t)pw * ph * sizeof(float));
-        if (rc) return rc;
-        pad = ctx->pad_buf.get();
         if (up2x) {
             const int py = phase_y;
             CU_CHECK(launch_pad_upsample2x(d_in, w + px, h + py, istride, n, std::min(rows_above, n) - py, std::min(rows_below, n), pad,
@@ -1012,13 +1029,21 @@ std::vector<FramePlan> frames_for(const PlanesPlan &p) {
 }
 
 // One step of a chain (w2x_convert_chain*, w2x_convert_planes*): every plane through one model, after the nearest 2x resize when
-// `up`.  A single-plane chain is a collection of one plane.
-struct PlaneIO { const float *src; size_t src_stride; float *dst; size_t dst_stride; };   // row strides in bytes
+// `up`.  A single-plane chain is a collection of one plane.  A step converts a window of each plane: the whole plane, except in the
+// region calls, which have no TTA step and never pack.
+// Where a plane comes from and goes to (row strides in bytes), and for a plane converted alone, convert_device's context around its
+// window (rows_above ... phase_y, all 0 for a whole plane).
+struct PlaneIO {
+    const float *src; size_t src_stride; float *dst; size_t dst_stride;
+    int above = 0, below = 0, left = 0, right = 0, phase_x = 0, phase_y = 0;
+};
 struct Step {
     const w2x_model *m;
     bool up;
     bool tta = false;                   // W2X_STEP_TTA: the model runs on the 8 variants of every plane, the mean is the output
-    std::vector<int> w, h;              // the step's output sizes
+    std::vector<int> w, h;              // the step's output sizes: of each plane's output window
+    std::vector<int> x0, y0;            // where each output window starts on the step's output plane
+    std::vector<Rect> in;               // each plane's input window on the step's input plane: what its source holds
     DevModel *dm = nullptr;
     bool packed = false;                // packs_frames: frames plus planes too large to pack, else every plane alone
     PlanesPlan plan;                    // packed: each converted plane's frame (-1: converted alone) and place
@@ -1046,10 +1071,12 @@ std::vector<Step> step_table(int n_steps, const w2x_model *const *models, const 
         s.m = models[k];
         s.up = (kinds[k] & W2X_STEP_UPSCALE2X) != 0;
         s.tta = (kinds[k] & W2X_STEP_TTA) != 0;
+        for (int i = 0; i < n_planes; i++) s.in.push_back(Rect{0, 0, w[(size_t)i], h[(size_t)i]});
         if (s.up)
             for (int i = 0; i < n_planes; i++) w[(size_t)i] *= 2, h[(size_t)i] *= 2;
         s.w = w;
         s.h = h;
+        s.x0 = s.y0 = std::vector<int>((size_t)n_planes, 0);
         for (int i = 0; i < n_planes && s.tta; i++)
             for (int j = 0; j < 8; j++) {
                 s.vof.push_back(8 * i + j);
@@ -1121,6 +1148,7 @@ struct Part {
     std::vector<FramePlan> frames;   // prepare_parts' working state
     Tables tables;
     size_t n_tta = 0;
+    int band_rows = 0;               // > 0: the last step's one plane is converted in row bands of at most this many rows (chain_host)
 };
 
 // Part p's steps: the call's steps on its planes, a TTA step's variants restricted to vof[k] (8 i + j each, ascending).
@@ -1135,6 +1163,9 @@ std::vector<Step> part_steps(const std::vector<Step> &all, const std::vector<int
         for (int i : own) {
             s.w.push_back(a.w[(size_t)i]);
             s.h.push_back(a.h[(size_t)i]);
+            s.x0.push_back(a.x0[(size_t)i]);
+            s.y0.push_back(a.y0[(size_t)i]);
+            s.in.push_back(a.in[(size_t)i]);
         }
         for (int v : vof[k]) {
             s.vof.push_back(v);
@@ -1146,12 +1177,14 @@ std::vector<Step> part_steps(const std::vector<Step> &all, const std::vector<int
 }
 
 // The first half of prepare_parts on one part: every device buffer and the model copies, where each plane and variant lives.  Its
-// planes come from and go to: step 0 reads ends[i].src, the last step writes ends[i].dst, step k < last writes its outputs densely into
-// chain_buf[k & 1]; a TTA step's variants (an upscaling step's are those of its half-resolution sources: the nearest 2x resize
-// commutes with every flip and transpose) lie dense in tta_buf[0] in vof order, their outputs dense in tta_buf[1].  With `pack`, each
-// step that packs_frames allows is planned into frames on its OUTPUT sizes, so that a plane may pack at one step and be converted
-// alone after a 2x step (without, every plane is converted alone); a TTA step's frames are planned on the variants it converts.
-int reserve_part(Part &P, bool pack) {
+// planes come from and go to: step 0 reads ends[i].src, the last step writes ends[i].dst, step k < last writes its outputs (output
+// windows) densely into chain_buf[k & 1]; a TTA step's variants (an upscaling step's are those of its half-resolution sources: the
+// nearest 2x resize commutes with every flip and transpose) lie dense in tta_buf[0] in vof order, their outputs dense in tta_buf[1].
+// With `pack`, each step that packs_frames allows is planned into frames on its OUTPUT sizes, so that a plane may pack at one step and
+// be converted alone after a 2x step (without, every plane is converted alone); a TTA step's frames are planned on the variants it
+// converts.  Every plane or variant converted alone gets the scratch of its convert_device call (reserve_convert, with the call's
+// block_splitting), so that the call's own reservations find it there.
+int reserve_part(Part &P, bool pack, int block_splitting) {
     w2x_ctx *ctx = P.ctx;
     DeviceGuard g(ctx->device);
     std::vector<Step> &steps = P.steps;
@@ -1185,15 +1218,23 @@ int reserve_part(Part &P, bool pack) {
         Step &s = steps[k];
         int rc = get_dev_model(ctx, s.m, &s.dm);
         if (rc) return rc;
-        s.packed = pack && !s.cw().empty() && packs_frames(ctx, s.m, s.dm, pick_engine(ctx, s.m));
+        const int engine = pick_engine(ctx, s.m), u = s.up ? 2 : 1;
+        s.packed = pack && !s.cw().empty() && packs_frames(ctx, s.m, s.dm, engine);
         s.io.resize(n_planes);
         size_t off = 0;
         for (size_t i = 0; i < n_planes; i++) {
+            // the source holds the input window, and the output window starts at its source pixel (o.y0 / u, o.x0 / u)
+            const Rect &in = s.in[i];
+            const Rect o{s.x0[i], s.y0[i], s.w[i], s.h[i]};
             PlaneIO &p = s.io[i];
-            p.src = k == 0 ? P.ends[i].src : steps[k - 1].io[i].dst;
+            const char *src = reinterpret_cast<const char *>(k == 0 ? P.ends[i].src : steps[k - 1].io[i].dst);
             p.src_stride = k == 0 ? P.ends[i].src_stride : steps[k - 1].io[i].dst_stride;
+            p.src = reinterpret_cast<const float *>(src + (size_t)(o.y0 / u - in.y0) * p.src_stride) + (o.x0 / u - in.x0);
             p.dst = k == last ? P.ends[i].dst : ctx->chain_buf[k & 1].get() + off;
             p.dst_stride = k == last ? P.ends[i].dst_stride : (size_t)s.w[i] * sizeof(float);
+            p.above = o.y0 - u * in.y0, p.below = u * in.y1() - o.y1();
+            p.left = o.x0 - u * in.x0, p.right = u * in.x1() - o.x1();
+            p.phase_x = o.x0 % u, p.phase_y = o.y0 % u;
             off += (size_t)s.w[i] * s.h[i];
         }
         if (s.tta) {
@@ -1208,20 +1249,26 @@ int reserve_part(Part &P, bool pack) {
             }
             P.n_tta += 2 * n_planes;   // the variants and the mean kernel's rows of the planes it owns
         }
-        if (!s.packed) continue;
         const std::vector<int> &cw = s.cw(), &ch = s.ch();
         const std::vector<PlaneIO> &cio = s.cio();
-        plan_for(ctx, s.m, (int)cw.size(), cw.data(), ch.data(), &s.plan);
-        s.f0 = P.frames.size();
-        for (FramePlan &f : frames_for(s.plan)) P.frames.push_back(std::move(f));
-        for (size_t i = 0; i < cw.size(); i++) {
-            const int f = s.plan.frame[i];
-            if (f >= 0)
-                P.frames[s.f0 + (size_t)f].rect.push_back(tc::PlaneRect{cio[i].src, cio[i].dst, (long)(cio[i].src_stride / 4), (long)(cio[i].dst_stride / 4),
-                                                                        cw[i], ch[i], s.plan.x0[i], s.plan.y0[i], 0});
+        if (s.packed) {
+            plan_for(ctx, s.m, (int)cw.size(), cw.data(), ch.data(), &s.plan);
+            s.f0 = P.frames.size();
+            for (FramePlan &f : frames_for(s.plan)) P.frames.push_back(std::move(f));
+            for (size_t i = 0; i < cw.size(); i++) {
+                const int f = s.plan.frame[i];
+                if (f >= 0)
+                    P.frames[s.f0 + (size_t)f].rect.push_back(tc::PlaneRect{cio[i].src, cio[i].dst, (long)(cio[i].src_stride / 4),
+                                                                            (long)(cio[i].dst_stride / 4), cw[i], ch[i], s.plan.x0[i], s.plan.y0[i], 0});
+            }
+            rc = reserve_frames(ctx, P.frames, s.f0, P.frames.size(), max_channels(s.m));
+            if (rc) return rc;
         }
-        rc = reserve_frames(ctx, P.frames, s.f0, P.frames.size(), max_channels(s.m));
-        if (rc) return rc;
+        for (size_t i = 0; i < cw.size(); i++) {   // the planes converted alone; band_rows: chain_host's copy bands of the last step
+            if (s.packed && s.plan.frame[i] >= 0) continue;
+            rc = reserve_convert(ctx, s.m, engine, cw[i], k == last && P.band_rows ? P.band_rows : ch[i], block_splitting);
+            if (rc) return rc;
+        }
     }
     P.tables = Tables();
     frame_tables(P.frames, &P.fd, &P.tables);
@@ -1229,13 +1276,13 @@ int reserve_part(Part &P, bool pack) {
     return ctx->plan_buf.reserve(P.tables.bytes(P.n_tta));
 }
 
-// Everything before the first launch of a call, on every part: first every buffer of every part (reserve_part), so that W2X_ERR_NOMEM
-// leaves nothing queued on any context; then on each part ONE upload of every step's frame tables and TTA kernel tables, so that no
+// Everything before the first line, on_step call or launch of a call, on every part: first every buffer of every part, convert_device's
+// scratch included (reserve_part), so that W2X_ERR_NOMEM leaves nothing queued on any context; then on each part ONE upload of every step's frame tables and TTA kernel tables, so that no
 // step waits for the host.  A TTA step's variants kernel on the part owning plane i writes variant j wherever the part converting it
 // keeps it, and the mean kernel reads its output there.
-int prepare_parts(std::vector<Part> &parts, bool pack) {
+int prepare_parts(std::vector<Part> &parts, bool pack, int block_splitting) {
     for (Part &P : parts)
-        if (int rc = reserve_part(P, pack)) return rc;
+        if (int rc = reserve_part(P, pack, block_splitting)) return rc;
     const size_t n_steps = parts[0].steps.size();
     std::vector<std::vector<const PlaneIO *>> var_at(n_steps);   // [k][8 i + j]: where variant j of plane i lives at TTA step k
     for (const Part &P : parts)
@@ -1311,7 +1358,8 @@ int run_unit(w2x_ctx *ctx, const Step &s, const std::vector<FrameDev> &fd, const
     if (u.frame < 0) {
         const size_t i = (size_t)u.planes[0];
         const PlaneIO &p = s.cio()[i];
-        return convert_device(ctx, s.m, p.src, s.cw()[i], s.ch()[i], p.src_stride, 0, 0, p.dst, p.dst_stride, block_splitting, s.up);
+        return convert_device(ctx, s.m, p.src, s.cw()[i], s.ch()[i], p.src_stride, p.above, p.below, p.dst, p.dst_stride, block_splitting,
+                              s.up, p.left, p.right, p.phase_x, p.phase_y);
     }
     const size_t f = s.f0 + (size_t)u.frame;
     int rc = run_packed_frame(ctx, s.m, s.dm, fd[f], s.up);
@@ -1377,7 +1425,7 @@ int planes_device(w2x_ctx *ctx, std::vector<Step> &steps, const float *const *d_
     Part &P = parts[0];
     P.ends.resize(P.own.size());
     for (size_t i = 0; i < P.ends.size(); i++) P.ends[i] = PlaneIO{d_in[i], in_strides[i], d_out[i], out_strides[i]};
-    int rc = prepare_parts(parts, pack);
+    int rc = prepare_parts(parts, pack, block_splitting);
     if (rc) return rc;
     return run_steps(ctx, P.steps, P.fd, 0, P.steps.size(), block_splitting, on_step, user, false);
 }
@@ -1412,7 +1460,7 @@ int planes_host(w2x_ctx *log, const std::vector<Step> &all, std::vector<Part> &p
         for (size_t i = 0; i < n; i++)
             P.ends[i] = PlaneIO{P.ctx->io_buf[0].get() + in_off[p][i], (size_t)widths[P.own[i]] * 4, P.ctx->io_buf[1].get() + out_off[p][i], (size_t)L.w[i] * 4};
     }
-    int rc = prepare_parts(parts, true);
+    int rc = prepare_parts(parts, true, 0);
     if (rc) return rc;
     std::vector<std::vector<HostGroup>> groups(np);
     std::vector<std::vector<int>> upto(np);   // [part][phase]: how many of the part's groups are queued by the end of the phase
@@ -1813,10 +1861,13 @@ int chain_host(w2x_ctx *ctx, std::vector<Step> &table, const float *in, int widt
     const w2x_model *m = steps[last].m;
     const bool up = steps[last].up, band_uploads = last == 0 && !steps[last].tta;
     const int n = (int)m->layers.size(), w = steps[last].w[0], h = steps[last].h[0];
+    const int nb = steps[last].tta ? 1 : host_copy_bands(ctx, n, w, h, block_splitting);
+    auto band_y = [&](int i) { return (int)((long)h * i / nb) & (up ? ~1 : ~0); };
+    for (int i = 0; i < nb && nb > 1; i++) parts[0].band_rows = std::max(parts[0].band_rows, band_y(i + 1) - band_y(i));
     const size_t in_dense = (size_t)width * 4;
     int rc = reserve_io(ctx, (size_t)width * height * sizeof(float), (size_t)w * h * sizeof(float));
     parts[0].ends = {PlaneIO{ctx->io_buf[0].get(), in_dense, ctx->io_buf[1].get(), (size_t)w * 4}};
-    if (!rc) rc = prepare_parts(parts, false);
+    if (!rc) rc = prepare_parts(parts, false, block_splitting);
     if (rc) return rc;
     if (!band_uploads)
         CU_CHECK(cudaMemcpy2DAsync(ctx->io_buf[0].get(), in_dense, in, in_stride_bytes, in_dense, (size_t)height, cudaMemcpyHostToDevice, ctx->stream));
@@ -1833,8 +1884,6 @@ int chain_host(w2x_ctx *ctx, std::vector<Step> &table, const float *in, int widt
         one[0].down = {{out, out_stride_bytes, io.dst, io.dst_stride, io.dst_stride, (size_t)h}};
         return run_host_groups(ctx, one);
     }
-    const int nb = host_copy_bands(ctx, n, w, h, block_splitting);
-    auto band_y = [&](int i) { return (int)((long)h * i / nb) & (up ? ~1 : ~0); };
     // band_uploads: upload i carries input rows [u(i), u(i + 1)); band i reads source rows up to (band_y(i + 1) + n - 1) >> up, its n
     // rows of context below included, so that it waits for its own upload only
     auto u = [&](int i) { return i == 0 ? 0 : i == nb ? height : std::min(height, ((band_y(i) + n - 1) >> (up ? 1 : 0)) + 1); };
@@ -1920,91 +1969,39 @@ int w2x_convert_chain(w2x_ctx *ctx, int n_steps, const w2x_model *const *models,
 }  // extern "C"
 
 // ---- a window of a chain's output (w2x_convert_chain_region*) ----------------------------------------------------------------
-// Step k converts only its output window wins[k + 1], reading its input window wins[k]: the source rectangle at step 0, else the
-// previous step's output window, dense in chain_buf[(k - 1) & 1].  The window is a plane of its own to convert_device, with the real
-// neighbours its input window holds beyond it as row and column context, so that only the plane's own border is replicated.
+// The steps of w2x_convert_chain* on a collection of one plane, step k converting only its output window wins[k + 1] from its input
+// window wins[k]: the source rectangle at step 0, else the previous step's output window, dense in chain_buf[(k - 1) & 1].  The
+// window is a plane of its own to convert_device, with the real neighbours its input window holds beyond it as row and column
+// context, so that only the plane's own border is replicated.  No step has TTA, none packs, and every buffer is reserved by
+// prepare_parts before the first launch, as for the other step-table calls.
 namespace {
-struct Region {
-    std::vector<const w2x_model *> m;
-    std::vector<bool> up;
-    std::vector<Rect> wins;   // region_windows
-};
-
-// Every argument of w2x_convert_chain_region*, before anything is printed, allocated or queued.
+// Every argument of w2x_convert_chain_region*, before anything is printed, allocated or queued: the steps (no TTA) and the window
+// by region_windows, then the buffers and each step's engine by check_steps.  Then *steps is the one-plane step table of the windows.
 int check_region(const char *fn, w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, int width, int height,
-                 const int *window, const void *src, size_t src_stride_bytes, const void *out, size_t out_stride_bytes, Region *r) {
+                 const int *window, const void *src, size_t src_stride_bytes, const void *out, size_t out_stride_bytes,
+                 std::vector<Step> *steps) {
     if (check_ctx(ctx)) return W2X_ERR_ARG;
-    int rc = region_windows(fn, n_steps, models, kinds, width, height, window, &r->wins);
+    std::vector<Rect> wins;
+    int rc = region_windows(fn, n_steps, models, kinds, width, height, window, &wins);
     if (rc) return rc;
-    const Rect &s = r->wins.front(), &o = r->wins.back();
-    if (!src) return fail(W2X_ERR_ARG, "%s: NULL source", fn);
-    if (src_stride_bytes % 4 || src_stride_bytes < (size_t)s.w * 4)
-        return fail(W2X_ERR_ARG, "%s: the source row stride must be a multiple of 4 bytes and >= the source rectangle's row (%d bytes)", fn,
-                    s.w * 4);
-    if (!out) return fail(W2X_ERR_ARG, "%s: NULL output", fn);
-    if (out_stride_bytes % 4 || out_stride_bytes < (size_t)o.w * 4)
-        return fail(W2X_ERR_ARG, "%s: the output row stride must be a multiple of 4 bytes and >= the window's row (%d bytes)", fn, o.w * 4);
-    for (int k = 0; k < n_steps; k++) {
-        if (pick_engine(ctx, models[k]) >= 0) continue;
-        const std::string why = w2x_last_error();
-        return fail(W2X_ERR_UNSUPPORTED, "%s: step %d: %s", fn, k, why.c_str());
+    const Rect &s = wins.front(), &o = wins.back();
+    rc = check_steps(fn, ctx, n_steps, models, kinds, 1, &s.w, &s.h, 0, [&](int) -> int {
+        if (!src) return fail(W2X_ERR_ARG, "%s: NULL source", fn);
+        if (src_stride_bytes % 4 || src_stride_bytes < (size_t)s.w * 4)
+            return fail(W2X_ERR_ARG, "%s: the source row stride must be a multiple of 4 bytes and >= the source rectangle's row (%d bytes)",
+                        fn, s.w * 4);
+        if (!out) return fail(W2X_ERR_ARG, "%s: NULL output", fn);
+        if (out_stride_bytes % 4 || out_stride_bytes < (size_t)o.w * 4)
+            return fail(W2X_ERR_ARG, "%s: the output row stride must be a multiple of 4 bytes and >= the window's row (%d bytes)", fn,
+                        o.w * 4);
+        return W2X_OK;
+    }, steps);
+    for (int k = 0; k < n_steps && !rc; k++) {
+        const Rect &w = wins[(size_t)k + 1];
+        Step &t = (*steps)[(size_t)k];
+        t.w = {w.w}, t.h = {w.h}, t.x0 = {w.x0}, t.y0 = {w.y0}, t.in = {wins[(size_t)k]};
     }
-    r->m.assign(models, models + n_steps);
-    for (int k = 0; k < n_steps; k++) r->up.push_back((kinds[k] & W2X_STEP_UPSCALE2X) != 0);
-    return W2X_OK;
-}
-
-// Every buffer of a region's steps: the models, the chain buffers of the intermediate windows, and the scratch that convert_device
-// and run_basic reserve for a plane the size of each output window (its scratch band's activation frames, and the fp32 engine's
-// padded plane), so that W2X_ERR_NOMEM comes before the first copy or launch.
-int reserve_region(w2x_ctx *ctx, const Region &r) {
-    const size_t last = r.m.size() - 1;
-    size_t need[2] = {0, 0}, act = 0, pad = 0;
-    for (size_t k = 0; k <= last; k++) {
-        const w2x_model *m = r.m[k];
-        DevModel *dm = nullptr;
-        int rc = get_dev_model(ctx, m, &dm);
-        if (rc) return rc;
-        const Rect &o = r.wins[k + 1];
-        const int n = (int)m->layers.size(), pw = o.w + 2 * n;
-        if (k < last) need[k & 1] = std::max(need[k & 1], (size_t)o.w * o.h * sizeof(float));
-        // both engines: 4 bytes per activation element (tc::act_bytes)
-        act = std::max(act, (size_t)max_channels(m) * pw * (scratch_band_rows(ctx, m, o.w, o.h) + 2 * n) * 4);
-        if (pick_engine(ctx, m) == W2X_ENGINE_FP32) pad = std::max(pad, (size_t)pw * (o.h + 2 * n) * sizeof(float));
-        else if ((rc = ensure_tc(ctx))) return rc;
-    }
-    for (int i = 0; i < 2; i++) {
-        if (!need[i]) continue;
-        if (int rc = ctx->chain_buf[i].reserve(need[i])) return rc;
-    }
-    for (int i = 0; i < 2; i++)
-        if (int rc = ctx->buf[i].reserve(act)) return rc;
-    return pad ? ctx->pad_buf.reserve(pad) : W2X_OK;
-}
-
-// The steps of a checked, reserved region on the context's stream: src is the source rectangle, out the window.
-int run_region(w2x_ctx *ctx, const Region &r, const float *src, size_t src_stride, float *out, size_t out_stride, w2x_step_fn on_step,
-               void *user) {
-    const size_t last = r.m.size() - 1;
-    for (size_t k = 0; k <= last; k++) {
-        const w2x_model *m = r.m[k];
-        const Rect &i = r.wins[k], &o = r.wins[k + 1];
-        if (on_step) on_step((int)k, user);
-        emit_plane_progress(ctx, m, o.w, o.h, 0, false);
-        // an upscaling step's window is in 2x pixels: it starts at source pixel (o.y0 >> 1, o.x0 >> 1), on the second copy of that
-        // pixel's row / column when o.y0 / o.x0 is odd, and its input window holds s * i of real 2x pixels
-        const int s = r.up[k] ? 2 : 1;
-        const float *in = reinterpret_cast<const float *>(reinterpret_cast<const char *>(src) + (size_t)(o.y0 / s - i.y0) * src_stride) +
-                          (o.x0 / s - i.x0);
-        float *dst = k == last ? out : ctx->chain_buf[k & 1].get();
-        const size_t dst_stride = k == last ? out_stride : (size_t)o.w * sizeof(float);
-        int rc = convert_device(ctx, m, in, o.w, o.h, src_stride, o.y0 - s * i.y0, s * i.y1() - o.y1(), dst, dst_stride, 0, r.up[k],
-                                o.x0 - s * i.x0, s * i.x1() - o.x1(), o.x0 % s, o.y0 % s);
-        if (rc) return rc;
-        src = dst;
-        src_stride = dst_stride;
-    }
-    return W2X_OK;
+    return rc;
 }
 }  // namespace
 
@@ -2013,37 +2010,38 @@ extern "C" {
 int w2x_convert_chain_region(w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, int width, int height,
                              const int *window, const float *src, size_t src_stride_bytes, float *out, size_t out_stride_bytes,
                              w2x_step_fn on_step, void *user) {
-    Region r;
+    std::vector<Step> table;
     int rc = check_region("w2x_convert_chain_region", ctx, n_steps, models, kinds, width, height, window, src, src_stride_bytes, out,
-                          out_stride_bytes, &r);
+                          out_stride_bytes, &table);
     if (rc) return rc;
     DeviceGuard g(ctx->device);
     NvtxRange nvtx("w2x convert chain region");
-    const Rect &s = r.wins.front(), &o = r.wins.back();
-    const size_t srow = (size_t)s.w * sizeof(float), orow = (size_t)o.w * sizeof(float);
-    rc = reserve_io(ctx, srow * s.h, orow * o.h);
-    if (!rc) rc = reserve_region(ctx, r);
+    std::vector<Part> parts{one_part(ctx, table)};
+    Part &P = parts[0];
+    const Rect s = P.steps.front().in[0];
+    const int ow = P.steps.back().w[0], oh = P.steps.back().h[0];
+    const size_t srow = (size_t)s.w * sizeof(float), orow = (size_t)ow * sizeof(float);
+    rc = reserve_io(ctx, srow * s.h, orow * oh);
+    P.ends = {PlaneIO{ctx->io_buf[0].get(), srow, ctx->io_buf[1].get(), orow}};
+    if (!rc) rc = prepare_parts(parts, false, 0);
     if (rc) return rc;
-    float *d_src = ctx->io_buf[0].get(), *d_out = ctx->io_buf[1].get();
     std::vector<HostGroup> one(1);
-    one[0].up = {{d_src, srow, src, src_stride_bytes, srow, (size_t)s.h}};
-    one[0].compute = [&] { return run_region(ctx, r, d_src, srow, d_out, orow, on_step, user); };
-    one[0].down = {{out, out_stride_bytes, d_out, orow, orow, (size_t)o.h}};
+    one[0].up = {{ctx->io_buf[0].get(), srow, src, src_stride_bytes, srow, (size_t)s.h}};
+    one[0].compute = [&] { return run_steps(ctx, P.steps, P.fd, 0, P.steps.size(), 0, on_step, user, false); };
+    one[0].down = {{out, out_stride_bytes, ctx->io_buf[1].get(), orow, orow, (size_t)oh}};
     return run_host_groups(ctx, one);
 }
 
 int w2x_convert_chain_region_device(w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, int width, int height,
                                     const int *window, const float *d_src, size_t src_stride_bytes, float *d_out, size_t out_stride_bytes,
                                     w2x_step_fn on_step, void *user) {
-    Region r;
+    std::vector<Step> steps;
     int rc = check_region("w2x_convert_chain_region_device", ctx, n_steps, models, kinds, width, height, window, d_src, src_stride_bytes,
-                          d_out, out_stride_bytes, &r);
+                          d_out, out_stride_bytes, &steps);
     if (rc) return rc;
     DeviceGuard g(ctx->device);
     NvtxRange nvtx("w2x convert chain region");
-    rc = reserve_region(ctx, r);
-    if (rc) return rc;
-    return run_region(ctx, r, d_src, src_stride_bytes, d_out, out_stride_bytes, on_step, user);
+    return planes_device(ctx, steps, &d_src, &src_stride_bytes, &d_out, &out_stride_bytes, false, 0, on_step, user);
 }
 
 }  // extern "C"
