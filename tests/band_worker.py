@@ -25,6 +25,9 @@ Case kinds (fields beyond "id", "kind", "model", "width"):
   forget    precision, rows (a band group), model2: w2x_ctx_forget_model while a band group, a slab and a w2x_multi plan
             hold the model -> log "<id>" the status of every forget, "<id>.<pass>" the band group's plane, run after the
             refused forgets
+  plans     precision, models [m1, m2, m3]: on one w2x_multi of 2 contexts, convert_plane(m1), convert_chain([m2, m3^]), a forget
+            of m1 and of m2, convert_plane(m1) again -> "<id>.plane", "<id>.chain", "<id>.plane again"; log "<id>" the status of
+            each forget and the per-context launches of each call
 """
 import json
 import os
@@ -269,7 +272,32 @@ def run_forget(c):
     log[c["id"]] = st
 
 
-RUN = {"slab": run_slabs, "slab_ipc": run_slab_ipc, "multi": run_multi, "forget": run_forget}
+def run_plans(c):
+    """a plane plan and a chain plan of one w2x_multi side by side: a plane, a chain, a forget of each plan's model, the plane again"""
+    pool.close()
+    m1, m2, m3 = (models[k] for k in c["models"])
+    x = inputs[c["id"]]
+    st = {}
+    multi = w2x.Multi([0, 0])
+
+    def counted(key, convert):
+        before = multi.launch_counts()
+        outs[f"{c['id']}.{key}"] = convert()
+        st[f"{key} launches"] = [a - b for a, b in zip(multi.launch_counts(), before)]
+
+    try:
+        multi.set_precision(c["precision"])
+        counted("plane", lambda: multi.convert_plane(m1, x))
+        counted("chain", lambda: multi.convert_chain([(m2, False), (m3, True)], x))
+        st["plane's model"] = forget_status(multi, m1)            # the first context refuses first
+        st["chain's model"] = forget_status(multi, m2)
+        counted("plane again", lambda: multi.convert_plane(m1, x))
+    finally:
+        multi.close()
+    log[c["id"]] = st
+
+
+RUN = {"slab": run_slabs, "slab_ipc": run_slab_ipc, "multi": run_multi, "forget": run_forget, "plans": run_plans}
 for c in cases:
     t0 = time.time()
     if c["kind"] == "band":

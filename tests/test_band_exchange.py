@@ -17,7 +17,8 @@ module builds the inputs and references and compares.
   * w2x_multi_* on k = 2..4 contexts of one device: heights on both sides of the cut-or-not rule, automatic sub-bands, the
     plan cache across precision / model / width / height changes, convert_tiles with fewer, as many and more tiles than
     devices, and the progress lines.
-  * w2x_ctx_forget_model while band sessions, slabs or a multi plan use the model.
+  * w2x_ctx_forget_model while band sessions, slabs or a multi plan use the model; a w2x_multi's plane plan and chain plan kept
+    side by side.
 
 Every group runs three passes (flag values, events and buffers are reused); every pass must give the reference's bits.
 """
@@ -404,3 +405,26 @@ def test_forget_model_refused_while_band_sessions_hold_it(layers, ref, tmp_path)
         assert st[k] == [0, ""], (k, st[k])
     fails = _check_passes(outs, "forget", ref("noise1", F16_F8X2, x), x.shape[1], cuts(rows))
     assert not fails, "\n".join(fails)
+
+
+def test_multi_keeps_the_plane_plan_beside_the_chain_plan(layers, ref, tmp_path):
+    """a chain between two plane calls leaves the plane's plan in place: both plans' models are refused by w2x_ctx_forget_model
+    after the chain, and the second plane call gives the first one's bits with the same launches"""
+    names = ["rand128", "noise1", "scale2.0x"]
+    job = Job({k: layers[k] for k in names})
+    x = seeded(60, 35, 303, "noise1")     # 60 rows: the plane (n = 4) and the chain (n = 7) are both cut for two contexts
+    job.add(dict(id="plans", kind="plans", models=names, precision=F16_F8X2), x)
+    job.write(tmp_path)
+    (outs, log), = run_worker(tmp_path)
+    st = log["plans"]
+    for k in ("plane's model", "chain's model"):
+        status, msg = st[k]
+        assert status == 1 and "band session" in msg, (k, st[k])
+    msg = mismatch(outs["plans.plane"], ref("rand128", F16_F8X2, x), _multi_seams(2, 4, 60))
+    assert not msg, msg
+    want = ref.ctx[F16_F8X2].convert_chain([(ref.models["noise1"], False), (ref.models["scale2.0x"], True)], x)
+    msg = mismatch(outs["plans.chain"], want, [0, 60, 120])
+    assert not msg, msg
+    assert np.array_equal(outs["plans.plane again"], outs["plans.plane"])
+    assert all(st["plane launches"]) and all(st["chain launches"]), st
+    assert st["plane again launches"] == st["plane launches"], st

@@ -16,6 +16,8 @@
 // The layer kernels never store a band's halo rows (their output tensor maps exclude them), so a neighbour may deliver
 // its row as early as it likes.  Results are bit-identical to the single-GPU pass: every output pixel sees the same
 // operands in the same order.
+#include <functional>
+
 #include "engine_internal.h"
 
 using namespace w2x;
@@ -28,32 +30,12 @@ int band_check(w2x_band *b) {
     return W2X_OK;
 }
 
-// The rows traded after `step` (-1 = the padded input frame): up to 4 contiguous ranges per row, each `bytes` long, at
-//   base + plane_mul * (pw * C * frame_rows) + row * pitch + in_row        (evaluated in the owner's OR the neighbour's frame)
-struct RowSeg { size_t plane_mul, pitch, in_row; };
-int row_segments(const w2x_band *b, int step, RowSeg seg[4], size_t *bytes, size_t *px_out) {
-    const int n = b->n;
-    if (step == -1) {
-        *bytes = (size_t)b->pw * sizeof(float);
-        seg[0] = {0, *bytes, 0};
-        *px_out = 0;
-        return 1;
-    }
-    if (step == n - 2) {              // per-pixel tap partials [hf][pw][12] fp32
-        *bytes = (size_t)b->pw * 12 * sizeof(float);
-        seg[0] = {0, *bytes, 0};
-        *px_out = 0;
-        return 1;
-    }
-    const size_t px = (size_t)b->pw * (size_t)b->model->layers[(size_t)step].n_out;
-    *px_out = px;
-    *bytes = 4 * px;                  // RECORD frame: a row is one contiguous range of 4 bytes per element
-    seg[0] = {0, 4 * px, 0};
-    return 1;
-}
-
-inline char *seg_at(char *base, int frame_rows, size_t px, const RowSeg &s, int row) {
-    return base + s.plane_mul * px * (size_t)frame_rows + s.pitch * (size_t)row + s.in_row;
+// The bytes of one row of the frame traded after `step` (-1 = the padded input frame).  A row is one contiguous range, and row r of
+// a frame, the owner's or the neighbour's, is at base + r * row_bytes.
+size_t row_bytes(const w2x_band *b, int step) {
+    if (step == -1) return (size_t)b->pw * sizeof(float);
+    if (step == b->n - 2) return (size_t)b->pw * 12 * sizeof(float);             // per-pixel tap partials [hf][pw][12] fp32
+    return 4 * (size_t)b->pw * (size_t)b->model->layers[(size_t)step].n_out;    // RECORD frame: 4 bytes per element
 }
 
 // w2x_band_load_rows, also through the nearest 2x resize: with up2x the band's rows are 2x rows of a half-resolution plane, the band
@@ -203,18 +185,14 @@ int w2x_band_halo(w2x_band *band, int step, int *n_segments, void **send_up, voi
     if (step != band->last_step || step < 0 || !n_segments || !send_up || !recv_up || !send_down || !recv_down || !seg_bytes)
         return fail(W2X_ERR_ARG, "w2x_band_halo: call it for the step that was queued last");
     char *base = reinterpret_cast<char *>(band->act[band->cur].get());
-    RowSeg seg[4];
-    size_t bytes, px;
-    const int nseg = row_segments(band, step, seg, &bytes, &px);
-    *n_segments = nseg;
+    const size_t bytes = row_bytes(band, step);
+    *n_segments = 1;
     *seg_bytes = bytes;
-    for (int s = 0; s < 4; s++) {
-        const bool on = s < nseg;
-        send_up[s] = on && band->up ? seg_at(base, band->hf, px, seg[s], 1) : nullptr;                       // first owned row
-        recv_up[s] = on && band->up ? seg_at(base, band->hf, px, seg[s], 0) : nullptr;                       // halo row above
-        send_down[s] = on && band->down ? seg_at(base, band->hf, px, seg[s], band->hf - 2) : nullptr;        // last owned row
-        recv_down[s] = on && band->down ? seg_at(base, band->hf, px, seg[s], band->hf - 1) : nullptr;        // halo row below
-    }
+    send_up[0] = band->up ? base + bytes : nullptr;                                   // first owned row
+    recv_up[0] = band->up ? base : nullptr;                                           // halo row above
+    send_down[0] = band->down ? base + bytes * (size_t)(band->hf - 2) : nullptr;      // last owned row
+    recv_down[0] = band->down ? base + bytes * (size_t)(band->hf - 1) : nullptr;      // halo row below
+    for (int s = 1; s < 4; s++) send_up[s] = recv_up[s] = send_down[s] = recv_down[s] = nullptr;
     return W2X_OK;
 }
 
@@ -324,26 +302,22 @@ int w2x_band_exchange(w2x_band *band, int step) {
     if (!band->up && !band->down) return W2X_OK;
     w2x_ctx *ctx = band->ctx;
     DeviceGuard g(ctx->device);
-    RowSeg seg[4];
-    size_t bytes, px;
-    const int nseg = row_segments(band, step, seg, &bytes, &px);
+    const size_t bytes = row_bytes(band, step);
     char *mine = step < 0 ? reinterpret_cast<char *>(band->pad.get()) : reinterpret_cast<char *>(band->act[band->cur].get());
     HaloXArgs a{};
-    for (int s = 0; s < nseg; s++) {
-        if (band->up) {      // my first owned row -> the up neighbour's halo row below (its last frame row)
-            const w2x_band::Peer &p = band->peer[0];
-            char *theirs = step < 0 ? reinterpret_cast<char *>(p.pad) : p.act[band->cur];
-            a.src[a.n] = seg_at(mine, band->hf, px, seg[s], 1);
-            a.dst[a.n] = seg_at(theirs, p.hf, px, seg[s], p.hf - 1);
-            a.n++;
-        }
-        if (band->down) {    // my last owned row -> the down neighbour's halo row above (its frame row 0)
-            const w2x_band::Peer &p = band->peer[1];
-            char *theirs = step < 0 ? reinterpret_cast<char *>(p.pad) : p.act[band->cur];
-            a.src[a.n] = seg_at(mine, band->hf, px, seg[s], band->hf - 2);
-            a.dst[a.n] = seg_at(theirs, p.hf, px, seg[s], 0);
-            a.n++;
-        }
+    if (band->up) {      // my first owned row -> the up neighbour's halo row below (its last frame row)
+        const w2x_band::Peer &p = band->peer[0];
+        char *theirs = step < 0 ? reinterpret_cast<char *>(p.pad) : p.act[band->cur];
+        a.src[a.n] = mine + bytes;
+        a.dst[a.n] = theirs + bytes * (size_t)(p.hf - 1);
+        a.n++;
+    }
+    if (band->down) {    // my last owned row -> the down neighbour's halo row above (its frame row 0)
+        const w2x_band::Peer &p = band->peer[1];
+        char *theirs = step < 0 ? reinterpret_cast<char *>(p.pad) : p.act[band->cur];
+        a.src[a.n] = mine + bytes * (size_t)(band->hf - 2);
+        a.dst[a.n] = theirs;
+        a.n++;
     }
     a.bytes = bytes;
     unsigned *const flags = band->flags.get();
@@ -617,33 +591,97 @@ int w2x_slab_convert(w2x_slab *s, const float *in, size_t in_stride_bytes, float
 // =========================================================================================================================
 struct w2x_multi {
     std::vector<w2x_ctx *> ctx;
-    // the slabs of the last (model, width, height): planes of one job usually share a shape
-    uint64_t plan_uid = 0;
-    int plan_w = 0, plan_h = 0, plan_precision = -1;
-    std::vector<w2x_slab *> slabs;
-    std::vector<int> r0;                       // first row of every slab (+ the plane height at the end)
-    // w2x_multi_convert_chain's plan, beside the one above: the slabs of the last (models, kinds, width, height), one per step and GPU
+    // The slabs of the last (models, kinds, width, height), one per step and GPU: jobs usually repeat a shape.
     struct Chain {
         std::vector<uint64_t> uids;
         std::vector<int> kinds;
         int w = 0, h = 0, precision = -1;
         std::vector<std::vector<w2x_slab *>> slabs;   // [step][GPU]; GPU i owns rows [r0[i] << u, r0[i + 1] << u) of a step after u upscales
         std::vector<int> r0;                          // in input rows
-    } chain;
+    };
+    // [0]: w2x_multi_convert_plane's (a one-step W2X_STEP_SAME chain); [1]: every other chain's.  Kept side by side, so a job that
+    // alternates planes and chains does not rebuild either.
+    Chain plan[2];
 };
 
 namespace {
 
-void multi_drop_plan(w2x_multi *m) {
-    for (auto b : m->slabs) w2x_slab_destroy(b);
-    m->slabs.clear();
-    m->plan_uid = 0;
+void drop(w2x_multi::Chain &c) {
+    for (auto &step : c.slabs)
+        for (auto b : step) w2x_slab_destroy(b);
+    c = w2x_multi::Chain();
 }
 
-void multi_drop_chain(w2x_multi *m) {
-    for (auto &step : m->chain.slabs)
-        for (auto b : step) w2x_slab_destroy(b);
-    m->chain = w2x_multi::Chain();
+// w2x_convert_chain over the row bands of nd >= 2 GPUs, HOST rows in and out, through the plan in `c` (built here unless the steps,
+// size, precision and nd are the plan's).  A nearest 2x step maps the rows [a, b) a GPU owns onto [2a, 2b), so the cut of step 0
+// stays a valid cut at every later step and no row ever changes GPU: the rows a GPU's slab of step k leaves in its d_out are, on
+// that GPU, the (half-resolution) source of its slab of step k + 1.  Only step 0 uploads and only the last step downloads; the one
+// cross-GPU traffic a step adds is the halo row of its input frame, which w2x_band_exchange(band, -1) already moves.  Every step
+// has sessions (frames, flags) of its own: a neighbour may deliver a halo row of step k + 1 while this GPU still reads step k.
+// begin(k) runs before step k is queued on any GPU.
+int multi_convert(w2x_multi *m, w2x_multi::Chain &c, int nd, int n_steps, const w2x_model *const *models, const int *kinds, const float *in,
+                  int width, int height, size_t in_stride_bytes, float *out, size_t out_stride_bytes, const std::function<void(int)> &begin) {
+    w2x_ctx *ctx0 = m->ctx[0];
+    int rc = W2X_OK;
+    // ---- plan: per step one slab per GPU, neighbours of a step wired through peer memory; all device memory is reserved here ----
+    std::vector<uint64_t> uids;
+    for (int k = 0; k < n_steps; k++) uids.push_back(models[k]->uid);
+    const std::vector<int> kv(kinds, kinds + n_steps);
+    if (c.uids != uids || c.kinds != kv || c.w != width || c.h != height || c.precision != ctx0->precision || c.slabs.empty() ||
+        (int)c.slabs[0].size() != nd) {
+        drop(c);
+        for (int i = 0; i <= nd; i++) c.r0.push_back((int)((long)height * i / nd));
+        c.slabs.resize((size_t)n_steps);
+        int u = 0;
+        for (int k = 0; k < n_steps && !rc; k++) {
+            const bool up = (kinds[k] & W2X_STEP_UPSCALE2X) != 0;
+            u += up;
+            for (int i = 0; i < nd && !rc; i++) {
+                m->ctx[(size_t)i]->precision = ctx0->precision;
+                w2x_slab *sl = nullptr;
+                rc = slab_create(m->ctx[(size_t)i], models[k], width << u, (c.r0[(size_t)i + 1] - c.r0[(size_t)i]) << u, i > 0, i + 1 < nd, i & 1, 0,
+                                 k == 0, up, &sl);
+                if (!rc) c.slabs[(size_t)k].push_back(sl);
+            }
+            for (int i = 0; i < nd && !rc; i++)
+                rc = w2x_slab_connect_local(c.slabs[(size_t)k][(size_t)i], i > 0 ? c.slabs[(size_t)k][(size_t)i - 1] : nullptr,
+                                            i + 1 < nd ? c.slabs[(size_t)k][(size_t)i + 1] : nullptr);
+        }
+        if (rc) { drop(c); return rc; }
+        c.uids = uids;
+        c.kinds = kv;
+        c.w = width;
+        c.h = height;
+        c.precision = ctx0->precision;
+    }
+    const size_t last = (size_t)n_steps - 1;
+    int u_last = 0;
+    for (int k = 0; k < n_steps; k++) u_last += (kinds[k] & W2X_STEP_UPSCALE2X) != 0;
+    const int ow = width << u_last;
+    HostPin pin_in(in, in_stride_bytes * (size_t)(height - 1) + (size_t)width * 4),
+        pin_out(out, out_stride_bytes * (size_t)(((size_t)height << u_last) - 1) + (size_t)ow * 4);
+    // ---- queue step-major, every GPU from this one thread: begin(k) comes before step k is queued anywhere, and a GPU's step k + 1
+    // follows its own step k in stream order.  Nothing queued here can block this thread on a GPU's progress. ----
+    for (size_t k = 0; k <= last && rc == W2X_OK; k++) {
+        begin((int)k);
+        for (int i = 0; i < nd && rc == W2X_OK; i++) {
+            w2x_slab *sl = c.slabs[k][(size_t)i];
+            if (k == 0) {
+                rc = slab_enqueue_compute(sl, reinterpret_cast<const float *>(reinterpret_cast<const char *>(in) + (size_t)c.r0[(size_t)i] * in_stride_bytes), in_stride_bytes);
+            } else {
+                const w2x_slab *prev = c.slabs[k - 1][(size_t)i];
+                rc = slab_enqueue_run(sl, prev->d_out.get(), (size_t)prev->width * 4, (kinds[k] & W2X_STEP_UPSCALE2X) != 0, false);
+            }
+        }
+    }
+    for (int i = 0; i < nd && rc == W2X_OK; i++)      // every GPU's layers are queued: a download (into pageable memory) may block this thread now
+        rc = slab_enqueue_download(c.slabs[last][(size_t)i], reinterpret_cast<float *>(reinterpret_cast<char *>(out) + ((size_t)c.r0[(size_t)i] << u_last) * out_stride_bytes),
+                                   out_stride_bytes);
+    for (int i = 0; i < nd; i++) {
+        int r2 = w2x_slab_synchronize(c.slabs[last][(size_t)i]);
+        if (rc == W2X_OK) rc = r2;
+    }
+    return rc;
 }
 
 }  // namespace
@@ -669,8 +707,7 @@ int w2x_multi_create(const int *devices, int n_devices, w2x_multi **out) {
 
 void w2x_multi_destroy(w2x_multi *m) {
     if (!m) return;
-    multi_drop_plan(m);
-    multi_drop_chain(m);
+    for (auto &c : m->plan) drop(c);
     for (auto c : m->ctx) w2x_ctx_destroy(c);
     delete m;
 }
@@ -689,48 +726,12 @@ int w2x_multi_convert_plane(w2x_multi *m, const w2x_model *model, const float *i
     nd = std::min(nd, height / (4 * n_layers));
     if (nd < 2 || !model->tc_eligible || m->ctx[0]->engine == W2X_ENGINE_FP32)
         return w2x_convert_plane(m->ctx[0], model, in, width, height, in_stride_bytes, out, out_stride_bytes, block_splitting);
-    // ---- plan: one slab per GPU (sub-bands for the copy pipeline), neighbours wired through peer memory ----
-    if (m->plan_uid != model->uid || m->plan_w != width || m->plan_h != height || (int)m->slabs.size() != nd ||
-        m->plan_precision != m->ctx[0]->precision) {
-        multi_drop_plan(m);
-        m->r0.assign((size_t)nd + 1, 0);
-        for (int i = 0; i <= nd; i++) m->r0[(size_t)i] = (int)((long)height * i / nd);
-        for (int i = 0; i < nd; i++) {
-            m->ctx[(size_t)i]->precision = m->ctx[0]->precision;
-            w2x_slab *sl = nullptr;
-            int rc = w2x_slab_create(m->ctx[(size_t)i], model, width, m->r0[(size_t)i + 1] - m->r0[(size_t)i], i > 0, i + 1 < nd, i & 1, 0, &sl);
-            if (rc) { multi_drop_plan(m); return rc; }
-            m->slabs.push_back(sl);
-        }
-        for (int i = 0; i < nd; i++) {
-            int rc = w2x_slab_connect_local(m->slabs[(size_t)i], i > 0 ? m->slabs[(size_t)i - 1] : nullptr, i + 1 < nd ? m->slabs[(size_t)i + 1] : nullptr);
-            if (rc) { multi_drop_plan(m); return rc; }
-        }
-        m->plan_uid = model->uid;
-        m->plan_w = width;
-        m->plan_h = height;
-        m->plan_precision = m->ctx[0]->precision;
-    }
-    emit_reference_progress(m->ctx[0], width, height, n_layers, block_splitting && w2x_requires_splitting(width, height));
-    HostPin pin_in(in, in_stride_bytes * (size_t)(height - 1) + (size_t)width * 4), pin_out(out, out_stride_bytes * (size_t)(height - 1) + (size_t)width * 4);
-    // ---- queue everything (uploads, the layer loops with their exchanges, downloads) for every GPU from this one thread ----
-    int rc = W2X_OK;
-    for (int i = 0; i < nd && rc == W2X_OK; i++)      // phase 1 on EVERY GPU before any download can block this thread
-        rc = slab_enqueue_compute(m->slabs[(size_t)i], reinterpret_cast<const float *>(reinterpret_cast<const char *>(in) + (size_t)m->r0[(size_t)i] * in_stride_bytes), in_stride_bytes);
-    for (int i = 0; i < nd && rc == W2X_OK; i++)
-        rc = slab_enqueue_download(m->slabs[(size_t)i], reinterpret_cast<float *>(reinterpret_cast<char *>(out) + (size_t)m->r0[(size_t)i] * out_stride_bytes), out_stride_bytes);
-    for (int i = 0; i < nd; i++) {
-        int r2 = w2x_slab_synchronize(m->slabs[(size_t)i]);
-        if (rc == W2X_OK) rc = r2;
-    }
-    return rc;
+    const int same = W2X_STEP_SAME;
+    return multi_convert(m, m->plan[0], nd, 1, &model, &same, in, width, height, in_stride_bytes, out, out_stride_bytes, [&](int) {
+        emit_reference_progress(m->ctx[0], width, height, n_layers, block_splitting && w2x_requires_splitting(width, height));
+    });
 }
 
-// w2x_convert_chain over row bands.  A nearest 2x step maps the rows [a, b) a GPU owns onto [2a, 2b), so the cut of step 0 stays a
-// valid cut at every later step and no row ever changes GPU: the rows a GPU's slab of step k leaves in its d_out are, on that GPU,
-// the (half-resolution) source of its slab of step k + 1.  Only step 0 uploads and only the last step downloads; the one cross-GPU
-// traffic a step adds is the halo row of its input frame, which w2x_band_exchange(band, -1) already moves.  Every step has sessions
-// (frames, flags) of its own: a neighbour may deliver a halo row of step k + 1 while this GPU still reads step k.
 int w2x_multi_convert_chain(w2x_multi *m, int n_steps, const w2x_model *const *models, const int *kinds, const float *in, int width,
                             int height, size_t in_stride_bytes, float *out, size_t out_stride_bytes, int block_splitting,
                             w2x_step_fn on_step, void *user) {
@@ -756,70 +757,12 @@ int w2x_multi_convert_chain(w2x_multi *m, int n_steps, const w2x_model *const *m
     const int nd = std::min((int)m->ctx.size(), height / (4 * n_max));
     if (nd < 2 || !tc)
         return w2x_convert_chain(ctx0, n_steps, models, kinds, in, width, height, in_stride_bytes, out, out_stride_bytes, block_splitting, on_step, user);
-    // ---- plan: per step one slab per GPU, neighbours of a step wired through peer memory; all device memory is reserved here ----
-    w2x_multi::Chain &c = m->chain;
-    std::vector<uint64_t> uids;
-    for (int k = 0; k < n_steps; k++) uids.push_back(models[k]->uid);
-    const std::vector<int> kv(kinds, kinds + n_steps);
-    if (c.uids != uids || c.kinds != kv || c.w != width || c.h != height || c.precision != ctx0->precision || c.slabs.empty() ||
-        (int)c.slabs[0].size() != nd) {
-        multi_drop_chain(m);
-        for (int i = 0; i <= nd; i++) c.r0.push_back((int)((long)height * i / nd));
-        c.slabs.resize((size_t)n_steps);
-        int u = 0;
-        for (int k = 0; k < n_steps && !rc; k++) {
-            const bool up = (kinds[k] & W2X_STEP_UPSCALE2X) != 0;
-            u += up;
-            for (int i = 0; i < nd && !rc; i++) {
-                m->ctx[(size_t)i]->precision = ctx0->precision;
-                w2x_slab *sl = nullptr;
-                rc = slab_create(m->ctx[(size_t)i], models[k], width << u, (c.r0[(size_t)i + 1] - c.r0[(size_t)i]) << u, i > 0, i + 1 < nd, i & 1, 0,
-                                 k == 0, up, &sl);
-                if (!rc) c.slabs[(size_t)k].push_back(sl);
-            }
-            for (int i = 0; i < nd && !rc; i++)
-                rc = w2x_slab_connect_local(c.slabs[(size_t)k][(size_t)i], i > 0 ? c.slabs[(size_t)k][(size_t)i - 1] : nullptr,
-                                            i + 1 < nd ? c.slabs[(size_t)k][(size_t)i + 1] : nullptr);
-        }
-        if (rc) { multi_drop_chain(m); return rc; }
-        c.uids = uids;
-        c.kinds = kv;
-        c.w = width;
-        c.h = height;
-        c.precision = ctx0->precision;
-    }
-    const size_t last = (size_t)n_steps - 1;
-    int u_last = 0;
-    for (int k = 0; k < n_steps; k++) u_last += (kinds[k] & W2X_STEP_UPSCALE2X) != 0;
-    const int ow = width << u_last;
-    HostPin pin_in(in, in_stride_bytes * (size_t)(height - 1) + (size_t)width * 4),
-        pin_out(out, out_stride_bytes * (size_t)(((size_t)height << u_last) - 1) + (size_t)ow * 4);
-    // ---- queue step-major, every GPU from this one thread: on_step(k) and step k's lines come before step k is queued anywhere, and a
-    // GPU's step k + 1 follows its own step k in stream order.  Nothing queued here can block this thread on a GPU's progress. ----
-    int w = width, h = height;
-    for (size_t k = 0; k <= last && rc == W2X_OK; k++) {
-        const bool up = (kinds[k] & W2X_STEP_UPSCALE2X) != 0;
-        if (up) w *= 2, h *= 2;
-        if (on_step) on_step((int)k, user);
+    int w = width, h = height;      // step k's output size: begin(k) runs once per step, in order
+    return multi_convert(m, m->plan[1], nd, n_steps, models, kinds, in, width, height, in_stride_bytes, out, out_stride_bytes, [&](int k) {
+        if (kinds[k] & W2X_STEP_UPSCALE2X) w *= 2, h *= 2;
+        if (on_step) on_step(k, user);
         emit_plane_progress(ctx0, models[k], w, h, block_splitting, true);
-        for (int i = 0; i < nd && rc == W2X_OK; i++) {
-            w2x_slab *sl = c.slabs[k][(size_t)i];
-            if (k == 0) {
-                rc = slab_enqueue_compute(sl, reinterpret_cast<const float *>(reinterpret_cast<const char *>(in) + (size_t)c.r0[(size_t)i] * in_stride_bytes), in_stride_bytes);
-            } else {
-                const w2x_slab *prev = c.slabs[k - 1][(size_t)i];
-                rc = slab_enqueue_run(sl, prev->d_out.get(), (size_t)prev->width * 4, up, false);
-            }
-        }
-    }
-    for (int i = 0; i < nd && rc == W2X_OK; i++)      // every GPU's layers are queued: a download may block this thread now
-        rc = slab_enqueue_download(c.slabs[last][(size_t)i], reinterpret_cast<float *>(reinterpret_cast<char *>(out) + ((size_t)c.r0[(size_t)i] << u_last) * out_stride_bytes),
-                                   out_stride_bytes);
-    for (int i = 0; i < nd; i++) {
-        int r2 = w2x_slab_synchronize(c.slabs[last][(size_t)i]);
-        if (rc == W2X_OK) rc = r2;
-    }
-    return rc;
+    });
 }
 
 int w2x_multi_convert_planes_chain(w2x_multi *m, int n_steps, const w2x_model *const *models, const int *kinds, int n_planes,
