@@ -396,7 +396,7 @@ FP32_MODELS = [(1, 3, 5, 1), (1, 17, 1), (1, 48, 33, 1)]
 @pytest.mark.gpu
 @pytest.mark.parametrize("dims", FP32_MODELS, ids=lambda d: "-".join(map(str, d)))
 def test_fp32_convert_plane_is_bit_exact(w2x, fp32_ctx, oracle_mod, dims):
-    """copyMakeBorder + layers + crop (pad_replicate_kernel, conv3x3_planar_fp32, crop_kernel); a plane that block-splits
+    """copyMakeBorder + layers + crop (pad_kernel, conv3x3_planar_fp32, crop_kernel); a plane that block-splits
     (64 x 64 blocks) in the fused and the literal walk (copy2d_kernel); convert_tiles"""
     om = oracle_mod.OracleModel.random(list(zip(dims[:-1], dims[1:])), seed=sum(dims))
     model = w2x.Model.from_arrays(om.weights, om.biases)

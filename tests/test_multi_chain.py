@@ -12,7 +12,7 @@ reference's bits.
     whose later steps get several sub-bands per GPU; row-strided pinned and pageable host planes.
   * progress lines and on_step order; a one-step W2X_STEP_SAME chain against Multi.convert_plane; the plan cache; refusals;
     w2x_ctx_forget_model against the chain plan.
-  * launch_pad_upsample2x_xy alone against a numpy restatement.
+  * launch_pad alone against a numpy restatement of its frame.
   * the CLI with W2X_DEVICES=0,0 against its one-GPU run.
 Without a GPU: the binding's signature, the numpy restatement's own sanity and the W2X_DEVICES parsing of host/w2xc.hpp.
 """
@@ -97,34 +97,42 @@ FORGET = [
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# the numpy restatement of launch_pad_upsample2x_xy
+# the numpy restatement of launch_pad's frame (FrameSource, csrc/kernels.h)
 # ---------------------------------------------------------------------------------------------------------------------
-def frame_of(src, row0, w2, h2, pad_x, pad_top, pad_bottom, rows_above, rows_below):
-    """the padded frame of the band of h2 2x rows starting at 2x row 2 * row0 of the nearest 2x resize of src (w2 columns of it)"""
-    up = np.repeat(np.repeat(src, 2, axis=0), 2, axis=1)[:, :w2]
-    y0 = 2 * row0
-    assert y0 >= rows_above and y0 + h2 + rows_below <= up.shape[0], "the real rows must exist"
-    real = up[y0 - min(rows_above, pad_top):y0 + h2 + min(rows_below, pad_bottom)]       # the band and the real rows the frame shows
-    return np.pad(real, ((max(pad_top - rows_above, 0), max(pad_bottom - rows_below, 0)), (pad_x, pad_x)), mode="edge")
+def frame_of(src, row0, col0, w, h, pad_x, pad_top, rows_above, rows_below, up2x, cols_left, cols_right, pw, ph):
+    """the pw x ph frame whose pixel (fy, fx) is the plane's pixel (clamp(fy - pad_top, -rows_above, h - 1 + rows_below),
+    clamp(fx - pad_x, -cols_left, w - 1 + cols_right)); the plane's pixel (y, x) is src[row0 + y][col0 + x], or with up2x (the
+    nearest 2x resize of src) src[row0 + (y >> 1)][col0 + (x >> 1)]"""
+    sh = 1 if up2x else 0
+    sy = row0 + (np.clip(np.arange(ph) - pad_top, -rows_above, h - 1 + rows_below) >> sh)
+    sx = col0 + (np.clip(np.arange(pw) - pad_x, -cols_left, w - 1 + cols_right) >> sh)
+    assert sy.min() >= 0 and sx.min() >= 0, "the real rows and columns must exist"
+    return src[np.ix_(sy, sx)]
 
 
 def test_frame_restatement_by_hand():
     src = np.arange(12, dtype=np.float32).reshape(4, 3)          # rows 0..3; the 2x plane has rows 0 0 1 1 2 2 3 3
-    f = frame_of(src, 2, 6, 4, 1, 3, 1, 3, 0)                    # band = 2x rows 4..7 (source rows 2, 3); 3 real rows above: 2x rows 1, 2, 3
+    f = frame_of(src, 2, 0, 6, 4, 1, 3, 3, 0, True, 0, 0, 8, 8)  # band = 2x rows 4..7 (source rows 2, 3); 3 real rows above: 2x rows 1, 2, 3
     assert f.shape == (8, 8)
     assert [r[1] for r in f.tolist()] == [0, 3, 3, 6, 6, 9, 9, 9]             # source rows 0 1 1 | 2 2 3 3 | replicated 3
     assert f[3].tolist() == [6, 6, 6, 7, 7, 8, 8, 8]
-    g = frame_of(src, 1, 6, 4, 2, 2, 2, 0, 0)                    # image borders on both sides: replicate the band's own rows
+    g = frame_of(src, 1, 0, 6, 4, 2, 2, 0, 0, True, 0, 0, 10, 8)  # image borders on both sides: replicate the band's own rows
     assert [r[2] for r in g.tolist()] == [3, 3, 3, 3, 6, 6, 6, 6] and g.shape == (8, 10)
-    h = frame_of(src, 0, 5, 2, 0, 0, 1, 0, 1)                    # an odd width cuts the 2x plane; one real row below
+    h = frame_of(src, 0, 0, 5, 2, 0, 0, 0, 1, True, 0, 0, 5, 3)  # an odd width cuts the 2x plane; one real row below
     assert h.tolist() == [[0, 0, 1, 1, 2], [0, 0, 1, 1, 2], [3, 3, 4, 4, 5]]
+    # no resize: the plane is src[1:3, 1:2], one real row and column on each side, pads of 2 left and right, 1 above and below
+    e = frame_of(src, 1, 1, 1, 2, 2, 1, 1, 1, False, 1, 1, 5, 4)
+    assert e.tolist() == [[0, 0, 1, 2, 2], [3, 3, 4, 5, 5], [6, 6, 7, 8, 8], [9, 9, 10, 11, 11]]
+    # a window of 2x columns [1, 3) with pad 2: it widens by one (the first copy of source column 0), its left pad and real columns
+    # one smaller, so that no pad shows 2x column 0
+    assert frame_of(src, 0, 0, 3, 1, 1, 0, 0, 0, True, -1, 0, 6, 1).tolist() == [[0, 0, 0, 1, 1, 1]]
 
 
-def test_binding_declares_the_multi_chain_entry(w2x):
+def test_binding_declares_the_multi_chain_and_pad_entries(w2x):
     L = w2x.lib()
     assert len(L.w2x_multi_convert_chain.argtypes) == len(L.w2x_convert_chain.argtypes) == 13
     assert L.w2x_multi_convert_chain.argtypes[1:] == L.w2x_convert_chain.argtypes[1:]
-    assert len(L.w2x_debug_pad_upsample2x_xy.argtypes) == 15
+    assert len(L.w2x_debug_pad.argtypes) == 20
     assert callable(w2x.Multi.convert_chain)
 
 
@@ -137,39 +145,60 @@ def test_device_list_parsing(w2x, tmp_path):
     assert p.returncode == 0 and "ALL OK" in p.stdout, p.stdout + p.stderr
 
 
+def pad_case(ctx, rng, w, h, pad_x, pad_top, ra, rb, up2x, cl, cr, pw, ph, y0, rows):
+    """launch_pad against frame_of on a source whose every row and column outside the clamps' reach is NaN: "" when they agree"""
+    sh = 1 if up2x else 0
+    r_lo, r_hi, c_lo, c_hi = -ra >> sh, (h - 1 + rb) >> sh, -cl >> sh, (w - 1 + cr) >> sh     # what the clamps reach, in src units
+    row0, col0 = 1 - r_lo, 2 - c_lo
+    src = np.full((row0 + r_hi + 2, col0 + c_hi + 4), np.nan, np.float32)
+    src[row0 + r_lo:row0 + r_hi + 1, col0 + c_lo:col0 + c_hi + 1] = rng.random((r_hi - r_lo + 1, c_hi - c_lo + 1), dtype=np.float32)
+    want = frame_of(src, row0, col0, w, h, pad_x, pad_top, ra, rb, up2x, cl, cr, pw, ph)
+    out = np.full(want.shape, -7.0, np.float32)
+    ctx.debug_pad(src, row0, col0, w, h, pad_x, pad_top, ra, rb, up2x, cl, cr, out, y0, rows)
+    want[:y0] = -7.0
+    want[y0 + rows:] = -7.0
+    return mismatch(out, want, [y0, y0 + rows])
+
+
 @gpu
-def test_pad_upsample2x_xy_against_numpy(w2x):
+def test_pad_against_numpy(w2x):
     ctx = w2x.Context(0)
     rng = np.random.default_rng(5)
     fails, checked = [], 0
     try:
-        # (source width, w2): even and odd 2x widths; (5, 10) with pad_x = 7 gives a 24-float frame row (the 16-byte stores)
+        # row bands of a 2x plane: (source width, w2): even and odd 2x widths; (5, 10) with pad_x = 7 gives a 24-float frame row (the
+        # 16-byte stores); a neighbour's side has one halo row, which the band's store window leaves out
         for (ws, w2), n in itertools.product(((1, 2), (1, 1), (2, 4), (2, 3), (3, 6), (5, 10), (5, 9), (9, 18)), (4, 7)):
             for ra, rb, st, sb in itertools.product((0, 1, n), (0, 1, n), (0, 1), (0, 1)):
-                pt, pb = (1 if st else n), (1 if sb else n)                   # a neighbour's side has one halo row, which is skipped
+                pt, pb = (1 if st else n), (1 if sb else n)
                 if ra > pt or rb > pb:
                     continue
-                h2 = 6
-                row0 = (n + 1) // 2
-                src = np.full((row0 + h2 // 2 + (n + 1) // 2, ws + 3), np.nan, np.float32)
-                src[:, :ws] = rng.random((src.shape[0], ws), dtype=np.float32)
-                want = frame_of(src[:, :ws], row0, w2, h2, n, pt, pb, ra, rb)
-                out = np.full(want.shape, -7.0, np.float32)
-                ctx.debug_pad_upsample2x_xy(src[:, :ws], row0, w2, h2, n, pt, pb, ra, rb, st, sb, out)
-                want[:st] = -7.0
-                want[want.shape[0] - sb:] = -7.0
+                ph = 6 + pt + pb
+                bad = pad_case(ctx, rng, w2, 6, n, pt, ra, rb, True, 0, 0, w2 + 2 * n, ph, st, ph - st - sb)
                 checked += 1
-                if not np.array_equal(out, want):
-                    fails.append(f"w2={w2} n={n} rows_above={ra} rows_below={rb} skip={st},{sb}: {mismatch(out, want, [pt, pt + h2])}")
+                if bad:
+                    fails.append(f"w2={w2} n={n} rows_above={ra} rows_below={rb} skip={st},{sb}: {bad}")
+        # with and without the resize: (left pad, right pad, cols_left, cols_right) and (top pad, bottom pad, rows_above, rows_below),
+        # among them real columns and rows beyond the plane, a right pad other than the left one, and the odd pads of windows
+        # starting on an odd 2x column / row (the plane one wider, its pad and real columns / rows before it one smaller: -1 when
+        # there are none); store windows that leave out rows at the top, the bottom, or both
+        for up2x, n, w in itertools.product((False, True), (4, 7), (5, 8, 10)):
+            for (pl, pr, cl, cr), (pt, pb, ra, rb) in itertools.product(
+                    ((n, n, 0, 0), (n, n, 2, n), (n - 1, n, -1, 0), (n - 1, n, n - 1, 1), (1, n, 1, 0), (n, 2, 0, 3)),
+                    ((n, n, 0, 0), (n - 1, n, -1, 0), (n - 1, n, n - 1, n), (1, n, 1, 0), (n, 1, 3, 1), (n, n, n, n))):
+                h = 7
+                pw, ph = w + pl + pr, h + pt + pb
+                for y0, rows in ((0, ph), (1, ph - 2), (3, ph - 5), (ph - 4, 4), (0, 2)):
+                    bad = pad_case(ctx, rng, w, h, pl, pt, ra, rb, up2x, cl, cr, pw, ph, y0, rows)
+                    checked += 1
+                    if bad:
+                        fails.append(f"up2x={up2x} w={w} h={h} x={pl, pr, cl, cr} y={pt, pb, ra, rb} window={y0, rows}: {bad}")
         # a taller band than one block of row pairs, odd pad, real rows on both sides
-        src = rng.random((40, 13), dtype=np.float32)
-        want = frame_of(src, 4, 26, 60, 7, 7, 7, 7, 7)
-        out = np.full(want.shape, -7.0, np.float32)
-        ctx.debug_pad_upsample2x_xy(src, 4, 26, 60, 7, 7, 7, 7, 7, 0, 0, out)
-        assert np.array_equal(out, want), mismatch(out, want, [7, 67])
+        bad = pad_case(ctx, rng, 26, 60, 7, 7, 7, 7, True, 0, 0, 40, 74, 0, 74)
+        assert not bad, bad
     finally:
         ctx.close()
-    assert checked >= 200 and not fails, "\n".join(fails[:20])
+    assert checked >= 1500 and not fails, "\n".join(fails[:20])
 
 
 # ---------------------------------------------------------------------------------------------------------------------

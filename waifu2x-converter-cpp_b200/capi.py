@@ -168,7 +168,7 @@ def lib():
     L.w2x_multi_convert_planes.argtypes = [vp, vp, ci, C.POINTER(vp), pi, pi, ps, C.POINTER(vp), ps]
     L.w2x_multi_convert_planes_chain.argtypes = [vp, ci, C.POINTER(vp), pi, ci, C.POINTER(vp), pi, pi, ps, C.POINTER(vp), ps, STEP_FN, vp]
     L.w2x_debug_plan_multi_planes.argtypes = [ci, ci, C.POINTER(vp), pi, ci, pi, pi, pi, C.POINTER(C.c_longlong)]
-    L.w2x_debug_pad_upsample2x_xy.argtypes = [vp, vp, ci, ci, C.c_long, ci, ci, ci, ci, ci, ci, ci, ci, ci, vp]
+    L.w2x_debug_pad.argtypes = [vp, vp, ci, C.c_long, ci, ci] + [ci] * 13 + [vp]
     L.w2x_debug_set_host_bands.argtypes = [vp, ci]
     L.w2x_debug_set_fuse_last.argtypes = [vp, ci]
     L.w2x_debug_set_num_sms.argtypes = [vp, ci]
@@ -382,12 +382,13 @@ class Context:
     def debug_set_num_sms(self, n): _check(lib().w2x_debug_set_num_sms(self._h, int(n)))
     def debug_tc_profile_enable(self, on=True): _check(lib().w2x_debug_tc_profile_enable(self._h, int(on)))
 
-    def debug_pad_upsample2x_xy(self, src, row0, w2, h2, pad_x, pad_top, pad_bottom, rows_above, rows_below, skip_top, skip_bottom, out):
-        """launch_pad_upsample2x_xy alone: src is the half-resolution plane (2-D float32, row-strided views pass as they are), its row
-        row0 holds 2x row 0 of the band; the frame is written into `out` (dense), whose skipped rows stay as they are."""
-        _check(lib().w2x_debug_pad_upsample2x_xy(self._h, C.c_void_p(src.ctypes.data), src.shape[0], row0, src.strides[0] // 4, w2, h2, pad_x,
-                                                 pad_top, pad_bottom, rows_above, rows_below, skip_top, skip_bottom,
-                                                 C.c_void_p(out.ctypes.data)))
+    def debug_pad(self, src, row0, col0, w, h, pad_x, pad_top, rows_above, rows_below, up2x, cols_left, cols_right, out, out_y0=0,
+                  out_rows=-1):
+        """launch_pad alone: the frame of the FrameSource whose `in` is pixel (row0, col0) of src (2-D float32, row-strided views pass
+        as they are) is written into `out` (dense, its shape is the frame's), whose rows outside the store window stay as they are."""
+        _check(lib().w2x_debug_pad(self._h, C.c_void_p(src.ctypes.data), src.shape[0], src.strides[0] // 4, row0, col0, w, h, pad_x, pad_top,
+                                   rows_above, rows_below, int(up2x), cols_left, cols_right, out.shape[1], out.shape[0], out_y0, out_rows,
+                                   C.c_void_p(out.ctypes.data)))
         return out
 
     def debug_tc_profile_read(self, layer):

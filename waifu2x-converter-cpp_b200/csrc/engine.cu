@@ -166,18 +166,15 @@ int launch_layer_tc(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int li, cons
     return W2X_OK;
 }
 
-// A pw x ph fp32 region (row stride `stride` floats) that already contains the n-pixel ring, as the first layer's source.
-tc::FirstSource padded(const float *p, long stride, int pw, int ph) { return tc::FirstSource{p, stride, pw, ph, 0, 0, 0, 0}; }
-
 // ---- convertWithModelsBasic on a pw x ph frame ------------------------------------------------
-// src: what the first layer reads: a padded region (padded()), or (tensor-core engine only) an unpadded plane with the replicate
-// padding folded into the loads.  The fp32 engine copies src.in / src.stride_floats, which is then always a padded region.
+// src: what the first layer reads: a padded region (FrameSource::padded()), or (tensor-core engine only) an unpadded plane with the
+// replicate padding folded into the loads.  The fp32 engine copies src.in / src.stride_floats, which is then always a padded region.
 // dst: receives the (pw-2n) x (ph-2n) interior.
 // packed (tensor-core engine with the fused last layer only): src is a packed frame of pw x ph holding many padded planes (see
 // tc::PlaneRect); the layers run ONCE on it -- the seams pollute only the rings that are cropped anyway -- and one gather writes
 // every plane's interior to its own destination; dst / dst_stride are then unused.
 struct PackedGather { const tc::PlaneRect *rect; int n_rect, n_blocks; };
-int run_basic(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int engine, const tc::FirstSource &src, int pw, int ph, float *dst,
+int run_basic(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int engine, const FrameSource &src, int pw, int ph, float *dst,
               long dst_stride, const PackedGather *packed = nullptr) {
     const int n = (int)m->layers.size();
     if (pw - 2 * n < 1 || ph - 2 * n < 1) return fail(W2X_ERR_ARG, "plane smaller than the model's receptive ring");
@@ -237,7 +234,8 @@ int run_basic(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int engine, const 
                 CU_CHECK(tc::launch_gather_planes(reinterpret_cast<const float *>(cur), pw, packed->rect, packed->n_rect, packed->n_blocks,
                                                   static_cast<float>(L.b[0]), n, ctx->stream));
             else
-                CU_CHECK(tc::launch_last_gather(reinterpret_cast<const float *>(cur), pw, ph, static_cast<float>(L.b[0]), n, dst, dst_stride, ctx->stream));
+                CU_CHECK(tc::launch_last_gather(reinterpret_cast<const float *>(cur), pw, ph, static_cast<float>(L.b[0]), n, n, n, dst, dst_stride,
+                                                ctx->stream));
             note_kernel(ctx, n - 1, "last_gather");
         } else {
             if (packed) return fail(W2X_ERR_UNSUPPORTED, "packed frames need the fused last layer");
@@ -440,28 +438,24 @@ int convert_device(w2x_ctx *ctx, const w2x_model *m, const float *d_in, int w, i
     const int pw = w + 2 * n;
     const long istride = (long)(in_stride_bytes / 4), ostride = (long)(out_stride_bytes / 4);
     const bool literal = literal_walk(ctx, w, h, block_splitting);
-    // cv::copyMakeBorder(in, temp, n, n, n, n, BORDER_REPLICATE)   (src/convertRoutine.cpp:35, :96): the tensor-core engine folds it
-    // into the first layer's loads and reads d_in directly, except on the literal walk, whose blocks are regions of the padded plane
+    // cv::copyMakeBorder(in, temp, n, n, n, n, BORDER_REPLICATE)   (src/convertRoutine.cpp:35, :96): the plane's frame.  The
+    // tensor-core engine folds it into the first layer's loads and reads d_in directly, except on the literal walk, whose blocks
+    // are regions of the padded plane.
+    const int px = up2x ? phase_x : 0, py = up2x ? phase_y : 0;
+    const FrameSource plane{d_in, istride, w + px, h + py, n - px, n - py, std::min(rows_above, n) - py, std::min(rows_below, n), up2x,
+                            std::min(cols_left, n) - px, std::min(cols_right, n)};
     const bool direct = engine == W2X_ENGINE_TC && !literal;
-    const int px = up2x ? phase_x : 0, cl = std::min(cols_left, n) - px, cr = std::min(cols_right, n);
     float *pad = direct ? nullptr : ctx->pad_buf.get();
     if (!direct) {
-        if (up2x) {
-            const int py = phase_y;
-            CU_CHECK(launch_pad_upsample2x(d_in, w + px, h + py, istride, n, std::min(rows_above, n) - py, std::min(rows_below, n), pad,
-                                           ctx->stream, cl, cr, n - px, n - py));
-        } else {
-            CU_CHECK(launch_pad_replicate(d_in, w, h, istride, n, std::min(rows_above, n), std::min(rows_below, n), pad, ctx->stream, cl,
-                                          cr));
-        }
+        CU_CHECK(launch_pad(plane, pw, h + 2 * n, pad, ctx->stream));
         ctx->launches++;
     }
     if (literal) {   // check_blocks has seen every block fit
         const std::vector<int> tab = blocks_of(w, h, n);
         for (size_t i = 0; i < tab.size(); i += 8) {
             const int *t = &tab[i];
-            rc = run_basic(ctx, m, dm, engine, padded(pad + (long)t[2] * pw + t[4], pw, t[5] - t[4], t[3] - t[2]), t[5] - t[4], t[3] - t[2],
-                           d_out + (long)t[6] * ostride + t[7], ostride);
+            rc = run_basic(ctx, m, dm, engine, FrameSource::padded(pad + (long)t[2] * pw + t[4], pw, t[5] - t[4], t[3] - t[2]), t[5] - t[4],
+                           t[3] - t[2], d_out + (long)t[6] * ostride + t[7], ostride);
             if (rc) return rc;
         }
         return W2X_OK;
@@ -470,12 +464,7 @@ int convert_device(w2x_ctx *ctx, const w2x_model *m, const float *d_in, int w, i
     const int band = scratch_band_rows(ctx, m, w, h);
     for (int y0 = 0; y0 < h; y0 += band) {
         const int bh = std::min(band, h - y0);
-        // up2x: the band's 2x rows [y0, y0 + bh) seen from source row yy >> 1; on an odd yy the band is 2x row 1 of that source row
-        const int yy = y0 + (up2x ? phase_y : 0), p = up2x ? yy & 1 : 0;
-        const tc::FirstSource src = direct ? tc::FirstSource{d_in + (long)(up2x ? yy >> 1 : y0) * istride, istride, w + px, bh + p, n - px,
-                                                             n - p, std::min(n, y0 + rows_above) - p, std::min(n, h - y0 - bh + rows_below),
-                                                             up2x, cl, cr}
-                                           : padded(pad + (long)y0 * pw, pw, pw, bh + 2 * n);
+        const FrameSource src = direct ? plane.band(y0, bh, n) : FrameSource::padded(pad + (long)y0 * pw, pw, pw, bh + 2 * n);
         rc = run_basic(ctx, m, dm, engine, src, pw, bh + 2 * n, d_out + (long)y0 * ostride, ostride);
         if (rc) return rc;
     }
@@ -922,7 +911,7 @@ int run_packed_frame(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, const Frame
     CU_CHECK(tc::launch_pack_planes(f.rect, f.shelf_y0, f.shelf_first, f.n_shelf, n, f.fw, f.fh, up2x, ctx->pad_buf.get(), ctx->stream));
     ctx->launches++;
     const PackedGather g{f.rect, f.n_rect, f.n_blocks};
-    return run_basic(ctx, m, dm, W2X_ENGINE_TC, padded(ctx->pad_buf.get(), f.fw, f.fw, f.fh), f.fw, f.fh, nullptr, 0, &g);
+    return run_basic(ctx, m, dm, W2X_ENGINE_TC, FrameSource::padded(ctx->pad_buf.get(), f.fw, f.fw, f.fh), f.fw, f.fh, nullptr, 0, &g);
 }
 
 int run_packed_frames(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, std::vector<FramePlan> &frames) {
@@ -972,9 +961,9 @@ int convert_tiles_dev(w2x_ctx *ctx, const w2x_model *m, const float *d_in, float
     rc = ctx->pad_buf.reserve((size_t)pw * ph * sizeof(float));
     if (rc) return rc;
     for (int t = 0; t < n_tiles; t++) {   // cv::copyMakeBorder per tile (src/convertRoutine.cpp:35)
-        CU_CHECK(launch_pad_replicate(d_in + (size_t)t * w * h, w, h, w, n, 0, 0, ctx->pad_buf.get(), ctx->stream));
+        CU_CHECK(launch_pad(FrameSource{d_in + (size_t)t * w * h, w, w, h, n, n, 0, 0}, pw, ph, ctx->pad_buf.get(), ctx->stream));
         ctx->launches++;
-        rc = run_basic(ctx, m, dm, engine, padded(ctx->pad_buf.get(), pw, pw, ph), pw, ph, d_out + (size_t)t * w * h, w);
+        rc = run_basic(ctx, m, dm, engine, FrameSource::padded(ctx->pad_buf.get(), pw, pw, ph), pw, ph, d_out + (size_t)t * w * h, w);
         if (rc) return rc;
     }
     return W2X_OK;

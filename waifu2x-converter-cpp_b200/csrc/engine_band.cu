@@ -46,9 +46,9 @@ int band_load_rows_from(w2x_band *band, const float *d_in, size_t in_stride_byte
         return fail(W2X_ERR_ARG, "w2x_band_load_rows: bad input");
     w2x_ctx *ctx = band->ctx;
     DeviceGuard g(ctx->device);
-    const auto pad = up2x ? launch_pad_upsample2x_xy : launch_pad_replicate_xy;
-    CU_CHECK(pad(d_in, band->width, band->rows, (long)(in_stride_bytes / 4), band->n, band->pt, band->pb, band->ov_up ? band->n : 0,
-                 band->ov_down ? band->n : 0, band->pad.get(), ctx->stream, band->up ? 1 : 0, band->down ? 1 : 0, 0, 0, -1));   // a pointer takes no defaults
+    const FrameSource src{d_in, (long)(in_stride_bytes / 4), band->width, band->rows, band->n, band->pt, band->ov_up ? band->n : 0,
+                          band->ov_down ? band->n : 0, up2x};
+    CU_CHECK(launch_pad(src, band->pw, band->hf, band->pad.get(), ctx->stream, band->win_y0, band->win_rows));
     ctx->launches++;
     band->last_step = -1;
     band->cur = 0;
@@ -106,6 +106,8 @@ int w2x_band_create(w2x_ctx *ctx, const w2x_model *model, int width, int band_ro
     b->pb = b->down ? 1 : b->n;
     b->pw = width + 2 * b->n;
     b->hf = band_rows + b->pt + b->pb;
+    b->win_y0 = b->up ? 1 : 0;
+    b->win_rows = b->hf - b->win_y0 - (b->down ? 1 : 0);
     b->act_bytes = tc::act_bytes(max_channels(model), b->pw, b->hf);
     auto nomem = [](cudaError_t e) {
         cudaGetLastError();
@@ -138,9 +140,9 @@ int w2x_band_load(w2x_band *band, const float *d_in, size_t in_stride_bytes) {
     DeviceGuard g(ctx->device);
     if (band->ov_up || band->ov_down) return fail(W2X_ERR_ARG, "w2x_band_load: overlap edges take their rows through w2x_band_load_rows");
     const long stride = (long)(in_stride_bytes / 4);
-    const float *band0 = d_in + (band->up ? stride : 0);
-    CU_CHECK(launch_pad_replicate_xy(band0, band->width, band->rows, stride, band->n, band->pt, band->pb, band->up ? 1 : 0,
-                                     band->down ? 1 : 0, band->pad.get(), ctx->stream));
+    const FrameSource src{d_in + (band->up ? stride : 0), stride, band->width, band->rows, band->n, band->pt, band->up ? 1 : 0,
+                          band->down ? 1 : 0};
+    CU_CHECK(launch_pad(src, band->pw, band->hf, band->pad.get(), ctx->stream));
     ctx->launches++;
     band->last_step = -1;
     band->cur = 0;
@@ -161,17 +163,16 @@ int w2x_band_step(w2x_band *band, int step) {
     DevModel *dm = band->dm;
     const Layer &L = m->layers[(size_t)step];
     const int f8 = ctx->precision == W2X_PRECISION_F16_F8X2 ? 1 : 0;
-    // the halo rows belong to the neighbours: they are not part of this layer's store window
-    const int y0 = band->up ? 1 : 0, rows = band->hf - y0 - (band->down ? 1 : 0);
     if (step == 0) {
         LayerTimer t(ctx, 0);
-        const tc::FirstSource fsrc{band->pad.get(), band->pw, band->pw, band->hf, 0, 0, 0, 0};       // the session's padded input frame (halo rows come from the neighbours)
-        CU_CHECK(tc::launch_first(fsrc, band->pw, band->hf, L.w.data(), dm->b_host[0].data(), L.n_out, band->act[0].get(), ctx->stream, f8, y0, rows));
+        CU_CHECK(tc::launch_first(FrameSource::padded(band->pad.get(), band->pw, band->pw, band->hf), band->pw, band->hf, L.w.data(),
+                                  dm->b_host[0].data(), L.n_out, band->act[0].get(), ctx->stream, f8, band->win_y0, band->win_rows));
         band->cur = 0;
         note_kernel(ctx, 0, "first_1xN");
         ctx->launches++;
     } else {
-        int rc = launch_layer_tc(ctx, m, dm, step, band->act[band->cur].get(), band->act[band->cur ^ 1].get(), band->pw, band->hf, step == band->n - 2, false, y0, rows);
+        int rc = launch_layer_tc(ctx, m, dm, step, band->act[band->cur].get(), band->act[band->cur ^ 1].get(), band->pw, band->hf, step == band->n - 2, false,
+                                 band->win_y0, band->win_rows);
         if (rc) return rc;
         band->cur ^= 1;
     }
@@ -205,9 +206,9 @@ int w2x_band_finish(w2x_band *band, float *d_out, size_t out_stride_bytes) {
     const Layer &L = band->model->layers.back();
     {
         LayerTimer t(ctx, band->n - 1);
-        CU_CHECK(tc::launch_last_gather_xy(reinterpret_cast<const float *>(band->act[band->cur].get()), band->pw, band->hf,
-                                           static_cast<float>(L.b[0]), band->n, band->pt, band->pb, d_out,
-                                           (long)(out_stride_bytes / 4), ctx->stream));
+        CU_CHECK(tc::launch_last_gather(reinterpret_cast<const float *>(band->act[band->cur].get()), band->pw, band->hf,
+                                        static_cast<float>(L.b[0]), band->n, band->pt, band->pb, d_out, (long)(out_stride_bytes / 4),
+                                        ctx->stream));
     }
     note_kernel(ctx, band->n - 1, "last_gather");
     ctx->launches++;
@@ -821,25 +822,29 @@ int w2x_multi_set_log(w2x_multi *m, w2x_log_fn fn, void *user) {
     return w2x_ctx_set_log(m->ctx[0], fn, user);
 }
 
-// Test hook: launch_pad_upsample2x_xy alone on HOST arrays.  `in` is in_rows x in_stride_floats, its row in_row0 holds 2x row 0 of the
-// band; `out` is the dense frame and comes back with the rows the kernel skipped as the caller left them.
-W2X_API int w2x_debug_pad_upsample2x_xy(w2x_ctx *ctx, const float *in, int in_rows, int in_row0, long in_stride_floats, int w2, int h2, int pad_x,
-                                        int pad_top, int pad_bottom, int rows_above, int rows_below, int skip_top, int skip_bottom, float *out) {
+// Test hook: launch_pad alone on HOST arrays.  `in` is in_rows x in_stride_floats and the source's pixel (0, 0) is its pixel
+// (in_row0, in_col0); every row and column the source's clamps allow must lie inside it.  `out` is the dense pw x ph frame and comes
+// back with the rows outside the store window [out_y0, out_y0 + out_rows) as the caller left them.
+W2X_API int w2x_debug_pad(w2x_ctx *ctx, const float *in, int in_rows, long in_stride_floats, int in_row0, int in_col0, int w, int h, int pad_x,
+                          int pad_top, int rows_above, int rows_below, int up2x, int cols_left, int cols_right, int pw, int ph, int out_y0,
+                          int out_rows, float *out) {
     if (check_ctx(ctx)) return W2X_ERR_ARG;
-    if (!in || !out || w2 < 1 || h2 < 1 || in_rows < 1 || pad_x < 0 || pad_top < 0 || pad_bottom < 0 || rows_above < 0 || rows_below < 0 ||
-        skip_top < 0 || skip_bottom < 0 || in_stride_floats < (w2 + 1) / 2 || in_row0 + ((-rows_above) >> 1) < 0 ||
-        in_row0 + ((h2 - 1 + rows_below) >> 1) >= in_rows)
-        return fail(W2X_ERR_ARG, "w2x_debug_pad_upsample2x_xy: bad argument");
+    const int sh = up2x ? 1 : 0;   // the source rows and columns the clamps can reach: [lo >> sh, hi >> sh] of each
+    if (!in || !out || w < 1 || h < 1 || in_rows < 1 || pw < 1 || ph < 1 || -rows_above > h - 1 + rows_below || -cols_left > w - 1 + cols_right ||
+        in_row0 + (-rows_above >> sh) < 0 || in_row0 + ((h - 1 + rows_below) >> sh) >= in_rows || in_col0 + (-cols_left >> sh) < 0 ||
+        in_col0 + ((w - 1 + cols_right) >> sh) >= in_stride_floats)
+        return fail(W2X_ERR_ARG, "w2x_debug_pad: bad argument");
     DeviceGuard g(ctx->device);
-    const size_t in_bytes = (size_t)in_rows * in_stride_floats * 4, out_bytes = (size_t)(w2 + 2 * pad_x) * (h2 + pad_top + pad_bottom) * 4;
+    const size_t in_bytes = (size_t)in_rows * in_stride_floats * 4, out_bytes = (size_t)pw * ph * 4;
     DevBuf<float> d_in, d_out;
     int rc = d_in.reserve(in_bytes);
     if (!rc) rc = d_out.reserve(out_bytes);
     if (rc) return rc;
     CU_CHECK(cudaMemcpyAsync(d_in.get(), in, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
     CU_CHECK(cudaMemcpyAsync(d_out.get(), out, out_bytes, cudaMemcpyHostToDevice, ctx->stream));
-    CU_CHECK(launch_pad_upsample2x_xy(d_in.get() + (size_t)in_row0 * in_stride_floats, w2, h2, in_stride_floats, pad_x, pad_top, pad_bottom, rows_above,
-                                      rows_below, d_out.get(), ctx->stream, skip_top, skip_bottom));
+    const FrameSource src{d_in.get() + (size_t)in_row0 * in_stride_floats + in_col0, in_stride_floats, w, h, pad_x, pad_top, rows_above,
+                          rows_below, up2x != 0, cols_left, cols_right};
+    CU_CHECK(launch_pad(src, pw, ph, d_out.get(), ctx->stream, out_y0, out_rows));
     ctx->launches++;
     CU_CHECK(cudaMemcpyAsync(out, d_out.get(), out_bytes, cudaMemcpyDeviceToHost, ctx->stream));
     CU_CHECK(cudaStreamSynchronize(ctx->stream));

@@ -140,6 +140,7 @@ struct w2x_band {
     bool ov_up = false, ov_down = false;   // the n rows above / below are REAL input rows supplied with the band (recomputed overlap, no exchange)
     int pt = 0, pb = 0;            // frame rows above / below the band: 1 (neighbour halo) or n (image border: replicated; overlap: real rows)
     int pw = 0, hf = 0;            // frame width / height
+    int win_y0 = 0, win_rows = 0;  // the store window of the input load and every step: all frame rows but the neighbours' halo rows
     w2x::eng::DevBuf<float> pad;   // padded fp32 input frame
     w2x::eng::DevBuf<__half> act[2];
     size_t act_bytes = 0;

@@ -7,34 +7,55 @@
 
 namespace w2x {
 
+// The padded input frame of a conversion, pw x ph pixels, read by the first layer (tc::launch_first) or materialised by launch_pad:
+// cv::copyMakeBorder(BORDER_REPLICATE) (src/convertRoutine.cpp:35,96) of a w x h plane, where the plane may have real rows and
+// columns beyond it (row bands, windows).  Frame pixel (fy, fx) is the plane's pixel
+//     (clamp(fy - pad_top, -rows_above, h - 1 + rows_below), clamp(fx - pad_x, -cols_left, w - 1 + cols_right))
+// of `in` (row stride stride_floats), whose pixel (0, 0) it points at.  pad_x and pad_top are the left and top pads; the right and
+// bottom ones are pw - w - pad_x and ph - h - pad_top.
+// up2x: the plane is the nearest-neighbour 2x resize of `in` (cv::resize INTER_NEAREST to exactly twice the size,
+// src/main.cpp:135-139), never materialised: the pixel (y, x) above is in[y >> 1][x >> 1] (>> floors, also above and to the left).
+// Every count is then in 2x rows and columns, and row 0 and column 0 of the plane are the first copies of in's row 0 and column 0: a
+// window or band that starts on an odd 2x row (column) widens by one, its h (w) one larger and pad_top and rows_above (pad_x and
+// cols_left) one smaller.
+struct FrameSource {
+    const float *in;
+    long stride_floats;
+    int w, h, pad_x, pad_top, rows_above, rows_below;
+    bool up2x = false;
+    int cols_left = 0, cols_right = 0;
+
+    // A pw x ph region (row stride `stride` floats) that already is a padded frame.
+    static FrameSource padded(const float *p, long stride, int pw, int ph) { return FrameSource{p, stride, pw, ph, 0, 0, 0, 0}; }
+    // The frame of rows [r, r + rows + 2 pad) of this one.  When this frame has pad rows above the plane it converts, that is the frame
+    // of the plane's rows [r, r + rows) with pad rows above and below, the plane's other rows being real rows beyond them.  An up2x
+    // band starting on an odd 2x row widens by one.
+    FrameSource band(int r, int rows, int pad) const {
+        const int v0 = r + pad - pad_top, p = up2x ? v0 & 1 : 0, o = v0 - p;    // plane rows: v0 the band's first, o its row 0 (even with up2x)
+        FrameSource b = *this;
+        b.in = in + (long)(up2x ? o >> 1 : o) * stride_floats;
+        b.h = rows + p;
+        b.pad_top = pad - p;
+        b.rows_above = rows_above + o;
+        b.rows_below = h + rows_below - v0 - rows;
+        return b;
+    }
+};
+
+#ifdef __CUDACC__
+// One axis of FrameSource's mapping: frame coordinate f -> the row (column) of `in` it reads.  The one definition of the clamp:
+// the first layer's loads and the padding kernel both call it.
+template <bool UP2X>
+__device__ __forceinline__ int frame_src(int f, int pad, int len, int before, int after) {
+    const int v = min(max(f - pad, -before), len - 1 + after);
+    return UP2X ? v >> 1 : v;
+}
+#endif
+
 // ---- kernels_fp32.cu --------------------------------------------------------------------------
-// cols_left / cols_right (all padding launchers): real columns readable left / right of the plane (windows), read instead of
-// replicating its edge columns, as rows_above / rows_below are for rows.
-cudaError_t launch_pad_replicate(const float *in, int w, int h, long in_stride_floats, int pad, int rows_above,
-                                 int rows_below, float *out, cudaStream_t s, int cols_left = 0, int cols_right = 0);
-// general form: left pad pad_x, right pad pad_right (-1: pad_x), vertical pads pad_top / pad_bottom (row-band sessions)
-// skip_top / skip_bottom: frame rows at the top / bottom that are NOT written (a neighbour GPU stores them)
-cudaError_t launch_pad_replicate_xy(const float *in, int w, int h, long in_stride_floats, int pad_x, int pad_top,
-                                    int pad_bottom, int rows_above, int rows_below, float *out, cudaStream_t s,
-                                    int skip_top = 0, int skip_bottom = 0, int cols_left = 0, int cols_right = 0,
-                                    int pad_right = -1);
-// launch_pad_replicate of the nearest-neighbour 2x resize of `in` (pixel (y, x) = in[y >> 1][x >> 1]) without materialising it:
-// w2 x h2 is the 2x plane (or a band of it starting on an even 2x row, `in` pointing at its first source row) and rows_above /
-// rows_below count real 2x rows beyond it.  Writes the dense (w2 + 2 pad) x (h2 + 2 pad) plane.
-// pad_left / pad_top >= 0 replace pad on that side (a window starting on an odd 2x column / row: w2 / h2 then include the 2x
-// column / row before it, which is the first copy of in's column / row 0, and the frame is (w2 + pad_left + pad) wide).
-cudaError_t launch_pad_upsample2x(const float *in, int w2, int h2, long in_stride_floats, int pad, int rows_above, int rows_below,
-                                  float *out, cudaStream_t s, int cols_left = 0, int cols_right = 0, int pad_left = -1,
-                                  int pad_top = -1);
-// The row-band form of launch_pad_upsample2x, with launch_pad_replicate_xy's frame: pixel (fy, fx) of the (w2 + 2 pad_x) x
-// (h2 + pad_top + pad_bottom) frame = in[clamp(fy - pad_top, -rows_above, h2 - 1 + rows_below) >> 1][clamp(fx - pad_x, 0, w2 - 1) >> 1]
-// (>> floors, so with an odd rows_above the first real row above is the SECOND 2x row of its source row).  `in` points at the source
-// row holding 2x row 0 of the band, which is an even 2x row of the plane; rows_above / rows_below count real 2x rows beyond the band;
-// the top skip_top / bottom skip_bottom frame rows are not written (a neighbour GPU stores them); the column clamp is
-// [-cols_left, w2 - 1 + cols_right] and the right pad pad_right (-1: pad_x).
-cudaError_t launch_pad_upsample2x_xy(const float *in, int w2, int h2, long in_stride_floats, int pad_x, int pad_top, int pad_bottom,
-                                     int rows_above, int rows_below, float *out, cudaStream_t s, int skip_top = 0, int skip_bottom = 0,
-                                     int cols_left = 0, int cols_right = 0, int pad_right = -1);
+// The frame of src, pw x ph, dense.  Only frame rows [out_y0, out_y0 + out_rows) are written (-1: the whole frame), as in
+// tc::launch_first; a row-band session leaves its halo rows to the neighbours that write them.
+cudaError_t launch_pad(const FrameSource &src, int pw, int ph, float *out, cudaStream_t s, int out_y0 = 0, int out_rows = -1);
 // Peer-memory halo exchange (engine_band.cu): ONE kernel copies up to 8 row segments into the neighbour GPUs' frames,
 // publishes `value` in their flag words once every byte is visible system-wide, then waits until the neighbours have
 // published the same value here.  Flag values only grow, so nothing is ever reset.
@@ -87,23 +108,10 @@ size_t layer_smem_bytes(int cin, int cout);
 // One-time per process: raise the dynamic shared memory limit of every instantiation.
 cudaError_t init_kernels();
 
-// First layer (Cin = 1): same-size 3x3 correlation with BORDER_REPLICATE (src/modelHandler.cpp:141-142) on the frame of pw x ph
-// whose pixel (fy, fx) is the source plane's pixel (clamp(fy - pad_top), clamp(fx - pad_x)) -- i.e. cv::copyMakeBorder
-// (src/convertRoutine.cpp:35,96) is folded into the loads; pad_x = pad_top = 0 with w x h = pw x ph reads an already padded ROI.
-// rows_above / rows_below: real rows readable beyond the plane (row bands); cols_left / cols_right: real columns readable beyond
-// it (windows), so that frame column fx reads column clamp(fx - pad_x, -cols_left, w - 1 + cols_right).  pad_x is the LEFT pad:
-// the right pad is pw - w - pad_x, as the bottom pad is ph - h - pad_top.  -> RECORD frame.
-// up2x: the source plane is the nearest-neighbour 2x resize of `in` (pixel (y, x) = in[y >> 1][x >> 1]); w, h, the pads and the
-// row and column counts are in 2x rows / columns, `in` points at the source pixel holding 2x pixel (0, 0) (see first_layer_kernel).
+// First layer (Cin = 1): same-size 3x3 correlation with BORDER_REPLICATE (src/modelHandler.cpp:141-142) on src's frame of pw x ph,
+// whose padding is folded into the loads (FrameSource::padded() reads an already padded region).  -> RECORD frame.
 // `wgt` ([C][9]) and `bias` ((float)bias) are HOST pointers: they travel as kernel parameters.
-struct FirstSource {
-    const float *in;
-    long stride_floats;
-    int w, h, pad_x, pad_top, rows_above, rows_below;
-    bool up2x = false;
-    int cols_left = 0, cols_right = 0;
-};
-cudaError_t launch_first(const FirstSource &src, int pw, int ph, const float *wgt /*[C][9]*/, const float *bias, int cout, __half *out,
+cudaError_t launch_first(const FrameSource &src, int pw, int ph, const float *wgt /*[C][9]*/, const float *bias, int cout, __half *out,
                          cudaStream_t s, int f8 = 0, int out_y0 = 0, int out_rows = -1);
 // Tensor-core (wgmma) layer: in/out NHWC frames (pw x ph); the tensor maps are built inside.
 // `bias` is a HOST pointer to the layer's (float)bias values (they travel as kernel parameters).
@@ -120,12 +128,10 @@ cudaError_t launch_tc_layer(const __half *in, const void *wpack, const float *bi
 // row-band session keeps its halo rows out of the window because its neighbours write them.
 // Fused last layer: launch_tc_layer(..., last_w = HOST pointer to [9][cout] fp32 tap-major, partial = [ph][pw][12] fp32) makes the
 // tensor-core layer emit per-pixel tap partials instead of activations; launch_last_gather sums the 3x3
-// neighbourhood of partials, adds the bias, applies the leaky-ReLU and writes the cropped fp32 plane.
-cudaError_t launch_last_gather(const float *partial, int pw, int ph, float bias, int crop, float *dst,
+// neighbourhood of partials, adds the bias, applies the leaky-ReLU and writes the fp32 plane cropped by crop_x columns left and
+// right, crop_top rows above and crop_bottom rows below.
+cudaError_t launch_last_gather(const float *partial, int pw, int ph, float bias, int crop_x, int crop_top, int crop_bottom, float *dst,
                                long dst_stride_floats, cudaStream_t s);
-// general form: crop_x columns left/right, crop_top / crop_bottom rows
-cudaError_t launch_last_gather_xy(const float *partial, int pw, int ph, float bias, int crop_x, int crop_top,
-                                  int crop_bottom, float *dst, long dst_stride_floats, cudaStream_t s);
 inline size_t partial_bytes(int Wp, int Hp) { return (size_t)Hp * Wp * 12 * sizeof(float); }
 // Packed frames: independent planes side by side in one frame, each inside its own padded rectangle of (w + 2 pad) x (h + 2 pad)
 // pixels (pad = the model's layer count).  A DEVICE table of PlaneRect lists them by shelf: ascending y0, then ascending x0;

@@ -23,87 +23,46 @@ namespace w2x {
 constexpr unsigned MAX_GRID_Y = 65535;
 __device__ __forceinline__ int row_blocks(int rows, unsigned block_rows) { return (int)((rows + block_rows - 1) / block_rows); }
 
-// ---- cv::copyMakeBorder(BORDER_REPLICATE) (src/convertRoutine.cpp:35,96) ----------------------
-// rows_above/rows_below > 0 mean real neighbour rows exist there (row-band mode): the source
-// pointer addresses band row 0 and may be read at rows [-rows_above, h + rows_below); likewise cols_left/cols_right for
-// columns (windows).  pad_x is the left pad, pad_right the right one.
-__global__ void pad_replicate_kernel(const float *__restrict__ in, int w, int h, long in_stride,
-                                     int pad_x, int pad_top, int pad_bottom, int rows_above, int rows_below,
-                                     float *__restrict__ out, int skip_top, int skip_bottom, int pad_right, int cols_left,
-                                     int cols_right) {
-    const int W = w + pad_x + pad_right, H = h + pad_top + pad_bottom;
-    const int x = blockIdx.x * blockDim.x + threadIdx.x;
-    if (x >= W) return;
-    const int sx = min(max(x - pad_x, -cols_left), w - 1 + cols_right);
-    for (int by = blockIdx.y; by < row_blocks(H, blockDim.y); by += gridDim.y) {
-        const int y = by * blockDim.y + threadIdx.y;
-        if (y >= H - skip_bottom || y < skip_top) continue;
-        const int sy = min(max(y - pad_top, -rows_above), h - 1 + rows_below);
-        out[(long)y * W + x] = in[(long)sy * in_stride + sx];
-    }
-}
-
-// The same padding of the nearest-neighbour 2x resize of `in` (cv::resize INTER_NEAREST to exactly twice the size,
-// src/main.cpp:135-139, whose pixel (y, x) is in[y >> 1][x >> 1]): w2 x h2 are the 2x plane's (or band's) size, the rows count
-// in 2x rows, and the band starts on an even 2x row, so that its first row is the first copy of in's row 0.  The left and top pads
-// may be smaller than pad (a window starting on an odd 2x column / row), and cols_left / cols_right count real 2x columns.
-__global__ void pad_upsample2x_kernel(const float *__restrict__ in, int w2, int h2, long in_stride, int pad, int rows_above,
-                                      int rows_below, float *__restrict__ out, int pad_left, int pad_top, int cols_left,
-                                      int cols_right) {
-    const int W = w2 + pad_left + pad, H = h2 + pad_top + pad;
-    const int x = blockIdx.x * blockDim.x + threadIdx.x;
-    if (x >= W) return;
-    const int sx = min(max(x - pad_left, -cols_left), w2 - 1 + cols_right) >> 1;   // arithmetic shift: floor, also left of the window
-    for (int by = blockIdx.y; by < row_blocks(H, blockDim.y); by += gridDim.y) {
-        const int y = by * blockDim.y + threadIdx.y;
-        if (y >= H) continue;
-        const int sy = min(max(y - pad_top, -rows_above), h2 - 1 + rows_below) >> 1;   // arithmetic shift: floor, also above the band
-        out[(long)y * W + x] = in[(long)sy * in_stride + sx];
-    }
-}
-
-// The band-frame form of pad_upsample2x_kernel (pad_replicate_kernel's frame, read through the resize): separate top / bottom pads
-// and frame rows left to a neighbour GPU.  A thread owns 4 frame columns of one 2x row PAIR (2q, 2q + 1): clamping either row to
-// [-rows_above, h2 - 1 + rows_below] and halving gives the same source row (a clamp bound inside the pair pulls the other row onto
-// its partner), so the at most 3 source floats behind the 4 columns are read once, through the read-only path, and stored to both
-// rows -- as one 16-byte store each when VEC (frame rows of a multiple of 4 floats in a 16-byte aligned frame).
-template <bool VEC>
-__global__ void __launch_bounds__(256) pad_upsample2x_xy_kernel(const float *__restrict__ in, int w2, int h2, long in_stride, int pad_x,
-                                                                int pad_top, int pad_bottom, int rows_above, int rows_below,
-                                                                float *__restrict__ out, int skip_top, int skip_bottom, int pad_right,
-                                                                int cols_left, int cols_right) {
-    const int W = w2 + pad_x + pad_right, H = h2 + pad_top + pad_bottom;
-    const int x0 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
-    if (x0 >= W) return;
-    const int q0 = -((pad_top + 1) >> 1);                  // the pair holding frame row 0 (2x row -pad_top)
-    const int pairs = ((h2 + pad_bottom - 1) >> 1) - q0 + 1;
-    int sx[4];
+// ---- cv::copyMakeBorder(BORDER_REPLICATE) (src/convertRoutine.cpp:35,96): a FrameSource's frame, materialised ----------------
+// A thread owns 4 columns of the two frame rows of a PAIR of plane rows (2q, 2q + 1), and writes those of frame rows [y_lo, y_hi).
+// Each row reads the source row its clamp gives; when both read the same one, it is read once and stored twice.  With UP2X that is
+// always so (a clamp bound inside the pair pulls the other row onto its partner), and the at most 3 source floats behind 4 adjacent
+// columns are read once too.  VEC (frame rows of a multiple of 4 floats in a 16-byte aligned frame): the 4 columns are adjacent and
+// leave as one 16-byte store per row; else they are 32 apart, so that each store of a warp covers 32 adjacent columns.
+template <bool UP2X, bool VEC>
+__global__ void __launch_bounds__(256) pad_kernel(const FrameSource src, int pw, float *__restrict__ out, int q0, int pairs, int y_lo,
+                                                  int y_hi) {
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    int x[4], sx[4];
 #pragma unroll
-    for (int j = 0; j < 4; j++) sx[j] = min(max(x0 + j - pad_x, -cols_left), w2 - 1 + cols_right) >> 1;
+    for (int j = 0; j < 4; j++) {
+        x[j] = VEC ? 4 * t + j : 4 * (t & ~31) + (t & 31) + 32 * j;
+        sx[j] = frame_src<UP2X>(x[j], src.pad_x, src.w, src.cols_left, src.cols_right);
+    }
+    if (x[0] >= pw) return;
     for (int by = blockIdx.y; by < row_blocks(pairs, blockDim.y); by += gridDim.y) {
         const int p = by * blockDim.y + threadIdx.y;
         if (p >= pairs) continue;
-        const int y = 2 * (q0 + p);                        // the pair's first 2x row; frame rows y + pad_top and y + pad_top + 1
-        const int fy = y + pad_top;
-        const bool st0 = fy >= skip_top && fy < H - skip_bottom, st1 = fy + 1 >= skip_top && fy + 1 < H - skip_bottom;
-        if (!st0 && !st1) continue;
-        const int sy = min(max(y, -rows_above), h2 - 1 + rows_below) >> 1;   // arithmetic shift: floor, also above the band
-        const float *row = in + (long)sy * in_stride;
+        const float *row = nullptr;
         float v[4];
-        v[0] = __ldg(row + sx[0]);
 #pragma unroll
-        for (int j = 1; j < 4; j++) v[j] = sx[j] == sx[j - 1] ? v[j - 1] : __ldg(row + sx[j]);
-        float *o = out + (long)fy * W + x0;
-        if (VEC) {
-            const float4 v4 = make_float4(v[0], v[1], v[2], v[3]);
-            if (st0) *reinterpret_cast<float4 *>(o) = v4;
-            if (st1) *reinterpret_cast<float4 *>(o + W) = v4;
-        } else {
+        for (int i = 0; i < 2; i++) {
+            const int fy = 2 * (q0 + p) + i + src.pad_top;
+            if (fy < y_lo || fy >= y_hi) continue;
+            const float *r = src.in + (long)frame_src<UP2X>(fy, src.pad_top, src.h, src.rows_above, src.rows_below) * src.stride_floats;
+            if (r != row) {
+                row = r;
+                v[0] = __ldg(row + sx[0]);
 #pragma unroll
-            for (int j = 0; j < 4; j++) {
-                if (x0 + j >= W) break;
-                if (st0) o[j] = v[j];
-                if (st1) o[W + j] = v[j];
+                for (int j = 1; j < 4; j++) v[j] = sx[j] == sx[j - 1] ? v[j - 1] : __ldg(row + sx[j]);
+            }
+            float *o = out + (long)fy * pw;
+            if (VEC) {
+                *reinterpret_cast<float4 *>(o + x[0]) = make_float4(v[0], v[1], v[2], v[3]);
+            } else {
+#pragma unroll
+                for (int j = 0; j < 4; j++)
+                    if (x[j] < pw) o[x[j]] = v[j];
             }
         }
     }
@@ -304,49 +263,22 @@ conv3x3_planar_fp32(const float *__restrict__ in, float *__restrict__ out,
 // ---- launchers --------------------------------------------------------------------------------
 static inline dim3 grid2d(int w, int h, dim3 b) { return dim3((w + b.x - 1) / b.x, std::min<unsigned>((h + b.y - 1) / b.y, MAX_GRID_Y)); }
 
-cudaError_t launch_pad_replicate(const float *in, int w, int h, long in_stride_floats, int pad,
-                                 int rows_above, int rows_below, float *out, cudaStream_t s, int cols_left, int cols_right) {
-    return launch_pad_replicate_xy(in, w, h, in_stride_floats, pad, pad, pad, rows_above, rows_below, out, s, 0, 0, cols_left, cols_right);
-}
-
-cudaError_t launch_pad_replicate_xy(const float *in, int w, int h, long in_stride_floats, int pad_x, int pad_top,
-                                    int pad_bottom, int rows_above, int rows_below, float *out, cudaStream_t s,
-                                    int skip_top, int skip_bottom, int cols_left, int cols_right, int pad_right) {
-    if (pad_right < 0) pad_right = pad_x;
-    dim3 b(32, 8);
-    pad_replicate_kernel<<<grid2d(w + pad_x + pad_right, h + pad_top + pad_bottom, b), b, 0, s>>>(
-        in, w, h, in_stride_floats, pad_x, pad_top, pad_bottom, rows_above, rows_below, out, skip_top, skip_bottom, pad_right,
-        cols_left, cols_right);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_pad_upsample2x(const float *in, int w2, int h2, long in_stride_floats, int pad, int rows_above, int rows_below,
-                                  float *out, cudaStream_t s, int cols_left, int cols_right, int pad_left, int pad_top) {
-    if (pad_left < 0) pad_left = pad;
-    if (pad_top < 0) pad_top = pad;
-    dim3 b(32, 8);
-    pad_upsample2x_kernel<<<grid2d(w2 + pad_left + pad, h2 + pad_top + pad, b), b, 0, s>>>(in, w2, h2, in_stride_floats, pad, rows_above,
-                                                                                          rows_below, out, pad_left, pad_top, cols_left,
-                                                                                          cols_right);
-    return cudaGetLastError();
-}
-
-// A row band's padded 2x input frame, materialised.  Folding the resize into the band's first-layer loads (the first_1xN+up2x form
-// of the one-GPU chain) is deliberately not done: the frame is 4 bytes per pixel beside 512 bytes per pixel of activations, and the
-// fold would need the halo exchange to deliver half-resolution rows into a side buffer instead of a row of the frame.
-cudaError_t launch_pad_upsample2x_xy(const float *in, int w2, int h2, long in_stride_floats, int pad_x, int pad_top, int pad_bottom,
-                                     int rows_above, int rows_below, float *out, cudaStream_t s, int skip_top, int skip_bottom,
-                                     int cols_left, int cols_right, int pad_right) {
-    if (pad_right < 0) pad_right = pad_x;
-    const int W = w2 + pad_x + pad_right, pairs = ((h2 + pad_bottom - 1) >> 1) + ((pad_top + 1) >> 1) + 1;
-    dim3 b(32, 8);
-    const dim3 g = grid2d((W + 3) / 4, pairs, b);
-    if (W % 4 == 0 && reinterpret_cast<uintptr_t>(out) % 16 == 0)
-        pad_upsample2x_xy_kernel<true><<<g, b, 0, s>>>(in, w2, h2, in_stride_floats, pad_x, pad_top, pad_bottom, rows_above, rows_below, out,
-                                                       skip_top, skip_bottom, pad_right, cols_left, cols_right);
-    else
-        pad_upsample2x_xy_kernel<false><<<g, b, 0, s>>>(in, w2, h2, in_stride_floats, pad_x, pad_top, pad_bottom, rows_above, rows_below, out,
-                                                        skip_top, skip_bottom, pad_right, cols_left, cols_right);
+// A row band's padded 2x input frame is materialised here too.  Folding the resize into the band's first-layer loads (the
+// first_1xN+up2x form of the one-GPU chain) is deliberately not done: the frame is 4 bytes per pixel beside 512 bytes per pixel of
+// activations, and the fold would need the halo exchange to deliver half-resolution rows into a side buffer instead of a row of the
+// frame.
+cudaError_t launch_pad(const FrameSource &src, int pw, int ph, float *out, cudaStream_t s, int out_y0, int out_rows) {
+    if (out_rows < 0) { out_y0 = 0; out_rows = ph; }
+    if (out_y0 < 0 || out_rows < 1 || out_y0 + out_rows > ph) return cudaErrorInvalidValue;
+    // the pairs of plane rows (2q, 2q + 1) behind the window: q0 .. q1
+    const int q0 = (out_y0 - src.pad_top) >> 1, q1 = (out_y0 + out_rows - 1 - src.pad_top) >> 1;
+    const dim3 b(32, 8), g = grid2d((pw + 3) / 4, q1 - q0 + 1, b);
+    const bool vec = pw % 4 == 0 && reinterpret_cast<uintptr_t>(out) % 16 == 0;
+    auto go = [&](void (*kernel)(const FrameSource, int, float *, int, int, int, int)) {
+        kernel<<<g, b, 0, s>>>(src, pw, out, q0, q1 - q0 + 1, out_y0, out_y0 + out_rows);
+    };
+    if (src.up2x) go(vec ? pad_kernel<true, true> : pad_kernel<true, false>);
+    else go(vec ? pad_kernel<false, true> : pad_kernel<false, false>);
     return cudaGetLastError();
 }
 

@@ -147,7 +147,7 @@ cudaError_t launch_tc_layer(const __half *in, const void *wpack, const float *bi
 }
 
 template <int COUT>
-static cudaError_t launch_first_c(const FirstSource &src, int pw, int ph, const float *wgt, const float *bias, __half *out, cudaStream_t s, int f8,
+static cudaError_t launch_first_c(const FrameSource &src, int pw, int ph, const float *wgt, const float *bias, __half *out, cudaStream_t s, int f8,
                                   int out_y0, int out_rows) {
     static_assert(FIRST_TILE_BYTES + 1024 <= 48 * 1024, "the first layer's staging tile stays under the default dynamic shared memory limit");
     FirstParams<COUT> prm;                                    // HOST pointers -> kernel parameters; ACT_SCALE folded in (exact: a power of two)
@@ -155,22 +155,21 @@ static cudaError_t launch_first_c(const FirstSource &src, int pw, int ph, const 
         for (int k = 0; k < 9; k++) prm.w[p * 9 + k] = make_float2(wgt[(2 * p) * 9 + k] * ACT_SCALE, wgt[(2 * p + 1) * 9 + k] * ACT_SCALE);
         prm.b[p] = make_float2(bias[2 * p] * ACT_SCALE, bias[2 * p + 1] * ACT_SCALE);
     }
-    FirstSrc fs{src.in, src.stride_floats, src.w, src.h, src.pad_x, src.pad_top, src.rows_above, src.rows_below, src.cols_left, src.cols_right};
     CUtensorMap omap;
     dim3 grid((pw + 31) / 32, (out_rows + 7) / 8);   // blocks tile the store window
     if (grid.y > 65535) return cudaErrorInvalidConfiguration;
     if (make_rec_map(&omap, out, COUT, pw, ph, 32, 8, out_y0, out_rows)) return cudaErrorInvalidValue;
     if (src.up2x) {
-        if (f8) first_layer_kernel<COUT, true, true><<<grid, 256, FIRST_TILE_BYTES + 1024, s>>>(fs, pw, ph, out_y0, omap, prm);
-        else first_layer_kernel<COUT, false, true><<<grid, 256, FIRST_TILE_BYTES + 1024, s>>>(fs, pw, ph, out_y0, omap, prm);
+        if (f8) first_layer_kernel<COUT, true, true><<<grid, 256, FIRST_TILE_BYTES + 1024, s>>>(src, pw, ph, out_y0, omap, prm);
+        else first_layer_kernel<COUT, false, true><<<grid, 256, FIRST_TILE_BYTES + 1024, s>>>(src, pw, ph, out_y0, omap, prm);
     } else {
-        if (f8) first_layer_kernel<COUT, true, false><<<grid, 256, FIRST_TILE_BYTES + 1024, s>>>(fs, pw, ph, out_y0, omap, prm);
-        else first_layer_kernel<COUT, false, false><<<grid, 256, FIRST_TILE_BYTES + 1024, s>>>(fs, pw, ph, out_y0, omap, prm);
+        if (f8) first_layer_kernel<COUT, true, false><<<grid, 256, FIRST_TILE_BYTES + 1024, s>>>(src, pw, ph, out_y0, omap, prm);
+        else first_layer_kernel<COUT, false, false><<<grid, 256, FIRST_TILE_BYTES + 1024, s>>>(src, pw, ph, out_y0, omap, prm);
     }
     return cudaGetLastError();
 }
 
-cudaError_t launch_first(const FirstSource &src, int pw, int ph, const float *wgt, const float *bias, int cout, __half *out, cudaStream_t s, int f8,
+cudaError_t launch_first(const FrameSource &src, int pw, int ph, const float *wgt, const float *bias, int cout, __half *out, cudaStream_t s, int f8,
                          int out_y0, int out_rows) {
     if (out_rows < 0) { out_y0 = 0; out_rows = ph; }
     switch (cout) {
@@ -200,13 +199,8 @@ cudaError_t launch_last(const __half *in, int cin, int pw, int ph, const float *
     return cudaGetLastError();
 }
 
-cudaError_t launch_last_gather(const float *partial, int pw, int ph, float bias, int crop, float *dst,
+cudaError_t launch_last_gather(const float *partial, int pw, int ph, float bias, int crop_x, int crop_top, int crop_bottom, float *dst,
                                long dst_stride_floats, cudaStream_t s) {
-    return launch_last_gather_xy(partial, pw, ph, bias, crop, crop, crop, dst, dst_stride_floats, s);
-}
-
-cudaError_t launch_last_gather_xy(const float *partial, int pw, int ph, float bias, int crop_x, int crop_top,
-                                  int crop_bottom, float *dst, long dst_stride_floats, cudaStream_t s) {
     const int ow = pw - 2 * crop_x, oh = ph - crop_top - crop_bottom;
     if (ow < 1 || oh < 1 || crop_x < 1 || crop_top < 1 || crop_bottom < 1) return cudaErrorInvalidValue;
     dim3 grid((ow + 31) / 32, (oh + 7) / 8);

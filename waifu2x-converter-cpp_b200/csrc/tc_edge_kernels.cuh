@@ -8,9 +8,8 @@
 // ================================================================================================
 // First layer: Model::filterWorker with nInputPlanes = 1 on the replicate-padded plane; writes the RECORD frame the tensor-core
 // layers consume.  One thread per pixel, 32 x 8 pixels per block.
-//   * the plane is NOT padded beforehand: `in` is the caller's plane (w x h, possibly a row band with real rows above / below)
-//     and frame pixel (fy, fx) reads in[clamp(fy - pad_y), clamp(fx - pad_x)] -- cv::copyMakeBorder(BORDER_REPLICATE)
-//     (src/convertRoutine.cpp:35,96) folded into the loads;
+//   * the plane is NOT padded beforehand: the frame is a FrameSource (kernels.h), whose pixels are read through frame_src --
+//     cv::copyMakeBorder(BORDER_REPLICATE) (src/convertRoutine.cpp:35,96) folded into the loads;
 //   * two output channels per step (channel pairs) with the weight PAIRS straight from the constant bank
 //     (kernel parameters -> uniform registers) and the pixel broadcast to both halves; every lane's arithmetic is the
 //     reference's: per tap an fma chain, + (float)bias, leaky = max(v, 0.1f v) (= min(v,0)*0.1f + max(v,0) bit for bit).
@@ -29,22 +28,10 @@ __device__ __forceinline__ float2 f32x2_fma(float2 a, float2 b, float2 c) { retu
 __device__ __forceinline__ float2 f32x2_mul(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 __device__ __forceinline__ float2 f32x2_add(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 
-// in: plane of w x h (row stride in_stride), readable at rows [-rows_above, h + rows_below) and columns [-cols_left, w + cols_right);
-// frame pixel (fy, fx) reads the plane at (fy - pad_top, fx - pad_x) clamped to that readable rectangle
-struct FirstSrc {
-    const float *in;
-    long in_stride;
-    int w, h, pad_x, pad_top, rows_above, rows_below, cols_left, cols_right;
-};
-
-// UP2X: the plane of w x h the frame pads is the nearest-neighbour 2x resize of `in` (cv::resize INTER_NEAREST to exactly twice
-// the size, src/main.cpp:135-139), never materialised: its pixel (y, x) is in[y >> 1][x >> 1].  Row 0 of that virtual plane is the
-// first copy of in's row 0, so a band starting on an odd 2x row has pad_top one smaller, rows_above one smaller and h one larger
-// than its even-row neighbour would (tc::FirstSource::up2x, set up by the engine); a window starting on an odd 2x column likewise
-// has pad_x and cols_left one smaller and w one larger.
+// UP2X = src.up2x.
 template <int COUT, bool F8, bool UP2X>
 __global__ void __launch_bounds__(256, 4)
-first_layer_kernel(const FirstSrc src, int pw, int ph, int out_y0, const __grid_constant__ CUtensorMap tmap_out,
+first_layer_kernel(const FrameSource src, int pw, int ph, int out_y0, const __grid_constant__ CUtensorMap tmap_out,
                    const __grid_constant__ FirstParams<COUT> prm) {
     extern __shared__ uint8_t first_smem[];
     const uint32_t tile = (smem_u32(first_smem) + 1023u) & ~1023u;
@@ -58,9 +45,9 @@ first_layer_kernel(const FirstSrc src, int pw, int ph, int out_y0, const __grid_
             // same-size correlation on the padded plane with BORDER_REPLICATE (src/modelHandler.cpp:141-142), the padded plane itself
             // being the replicate-padded input: clamp to the frame, then to the rows / columns that really exist
             const int fy = min(max(y + ky - 1, 0), ph - 1), fx = min(max(x + kx - 1, 0), pw - 1);
-            const int sy = min(max(fy - src.pad_top, -src.rows_above), src.h - 1 + src.rows_below), sx = min(max(fx - src.pad_x, -src.cols_left), src.w - 1 + src.cols_right);
-            const int ry = UP2X ? sy >> 1 : sy, rx = UP2X ? sx >> 1 : sx;   // arithmetic shift: floor, also above and to the left
-            v[ky * 3 + kx] = __ldg(src.in + (long)ry * src.in_stride + rx);
+            const int ry = frame_src<UP2X>(fy, src.pad_top, src.h, src.rows_above, src.rows_below);
+            const int rx = frame_src<UP2X>(fx, src.pad_x, src.w, src.cols_left, src.cols_right);
+            v[ky * 3 + kx] = __ldg(src.in + (long)ry * src.stride_floats + rx);
         }
     const uint32_t r = (uint32_t)threadIdx.x;                            // pixel index inside the block = row of the staged image
     const uint32_t sw128 = r & 7u;
@@ -207,7 +194,7 @@ last_gather_kernel(const float *__restrict__ partial, int pw, int ph, float bias
 // Frame pixel (y, x) of the padded fp32 image: cv::copyMakeBorder(plane, pad, BORDER_REPLICATE) (src/convertRoutine.cpp:35)
 // inside a rectangle, 0 everywhere else.  One thread per frame pixel, 32 x 8 per block.
 // UP2X: the plane of R.w x R.h is the nearest-neighbour 2x resize of R.src (src/main.cpp:135-139), never materialised: its pixel
-// (y, x) is src[y >> 1][x >> 1], as in first_layer_kernel<..., true> and pad_upsample2x_kernel.
+// (y, x) is src[y >> 1][x >> 1], as in FrameSource::up2x.
 template <bool UP2X>
 __global__ void __launch_bounds__(256)
 pack_planes_kernel(const PlaneRect *__restrict__ rect, const int *__restrict__ shelf_y0, const int *__restrict__ shelf_first,
@@ -230,8 +217,7 @@ pack_planes_kernel(const PlaneRect *__restrict__ rect, const int *__restrict__ s
     const int px = x - R.x0, py = y - R.y0;
     float v = 0.f;
     if (px >= 0 && py >= 0 && px < R.w + 2 * pad && py < R.h + 2 * pad) {
-        const int sx = min(max(px - pad, 0), R.w - 1), sy = min(max(py - pad, 0), R.h - 1);
-        v = __ldg(R.src + (long)(UP2X ? sy >> 1 : sy) * R.src_stride + (UP2X ? sx >> 1 : sx));
+        v = __ldg(R.src + (long)frame_src<UP2X>(py, pad, R.h, 0, 0) * R.src_stride + frame_src<UP2X>(px, pad, R.w, 0, 0));
     }
     frame[(size_t)y * fw + x] = v;
 }
