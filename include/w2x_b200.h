@@ -168,8 +168,8 @@ W2X_API void *w2x_host_alloc(size_t bytes);
 W2X_API void w2x_host_free(void *p);
 
 /* ---- the hot path ------------------------------------------------------------------------- */
-/* Device memory of w2x_convert_plane*, w2x_convert_planes*, w2x_convert_chain*, w2x_convert_planes_chain* and
- * w2x_convert_chain_region*: every buffer a call uses (the host entries' staging, the planes between steps, TTA variants, packed
+/* Device memory of w2x_convert_plane*, w2x_convert_planes*, w2x_convert_chain*, w2x_convert_planes_chain*,
+ * w2x_convert_chain_region* and w2x_convert_chain_regions*: every buffer a call uses (the host entries' staging, the planes between steps, TTA variants, packed
  * frames, activation and padding scratch) is reserved before its first progress line, on_step call, copy or launch, so
  * W2X_ERR_NOMEM leaves nothing logged, called back or queued.  The context keeps its buffers for later calls. */
 /* Replaces bool w2xc::convertWithModels(cv::Mat& in, cv::Mat& out, models, bool blockSplitting)
@@ -383,6 +383,37 @@ W2X_API int w2x_convert_chain_region(w2x_ctx *ctx, int n_steps, const w2x_model 
 W2X_API int w2x_convert_chain_region_device(w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, int width,
                                             int height, const int *window, const float *d_src, size_t src_stride_bytes, float *d_out,
                                             size_t out_stride_bytes, w2x_step_fn on_step, void *user);
+/* Many windows in one call, packed side by side into shared frames: the tiles of a scan too large to hold, the visible tiles of a
+ * viewer, patches of many images for a dataset.  Window i is windows[4 i .. 4 i + 3] = {x0, y0, w, h} of the chain's output on a
+ * widths[i] x heights[i] input plane; the steps are shared by every window.  src[i] points at the top-left pixel of window i's
+ * source rectangle (w2x_chain_region_source), row stride src_strides[i] bytes, and nothing outside that rectangle is read; out[i]
+ * receives the w x h window, row stride out_strides[i] bytes.  Several windows may come from one plane, and their source rectangles
+ * may overlap or share memory; the outputs must not overlap one another or any source (as in w2x_convert_planes_chain).
+ * Bits: every window is bit-identical to w2x_convert_chain_region on that window alone, and so to the same window of
+ * w2x_convert_chain(..., block_splitting = 0), on the same context settings (both engines, every precision).
+ * Packing: each step packs the windows' step outputs into frames as w2x_convert_planes* does, planned by their output-window sizes;
+ * a frame's rectangle holds the window's real neighbours as its padding, so that only the plane's own border is replicated.  A
+ * window too large for a frame is converted alone, in scratch bands if needed.  The fp32 engine, or a model without the fused last
+ * layer, converts window by window.  Step k launches what w2x_convert_planes_device launches for planes of the step's output-window
+ * sizes.
+ * Before step k is queued, on_step(k, user) is called (if not NULL); then the step logs, window by window in order, the lines
+ * w2x_convert_chain_region logs for that window at step k (both entries log them so).
+ * Every argument is checked before anything is printed, allocated or queued.  W2X_ERR_ARG names the step or the window: n_windows
+ * < 1 or a NULL array; a W2X_STEP_TTA step, an unknown kind or a model that does not map 1 plane to 1 plane (naming the step);
+ * per window, every check of w2x_convert_chain_region, its message prefixed by "window i: ".  A model the context's engine refuses
+ * gives W2X_ERR_UNSUPPORTED naming the step.  Every buffer is reserved first, so W2X_ERR_NOMEM leaves nothing queued.
+ * HOST buffers, synchronous: each source rectangle is staged densely on the device, uploads overlap step 0 and downloads the last
+ * step. */
+W2X_API int w2x_convert_chain_regions(w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, int n_windows,
+                                      const int *widths, const int *heights, const int *windows, const float *const *src,
+                                      const size_t *src_strides, float *const *out, const size_t *out_strides, w2x_step_fn on_step,
+                                      void *user);
+/* Same on DEVICE buffers (the pointer, size, window and stride arrays themselves are host arrays), asynchronous on the context's
+ * stream. */
+W2X_API int w2x_convert_chain_regions_device(w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds,
+                                             int n_windows, const int *widths, const int *heights, const int *windows,
+                                             const float *const *d_src, const size_t *src_strides, float *const *d_out,
+                                             const size_t *out_strides, w2x_step_fn on_step, void *user);
 
 /* ---- a chain of conversions on a collection of planes of any sizes ------------------------------------ */
 /* w2x_convert_chain for every plane of a w2x_convert_planes collection, in one call: the default noise_scale mode of a sprite set,

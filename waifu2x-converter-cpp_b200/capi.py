@@ -43,7 +43,7 @@ ABI_SYMBOLS = (
     "w2x_convert_planes", "w2x_convert_planes_device", "w2x_convert_chain", "w2x_convert_chain_device",
     "w2x_convert_planes_chain", "w2x_convert_planes_chain_device", "w2x_multi_convert_chain",
     "w2x_multi_convert_planes", "w2x_multi_convert_planes_chain", "w2x_chain_region_source", "w2x_convert_chain_region",
-    "w2x_convert_chain_region_device",
+    "w2x_convert_chain_region_device", "w2x_convert_chain_regions", "w2x_convert_chain_regions_device",
 )
 BAND_BLOB_BYTES = 320
 
@@ -151,6 +151,8 @@ def lib():
     L.w2x_chain_region_source.argtypes = [ci, C.POINTER(vp), pi, ci, ci, pi, pi]
     L.w2x_convert_chain_region.argtypes = [vp, ci, C.POINTER(vp), pi, ci, ci, pi, vp, cs, vp, cs, STEP_FN, vp]
     L.w2x_convert_chain_region_device.argtypes = [vp, ci, C.POINTER(vp), pi, ci, ci, pi, vp, cs, vp, cs, STEP_FN, vp]
+    L.w2x_convert_chain_regions.argtypes = [vp, ci, C.POINTER(vp), pi, ci, pi, pi, pi, C.POINTER(vp), ps, C.POINTER(vp), ps, STEP_FN, vp]
+    L.w2x_convert_chain_regions_device.argtypes = [vp, ci, C.POINTER(vp), pi, ci, pi, pi, pi, C.POINTER(vp), ps, C.POINTER(vp), ps, STEP_FN, vp]
     L.w2x_convert_planes_chain.argtypes = [vp, ci, C.POINTER(vp), pi, ci, C.POINTER(vp), pi, pi, ps, C.POINTER(vp), ps, STEP_FN, vp]
     L.w2x_convert_planes_chain_device.argtypes = [vp, ci, C.POINTER(vp), pi, ci, C.POINTER(vp), pi, pi, ps, C.POINTER(vp), ps, STEP_FN, vp]
     L.w2x_debug_plan_planes.argtypes = [ci, pi, pi, ci, ci, cs, pi, pi, pi, pi, ci]
@@ -263,6 +265,14 @@ def debug_plan_multi_planes(n_devices, steps, widths, heights):
     if nd < 0:
         raise W2xError(-nd, lib().w2x_last_error().decode())
     return nd, owner, load[:nd]
+
+
+def _c_view(p):
+    """p as float32, copied only when its rows are not evenly strided unit-stride rows the C ABI can take"""
+    x = np.asarray(p, np.float32)
+    if x.ndim == 2 and (x.strides[1] != 4 or x.strides[0] % 4 or x.strides[0] < x.shape[1] * 4):
+        x = np.ascontiguousarray(x)
+    return x
 
 
 def _plane_arrays(planes, fix):
@@ -473,12 +483,7 @@ class Context:
     @staticmethod
     def _planes_args(planes, out, ups):
         """inputs and outputs of a planes call whose planes come out (h << ups) x (w << ups)"""
-        def fix(p):
-            x = np.asarray(p, np.float32)
-            if x.ndim == 2 and (x.strides[1] != 4 or x.strides[0] % 4 or x.strides[0] < x.shape[1] * 4):
-                x = np.ascontiguousarray(x)
-            return x
-        xs, ip, ws, hs, ist = _plane_arrays(planes, fix)
+        xs, ip, ws, hs, ist = _plane_arrays(planes, _c_view)
         shapes = [(x.shape[0] << ups, x.shape[1] << ups) for x in xs]
         if out is None:
             out = [np.empty(s, np.float32) for s in shapes]
@@ -573,6 +578,55 @@ class Context:
         win = (C.c_int * 4)(*[int(v) for v in window])
         _check(lib().w2x_convert_chain_region_device(self._h, n, models, kinds, int(size[0]), int(size[1]), win, C.c_void_p(d_src),
                                                      src_stride_bytes, C.c_void_p(d_out), out_stride_bytes, cb, None))
+
+    # many windows of chains' outputs in one call, each step packing the windows into frames
+    def convert_chain_regions(self, steps, sources, sizes, windows, out=None, on_step=None):
+        """Window i = windows[i] (x0, y0, w, h) of convert_chain(steps, plane_i, block_splitting=False) on a plane of sizes[i] =
+        (width, height), from sources[i] alone: the 2-D float32 source rectangle chain_region_source(steps, sizes[i], windows[i]) of
+        that plane (row-strided views, such as slices of the whole plane, are passed as they are; several may share one plane) ->
+        the list of h x w windows; `out` may be such a list (strided views included), written in place.  on_step(k) is called before
+        step k."""
+        if not (len(sources) == len(sizes) == len(windows)):
+            raise ValueError("sources, sizes and windows must have one entry per window")
+        xs, sp, _, _, sst = _plane_arrays(sources, _c_view)
+        for i, (x, size, win) in enumerate(zip(xs, sizes, windows)):
+            try:
+                sx0, sy0, sw, sh = chain_region_source(steps, size, win)
+            except W2xError:            # the call below refuses the same arguments, in its own name
+                continue
+            if x.shape != (sh, sw):
+                raise ValueError(f"window {i}: source must be the source rectangle {(sx0, sy0, sw, sh)}: shape {(sh, sw)}, not {x.shape}")
+        shapes = [(int(win[3]), int(win[2])) for win in windows]
+        if out is None:
+            out = [np.empty(s, np.float32) for s in shapes]
+        if len(out) != len(xs) or any(o.ndim != 2 or o.dtype != np.float32 or o.shape != s for o, s in zip(out, shapes)):
+            raise ValueError("out must hold one 2-D float32 array per window, of the window's shape")
+        if any(o.strides[1] != 4 or o.strides[0] % 4 for o in out):
+            raise ValueError("out arrays need unit column stride and row strides that are multiples of 4 bytes")
+        _, op, _, _, ost = _plane_arrays(out, lambda o: o)
+        n, models, kinds, cb, _ = self._chain_args(steps, on_step)
+        k = len(xs)
+        ws, hs, wins = self._regions_args(sizes, windows)
+        _check(lib().w2x_convert_chain_regions(self._h, n, models, kinds, k, ws, hs, wins, sp, sst, op, ost, cb, None))
+        return out
+
+    @staticmethod
+    def _regions_args(sizes, windows):
+        k = len(windows)
+        ws = (C.c_int * max(k, 1))(*[int(s[0]) for s in sizes])
+        hs = (C.c_int * max(k, 1))(*[int(s[1]) for s in sizes])
+        wins = (C.c_int * max(4 * k, 1))(*[int(v) for win in windows for v in win])
+        return ws, hs, wins
+
+    def convert_chain_regions_device(self, steps, d_src, sizes, windows, src_strides, d_out, out_strides, on_step=None):
+        """Device pointers (ints): d_src[i] at window i's source rectangle's top-left pixel, d_out[i] receiving window i; host lists
+        of plane sizes, windows and row strides in bytes; asynchronous on the context's stream."""
+        n, models, kinds, cb, _ = self._chain_args(steps, on_step)
+        k = len(d_src)
+        ws, hs, wins = self._regions_args(sizes, windows)
+        _check(lib().w2x_convert_chain_regions_device(self._h, n, models, kinds, k, ws, hs, wins, (C.c_void_p * max(k, 1))(*d_src),
+                                                      (C.c_size_t * max(k, 1))(*src_strides), (C.c_void_p * max(k, 1))(*d_out),
+                                                      (C.c_size_t * max(k, 1))(*out_strides), cb, None))
 
     # convert_chain for every plane of a convert_planes collection, each step packing the planes into frames
     def convert_planes_chain(self, steps, planes, out=None, on_step=None):

@@ -419,11 +419,27 @@ int reserve_convert(w2x_ctx *ctx, const w2x_model *m, int engine, int w, int h, 
     return rc;
 }
 
+// Where a plane (or a window of one) comes from and goes to (row strides in bytes), and the real neighbours its source holds
+// beyond it: rows above and below, columns left and right (all 0 for a whole plane).  up2x (an upscaling step): the counts are in
+// 2x pixels, src points at the source pixel holding the window's first row and column, and phase_y / phase_x = 1 when those are
+// that pixel's second copies (a window starting on an odd 2x row / column).
+struct PlaneIO {
+    const float *src; size_t src_stride; float *dst; size_t dst_stride;
+    int above = 0, below = 0, left = 0, right = 0, phase_x = 0, phase_y = 0;
+};
+
+// The frame a model of n layers converts for the w x h window of p: cv::copyMakeBorder(BORDER_REPLICATE) by n
+// (src/convertRoutine.cpp:35, :96) at the plane's own border, up to n real neighbour rows and columns elsewhere.  The one
+// description of a window's frame: convert_device's first layer or padding kernel reads it, and a packed frame's rectangle holds it.
+FrameSource window_frame(const PlaneIO &p, int w, int h, int n, bool up2x) {
+    const int px = up2x ? p.phase_x : 0, py = up2x ? p.phase_y : 0;
+    return FrameSource{p.src, (long)(p.src_stride / 4), w + px, h + py, n - px, n - py, std::min(p.above, n) - py, std::min(p.below, n), up2x,
+                       std::min(p.left, n) - px, std::min(p.right, n)};
+}
+
 // convertWithModels on checked device buffers (rows_above / rows_below: real neighbour rows available around the band;
 // cols_left / cols_right: real neighbour columns left and right of it, for a window).  up2x: the plane converted is the
-// nearest-neighbour 2x resize of d_in, never materialised; w x h is its (2x) size, the row and column counts are in 2x pixels, and
-// d_in points at the source pixel holding its first row and column, which are the first copies of that pixel's row and column --
-// or, with phase_y / phase_x = 1 (a window starting on an odd 2x row / column), the second ones.
+// nearest-neighbour 2x resize of d_in, never materialised; w x h is its (2x) size, and the counts and phases are PlaneIO's.
 int convert_device(w2x_ctx *ctx, const w2x_model *m, const float *d_in, int w, int h, size_t in_stride_bytes,
                    int rows_above, int rows_below, float *d_out, size_t out_stride_bytes, int block_splitting, bool up2x = false,
                    int cols_left = 0, int cols_right = 0, int phase_x = 0, int phase_y = 0) {
@@ -436,14 +452,14 @@ int convert_device(w2x_ctx *ctx, const w2x_model *m, const float *d_in, int w, i
     if (rc) return rc;
     const int n = (int)m->layers.size();
     const int pw = w + 2 * n;
-    const long istride = (long)(in_stride_bytes / 4), ostride = (long)(out_stride_bytes / 4);
+    const long ostride = (long)(out_stride_bytes / 4);
     const bool literal = literal_walk(ctx, w, h, block_splitting);
     // cv::copyMakeBorder(in, temp, n, n, n, n, BORDER_REPLICATE)   (src/convertRoutine.cpp:35, :96): the plane's frame.  The
     // tensor-core engine folds it into the first layer's loads and reads d_in directly, except on the literal walk, whose blocks
     // are regions of the padded plane.
-    const int px = up2x ? phase_x : 0, py = up2x ? phase_y : 0;
-    const FrameSource plane{d_in, istride, w + px, h + py, n - px, n - py, std::min(rows_above, n) - py, std::min(rows_below, n), up2x,
-                            std::min(cols_left, n) - px, std::min(cols_right, n)};
+    const FrameSource plane = window_frame(PlaneIO{d_in, in_stride_bytes, d_out, out_stride_bytes, rows_above, rows_below, cols_left, cols_right,
+                                                   phase_x, phase_y},
+                                           w, h, n, up2x);
     const bool direct = engine == W2X_ENGINE_TC && !literal;
     float *pad = direct ? nullptr : ctx->pad_buf.get();
     if (!direct) {
@@ -952,7 +968,8 @@ int convert_tiles_dev(w2x_ctx *ctx, const w2x_model *m, const float *d_in, float
             f.fh = std::min(group, n_tiles - t0) * ph;
             for (int t = 0; t0 + t < n_tiles && t < group; t++) {
                 const size_t off = (size_t)(t0 + t) * w * h;
-                f.rect.push_back(tc::PlaneRect{d_in + off, d_out + off, w, w, w, h, 0, t * ph, 0});
+                f.rect.push_back(tc::PlaneRect{window_frame(PlaneIO{d_in + off, (size_t)w * 4, d_out + off, (size_t)w * 4}, w, h, n, false),
+                                               d_out + off, w, w, h, 0, t * ph, 0});
             }
             frames.push_back(std::move(f));
         }
@@ -1019,13 +1036,8 @@ std::vector<FramePlan> frames_for(const PlanesPlan &p) {
 
 // One step of a chain (w2x_convert_chain*, w2x_convert_planes*): every plane through one model, after the nearest 2x resize when
 // `up`.  A single-plane chain is a collection of one plane.  A step converts a window of each plane: the whole plane, except in the
-// region calls, which have no TTA step and never pack.
-// Where a plane comes from and goes to (row strides in bytes), and for a plane converted alone, convert_device's context around its
-// window (rows_above ... phase_y, all 0 for a whole plane).
-struct PlaneIO {
-    const float *src; size_t src_stride; float *dst; size_t dst_stride;
-    int above = 0, below = 0, left = 0, right = 0, phase_x = 0, phase_y = 0;
-};
+// region calls (w2x_convert_chain_region*, w2x_convert_chain_regions*), which have no TTA step.  Each plane's PlaneIO carries the
+// context around its window, which its frame (window_frame) reads, converted alone or packed.
 struct Step {
     const w2x_model *m;
     bool up;
@@ -1247,8 +1259,9 @@ int reserve_part(Part &P, bool pack, int block_splitting) {
             for (size_t i = 0; i < cw.size(); i++) {
                 const int f = s.plan.frame[i];
                 if (f >= 0)
-                    P.frames[s.f0 + (size_t)f].rect.push_back(tc::PlaneRect{cio[i].src, cio[i].dst, (long)(cio[i].src_stride / 4),
-                                                                            (long)(cio[i].dst_stride / 4), cw[i], ch[i], s.plan.x0[i], s.plan.y0[i], 0});
+                    P.frames[s.f0 + (size_t)f].rect.push_back(tc::PlaneRect{window_frame(cio[i], cw[i], ch[i], (int)s.m->layers.size(), s.up),
+                                                                            cio[i].dst, (long)(cio[i].dst_stride / 4), cw[i], ch[i],
+                                                                            s.plan.x0[i], s.plan.y0[i], 0});
             }
             rc = reserve_frames(ctx, P.frames, s.f0, P.frames.size(), max_channels(s.m));
             if (rc) return rc;
@@ -1427,8 +1440,10 @@ int planes_device(w2x_ctx *ctx, std::vector<Step> &steps, const float *const *d_
 // queued before any part is waited for, phase by phase (a plain step is one phase, a TTA step three), and on_step(k) and step k's lines
 // (through `log`) come before its first phase.  Between parts, the units of a TTA step wait for every other part's variants kernel
 // (tta_ev[0]) and a mean kernel for every other part's units (tta_ev[1]): every record is queued before the waits that name it.
+// host_lines: each step logs its planes' lines as the host entry points do (emit_plane_progress), else as the device ones.
 int planes_host(w2x_ctx *log, const std::vector<Step> &all, std::vector<Part> &parts, const float *const *in, const int *widths,
-                const int *heights, const size_t *in_strides, float *const *out, const size_t *out_strides, w2x_step_fn on_step, void *user) {
+                const int *heights, const size_t *in_strides, float *const *out, const size_t *out_strides, w2x_step_fn on_step, void *user,
+                bool host_lines = true) {
     const size_t np = parts.size(), last = all.size() - 1;
     std::vector<std::vector<size_t>> in_off(np), out_off(np);
     for (size_t p = 0; p < np; p++) {
@@ -1527,7 +1542,7 @@ int planes_host(w2x_ctx *log, const std::vector<Step> &all, std::vector<Part> &p
     for (size_t p = 0; p < np; p++) pipes.push_back(HostPipe{parts[p].ctx, groups[p]});
     for (size_t p = 0; p < np && !rc; p++) rc = pipes[p].start();
     for (size_t k = 0, ph = 0; k <= last && !rc; k++) {
-        begin_step(log, all, k, 0, on_step, user, true);
+        begin_step(log, all, k, 0, on_step, user, host_lines);
         for (int t = 0; t < (all[k].tta ? 3 : 1) && !rc; t++, ph++)
             for (size_t p = 0; p < np && !rc; p++) rc = pipes[p].queue(upto[p][ph]);
     }
@@ -1540,9 +1555,10 @@ int planes_host(w2x_ctx *log, const std::vector<Step> &all, std::vector<Part> &p
 
 // The one-context host call.
 int planes_host(w2x_ctx *ctx, std::vector<Step> &steps, const float *const *in, const int *widths, const int *heights,
-                const size_t *in_strides, float *const *out, const size_t *out_strides, w2x_step_fn on_step, void *user) {
+                const size_t *in_strides, float *const *out, const size_t *out_strides, w2x_step_fn on_step, void *user,
+                bool host_lines = true) {
     std::vector<Part> parts{one_part(ctx, steps)};
-    return planes_host(ctx, parts[0].steps, parts, in, widths, heights, in_strides, out, out_strides, on_step, user);
+    return planes_host(ctx, parts[0].steps, parts, in, widths, heights, in_strides, out, out_strides, on_step, user, host_lines);
 }
 
 // ---- a collection across the GPUs of a w2x_multi (w2x_multi_convert_planes*) ----------------------------------------------------
@@ -1957,40 +1973,66 @@ int w2x_convert_chain(w2x_ctx *ctx, int n_steps, const w2x_model *const *models,
 
 }  // extern "C"
 
-// ---- a window of a chain's output (w2x_convert_chain_region*) ----------------------------------------------------------------
-// The steps of w2x_convert_chain* on a collection of one plane, step k converting only its output window wins[k + 1] from its input
-// window wins[k]: the source rectangle at step 0, else the previous step's output window, dense in chain_buf[(k - 1) & 1].  The
-// window is a plane of its own to convert_device, with the real neighbours its input window holds beyond it as row and column
-// context, so that only the plane's own border is replicated.  No step has TTA, none packs, and every buffer is reserved by
-// prepare_parts before the first launch, as for the other step-table calls.
+// ---- windows of a chain's output (w2x_convert_chain_region*, w2x_convert_chain_regions*) ----------------------------------------
+// The steps of w2x_convert_planes_chain* on a collection of windows, step k converting each window's output window wins[k + 1] from
+// its input window wins[k]: the source rectangle at step 0, else the previous step's output window, dense in chain_buf[(k - 1) & 1].
+// A window is a plane of its own, with the real neighbours its input window holds beyond it as row and column context, so that
+// only the plane's own border is replicated: converted alone by convert_device, or packed into a frame whose rectangle holds the
+// same frame (window_frame).  No step has TTA, and every buffer is reserved by prepare_parts before the first launch, as for the
+// other step-table calls.
 namespace {
-// Every argument of w2x_convert_chain_region*, before anything is printed, allocated or queued: the steps (no TTA) and the window
-// by region_windows, then the buffers and each step's engine by check_steps.  Then *steps is the one-plane step table of the windows.
+// Every argument of a region call on n_windows windows, before anything is printed, allocated or queued: the steps (no TTA) by
+// region_windows, then each window by region_windows and its buffers, then each step's engine by check_steps.  numbered: the
+// messages of a window's checks name it ("window i: ..."); the one-window call's do not.  Then *steps is the step table of the
+// windows: step k converts window i's output window from its input window.
+int check_regions(const char *fn, w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, int n_windows,
+                  const int *widths, const int *heights, const int *windows, const void *const *src, const size_t *src_strides,
+                  const void *const *out, const size_t *out_strides, bool numbered, std::vector<Step> *steps) {
+    if (check_ctx(ctx)) return W2X_ERR_ARG;
+    if (numbered) {
+        if (n_windows < 1) return fail(W2X_ERR_ARG, "%s: n_windows is %d, at least 1 window is needed", fn, n_windows);
+        if (!widths || !heights || !windows || !src || !src_strides || !out || !out_strides) return fail(W2X_ERR_ARG, "%s: NULL array argument", fn);
+        // the steps alone: every window's checks begin with them, and a 1 x 1 window of a 1 x 1 plane passes every other one
+        const int unit[4] = {0, 0, 1, 1};
+        std::vector<Rect> wins;
+        if (int rc = region_windows(fn, n_steps, models, kinds, 1, 1, unit, &wins)) return rc;
+    }
+    std::vector<std::vector<Rect>> wins((size_t)n_windows);
+    std::vector<int> sw((size_t)n_windows), sh((size_t)n_windows);
+    for (int i = 0; i < n_windows; i++) {
+        const std::string name = numbered ? std::string(fn) + ": window " + std::to_string(i) : std::string(fn);
+        const char *wn = name.c_str();
+        int rc = region_windows(wn, n_steps, models, kinds, widths[i], heights[i], windows + 4 * i, &wins[(size_t)i]);
+        if (rc) return rc;
+        const Rect &s = wins[(size_t)i].front(), &o = wins[(size_t)i].back();
+        if (!src[i]) return fail(W2X_ERR_ARG, "%s: NULL source", wn);
+        if (src_strides[i] % 4 || src_strides[i] < (size_t)s.w * 4)
+            return fail(W2X_ERR_ARG, "%s: the source row stride must be a multiple of 4 bytes and >= the source rectangle's row (%d bytes)",
+                        wn, s.w * 4);
+        if (!out[i]) return fail(W2X_ERR_ARG, "%s: NULL output", wn);
+        if (out_strides[i] % 4 || out_strides[i] < (size_t)o.w * 4)
+            return fail(W2X_ERR_ARG, "%s: the output row stride must be a multiple of 4 bytes and >= the window's row (%d bytes)", wn,
+                        o.w * 4);
+        sw[(size_t)i] = s.w;
+        sh[(size_t)i] = s.h;
+    }
+    int rc = check_steps(fn, ctx, n_steps, models, kinds, n_windows, sw.data(), sh.data(), 0, [](int) { return W2X_OK; }, steps);
+    for (int k = 0; k < n_steps && !rc; k++) {
+        Step &t = (*steps)[(size_t)k];
+        for (int i = 0; i < n_windows; i++) {
+            const Rect &w = wins[(size_t)i][(size_t)k + 1];
+            t.w[(size_t)i] = w.w, t.h[(size_t)i] = w.h, t.x0[(size_t)i] = w.x0, t.y0[(size_t)i] = w.y0;
+            t.in[(size_t)i] = wins[(size_t)i][(size_t)k];
+        }
+    }
+    return rc;
+}
+
 int check_region(const char *fn, w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, int width, int height,
                  const int *window, const void *src, size_t src_stride_bytes, const void *out, size_t out_stride_bytes,
                  std::vector<Step> *steps) {
-    if (check_ctx(ctx)) return W2X_ERR_ARG;
-    std::vector<Rect> wins;
-    int rc = region_windows(fn, n_steps, models, kinds, width, height, window, &wins);
-    if (rc) return rc;
-    const Rect &s = wins.front(), &o = wins.back();
-    rc = check_steps(fn, ctx, n_steps, models, kinds, 1, &s.w, &s.h, 0, [&](int) -> int {
-        if (!src) return fail(W2X_ERR_ARG, "%s: NULL source", fn);
-        if (src_stride_bytes % 4 || src_stride_bytes < (size_t)s.w * 4)
-            return fail(W2X_ERR_ARG, "%s: the source row stride must be a multiple of 4 bytes and >= the source rectangle's row (%d bytes)",
-                        fn, s.w * 4);
-        if (!out) return fail(W2X_ERR_ARG, "%s: NULL output", fn);
-        if (out_stride_bytes % 4 || out_stride_bytes < (size_t)o.w * 4)
-            return fail(W2X_ERR_ARG, "%s: the output row stride must be a multiple of 4 bytes and >= the window's row (%d bytes)", fn,
-                        o.w * 4);
-        return W2X_OK;
-    }, steps);
-    for (int k = 0; k < n_steps && !rc; k++) {
-        const Rect &w = wins[(size_t)k + 1];
-        Step &t = (*steps)[(size_t)k];
-        t.w = {w.w}, t.h = {w.h}, t.x0 = {w.x0}, t.y0 = {w.y0}, t.in = {wins[(size_t)k]};
-    }
-    return rc;
+    return check_regions(fn, ctx, n_steps, models, kinds, 1, &width, &height, window, &src, &src_stride_bytes, &out, &out_stride_bytes, false,
+                         steps);
 }
 }  // namespace
 
@@ -2031,6 +2073,35 @@ int w2x_convert_chain_region_device(w2x_ctx *ctx, int n_steps, const w2x_model *
     DeviceGuard g(ctx->device);
     NvtxRange nvtx("w2x convert chain region");
     return planes_device(ctx, steps, &d_src, &src_stride_bytes, &d_out, &out_stride_bytes, false, 0, on_step, user);
+}
+
+int w2x_convert_chain_regions(w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, int n_windows, const int *widths,
+                              const int *heights, const int *windows, const float *const *src, const size_t *src_strides, float *const *out,
+                              const size_t *out_strides, w2x_step_fn on_step, void *user) {
+    std::vector<Step> steps;
+    int rc = check_regions("w2x_convert_chain_regions", ctx, n_steps, models, kinds, n_windows, widths, heights, windows,
+                           reinterpret_cast<const void *const *>(src), src_strides, reinterpret_cast<const void *const *>(out), out_strides,
+                           true, &steps);
+    if (rc) return rc;
+    DeviceGuard g(ctx->device);
+    NvtxRange nvtx("w2x convert chain regions");
+    std::vector<int> sw((size_t)n_windows), sh((size_t)n_windows);   // the source rectangles, staged densely
+    for (size_t i = 0; i < sw.size(); i++) sw[i] = steps[0].in[i].w, sh[i] = steps[0].in[i].h;
+    return planes_host(ctx, steps, src, sw.data(), sh.data(), src_strides, out, out_strides, on_step, user, false);
+}
+
+int w2x_convert_chain_regions_device(w2x_ctx *ctx, int n_steps, const w2x_model *const *models, const int *kinds, int n_windows,
+                                     const int *widths, const int *heights, const int *windows, const float *const *d_src,
+                                     const size_t *src_strides, float *const *d_out, const size_t *out_strides, w2x_step_fn on_step,
+                                     void *user) {
+    std::vector<Step> steps;
+    int rc = check_regions("w2x_convert_chain_regions_device", ctx, n_steps, models, kinds, n_windows, widths, heights, windows,
+                           reinterpret_cast<const void *const *>(d_src), src_strides, reinterpret_cast<const void *const *>(d_out),
+                           out_strides, true, &steps);
+    if (rc) return rc;
+    DeviceGuard g(ctx->device);
+    NvtxRange nvtx("w2x convert chain regions");
+    return planes_device(ctx, steps, d_src, src_strides, d_out, out_strides, true, 0, on_step, user);
 }
 
 }  // extern "C"

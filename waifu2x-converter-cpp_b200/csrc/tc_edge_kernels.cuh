@@ -188,13 +188,15 @@ last_gather_kernel(const float *__restrict__ partial, int pw, int ph, float bias
 // ---- packed frames: independent planes of any sizes side by side in one frame (w2x_convert_planes, w2x_convert_tiles) ----
 // Each plane owns the padded rectangle (w + 2 pad) x (h + 2 pad) at (x0, y0).  An interior pixel's receptive field has radius
 // pad = the layer count, so it never leaves its own rectangle: every plane's interior sees exactly the operands, in the same
-// order, as a pass on the plane alone.  The table lists the rectangles by shelf: ascending y0, then ascending x0; rectangles
+// order, as a pass on the plane (or window, with its context) alone.  The table lists the rectangles by shelf: ascending y0, then ascending x0; rectangles
 // with one y0 form a shelf, no rectangle reaches below the next shelf's y0 or right of its successor's x0.
 
-// Frame pixel (y, x) of the padded fp32 image: cv::copyMakeBorder(plane, pad, BORDER_REPLICATE) (src/convertRoutine.cpp:35)
-// inside a rectangle, 0 everywhere else.  One thread per frame pixel, 32 x 8 per block.
-// UP2X: the plane of R.w x R.h is the nearest-neighbour 2x resize of R.src (src/main.cpp:135-139), never materialised: its pixel
-// (y, x) is src[y >> 1][x >> 1], as in FrameSource::up2x.
+// Frame pixel (y, x) of the padded fp32 image: pixel (py, px) of the rectangle's FrameSource inside a rectangle --
+// cv::copyMakeBorder(plane, pad, BORDER_REPLICATE) (src/convertRoutine.cpp:35) of a whole plane, or a window's frame with its real
+// neighbour rows and columns -- read through frame_src as tc::launch_first and launch_pad read it; 0 everywhere else.  One thread
+// per frame pixel, 32 x 8 per block.
+// UP2X = every rectangle's src.up2x: its plane is the nearest-neighbour 2x resize of src.in (src/main.cpp:135-139), never
+// materialised.
 template <bool UP2X>
 __global__ void __launch_bounds__(256)
 pack_planes_kernel(const PlaneRect *__restrict__ rect, const int *__restrict__ shelf_y0, const int *__restrict__ shelf_first,
@@ -217,7 +219,9 @@ pack_planes_kernel(const PlaneRect *__restrict__ rect, const int *__restrict__ s
     const int px = x - R.x0, py = y - R.y0;
     float v = 0.f;
     if (px >= 0 && py >= 0 && px < R.w + 2 * pad && py < R.h + 2 * pad) {
-        v = __ldg(R.src + (long)frame_src<UP2X>(py, pad, R.h, 0, 0) * R.src_stride + frame_src<UP2X>(px, pad, R.w, 0, 0));
+        const FrameSource &S = R.src;
+        v = __ldg(S.in + (long)frame_src<UP2X>(py, S.pad_top, S.h, S.rows_above, S.rows_below) * S.stride_floats +
+                  frame_src<UP2X>(px, S.pad_x, S.w, S.cols_left, S.cols_right));
     }
     frame[(size_t)y * fw + x] = v;
 }
