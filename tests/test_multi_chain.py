@@ -7,8 +7,9 @@ compares.  Every chain call runs three passes (flags, events and the cached plan
 reference's bits.
 
   * k = 2, 3, 4; chains [noise], [scale^], [noise, scale^], [noise, scale^, scale^], [scale^, noise], the shipped n = 7 models,
-    the random n = 4 model of test_band_exchange.py and a chain mixing both depths; all three precisions; odd sizes; cuts on odd
-    and even rows; step-0 frame widths with (w + 2n) % 4 in {1, 2, 3}; heights on both sides of the height / (4 n) rule; a plane
+    the random n = 4 model of test_band_exchange.py and a chain mixing both depths, and chains of the selection models of
+    test_chain_exact.py (n = 3, 4, 6), whose reference is the chain emulator (which one-context convert_chain must match too);
+    all three precisions; odd sizes; cuts on odd and even rows; step-0 frame widths with (w + 2n) % 4 in {1, 2, 3}; heights on both sides of the height / (4 n) rule; a plane
     whose later steps get several sub-bands per GPU; row-strided pinned and pageable host planes.
   * progress lines and on_step order; a one-step W2X_STEP_SAME chain against Multi.convert_plane; the plan cache; refusals;
     w2x_ctx_forget_model against the chain plan.
@@ -26,6 +27,7 @@ import pytest
 
 from conftest import ROOT
 from test_band_exchange import ENV, RANDOM, Job, mismatch, slab_cuts
+from test_chain_exact import LAYERS as SEL_LAYERS, emulate_chain, spec_of
 
 gpu = pytest.mark.gpu
 PKG = os.path.join(ROOT, "waifu2x-converter-cpp_b200")
@@ -33,7 +35,10 @@ CLI = os.path.join(PKG, "w2x-converter")
 WORKER = os.path.join(ROOT, "tests", "multi_chain_worker.py")
 PASSES = 3
 F16X3, F16_F8X2, F16 = 0, 1, 2
-N_OF = {"noise1": 7, "scale2.0x": 7, "rand128": 4}
+N_OF = {"noise1": 7, "scale2.0x": 7, "rand128": 4, "selA": 3, "selB": 4, "selC": 6}
+# the selection models of test_chain_exact.py (n = 3, 4, 6): their chains are compared with the chain emulator as well
+SELS = {"selA": "A", "selB": "B", "selC": "C"}
+PREC_NAMES = {F16X3: "f16x3", F16_F8X2: "f16+f8x2", F16: "f16"}
 
 NOISE, SCALE, RAND = "noise1", "scale2.0x", "rand128"
 S = lambda m, up=False, tta=False: [m, up, tta]   # noqa: E731  (a step)
@@ -76,6 +81,14 @@ CASES = [
         chain([S(NOISE), S(SCALE, True), S(SCALE, True)], F16, 20, 113, 15),                    # cuts at rows 28, 56 and 84
         chain([S(RAND), S(RAND, True)], F16_F8X2, 19, 70, 16), chain([S(SCALE, True)], F16X3, 17, 111, 17),   # 111 rows: 3 of the 4 contexts
     ]),
+    # selection chains whose steps differ in depth (3, 4, 6) and width, shallow -> deep and deep -> shallow; every height cuts
+    # for every context (height / (4 n_max) >= k)
+    (2, [
+        chain([S("selA"), S("selC", True)], F16X3, 23, 50, 40), chain([S("selC", True), S("selA")], F16, 19, 49, 41),
+    ]),
+    (3, [
+        chain([S("selC", True), S("selA")], F16_F8X2, 17, 75, 42), chain([S("selB", True), S("selA", True), S("selC")], F16X3, 9, 72, 43),
+    ]),
 ]
 # refusals (k = 2): status, the step named in the message, nothing logged, no on_step call
 REFUSALS = [
@@ -108,6 +121,15 @@ def frame_of(src, row0, col0, w, h, pad_x, pad_top, rows_above, rows_below, up2x
     sx = col0 + (np.clip(np.arange(pw) - pad_x, -cols_left, w - 1 + cols_right) >> sh)
     assert sy.min() >= 0 and sx.min() >= 0, "the real rows and columns must exist"
     return src[np.ix_(sy, sx)]
+
+
+def selection_chain_cases():
+    """(chain, input, precision) of every selection-model chain call above, for test_chain_exact.py's check of the emulator's
+    conditions"""
+    for _, calls in CASES:
+        for c in calls:
+            if c["op"] == "chain" and all(m in SELS for m, _, _ in c["steps"]):
+                yield spec_of(c["steps"], SELS), np.random.default_rng(c["seed"]).random(c["size"], dtype=np.float32), PREC_NAMES[c["precision"]]
 
 
 def test_frame_restatement_by_hand():
@@ -210,6 +232,7 @@ def layers(oracle_models, oracle_mod):
     dims, seed = RANDOM[RAND]
     om = oracle_mod.OracleModel.random(dims, seed=seed)
     out[RAND] = list(zip(om.weights, om.biases))
+    out.update({k: SEL_LAYERS[v] for k, v in SELS.items()})
     return out
 
 
@@ -238,7 +261,8 @@ def worker_run(layers, tmp_path_factory):
 
 
 class Reference:
-    """Context.convert_chain on one context per precision, with its lines, on_step calls and launch count"""
+    """Context.convert_chain on one context per precision, with its lines, on_step calls and launch count; for a chain of
+    selection models the planes are the chain emulator's, which the one-context call must give as well"""
 
     def __init__(self, w2x, models):
         self.models = models
@@ -260,6 +284,11 @@ class Reference:
                 y = ctx.convert_chain(steps, x, block_splitting=call.get("block_splitting", True), on_step=lambda k: events.append(f"step {k}"))
             finally:
                 ctx.set_log(None)
+            if all(m in SELS for m, _, _ in call["steps"]):
+                want = emulate_chain(spec_of(call["steps"], SELS), x, PREC_NAMES[call["precision"]])
+                msg = mismatch(y, want, [0])
+                assert not msg, f"one-context convert_chain {call['steps']} against the emulator: {msg}"
+                y = want
             self.memo[key] = (y, events, ctx.launch_count() - before)
         return self.memo[key]
 

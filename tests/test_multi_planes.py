@@ -6,7 +6,8 @@ collections -- the GPUs used, every owner and every GPU's load -- and the balanc
 On the GPU: the "GPUs" are 2, 3 and 4 contexts of device 0, driven in tests/multi_planes_worker.py (a child process with
 CUDA_DEVICE_MAX_CONNECTIONS set before CUDA starts).  Every call runs twice and must give, bit for bit, what Context.convert_planes_chain
 gives on one context, with the same progress lines and on_step calls; step patterns S, U, SU, SUU and US with TTA on no, some and all
-steps; all three precisions and the fp32 engine; one plane (a single image's TTA across GPUs), fewer planes than GPUs, 300 planes with
+steps; chains of the selection models of test_chain_exact.py (n = 3, 4, 6), also compared with its chain emulator; all three
+precisions and the fp32 engine; one plane (a single image's TTA across GPUs), fewer planes than GPUs, 300 planes with
 sides 1-160, a plane too large to pack among small ones, row-strided pinned and pageable host planes; the one-step W2X_STEP_SAME call
 against Multi.convert_planes and Context.convert_planes; a call on one GPU against the one-context call's launches; the launches of
 collection A against its frames; refusals and W2X_ERR_NOMEM, which queue nothing on any context.
@@ -22,12 +23,16 @@ import pytest
 
 from conftest import ROOT
 from test_band_exchange import ENV, RANDOM, Job, mismatch
+from test_chain_exact import LAYERS as SEL_LAYERS, emulate_chain, spec_of
 
 gpu = pytest.mark.gpu
 WORKER = os.path.join(ROOT, "tests", "multi_planes_worker.py")
 F16X3, F16_F8X2, F16 = 0, 1, 2
 ENGINE_FP32 = 1
 NOISE, SCALE, RAND = "noise1", "scale2.0x", "rand128"
+# the selection models of test_chain_exact.py (n = 3, 4, 6): their chains are compared with the chain emulator as well
+SELS = {"selA": "A", "selB": "B", "selC": "C"}
+PREC_NAMES = {F16X3: "f16x3", F16_F8X2: "f16+f8x2", F16: "f16"}
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -177,6 +182,7 @@ COLLECTIONS = {
     "mix": [(300, 200)] + sizes_with_edges(4, 40, 4, 40),
     "A": [(int(w), int(h)) for w, h in np.random.default_rng(1).integers(16, 129, size=(2000, 2))],
     "big": [(2048, 2048)],
+    "sel": sizes_with_edges(5, 6, 1, 16),
 }
 PATTERNS = {"S": [False], "U": [True], "SU": [False, True], "SUU": [False, True, True], "US": [True, False]}
 
@@ -219,6 +225,15 @@ def groups():
         chain([[NOISE, False, False], [SCALE, True, False]], "two"),                               # 2 planes, no TTA: 2 of 4 GPUs
         chain([[SCALE, True, True]], "c300"),
     ]))
+    # selection chains whose steps differ in depth (3, 4, 6) and width, TTA on the first step and on a deep step after an upscale
+    out.append((2, [
+        chain([["selA", False, True], ["selC", True, False]], "sel", precision=F16X3),
+        chain([["selC", True, False], ["selA", False, False]], "sel", precision=F16),
+    ]))
+    out.append((3, [
+        chain([["selB", True, False], ["selA", False, False], ["selC", False, True]], "sel", precision=F16_F8X2),
+        chain([["selC", True, False], ["selB", False, False]], "sel", precision=F16X3),
+    ]))
     return out
 
 
@@ -231,16 +246,32 @@ def layers(oracle_models, oracle_mod):
     dims, seed = RANDOM[RAND]
     om = oracle_mod.OracleModel.random(dims, seed=seed)
     out[RAND] = list(zip(om.weights, om.biases))
+    out.update({k: SEL_LAYERS[v] for k, v in SELS.items()})
     return out
+
+
+def collection(name):
+    """the planes of collection `name`"""
+    rng = np.random.default_rng(100 + list(COLLECTIONS).index(name))
+    return [rng.random((h, w), dtype=np.float32) for w, h in COLLECTIONS[name]]
+
+
+def selection_planes_cases():
+    """(chain, plane, precision) of every plane of every selection-model call above, for test_chain_exact.py's check of the
+    emulator's conditions"""
+    for _, calls in groups():
+        for c in calls:
+            if all(m in SELS for m, _, _ in c["steps"]):
+                for x in collection(c["coll"]):
+                    yield spec_of(c["steps"], SELS), x, PREC_NAMES[c.get("precision", F16_F8X2)]
 
 
 @pytest.fixture(scope="module")
 def worker_run(layers, tmp_path_factory):
     job = Job(layers)
-    for seed, (name, sizes) in enumerate(COLLECTIONS.items()):
-        rng = np.random.default_rng(100 + seed)
-        for i, (w, h) in enumerate(sizes):
-            job.inputs[f"{name}/{i}"] = rng.random((h, w), dtype=np.float32)
+    for name in COLLECTIONS:
+        for i, x in enumerate(collection(name)):
+            job.inputs[f"{name}/{i}"] = x
     gs = groups() + [(2, [dict(op="raw", steps=[[NOISE, False, False], [SCALE, True, True]], coll="c7", bad=b) for b in REFUSALS]),
                      (2, [dict(op="nomem", steps=[[NOISE, False, True]], coll="big")])]
     for i, (k, calls) in enumerate(gs):
@@ -273,22 +304,35 @@ def models(w2x, layers):
 
 @gpu
 def test_every_pass_is_bit_identical_to_one_context(worker_run):
+    """and, for chains of selection models, the one-context call and every pass to the chain emulator"""
     job, outs, log = worker_run
-    fails, checked = [], 0
+    fails, checked, emulated = [], 0, 0
     for c, call, key in chain_calls(job):
         n = len(COLLECTIONS[call["coll"]])
-        for p in range(len(log[key]["passes"])):
-            for i in range(n):
+        sel = all(m in SELS for m, _, _ in call["steps"])
+        xs = collection(call["coll"]) if sel else None
+        for i in range(n):
+            if sel:
+                em = emulate_chain(spec_of(call["steps"], SELS), xs[i], PREC_NAMES[call.get("precision", F16_F8X2)])
+                msg = mismatch(outs[f"{key}.ref.{i}"], em, [0])
+                if msg:
+                    fails.append(f"{key} {call['steps']} one context plane {i} {em.shape} against the emulator: {msg}")
+                emulated += 1
+            for p in range(len(log[key]["passes"])):
                 want, got = outs[f"{key}.ref.{i}"], outs[f"{key}.{p}.{i}"]
                 W = want.shape[1]
                 msg = mismatch(got[:, :W], want, [0])
                 if msg:
                     fails.append(f"{key} k={c['k']} {call['steps']} {call['coll']} pass {p} plane {i} {want.shape}: {msg}")
+                if sel:
+                    msg = mismatch(got[:, :W], em, [0])
+                    if msg:
+                        fails.append(f"{key} k={c['k']} {call['steps']} pass {p} plane {i} {em.shape} against the emulator: {msg}")
                 if got.shape[1] > W and not np.all(np.isnan(got[:, W:])):
                     fails.append(f"{key} pass {p} plane {i}: wrote into the row padding")
                 checked += 1
         assert len(log[key]["passes"]) == 2, key
-    assert checked > 2000 and not fails, "\n".join(fails[:30])
+    assert checked > 2000 and emulated >= 24 and not fails, "\n".join(fails[:30])
 
 
 @gpu
