@@ -525,6 +525,33 @@ W2X_API int w2x_multi_convert_planes_chain(w2x_multi *multi, int n_steps, const 
                                            const size_t *in_strides, float *const *out, const size_t *out_strides,
                                            w2x_step_fn on_step, void *user);
 
+/* w2x_convert_chain_regions on N GPUs: the tiles of a scan too large to hold, the visible tiles of a viewer or patches of many images,
+ * each window on one GPU.  The arguments mean what they mean for w2x_convert_chain_regions.
+ * Every window is bit-identical to w2x_convert_chain_regions on the first context with the same precision and engine, and so to the
+ * same window of w2x_convert_chain(..., block_splitting = 0): every context the call uses takes the first context's precision and
+ * engine.
+ * Arguments are checked exactly as w2x_convert_chain_regions checks them, with the same messages naming the step or "window i: ",
+ * before anything is printed, allocated or queued on any context.  A W2X_STEP_TTA step is refused: windows have no TTA form.
+ * Before step k is queued on any GPU, on_step(k, user) is called (if not NULL); then, through the first context's log function
+ * (w2x_multi_set_log), the lines w2x_convert_chain_regions logs for step k, window by window in order.
+ * Placement (a pure function of the windows, the steps and N): the work of a window is, summed over the steps, its output-window
+ * pixels at the step times the step model's multiply-adds per pixel.  Every window has one owner GPU, which stages its source
+ * rectangle, holds its intermediate windows and writes its output; owners are chosen as in w2x_multi_convert_planes_chain: windows
+ * in decreasing order of work (ties: the lower index), each on the owner that minimises the largest per-GPU load once its work is
+ * added (ties: the owner with the smaller load before it, then the lower GPU index).  Each context launches what
+ * w2x_convert_chain_regions launches on the windows it owns, in order, under its own scratch limit.
+ * GPUs used: nd = min(n_devices, n_windows).  With nd == 1 the call is w2x_convert_chain_regions on the first context: same bits,
+ * same lines, same launches.  No window leaves its GPU, so the call needs no peer access.
+ * Device memory: each GPU holds what w2x_convert_chain_regions holds for its windows.  All of it is reserved on every GPU before the
+ * first copy or launch anywhere: W2X_ERR_NOMEM leaves nothing queued on any context.
+ * HOST buffers, synchronous; pageable buffers are pinned for the call: the page-rounded union of every source rectangle's and every
+ * output's rows, registered as merged intervals of 4 MiB and more, so that windows sharing pages are pinned too.  Every GPU's work
+ * is queued before any is waited for. */
+W2X_API int w2x_multi_convert_chain_regions(w2x_multi *multi, int n_steps, const w2x_model *const *models, const int *kinds,
+                                            int n_windows, const int *widths, const int *heights, const int *windows,
+                                            const float *const *src, const size_t *src_strides, float *const *out,
+                                            const size_t *out_strides, w2x_step_fn on_step, void *user);
+
 /* ---- instrumentation ---------------------------------------------------------------------- */
 /* Number of kernels of THIS library launched by the context so far. */
 W2X_API int w2x_ctx_launch_count(const w2x_ctx *ctx, uint64_t *n_launches);

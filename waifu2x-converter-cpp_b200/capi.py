@@ -44,6 +44,7 @@ ABI_SYMBOLS = (
     "w2x_convert_planes_chain", "w2x_convert_planes_chain_device", "w2x_multi_convert_chain",
     "w2x_multi_convert_planes", "w2x_multi_convert_planes_chain", "w2x_chain_region_source", "w2x_convert_chain_region",
     "w2x_convert_chain_region_device", "w2x_convert_chain_regions", "w2x_convert_chain_regions_device",
+    "w2x_multi_convert_chain_regions",
 )
 BAND_BLOB_BYTES = 320
 
@@ -170,6 +171,8 @@ def lib():
     L.w2x_multi_convert_planes.argtypes = [vp, vp, ci, C.POINTER(vp), pi, pi, ps, C.POINTER(vp), ps]
     L.w2x_multi_convert_planes_chain.argtypes = [vp, ci, C.POINTER(vp), pi, ci, C.POINTER(vp), pi, pi, ps, C.POINTER(vp), ps, STEP_FN, vp]
     L.w2x_debug_plan_multi_planes.argtypes = [ci, ci, C.POINTER(vp), pi, ci, pi, pi, pi, C.POINTER(C.c_longlong)]
+    L.w2x_multi_convert_chain_regions.argtypes = [vp, ci, C.POINTER(vp), pi, ci, pi, pi, pi, C.POINTER(vp), ps, C.POINTER(vp), ps, STEP_FN, vp]
+    L.w2x_debug_plan_multi_regions.argtypes = [ci, ci, C.POINTER(vp), pi, ci, pi, pi, pi, pi, C.POINTER(C.c_longlong)]
     L.w2x_debug_pad.argtypes = [vp, vp, ci, C.c_long, ci, ci] + [ci] * 13 + [vp]
     L.w2x_debug_set_host_bands.argtypes = [vp, ci]
     L.w2x_debug_set_fuse_last.argtypes = [vp, ci]
@@ -265,6 +268,22 @@ def debug_plan_multi_planes(n_devices, steps, widths, heights):
     if nd < 0:
         raise W2xError(-nd, lib().w2x_last_error().decode())
     return nd, owner, load[:nd]
+
+
+def debug_plan_multi_regions(n_devices, steps, sizes, windows):
+    """The placement of w2x_multi_convert_chain_regions on n_devices GPUs (no device needed); steps as in Context.convert_chain_regions,
+    sizes and windows one per window -> (nd, owner [n], load [nd]): the GPUs used, every window's owner and the planned work
+    (multiply-adds) per GPU."""
+    n, models, kinds, _, _ = Context._chain_args(steps, None)
+    ws, hs, wins = Context._regions_args(sizes, windows)
+    k = len(windows)
+    owner = np.zeros(max(k, 1), np.int32)
+    load = np.zeros(max(n_devices, 1), np.int64)
+    nd = lib().w2x_debug_plan_multi_regions(n_devices, n, models, kinds, k, ws, hs, wins, owner.ctypes.data_as(C.POINTER(C.c_int)),
+                                            load.ctypes.data_as(C.POINTER(C.c_longlong)))
+    if nd < 0:
+        raise W2xError(-nd, lib().w2x_last_error().decode())
+    return nd, owner[:k], load[:nd]
 
 
 def _c_view(p):
@@ -586,6 +605,16 @@ class Context:
         that plane (row-strided views, such as slices of the whole plane, are passed as they are; several may share one plane) ->
         the list of h x w windows; `out` may be such a list (strided views included), written in place.  on_step(k) is called before
         step k."""
+        args, out, xs = self._regions_host_args(steps, sources, sizes, windows, out, on_step)
+        _check(lib().w2x_convert_chain_regions(self._h, *args))
+        del xs
+        return out
+
+    @staticmethod
+    def _regions_host_args(steps, sources, sizes, windows, out, on_step):
+        """-> (the arguments of w2x_convert_chain_regions after the handle, the output list, the source arrays): the source arrays
+        include the float32 unit-column-stride copies _c_view made, which the arguments point into without holding them, so the
+        caller keeps them until the call returns"""
         if not (len(sources) == len(sizes) == len(windows)):
             raise ValueError("sources, sizes and windows must have one entry per window")
         xs, sp, _, _, sst = _plane_arrays(sources, _c_view)
@@ -604,11 +633,9 @@ class Context:
         if any(o.strides[1] != 4 or o.strides[0] % 4 for o in out):
             raise ValueError("out arrays need unit column stride and row strides that are multiples of 4 bytes")
         _, op, _, _, ost = _plane_arrays(out, lambda o: o)
-        n, models, kinds, cb, _ = self._chain_args(steps, on_step)
-        k = len(xs)
-        ws, hs, wins = self._regions_args(sizes, windows)
-        _check(lib().w2x_convert_chain_regions(self._h, n, models, kinds, k, ws, hs, wins, sp, sst, op, ost, cb, None))
-        return out
+        n, models, kinds, cb, _ = Context._chain_args(steps, on_step)
+        ws, hs, wins = Context._regions_args(sizes, windows)
+        return (n, models, kinds, len(xs), ws, hs, wins, sp, sst, op, ost, cb, None), out, xs
 
     @staticmethod
     def _regions_args(sizes, windows):
@@ -820,6 +847,14 @@ class Multi:
         n, models, kinds, cb, ups = Context._chain_args(steps, on_step)
         xs, ip, ws, hs, ist, out, op, ost = Context._planes_args(planes, out, ups)
         _check(lib().w2x_multi_convert_planes_chain(self._h, n, models, kinds, len(xs), ip, ws, hs, ist, op, ost, cb, None))
+        return out
+
+    def convert_chain_regions(self, steps, sources, sizes, windows, out=None, on_step=None):
+        """Context.convert_chain_regions across this handle's GPUs (w2x_multi_convert_chain_regions): each window on one GPU.  Same
+        arguments, same bits."""
+        args, out, xs = Context._regions_host_args(steps, sources, sizes, windows, out, on_step)
+        _check(lib().w2x_multi_convert_chain_regions(self._h, *args))
+        del xs
         return out
 
     def launch_counts(self):

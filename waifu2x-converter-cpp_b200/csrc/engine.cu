@@ -1981,6 +1981,19 @@ int w2x_convert_chain(w2x_ctx *ctx, int n_steps, const w2x_model *const *models,
 // same frame (window_frame).  No step has TTA, and every buffer is reserved by prepare_parts before the first launch, as for the
 // other step-table calls.
 namespace {
+// The step table of the windows from the step table of their source rectangles: step k converts window i's output window
+// wins[i][k + 1] from its input window wins[i][k] (region_windows).
+void set_region_windows(std::vector<Step> &steps, const std::vector<std::vector<Rect>> &wins) {
+    for (size_t k = 0; k < steps.size(); k++) {
+        Step &t = steps[k];
+        for (size_t i = 0; i < wins.size(); i++) {
+            const Rect &w = wins[i][k + 1];
+            t.w[i] = w.w, t.h[i] = w.h, t.x0[i] = w.x0, t.y0[i] = w.y0;
+            t.in[i] = wins[i][k];
+        }
+    }
+}
+
 // Every argument of a region call on n_windows windows, before anything is printed, allocated or queued: the steps (no TTA) by
 // region_windows, then each window by region_windows and its buffers, then each step's engine by check_steps.  numbered: the
 // messages of a window's checks name it ("window i: ..."); the one-window call's do not.  Then *steps is the step table of the
@@ -2017,14 +2030,7 @@ int check_regions(const char *fn, w2x_ctx *ctx, int n_steps, const w2x_model *co
         sh[(size_t)i] = s.h;
     }
     int rc = check_steps(fn, ctx, n_steps, models, kinds, n_windows, sw.data(), sh.data(), 0, [](int) { return W2X_OK; }, steps);
-    for (int k = 0; k < n_steps && !rc; k++) {
-        Step &t = (*steps)[(size_t)k];
-        for (int i = 0; i < n_windows; i++) {
-            const Rect &w = wins[(size_t)i][(size_t)k + 1];
-            t.w[(size_t)i] = w.w, t.h[(size_t)i] = w.h, t.x0[(size_t)i] = w.x0, t.y0[(size_t)i] = w.y0;
-            t.in[(size_t)i] = wins[(size_t)i][(size_t)k];
-        }
-    }
+    if (!rc) set_region_windows(*steps, wins);
     return rc;
 }
 
@@ -2104,4 +2110,72 @@ int w2x_convert_chain_regions_device(w2x_ctx *ctx, int n_steps, const w2x_model 
     return planes_device(ctx, steps, d_src, src_strides, d_out, out_strides, true, 0, on_step, user);
 }
 
+// Test hook (not part of the stable ABI): the placement of w2x_multi_convert_chain_regions on n_devices GPUs, without a device.
+// owner gets every window's GPU, load (n_devices entries) the planned work per GPU used.  Returns the number of GPUs used, or
+// -W2X_ERR_ARG.
+W2X_API int w2x_debug_plan_multi_regions(int n_devices, int n_steps, const w2x_model *const *models, const int *kinds, int n_windows,
+                                         const int *widths, const int *heights, const int *windows, int *owner, long long *load) {
+    const char *fn = "w2x_debug_plan_multi_regions";
+    if (n_devices < 1 || n_windows < 1 || !widths || !heights || !windows || !owner || !load) return -fail(W2X_ERR_ARG, "%s: bad argument", fn);
+    std::vector<std::vector<Rect>> wins((size_t)n_windows);
+    std::vector<int> sw((size_t)n_windows), sh((size_t)n_windows);
+    for (int i = 0; i < n_windows; i++) {
+        const std::string name = std::string(fn) + ": window " + std::to_string(i);
+        if (int rc = region_windows(name.c_str(), n_steps, models, kinds, widths[i], heights[i], windows + 4 * i, &wins[(size_t)i])) return -rc;
+        sw[(size_t)i] = wins[(size_t)i][0].w;
+        sh[(size_t)i] = wins[(size_t)i][0].h;
+    }
+    std::vector<Step> steps = step_table(n_steps, models, kinds, n_windows, sw.data(), sh.data());
+    set_region_windows(steps, wins);
+    std::vector<int> own;
+    std::vector<long long> ld;
+    const int nd = plan_multi(n_devices, steps, &own, &ld);
+    std::copy(own.begin(), own.end(), owner);
+    std::copy(ld.begin(), ld.end(), load);
+    return nd;
+}
+
 }  // extern "C"
+
+namespace w2x {
+namespace eng {
+// w2x_convert_chain_regions with every window on one owner GPU (plan_multi on the windows' step table): the owner stages its
+// source rectangle, holds its intermediate windows and writes its output, so nothing crosses devices.
+int multi_regions(const char *fn, const std::vector<w2x_ctx *> &ctxs, int n_steps, const w2x_model *const *models, const int *kinds,
+                  int n_windows, const int *widths, const int *heights, const int *windows, const float *const *src,
+                  const size_t *src_strides, float *const *out, const size_t *out_strides, w2x_step_fn on_step, void *user) {
+    w2x_ctx *ctx0 = ctxs[0];
+    std::vector<Step> all;
+    int rc = check_regions(fn, ctx0, n_steps, models, kinds, n_windows, widths, heights, windows,
+                           reinterpret_cast<const void *const *>(src), src_strides, reinterpret_cast<const void *const *>(out), out_strides,
+                           true, &all);
+    if (rc) return rc;
+    std::vector<int> owner;
+    std::vector<long long> load;
+    const int nd = plan_multi((int)ctxs.size(), all, &owner, &load);
+    if (nd == 1)
+        return w2x_convert_chain_regions(ctx0, n_steps, models, kinds, n_windows, widths, heights, windows, src, src_strides, out,
+                                         out_strides, on_step, user);
+    std::vector<Part> parts((size_t)nd);
+    for (int i = 0; i < n_windows; i++) parts[(size_t)owner[(size_t)i]].own.push_back(i);
+    for (int d = 0; d < nd; d++) {
+        Part &P = parts[(size_t)d];
+        P.ctx = ctxs[(size_t)d];
+        P.ctx->precision = ctx0->precision;
+        P.ctx->engine = ctx0->engine;
+        P.steps = part_steps(all, P.own, std::vector<std::vector<int>>(all.size()));
+    }
+    NvtxRange nvtx("w2x multi convert chain regions");
+    const Step &L = all.back();
+    std::vector<int> sw((size_t)n_windows), sh((size_t)n_windows);   // the source rectangles, staged densely
+    std::vector<HostRange> ranges;
+    for (size_t i = 0; i < sw.size(); i++) {
+        sw[i] = all[0].in[i].w, sh[i] = all[0].in[i].h;
+        ranges.push_back({src[i], src_strides[i] * (size_t)(sh[i] - 1) + (size_t)sw[i] * 4});
+        ranges.push_back({out[i], out_strides[i] * (size_t)(L.h[i] - 1) + (size_t)L.w[i] * 4});
+    }
+    HostPins pins(ranges);
+    return planes_host(ctx0, all, parts, src, sw.data(), sh.data(), src_strides, out, out_strides, on_step, user, false);
+}
+}  // namespace eng
+}  // namespace w2x

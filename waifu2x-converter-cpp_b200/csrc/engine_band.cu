@@ -774,6 +774,15 @@ int w2x_multi_convert_planes_chain(w2x_multi *m, int n_steps, const w2x_model *c
                               out, out_strides, on_step, user);
 }
 
+int w2x_multi_convert_chain_regions(w2x_multi *m, int n_steps, const w2x_model *const *models, const int *kinds, int n_windows,
+                                    const int *widths, const int *heights, const int *windows, const float *const *src,
+                                    const size_t *src_strides, float *const *out, const size_t *out_strides, w2x_step_fn on_step,
+                                    void *user) {
+    if (!m || m->ctx.empty()) return fail(W2X_ERR_ARG, "w2x_multi_convert_chain_regions: NULL handle");
+    return multi_regions("w2x_multi_convert_chain_regions", m->ctx, n_steps, models, kinds, n_windows, widths, heights, windows, src,
+                         src_strides, out, out_strides, on_step, user);
+}
+
 int w2x_multi_convert_planes(w2x_multi *m, const w2x_model *model, int n_planes, const float *const *in, const int *widths,
                              const int *heights, const size_t *in_strides, float *const *out, const size_t *out_strides) {
     if (!m || m->ctx.empty()) return fail(W2X_ERR_ARG, "w2x_multi_convert_planes: NULL handle");

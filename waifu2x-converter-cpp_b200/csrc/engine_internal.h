@@ -5,14 +5,17 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <nvtx3/nvToolsExt.h>   // header-only NVTX v3: ranges cost a few nanoseconds when no tool is attached
+#include <unistd.h>
 
 #include <algorithm>
+#include <cstdint>
 #include <cstdlib>
 #include <cstring>
 #include <map>
 #include <memory>
 #include <mutex>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "kernels.h"
@@ -216,6 +219,10 @@ int launch_layer_tc(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int li, cons
 int multi_planes_chain(const char *fn, const std::vector<w2x_ctx *> &ctxs, int n_steps, const w2x_model *const *models, const int *kinds,
                        int n_planes, const float *const *in, const int *widths, const int *heights, const size_t *in_strides,
                        float *const *out, const size_t *out_strides, w2x_step_fn on_step, void *user);
+// w2x_multi_convert_chain_regions on the contexts of a w2x_multi (engine.cu): `fn` names the entry point in messages.
+int multi_regions(const char *fn, const std::vector<w2x_ctx *> &ctxs, int n_steps, const w2x_model *const *models, const int *kinds,
+                  int n_windows, const int *widths, const int *heights, const int *windows, const float *const *src,
+                  const size_t *src_strides, float *const *out, const size_t *out_strides, w2x_step_fn on_step, void *user);
 
 int tiles_enqueue_compute(w2x_ctx *ctx, const w2x_model *model, const float *const *in_tiles, float *const *out_tiles, int n_tiles, int width, int height, size_t in_stride_bytes, size_t out_stride_bytes);
 int tiles_enqueue_download(w2x_ctx *ctx, float *const *out_tiles, int n_tiles, int width, int height, size_t out_stride_bytes);
@@ -234,6 +241,34 @@ struct HostPin {
     HostPin &operator=(const HostPin &) = delete;
     ~HostPin() {
         if (p) cudaHostUnregister(p);
+    }
+};
+
+// Pinned views of many caller ranges for one call.  The ranges may overlap or share pages (windows whose sources are strided views
+// of one plane, outputs that are strided views of one array), and cudaHostRegister refuses a range that shares a page with a
+// registered one.  So the ranges not already pinned are rounded out to whole pages and merged, and each merged interval is one
+// HostPin (4 MiB and more).  Every page of an interval belongs to one of the ranges, so all of it is mapped.  A range is {first
+// byte, bytes from the first to the last byte}.
+struct HostRange { const void *p; size_t span; };
+struct HostPins {
+    std::vector<std::unique_ptr<HostPin>> pins;
+    explicit HostPins(const std::vector<HostRange> &ranges) {
+        const uintptr_t page = (uintptr_t)sysconf(_SC_PAGESIZE);
+        std::vector<std::pair<uintptr_t, uintptr_t>> iv;
+        for (const HostRange &r : ranges) {
+            cudaPointerAttributes at{};
+            if (cudaPointerGetAttributes(&at, r.p) == cudaSuccess && at.type != cudaMemoryTypeUnregistered) continue;
+            cudaGetLastError();
+            const uintptr_t a = reinterpret_cast<uintptr_t>(r.p);
+            iv.push_back({a / page * page, (a + r.span + page - 1) / page * page});
+        }
+        std::sort(iv.begin(), iv.end());
+        for (size_t i = 0; i < iv.size();) {
+            const uintptr_t a = iv[i].first;
+            uintptr_t b = iv[i].second;
+            for (i++; i < iv.size() && iv[i].first <= b; i++) b = std::max(b, iv[i].second);
+            pins.push_back(std::make_unique<HostPin>(reinterpret_cast<const void *>(a), (size_t)(b - a)));
+        }
     }
 };
 
