@@ -393,6 +393,55 @@ inline bool convertChainWithModels(Plane &inputPlane, Plane &outputPlane, const 
     return true;
 }
 
+// Not in the reference: convertChainWithModels for a collection of planes of any sizes in ONE call, packed into shared frames on the
+// GPU (w2x_convert_planes_chain; with several GPUs w2x_multi_convert_planes_chain, each plane on one GPU and each tta step's 8
+// variants spread over them).  outputPlanes[i] is bit-identical to convertChainWithModels on inputPlanes[i] alone, with the same
+// steps, precision and engine; it is (re)allocated to its final size unless it already has that size.  Same argument checks and error
+// reporting as convertChainWithModels, but no progress lines: a collection's would be one set per plane and step.
+inline bool convertPlanesChainWithModels(std::vector<Plane> &inputPlanes, std::vector<Plane> &outputPlanes,
+                                         const std::vector<ChainStep> &steps) {
+    w2x_ctx *ctx = gpuRuntime::context();
+    if (!ctx || steps.empty() || inputPlanes.empty()) return false;
+    std::vector<const w2x_model *> files;
+    std::vector<int> kinds;
+    int upscales = 0;
+    for (const ChainStep &s : steps) {
+        const w2x_model *f = s.models ? modelFileOf(*s.models) : nullptr;
+        if (!f) return false;
+        files.push_back(f);
+        kinds.push_back((s.upscale2x ? W2X_STEP_UPSCALE2X : W2X_STEP_SAME) | (s.tta ? W2X_STEP_TTA : 0));
+        if (s.upscale2x) upscales++;
+    }
+    const size_t n = inputPlanes.size();
+    outputPlanes.resize(n);
+    std::vector<const float *> in(n);
+    std::vector<float *> out(n);
+    std::vector<int> widths(n), heights(n);
+    std::vector<size_t> inStrides(n), outStrides(n);
+    for (size_t i = 0; i < n; i++) {
+        Plane &p = inputPlanes[i], &o = outputPlanes[i];
+        if (p.empty()) return false;
+        int w = p.width, h = p.height;
+        for (int k = 0; k < upscales; k++) { w *= 2; h *= 2; }
+        if (o.data == p.data || o.width != w || o.height != h) o.create(w, h);
+        in[i] = p.data; widths[i] = p.width; heights[i] = p.height; inStrides[i] = p.stride_bytes;
+        out[i] = o.data; outStrides[i] = o.stride_bytes;
+    }
+    w2x_ctx_set_log(ctx, nullptr, nullptr);   // with several GPUs the first context's log is the call's
+    int rc;
+    if (w2x_multi *mg = gpuRuntime::multi())
+        rc = w2x_multi_convert_planes_chain(mg, (int)steps.size(), files.data(), kinds.data(), (int)n, in.data(), widths.data(), heights.data(),
+                                            inStrides.data(), out.data(), outStrides.data(), nullptr, nullptr);
+    else
+        rc = w2x_convert_planes_chain(ctx, (int)steps.size(), files.data(), kinds.data(), (int)n, in.data(), widths.data(), heights.data(),
+                                      inStrides.data(), out.data(), outStrides.data(), nullptr, nullptr);
+    if (rc != W2X_OK) {
+        std::cerr << w2x_last_error() << std::endl;
+        return false;
+    }
+    return true;
+}
+
 #ifdef W2X_WITH_OPENCV
 // The reference's own signatures (src/modelHandler.hpp:87-88, src/convertRoutine.hpp:25-28) on cv::Mat: CV_32FC1 planes are
 // viewed in place (no copy), outputs are allocated like the reference does (cv::Mat::zeros).
