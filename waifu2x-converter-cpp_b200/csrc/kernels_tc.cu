@@ -30,6 +30,9 @@
 //                            K = 16 (fp16) / 32 (e4m3) per instruction; each drains its own accumulators: scale,
 //                            +bias, leaky-ReLU -> either the frame's records, staged in the TMA swizzle pattern and
 //                            TMA-stored, or (FUSE) the last layer's nine tap partials
+//               Cout = 64 layers (not fused) swap the roles: A = the 64 weight rows, B = the M-tile's 128 pixels, one
+//               m64n128 per K step (Cfg::SWAP, consume_swapped): a quarter less shared-memory operand traffic, same bits.
+//               Cout = 32 would fill half an m64 A; at Cout = 128 the accumulators and correction buffers do not fit.
 //
 #include <cuda.h>
 #include <cuda_fp16.h>

@@ -34,10 +34,19 @@ struct Cfg {
     static constexpr int B_BLOCK = COUT * B_ROWB;
     static constexpr int B_STAGE = 2 * B_BLOCK;
     static constexpr int STAGES_PER_TILESET = NCHUNK * 9;
+    // ---- operand roles (see tc_kernel.cuh) ----
+    //   SWAP = false: A = an m64 half of the M-tile's pixels, B = the Cout weight rows (N = Cout)
+    //   SWAP = true : A = the 64 weight rows (M = Cout), B = all 128 pixels of the M-tile (N = 128).  The stage image and the
+    //                 record boxes are read as they are; only the descriptors change.  Cout = 64 only: a 32-row A would
+    //                 leave half of every m64 wgmma empty, and at Cout = 128 two m64 channel halves would need 128
+    //                 accumulators plus two 64-register correction buffers per thread.  The fused last layer keeps
+    //                 SWAP = false (epilogue_fuse sums a pixel's channels across the lanes of a quad).
+    static constexpr bool SWAP = COUT == 64 && !FUSE;
     // ---- shared memory map: [A slots][B stages][store staging][barriers (1 KB)][bias | last-layer weights] ----
     static constexpr int BAR_BYTES = 1024;
     static constexpr int PRM_BYTES = 4 * COUT * (FUSE ? 10 : 1);             // the epilogue indexes them per lane: shared, not parameter space
-    static constexpr int STG_WG = 128 * 128;                                 // one 32-channel record block of an M-tile (128 px)
+    // one 32-channel record block of an M-tile (128 px); SWAP: both blocks, each written by the two warps holding its channels
+    static constexpr int STG_WG = (SWAP ? 2 : 1) * 128 * 128;
     static constexpr int STG_BYTES = FUSE ? 0 : 2 * STG_WG;
     static constexpr int SMEM_MAX = 227 * 1024;
     static constexpr int NB_FIT = (SMEM_MAX - 1024 - BAR_BYTES - PRM_BYTES - STG_BYTES - A_SLOTS * A_SLOT) / B_STAGE;

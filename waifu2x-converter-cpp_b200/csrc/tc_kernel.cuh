@@ -9,6 +9,27 @@ __device__ __forceinline__ float activate(float acc, float scale, float bias) {
     return fmaxf(v, 0.1f * v);                                           // leaky 0.1: min(v,0)*0.1 + max(v,0)
 }
 
+// The record of activated channels cc, cc + 1 (cc even, within the 32-channel block) of one pixel, written into the staging
+// row at rowaddr (swizzle phase sw = row & 7) in the TMA SWIZZLE_128B pattern: fp16 at byte 2 cc, then xh8 at 64 + cc and
+// xl8 at 96 + cc (F8) or lo fp16 at 64 + 2 cc.
+template <bool F8>
+__device__ __forceinline__ void store_record_pair(uint32_t rowaddr, uint32_t sw, uint32_t cc, float v0, float v1) {
+    const __half2 hh = f32x2_to_f16x2_sat(v0, v1);
+    const float2 hf = __half22float2(hh);
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(rowaddr + (((cc >> 3) ^ sw) << 4) + 2u * (cc & 7u)), "r"(*reinterpret_cast<const uint32_t *>(&hh)) : "memory");
+    if constexpr (F8) {
+        constexpr float kDown = 1.0f / (float)(1 << F8_C), kUp = (float)(1 << F8_A);
+        const __half2 hd = __hmul2(hh, __float2half2_rn(kDown));
+        const uint16_t h8 = __nv_cvt_halfraw2_to_fp8x2(static_cast<__half2_raw>(hd), __NV_SATFINITE, __NV_E4M3);
+        const uint16_t l8 = __nv_cvt_float2_to_fp8x2(make_float2((v0 - hf.x) * kUp, (v1 - hf.y) * kUp), __NV_SATFINITE, __NV_E4M3);
+        asm volatile("st.shared.b16 [%0], %1;" ::"r"(rowaddr + (((4u + (cc >> 4)) ^ sw) << 4) + (cc & 15u)), "h"(h8) : "memory");
+        asm volatile("st.shared.b16 [%0], %1;" ::"r"(rowaddr + (((6u + (cc >> 4)) ^ sw) << 4) + (cc & 15u)), "h"(l8) : "memory");
+    } else {
+        const __half2 lo = f32x2_to_f16x2_sat(v0 - hf.x, v1 - hf.y);
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(rowaddr + (((4u + (cc >> 3)) ^ sw) << 4) + 2u * (cc & 7u)), "r"(*reinterpret_cast<const uint32_t *>(&lo)) : "memory");
+    }
+}
+
 // One consumer warpgroup's M-tile (8 wide x 16 tall pixels = two m64 halves) of a tile-set: accumulators -> scale, bias,
 // leaky-ReLU -> records of each 32-channel block written into the warpgroup's staging tile in the TMA SWIZZLE_128B pattern
 // (staging row = pixel = y * 8 + x, conflict-free: the eight rows a warp writes at once fall into eight different 16-byte
@@ -34,21 +55,7 @@ __device__ __forceinline__ void epilogue_store(const TcParams &p, const float *b
                     const int jj = cb * 4 + j, ch = 8 * jj + 2 * q;
                     const float v0 = activate(acc[h][4 * jj + 2 * e], p.out_scale, bias[ch]);
                     const float v1 = activate(acc[h][4 * jj + 2 * e + 1], p.out_scale, bias[ch + 1]);
-                    const __half2 hh = f32x2_to_f16x2_sat(v0, v1);
-                    const float2 hf = __half22float2(hh);
-                    asm volatile("st.shared.b32 [%0], %1;" ::"r"(rowaddr + (((uint32_t)j ^ sw) << 4) + 4u * q), "r"(*reinterpret_cast<const uint32_t *>(&hh)) : "memory");
-                    if constexpr (F8) {
-                        constexpr float kDown = 1.0f / (float)(1 << F8_C), kUp = (float)(1 << F8_A);
-                        const __half2 hd = __hmul2(hh, __float2half2_rn(kDown));
-                        const uint16_t h8 = __nv_cvt_halfraw2_to_fp8x2(static_cast<__half2_raw>(hd), __NV_SATFINITE, __NV_E4M3);
-                        const uint16_t l8 = __nv_cvt_float2_to_fp8x2(make_float2((v0 - hf.x) * kUp, (v1 - hf.y) * kUp), __NV_SATFINITE, __NV_E4M3);
-                        const uint32_t in_unit = 8u * (uint32_t)(j & 1) + 2u * q;
-                        asm volatile("st.shared.b16 [%0], %1;" ::"r"(rowaddr + (((uint32_t)(4 + (j >> 1)) ^ sw) << 4) + in_unit), "h"(h8) : "memory");
-                        asm volatile("st.shared.b16 [%0], %1;" ::"r"(rowaddr + (((uint32_t)(6 + (j >> 1)) ^ sw) << 4) + in_unit), "h"(l8) : "memory");
-                    } else {
-                        const __half2 lo = f32x2_to_f16x2_sat(v0 - hf.x, v1 - hf.y);
-                        asm volatile("st.shared.b32 [%0], %1;" ::"r"(rowaddr + (((uint32_t)(4 + j) ^ sw) << 4) + 4u * q), "r"(*reinterpret_cast<const uint32_t *>(&lo)) : "memory");
-                    }
+                    store_record_pair<F8>(rowaddr, sw, (uint32_t)(8 * j + 2 * q), v0, v1);
                 }
             }
         }
@@ -58,6 +65,45 @@ __device__ __forceinline__ void epilogue_store(const TcParams &p, const float *b
             tma_store_4d(tmap_out, stg, 0, cb, gx0, gy0);
             bulk_commit();
         }
+    }
+}
+
+// epilogue_store for channel-major accumulators (Cfg::SWAP, Cout = 64): the thread holds channels ch = 16 wq + r + 8e
+// (r = lane / 4) of the pixels n = 8j + 2q + {0, 1} (y = j, x = 2q + {0, 1}) at acc[4j + 2e + {0, 1}].  Lanes r and r ^ 1
+// swap one value each, so the even lane holds channels ch, ch + 1 of pixel x = 2q and the odd lane those of x = 2q + 1:
+// the same channel pairs, expressions and stores as epilogue_store.  Warps 0, 1 hold block 0 and warps 2, 3 block 1, each
+// written into its own staging tile; warp 0 sends both boxes.
+template <bool F8>
+__device__ __forceinline__ void epilogue_store_swapped(const TcParams &p, const float *bias, const CUtensorMap *tmap_out, const float (&acc)[64],
+                                                       uint32_t stg, int wg, int wq, int lane, int gx0, int gy0) {
+    const int q = lane & 3, r = lane >> 2, odd = r & 1;
+    const uint32_t blk = stg + (uint32_t)(wq >> 1) * (128u * 128u), x = (uint32_t)(2 * q + odd);
+    if (wq == 0) {                        // the lanes of warp 0 wait for their own stores of the previous tile-set to have left
+        bulk_wait_read();
+        __syncwarp();
+    }
+    named_sync(1 + wg, 128);
+#pragma unroll
+    for (int e = 0; e < 2; e++) {
+        const int ch = 16 * wq + (r & ~1) + 8 * e;
+        const float b0 = bias[ch], b1 = bias[ch + 1];
+        const uint32_t cc = (uint32_t)(ch & 31);
+#pragma unroll
+        for (int j = 0; j < 16; j++) {
+            const float a0 = acc[4 * j + 2 * e], a1 = acc[4 * j + 2 * e + 1];
+            const float other = __shfl_xor_sync(0xffffffffu, odd ? a0 : a1, 4);
+            const float v0 = activate(odd ? other : a0, p.out_scale, b0);
+            const float v1 = activate(odd ? a1 : other, p.out_scale, b1);
+            const uint32_t row = 8u * (uint32_t)j + x;
+            store_record_pair<F8>(blk + row * 128u, x, cc, v0, v1);
+        }
+    }
+    fence_proxy_async();
+    named_sync(1 + wg, 128);
+    if (wq == 0) {
+        tma_store_4d(tmap_out, stg, 0, 0, gx0, gy0);
+        tma_store_4d(tmap_out, stg + 128u * 128u, 0, 1, gx0, gy0);
+        bulk_commit();
     }
 }
 
@@ -135,6 +181,153 @@ __device__ __forceinline__ void epilogue_fuse(const TcParams &p, const float *bi
 // PRODUCER_REGS, and the consumer warpgroups take the rest: the accumulators alone are COUT fp32 registers per thread.
 constexpr uint32_t PRODUCER_REGS = 40, CONSUMER_REGS = 232;
 static_assert(128 * PRODUCER_REGS + 256 * CONSUMER_REGS == NUM_THREADS * 168, "register hand-off must balance");
+
+// The consumer warpgroup of a Cout = 64 layer (Cfg::SWAP): D[channel][pixel], A = the stage's 64 weight rows (the packed
+// image as it is: fp16 rows of 64 B, SWIZZLE_64B; e4m3 rows of 32 B, SWIZZLE_32B), B = the M-tile's 128 pixels (N = 128;
+// the record box with the same descriptor the m64 halves use, eight pixels per halo row).  Per (tap, chunk) one m64n128
+// per K step reads 24 KB of shared memory where two m64n64 halves read 32 KB: a tile-set of these layers is bound by the
+// shared-memory operand traffic, not by the tensor cores.  Each element sees the same products in the same order, and
+// the tensor cores' sums do not depend on which operand is A.
+//   f16x3 / xh_only: one group per tap, as in the kernel below.
+//   F8: F_t = the f16 product of tap t into acc, X_t = its e4m3 corrections into the fresh buffer corr[t & 1].  Issue order
+//   F_0 X_0 | X_1 [wait: F_0, X_0 done; acc += corr[0]] F_1 | X_2 [wait; acc += corr[1]] F_2 | ... F_8 [wait all]: the
+//   next tap's corrections run while the adds do, and per element the order stays f16 product of tap t, correction of
+//   tap t, f16 product of tap t + 1.  Taps unrolled, the chunk ends with an empty pipe (see below).
+template <int CIN, bool F8>
+__device__ __forceinline__ void consume_swapped(const TcParams &p, const CUtensorMap *tmap_out, uint32_t a_base, uint32_t b_base, uint32_t stg,
+                                                uint32_t bar_base, const float *prm, int wg, int wq, int lane, unsigned long long *prof) {
+    using C = Cfg<CIN, 64, false, F8>;
+    auto a_full = [&](uint32_t i) { return bar_base + 8u * i; };
+    auto a_empty = [&](uint32_t i) { return bar_base + 8u * (2u + i); };
+    auto b_full = [&](uint32_t i) { return bar_base + 8u * (4u + i); };
+    auto b_empty = [&](uint32_t i) { return bar_base + 8u * (4u + C::NB + i); };
+    constexpr uint32_t ROWB = C::ROWB;
+    constexpr uint32_t X_HI = desc_hi(HALO * ROWB, SW128);      // B: next 8-pixel group = next halo row
+    constexpr uint32_t W_HI = desc_hi(8 * 64, SW64);             // A: fp16 weight rows of 64 B
+    constexpr uint32_t W8_HI = desc_hi(8 * 32, SW32);            // A: e4m3 weight rows of 32 B
+    const bool prof_on = prof != nullptr;
+    float acc[64];
+    float corr[F8 ? 2 : 1][64];
+#pragma unroll
+    for (int i = 0; i < 64; i++) acc[i] = 0.f;
+    uint32_t a_it = 0, stage = 0, phase = 0, n = 0;
+    unsigned long long w_af = 0, w_bf = 0;
+    // the next weight stage, once it has arrived
+    auto next_stage = [&]() -> uint32_t {
+        if (!C::RESIDENT) mbar_wait_prof(b_full(stage), phase, prof_on, w_bf);
+        else if (n == 0) mbar_wait_prof(b_full(stage), 0u, prof_on, w_bf);   // the stages arrive once, during the first tile-set
+        const uint32_t s = stage;
+        if (++stage == (uint32_t)C::NB) { stage = 0; phase ^= 1u; }
+        return s;
+    };
+    const long long t_begin = clock64();
+    for (int ts = blockIdx.x; ts < p.n_tilesets; ts += gridDim.x, n++) {
+        const int ty = ts / p.tiles_x, tx = ts - ty * p.tiles_x;
+        if constexpr (F8) {
+            for (int c = 0; c < C::NCHUNK; c++, a_it++) {
+                const uint32_t slot = a_it & 1u;
+                mbar_wait_prof(a_full(slot), (a_it >> 1) & 1u, prof_on, w_af);
+                const uint32_t x0 = a_base + slot * C::A_SLOT + (uint32_t)wg * 8u * ROWB;
+                auto px = [&](int t) { return x0 + (uint32_t)((t / 3) * HALO + t % 3) * ROWB; };
+                auto issue_f16 = [&](int t, uint32_t s, uint32_t scale_d) {
+                    const uint32_t w = b_base + s * C::B_STAGE, x = px(t);
+                    acc_fence(acc);
+                    wgmma_fence();
+                    Wgmma<128>::f16(acc, make_desc(W_HI, w), make_desc(X_HI, x), scale_d);               // wh * xh
+                    Wgmma<128>::f16(acc, make_desc(W_HI, w + 32u), make_desc(X_HI, x + 32u), 1u);
+                    wgmma_commit();
+                };
+                auto issue_corr = [&](int t, uint32_t s) {
+                    const uint32_t w = b_base + s * C::B_STAGE, x = px(t);
+                    acc_fence(corr[t & 1]);
+                    wgmma_fence();
+                    Wgmma<128>::e4m3(corr[t & 1], make_desc(W8_HI, w + 64u * 64u), make_desc(X_HI, x + 96u), 0u);   // wh8 * xl8
+                    Wgmma<128>::e4m3(corr[t & 1], make_desc(W8_HI, w + 64u * 96u), make_desc(X_HI, x + 64u), 1u);   // wl8 * xh8
+                    wgmma_commit();
+                };
+                uint32_t st_cur = next_stage();
+                issue_f16(0, st_cur, c != 0 ? 1u : 0u);
+                issue_corr(0, st_cur);
+#pragma unroll 9
+                for (int t = 0; t < 9; t++) {
+                    uint32_t st_next = 0;
+                    if (t < 8) {
+                        st_next = next_stage();
+                        issue_corr(t + 1, st_next);
+                        wgmma_wait<1>();                     // all but X_{t+1}: F_t and X_t have completed
+                    } else {
+                        wgmma_wait<0>();
+                    }
+                    acc_fence(acc);
+                    acc_fence(corr[t & 1]);
+#pragma unroll
+                    for (int i = 0; i < 64; i++) acc[i] += corr[t & 1][i];
+                    acc_fence(acc);
+                    if (lane == 0) {                         // tap t's stage (and after tap 8 the slot) is read by no group any more
+                        if (!C::RESIDENT) mbar_arrive(b_empty(st_cur));
+                        if (t == 8) mbar_arrive(a_empty(slot));
+                    }
+                    if (t < 8) {
+                        issue_f16(t + 1, st_next, 1u);
+                        st_cur = st_next;
+                    }
+                }
+            }
+        } else {
+            // f16x3, or with p.xh_only the xh * wh K steps alone, chosen once per tile-set (no group in flight)
+            auto chunks = [&](auto xh_only_tag) {
+                constexpr bool XH_ONLY = decltype(xh_only_tag)::value;
+                int pend_b = -1, pend_a = -1;                // stage / slot read by the previous tap's group
+                for (int c = 0; c < C::NCHUNK; c++, a_it++) {
+                    const uint32_t slot = a_it & 1u;
+                    mbar_wait_prof(a_full(slot), (a_it >> 1) & 1u, prof_on, w_af);
+                    const uint32_t x0 = a_base + slot * C::A_SLOT + (uint32_t)wg * 8u * ROWB;
+#pragma unroll 1
+                    for (int t = 0; t < 9; t++) {
+                        const uint32_t x = x0 + (uint32_t)((t / 3) * HALO + t % 3) * ROWB;
+                        const uint32_t s = next_stage(), w = b_base + s * C::B_STAGE, wl = w + 64u * 64u;
+                        const uint32_t first = (c | t) != 0 ? 1u : 0u;
+                        acc_fence(acc);
+                        wgmma_fence();
+                        Wgmma<128>::f16(acc, make_desc(W_HI, w), make_desc(X_HI, x), first);              // wh * xh
+                        Wgmma<128>::f16(acc, make_desc(W_HI, w + 32u), make_desc(X_HI, x + 32u), 1u);
+                        if constexpr (!XH_ONLY) {
+                            Wgmma<128>::f16(acc, make_desc(W_HI, w), make_desc(X_HI, x + 64u), 1u);       // wh * xl
+                            Wgmma<128>::f16(acc, make_desc(W_HI, w + 32u), make_desc(X_HI, x + 96u), 1u);
+                            Wgmma<128>::f16(acc, make_desc(W_HI, wl), make_desc(X_HI, x), 1u);             // wl * xh
+                            Wgmma<128>::f16(acc, make_desc(W_HI, wl + 32u), make_desc(X_HI, x + 32u), 1u);
+                        }
+                        wgmma_commit();
+                        wgmma_wait<1>();                             // the previous group is done: its stage / slot may be refilled
+                        acc_fence(acc);
+                        if (lane == 0) {
+                            if (!C::RESIDENT && pend_b >= 0) mbar_arrive(b_empty((uint32_t)pend_b));
+                            if (pend_a >= 0) mbar_arrive(a_empty((uint32_t)pend_a));
+                        }
+                        pend_b = (int)s;
+                        pend_a = t == 8 ? (int)slot : -1;
+                    }
+                }
+                wgmma_wait<0>();
+                acc_fence(acc);
+                if (lane == 0) {
+                    if (!C::RESIDENT && pend_b >= 0) mbar_arrive(b_empty((uint32_t)pend_b));
+                    if (pend_a >= 0) mbar_arrive(a_empty((uint32_t)pend_a));
+                }
+            };
+            if (p.xh_only) chunks(std::true_type{});
+            else chunks(std::false_type{});
+        }
+        epilogue_store_swapped<F8>(p, prm, tmap_out, acc, stg, wg, wq, lane, tx * REGION + 8 * wg, ty * REGION);
+    }
+    if (wq == 0) bulk_wait_all();    // this warpgroup's TMA stores are complete before the CTA may exit
+    if (prof_on && wg == 0 && wq == 0 && lane == 0) {
+        prof[PROF_TOTAL] += (unsigned long long)(clock64() - t_begin);
+        prof[PROF_MMA_WAIT_A] += w_af;
+        prof[PROF_MMA_WAIT_B] += w_bf;
+        prof[PROF_TILESETS] += n;
+    }
+}
 
 template <int CIN, int COUT, bool FUSE, bool F8>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
@@ -215,6 +408,10 @@ tc_conv3x3_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_cons
             }
             if (prof_on && lane == 0) prof[PROF_BPROD_WAIT] += w_b;
         }
+    } else if constexpr (C::SWAP) {
+        setmaxnreg_inc<CONSUMER_REGS>();
+        consume_swapped<CIN, F8>(p, &tmap_out, a_base, b_base, stg_base + (uint32_t)((warp - 4) >> 2) * C::STG_WG, bar_base, prm, (warp - 4) >> 2,
+                                 warp & 3, lane, prof);
     } else {
         setmaxnreg_inc<CONSUMER_REGS>();
         // ===================== consumers: warpgroup wg = M-tile wg (pixels x in [8 wg, 8 wg + 8) of the tile-set) ===========
