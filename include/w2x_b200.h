@@ -130,7 +130,19 @@ W2X_API int w2x_ctx_get_engine(const w2x_ctx *ctx);
  *                           <= 1e-3 relative for a < 4094 (about 1e-4 at a = 150 to 300)
  *   W2X_PRECISION_F16       <= 4e-3 relative for a < 4094
  * Beyond a = 4094 every precision saturates its records at +-65504 (fp16 hi and lo): outputs stay finite, with no
- * accuracy bound (they no longer follow the reference).  The fp32 engine has no such limit. */
+ * accuracy bound (they no longer follow the reference).  The fp32 engine has no such limit.
+ * Model scale: the records hold 16 a at a fixed scale, so a layer whose activations are small loses their low bits
+ * (fp16 subnormals; e4m3 underflow of the default precision's copies) and later layers amplify the loss.  With
+ * g = the largest ratio, over the inputs of the tensor-core layers (layers 1 .. L-2), of max(1, max |output|) to that
+ * input's largest |activation| (about 7 for the shipped models on planes in [0, 1]), the ranges above hold for g <= 64
+ * (the default precision also needs max |w| >= 1/16 in every tensor-core layer: below, the weight scale of the packed
+ * operands, at most 2^14, no longer lifts them to the e4m3 copies' range).  Beyond, for a < 4094:
+ *   W2X_PRECISION_F16X3     <= 4e-8 g relative to float64 (about 1.3e-4 at g = 3e4)
+ *   W2X_PRECISION_F16_F8X2  <= 1e-3 relative (about 4e-4 at g = 3e4)
+ * Asserted by tests/test_model_scale.py on power-of-two rescalings of the shipped models (one layer's output x 2^-12 to
+ * 2^12), which the reference and the fp32 engine compute bit for bit as the originals.  A model whose tensor-core layers
+ * hold a non-finite weight or one of |w| >= 65520 (past the fp16 limit) runs on the fp32 engine: W2X_ENGINE_AUTO picks
+ * it; W2X_ENGINE_TC returns W2X_ERR_UNSUPPORTED for it, and for w2x_filter_layer of such a layer. */
 /* The environment variable W2X_PRECISION=f16x3|f8|f16 sets the initial value of new contexts. */
 #define W2X_PRECISION_F16X3 0
 #define W2X_PRECISION_F16_F8X2 1

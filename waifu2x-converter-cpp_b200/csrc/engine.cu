@@ -133,7 +133,7 @@ int pick_engine(w2x_ctx *ctx, const w2x_model *m) {
     int e = ctx->engine;
     if (e == W2X_ENGINE_AUTO) e = m->tc_eligible ? W2X_ENGINE_TC : W2X_ENGINE_FP32;
     if (e == W2X_ENGINE_TC && !m->tc_eligible) {
-        fail(W2X_ERR_UNSUPPORTED, "tensor-core engine needs a 1->{32,64,128}...->1 layer chain");
+        fail(W2X_ERR_UNSUPPORTED, "tensor-core engine needs a 1->{32,64,128}...->1 layer chain with finite inner weights below 65520");
         return -1;
     }
     return e;
@@ -708,6 +708,8 @@ int w2x_filter_layer_device(w2x_ctx *ctx, const w2x_model *model, int layer, con
     if (engine == W2X_ENGINE_TC) {
         if (!tc::layer_supported(L.n_in, L.n_out))
             return fail(W2X_ERR_UNSUPPORTED, "tensor-core engine does not support a %d->%d layer", L.n_in, L.n_out);
+        if (model->tc[(size_t)layer].bytes.empty())
+            return fail(W2X_ERR_UNSUPPORTED, "tensor-core engine needs finite layer weights below 65520 in magnitude");
         rc = ensure_tc(ctx);
         if (rc) return rc;
         // Model::filter semantics (same size, BORDER_REPLICATE): stage a frame with a replicated ring

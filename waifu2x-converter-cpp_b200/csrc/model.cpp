@@ -453,6 +453,14 @@ static void pack_tc_layer_strip(const Layer &L, TcPack &P) {
         }
 }
 
+// Whether the tensor-core operand images can hold the layer's weights: wscale is never below 1, so a weight of
+// |w| >= 65520 (or a non-finite one) would pack as an fp16 infinity.
+static bool tc_packable(const Layer &L) {
+    for (float v : L.w)
+        if (!(std::fabs(v) < 65520.f)) return false;
+    return true;
+}
+
 int finalize_model(w2x_model *m) {
     if (m->layers.empty()) return fail(W2X_ERR_MODEL, "Error : model has no layers");
     for (size_t i = 0; i < m->layers.size(); i++) {
@@ -463,17 +471,17 @@ int finalize_model(w2x_model *m) {
             return fail(W2X_ERR_MODEL, "Error : model layer %zu : nInputPlane %d does not match previous nOutputPlane %d",
                         i, L.n_in, m->layers[i - 1].n_out);
     }
-    // tensor-core eligibility: 1 -> C1 -> ... -> Cn -> 1 with every inner width in {32, 64, 128}
+    // tensor-core eligibility: 1 -> C1 -> ... -> Cn -> 1 with every inner width in {32, 64, 128} and every inner layer packable
     auto okc = [](int c) { return c == 32 || c == 64 || c == 128; };
     size_t n = m->layers.size();
     bool ok = n >= 3 && m->layers.front().n_in == 1 && m->layers.back().n_out == 1 &&
               okc(m->layers.front().n_out) && okc(m->layers.back().n_in);
-    for (size_t i = 1; ok && i + 1 < n; i++) ok = okc(m->layers[i].n_in) && okc(m->layers[i].n_out);
+    for (size_t i = 1; ok && i + 1 < n; i++) ok = okc(m->layers[i].n_in) && okc(m->layers[i].n_out) && tc_packable(m->layers[i]);
     m->tc_eligible = ok;
     m->tc.assign(n, TcPack());
     for (size_t i = 0; i < n; i++) {
         const Layer &L = m->layers[i];
-        if (okc(L.n_in) && okc(L.n_out)) {
+        if (okc(L.n_in) && okc(L.n_out) && tc_packable(L)) {
             pack_tc_layer(L, m->tc[i]);
             pack_tc_layer_f8(L, m->tc[i]);
         }
