@@ -142,11 +142,26 @@ W2X_API int w2x_ctx_get_engine(const w2x_ctx *ctx);
  * Asserted by tests/test_model_scale.py on power-of-two rescalings of the shipped models (one layer's output x 2^-12 to
  * 2^12), which the reference and the fp32 engine compute bit for bit as the originals.  A model whose tensor-core layers
  * hold a non-finite weight or one of |w| >= 65520 (past the fp16 limit) runs on the fp32 engine: W2X_ENGINE_AUTO picks
- * it; W2X_ENGINE_TC returns W2X_ERR_UNSUPPORTED for it, and for w2x_filter_layer of such a layer. */
-/* The environment variable W2X_PRECISION=f16x3|f8|f16 sets the initial value of new contexts. */
+ * it; W2X_ENGINE_TC returns W2X_ERR_UNSUPPORTED for it, and for w2x_filter_layer of such a layer.
+ *   W2X_PRECISION_BF16X3    x*w = xh*wh + xl*wh + xh*wl with h = the bf16 rounding: three bf16 tensor-core products
+ *                           on records hi = bf16(16 a), lo = bf16(16 a - hi) and weights packed at scale 1.  bf16 has
+ *                           fp32's exponent range, so nothing saturates or underflows where fp16 and e4m3 do:
+ *                           <= 3e-5 relative to float64 for any activation and model scale whose activations stay
+ *                           within fp32's normal range (measured on H100: 7e-6 to 1.5e-5 at input scales x1 to x1e6;
+ *                           f16x3 stays the more accurate choice at a < 4094 and g <= 64).  A power-of-two rescaling of
+ *                           a model's layers (as above) gives bit-identical outputs.  Eligibility: the same layer shapes
+ *                           with finite inner weights, no 65520 limit; W2X_ENGINE_AUTO runs such a model on the tensor
+ *                           cores in this precision only (every other precision still sends a weight of |w| >= 65520 to
+ *                           the fp32 engine), and W2X_ENGINE_TC refuses only non-finite inner weights.  Measured with
+ *                           tools/precision_bench.py on a 4096x4096 scale2.0x pass: 380 Mpix/s against f16x3's 366 in
+ *                           the same run, H100 80GB HBM3 at a 700 W power limit and a 1980 MHz max SM clock.
+ *                           Asserted by tests/test_precision_bf16.py. */
+/* The environment variable W2X_PRECISION=f16x3|f8|f16|bf16x3 sets the initial value of new contexts. */
 #define W2X_PRECISION_F16X3 0
 #define W2X_PRECISION_F16_F8X2 1
 #define W2X_PRECISION_F16 2
+/* 3 is not a precision and stays one: w2x_ctx_set_precision(ctx, 3) returns W2X_ERR_ARG.  bf16x3 is 4. */
+#define W2X_PRECISION_BF16X3 4
 W2X_API int w2x_ctx_set_precision(w2x_ctx *ctx, int precision);
 W2X_API int w2x_ctx_get_precision(const w2x_ctx *ctx);
 /* Run on a caller-owned CUDA stream (cudaStream_t passed as void*); NULL = the ctx's own stream.

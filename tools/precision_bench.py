@@ -1,4 +1,4 @@
-"""precision_bench.py -- the tensor-core engine's three precisions side by side, in one process:
+"""precision_bench.py -- the tensor-core engine's four precisions side by side, in one process:
 
     python tools/precision_bench.py [--size 4096] [--rounds 3] [--steps 5] [--out DIR]
 
@@ -67,7 +67,8 @@ def main():
     if not torch.cuda.is_available():
         sys.exit("precision_bench.py needs a CUDA device")
     w2x = w2x_loader.load()
-    precs = {"f16x3": w2x.PRECISION_F16X3, "f16+f8x2": w2x.PRECISION_F16_F8X2, "f16": w2x.PRECISION_F16}
+    precs = {"f16x3": w2x.PRECISION_F16X3, "f16+f8x2": w2x.PRECISION_F16_F8X2, "f16": w2x.PRECISION_F16,
+             "bf16x3": w2x.PRECISION_BF16X3}
     stream = torch.cuda.Stream()                                      # the contexts run on it, the CUDA events are recorded on it
     torch.cuda.set_stream(stream)
     ctxs = {}

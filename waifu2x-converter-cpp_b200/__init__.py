@@ -17,7 +17,7 @@ The directory name is not a valid Python identifier; load it with
 (tests/conftest.py, bench.py and __graft_entry__.py do exactly this through w2x_loader.py).
 """
 from .capi import (  # noqa: F401
-    ENGINE_AUTO, ENGINE_FP32, ENGINE_TC, PRECISION_F16X3, PRECISION_F16_F8X2, PRECISION_F16, STEP_SAME, STEP_UPSCALE2X, WALK_BLOCKS, WALK_FUSED, Band, Context, DevBytes, Model, Multi, Slab, W2xError,
+    ENGINE_AUTO, ENGINE_FP32, ENGINE_TC, PRECISION_F16X3, PRECISION_F16_F8X2, PRECISION_F16, PRECISION_BF16X3, STEP_SAME, STEP_UPSCALE2X, WALK_BLOCKS, WALK_FUSED, Band, Context, DevBytes, Model, Multi, Slab, W2xError,
     block_table, chain_region_source, debug_plan_multi_planes, debug_plan_multi_regions, debug_plan_planes, get_block_size, get_jobs, lib, lib_path, requires_splitting, set_block_size,
     set_block_size_exp2_square, set_jobs, version,
 )

@@ -17,6 +17,7 @@ _LIB_PATH = os.path.join(_HERE, "libw2x_b200.so")
 
 ENGINE_AUTO, ENGINE_FP32, ENGINE_TC = 0, 1, 2
 PRECISION_F16X3, PRECISION_F16_F8X2, PRECISION_F16 = 0, 1, 2
+PRECISION_BF16X3 = 4                 # 3 is not a precision
 WALK_FUSED, WALK_BLOCKS = 0, 1
 STEP_SAME, STEP_UPSCALE2X, STEP_TTA = 0, 1, 4
 
@@ -178,6 +179,7 @@ def lib():
     L.w2x_debug_set_fuse_last.argtypes = [vp, ci]
     L.w2x_debug_set_num_sms.argtypes = [vp, ci]
     L.w2x_debug_tc_pack8.argtypes = [vp, ci, C.POINTER(C.POINTER(C.c_uint8)), C.POINTER(cs)]
+    L.w2x_debug_tc_pack_bf16.argtypes = [vp, ci, C.POINTER(C.POINTER(C.c_uint16)), C.POINTER(cs)]
     L.w2x_debug_tc_strip.argtypes = [vp, ci, ci, C.POINTER(C.POINTER(C.c_uint8)), C.POINTER(cs)]
     L.w2x_debug_tc_profile_enable.argtypes = [vp, ci]
     L.w2x_debug_tc_profile_read.argtypes = [vp, ci, C.POINTER(C.c_uint64), C.POINTER(ci)]
@@ -369,6 +371,14 @@ class Model:
         """uint8 image [chunk][tap][kblock][wh fp16 n_out*64 B | wh8 n_out*32 B | wl8 n_out*32 B] of the f8 flavour."""
         dp, n = C.POINTER(C.c_uint8)(), C.c_size_t()
         _check(lib().w2x_debug_tc_pack8(self._h, layer, C.byref(dp), C.byref(n)))
+        return None if n.value == 0 else np.ctypeslib.as_array(dp, shape=(n.value,)).copy()
+
+
+    def debug_tc_pack_bf16(self, layer):
+        """bf16 bit patterns [chunk][tap][hi|lo][n_out*32] of the bf16x3 flavour (debug_tc_pack's layout, wscale 1); None when the
+        layer has none."""
+        dp, n = C.POINTER(C.c_uint16)(), C.c_size_t()
+        _check(lib().w2x_debug_tc_pack_bf16(self._h, layer, C.byref(dp), C.byref(n)))
         return None if n.value == 0 else np.ctypeslib.as_array(dp, shape=(n.value,)).copy()
 
 

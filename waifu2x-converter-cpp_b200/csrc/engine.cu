@@ -55,6 +55,7 @@ int get_dev_model(w2x_ctx *ctx, const w2x_model *m, DevModel **out) {
     dm.b.resize(n);
     dm.pack.resize(n);
     dm.pack8.resize(n);
+    dm.pack_bf16.resize(n);
     dm.out_scale.assign(n, 1.f);
     for (size_t i = 0; i < n; i++) {
         const Layer &L = m->layers[i];
@@ -75,7 +76,7 @@ int get_dev_model(w2x_ctx *ctx, const w2x_model *m, DevModel **out) {
             CU_CHECK(cudaMemcpyAsync(dm.pack8[i].get(), P.bytes8.data(), P.bytes8.size(), cudaMemcpyHostToDevice, ctx->stream));
         }
     }
-    if (m->tc_eligible) {
+    if (m->tc_eligible || m->tc_eligible_bf16) {
         const Layer &L = m->layers.back();                // n_out == 1: w is [1][Cin][9]
         dm.last_w_t.assign((size_t)9 * L.n_in, 0.f);
         for (int c = 0; c < L.n_in; c++)
@@ -84,6 +85,16 @@ int get_dev_model(w2x_ctx *ctx, const w2x_model *m, DevModel **out) {
     CU_CHECK(cudaStreamSynchronize(ctx->stream));
     auto res = ctx->models.emplace(m->uid, std::move(dm));
     *out = &res.first->second;
+    return W2X_OK;
+}
+
+int upload_pack_bf16(w2x_ctx *ctx, const w2x_model *m, DevModel *dm) {
+    for (size_t i = 0; i < m->layers.size(); i++) {
+        const std::vector<uint16_t> &v = m->tc[i].bytes_bf16;
+        if (v.empty() || dm->pack_bf16[i].get()) continue;
+        CU_CHECK(dm->pack_bf16[i].grow(v.size() * 2));
+        CU_CHECK(cudaMemcpyAsync(dm->pack_bf16[i].get(), v.data(), v.size() * 2, cudaMemcpyHostToDevice, ctx->stream));
+    }
     return W2X_OK;
 }
 
@@ -131,9 +142,12 @@ void emit_reference_progress(w2x_ctx *ctx, int w, int h, int n_layers, bool spli
 
 int pick_engine(w2x_ctx *ctx, const w2x_model *m) {
     int e = ctx->engine;
-    if (e == W2X_ENGINE_AUTO) e = m->tc_eligible ? W2X_ENGINE_TC : W2X_ENGINE_FP32;
-    if (e == W2X_ENGINE_TC && !m->tc_eligible) {
-        fail(W2X_ERR_UNSUPPORTED, "tensor-core engine needs a 1->{32,64,128}...->1 layer chain with finite inner weights below 65520");
+    const bool ok = tc_eligible(m, ctx->precision);
+    if (e == W2X_ENGINE_AUTO) e = ok ? W2X_ENGINE_TC : W2X_ENGINE_FP32;
+    if (e == W2X_ENGINE_TC && !ok) {
+        fail(W2X_ERR_UNSUPPORTED, ctx->precision == W2X_PRECISION_BF16X3
+                                      ? "tensor-core engine needs a 1->{32,64,128}...->1 layer chain with finite inner weights"
+                                      : "tensor-core engine needs a 1->{32,64,128}...->1 layer chain with finite inner weights below 65520");
         return -1;
     }
     return e;
@@ -151,16 +165,24 @@ int launch_layer_tc(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int li, cons
                     bool fused, bool profile, int out_y0, int out_rows) {
     if (out_rows < 0) { out_y0 = 0; out_rows = ph; }
     const Layer &L = m->layers[(size_t)li];
-    const int f8 = ctx->precision == W2X_PRECISION_F16_F8X2 ? 1 : 0;
+    const tc::Rec rec = tc::rec_format(ctx->precision);
+    if (rec == tc::Rec::BF16 && !dm->pack_bf16[(size_t)li].get()) {
+        const int rc = upload_pack_bf16(ctx, m, dm);
+        if (rc) return rc;
+    }
+    const void *wpack = rec == tc::Rec::F8     ? (const void *)dm->pack8[(size_t)li].get()
+                        : rec == tc::Rec::BF16 ? (const void *)dm->pack_bf16[(size_t)li].get()
+                                               : (const void *)dm->pack[(size_t)li].get();
+    const float out_scale = rec == tc::Rec::BF16 ? 1.0f / tc::ACT_SCALE : dm->out_scale[(size_t)li];   // bf16x3 packs at wscale 1
     {
         LayerTimer t(ctx, li);
-        CU_CHECK(tc::launch_tc_layer(in, f8 ? (const void *)dm->pack8[(size_t)li].get() : (const void *)dm->pack[(size_t)li].get(),
-                                     dm->b_host[(size_t)li].data(), out, L.n_in, L.n_out, pw, ph, dm->out_scale[(size_t)li], ctx->precision,
+        CU_CHECK(tc::launch_tc_layer(in, wpack, dm->b_host[(size_t)li].data(), out, L.n_in, L.n_out, pw, ph, out_scale, ctx->precision,
                                      ctx->num_sms, ctx->stream,
                                      profile && ctx->prof_buf.get() ? ctx->prof_buf.get() + (size_t)li * tc::PROF_MAX_CTAS * tc::PROF_WORDS : nullptr,
                                      fused ? dm->last_w_t.data() : nullptr, fused ? reinterpret_cast<float *>(out) : nullptr, out_y0, out_rows));
     }
-    static const char *const names[3][2] = {{"wgmma_f16x3", "wgmma_f16x3+last"}, {"wgmma_f16+f8x2", "wgmma_f16+f8x2+last"}, {"wgmma_f16", "wgmma_f16+last"}};
+    static const char *const names[5][2] = {{"wgmma_f16x3", "wgmma_f16x3+last"}, {"wgmma_f16+f8x2", "wgmma_f16+f8x2+last"}, {"wgmma_f16", "wgmma_f16+last"},
+                                            {nullptr, nullptr}, {"wgmma_bf16x3", "wgmma_bf16x3+last"}};
     note_kernel(ctx, li, names[ctx->precision][fused ? 1 : 0]);
     ctx->launches++;
     return W2X_OK;
@@ -204,7 +226,7 @@ int run_basic(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int engine, const 
         return W2X_OK;
     }
     // ---- tensor-core engine ----
-    const int f8 = ctx->precision == W2X_PRECISION_F16_F8X2 ? 1 : 0;
+    const tc::Rec rec = tc::rec_format(ctx->precision);
     int rc = ensure_tc(ctx);
     if (rc) return rc;
     const size_t need = tc::act_bytes(maxc, pw, ph);
@@ -216,7 +238,7 @@ int run_basic(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int engine, const 
     {
         const Layer &L = m->layers[0];
         LayerTimer t(ctx, 0);
-        CU_CHECK(tc::launch_first(src, pw, ph, L.w.data(), dm->b_host[0].data(), L.n_out, cur, ctx->stream, f8));
+        CU_CHECK(tc::launch_first(src, pw, ph, L.w.data(), dm->b_host[0].data(), L.n_out, cur, ctx->stream, rec));
         note_kernel(ctx, 0, src.up2x ? "first_1xN+up2x" : "first_1xN");
         ctx->launches++;
     }
@@ -240,7 +262,7 @@ int run_basic(w2x_ctx *ctx, const w2x_model *m, DevModel *dm, int engine, const 
         } else {
             if (packed) return fail(W2X_ERR_UNSUPPORTED, "packed frames need the fused last layer");
             CU_CHECK(tc::launch_last(cur, L.n_in, pw, ph, dm->w[(size_t)n - 1].get(), static_cast<float>(L.b[0]), n, dst,
-                                     dst_stride, ctx->stream, f8));
+                                     dst_stride, ctx->stream, rec));
             note_kernel(ctx, n - 1, "last_Nx1");
         }
         ctx->launches++;
@@ -525,6 +547,7 @@ int w2x_ctx_create(int device, w2x_ctx **out_ctx) {
         if (!std::strcmp(pe, "f16x3")) ctx->precision = W2X_PRECISION_F16X3;
         else if (!std::strcmp(pe, "f16+f8x2") || !std::strcmp(pe, "f8")) ctx->precision = W2X_PRECISION_F16_F8X2;
         else if (!std::strcmp(pe, "f16")) ctx->precision = W2X_PRECISION_F16;
+        else if (!std::strcmp(pe, "bf16x3")) ctx->precision = W2X_PRECISION_BF16X3;
     }
     CU_CHECK(cudaStreamCreateWithFlags(&ctx->copy_in, cudaStreamNonBlocking));
     CU_CHECK(cudaStreamCreateWithFlags(&ctx->copy_out, cudaStreamNonBlocking));
@@ -574,7 +597,9 @@ int w2x_ctx_get_engine(const w2x_ctx *ctx) { return ctx ? ctx->engine : -1; }
 
 int w2x_ctx_set_precision(w2x_ctx *ctx, int precision) {
     if (check_ctx(ctx)) return W2X_ERR_ARG;
-    if (precision != W2X_PRECISION_F16X3 && precision != W2X_PRECISION_F16_F8X2 && precision != W2X_PRECISION_F16) return fail(W2X_ERR_ARG, "unknown precision mode %d", precision);
+    if (precision != W2X_PRECISION_F16X3 && precision != W2X_PRECISION_F16_F8X2 && precision != W2X_PRECISION_F16 &&
+        precision != W2X_PRECISION_BF16X3)
+        return fail(W2X_ERR_ARG, "unknown precision mode %d", precision);
     ctx->precision = precision;
     return W2X_OK;
 }
@@ -708,8 +733,10 @@ int w2x_filter_layer_device(w2x_ctx *ctx, const w2x_model *model, int layer, con
     if (engine == W2X_ENGINE_TC) {
         if (!tc::layer_supported(L.n_in, L.n_out))
             return fail(W2X_ERR_UNSUPPORTED, "tensor-core engine does not support a %d->%d layer", L.n_in, L.n_out);
-        if (model->tc[(size_t)layer].bytes.empty())
-            return fail(W2X_ERR_UNSUPPORTED, "tensor-core engine needs finite layer weights below 65520 in magnitude");
+        const tc::Rec rec = tc::rec_format(ctx->precision);
+        if (rec == tc::Rec::BF16 ? model->tc[(size_t)layer].bytes_bf16.empty() : model->tc[(size_t)layer].bytes.empty())
+            return fail(W2X_ERR_UNSUPPORTED, rec == tc::Rec::BF16 ? "tensor-core engine needs finite layer weights"
+                                                                  : "tensor-core engine needs finite layer weights below 65520 in magnitude");
         rc = ensure_tc(ctx);
         if (rc) return rc;
         // Model::filter semantics (same size, BORDER_REPLICATE): stage a frame with a replicated ring
@@ -720,11 +747,10 @@ int w2x_filter_layer_device(w2x_ctx *ctx, const w2x_model *model, int layer, con
         rc = ctx->buf[1].reserve(tc::act_bytes(L.n_out, pw, ph));
         if (rc) return rc;
         __half *fin = static_cast<__half *>(ctx->buf[0].get()), *fout = static_cast<__half *>(ctx->buf[1].get());
-        const int f8 = ctx->precision == W2X_PRECISION_F16_F8X2 ? 1 : 0;
-        CU_CHECK(tc::launch_planar_to_nhwc(d_in, L.n_in, width, height, fin, ctx->stream, f8));
+        CU_CHECK(tc::launch_planar_to_nhwc(d_in, L.n_in, width, height, fin, ctx->stream, rec));
         rc = launch_layer_tc(ctx, model, dm, layer, fin, fout, pw, ph, false, false);
         if (rc) return rc;
-        CU_CHECK(tc::launch_nhwc_to_planar(fout, L.n_out, width, height, d_out, ctx->stream, f8));
+        CU_CHECK(tc::launch_nhwc_to_planar(fout, L.n_out, width, height, d_out, ctx->stream, rec));
         ctx->launches += 2;
         return W2X_OK;
     }

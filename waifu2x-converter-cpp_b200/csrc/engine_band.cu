@@ -76,7 +76,7 @@ int w2x_band_create(w2x_ctx *ctx, const w2x_model *model, int width, int band_ro
     if (check_ctx(ctx)) return W2X_ERR_ARG;
     if (!model || !out_band || width < 1 || band_rows < 1) return fail(W2X_ERR_ARG, "w2x_band_create: bad argument");
     *out_band = nullptr;
-    if (!model->tc_eligible || ctx->engine == W2X_ENGINE_FP32)
+    if (!tc_eligible(model, ctx->precision) || ctx->engine == W2X_ENGINE_FP32)
         return fail(W2X_ERR_UNSUPPORTED, "w2x_band_create: the per-layer halo mode needs the tensor-core engine and a 1->{32,64,128}..->1 model");
     if (has_up < 0 || has_up > 2 || has_down < 0 || has_down > 2) return fail(W2X_ERR_ARG, "w2x_band_create: edge kind must be 0 (image border), 1 (neighbour GPU) or 2 (overlap rows)");
     // Refused here, before anything is allocated or queued: a band whose layers failed mid-pass would leave its neighbours'
@@ -94,6 +94,10 @@ int w2x_band_create(w2x_ctx *ctx, const w2x_model *model, int width, int band_ro
     b->model = model;
     rc = get_dev_model(ctx, model, &b->dm);
     if (rc) return rc;
+    if (ctx->precision == W2X_PRECISION_BF16X3) {   // now, not in the first pass: a pass must not stall neighbours that wait for its rows
+        rc = upload_pack_bf16(ctx, model, b->dm);
+        if (rc) return rc;
+    }
     b->dm->band_sessions++;        // w2x_ctx_forget_model refuses until the session goes
     b->n = (int)model->layers.size();
     b->width = width;
@@ -162,11 +166,10 @@ int w2x_band_step(w2x_band *band, int step) {
     const w2x_model *m = band->model;
     DevModel *dm = band->dm;
     const Layer &L = m->layers[(size_t)step];
-    const int f8 = ctx->precision == W2X_PRECISION_F16_F8X2 ? 1 : 0;
     if (step == 0) {
         LayerTimer t(ctx, 0);
         CU_CHECK(tc::launch_first(FrameSource::padded(band->pad.get(), band->pw, band->pw, band->hf), band->pw, band->hf, L.w.data(),
-                                  dm->b_host[0].data(), L.n_out, band->act[0].get(), ctx->stream, f8, band->win_y0, band->win_rows));
+                                  dm->b_host[0].data(), L.n_out, band->act[0].get(), ctx->stream, tc::rec_format(ctx->precision), band->win_y0, band->win_rows));
         band->cur = 0;
         note_kernel(ctx, 0, "first_1xN");
         ctx->launches++;
@@ -725,7 +728,7 @@ int w2x_multi_convert_plane(w2x_multi *m, const w2x_model *model, const float *i
     int nd = (int)m->ctx.size();
     // every band needs a few rows of its own; small planes (and models without a tensor-core form) stay on one GPU
     nd = std::min(nd, height / (4 * n_layers));
-    if (nd < 2 || !model->tc_eligible || m->ctx[0]->engine == W2X_ENGINE_FP32)
+    if (nd < 2 || !tc_eligible(model, m->ctx[0]->precision) || m->ctx[0]->engine == W2X_ENGINE_FP32)
         return w2x_convert_plane(m->ctx[0], model, in, width, height, in_stride_bytes, out, out_stride_bytes, block_splitting);
     const int same = W2X_STEP_SAME;
     return multi_convert(m, m->plan[0], nd, 1, &model, &same, in, width, height, in_stride_bytes, out, out_stride_bytes, [&](int) {
@@ -752,7 +755,7 @@ int w2x_multi_convert_chain(w2x_multi *m, int n_steps, const w2x_model *const *m
     bool tc = ctx0->engine != W2X_ENGINE_FP32;
     for (int k = 0; k < n_steps; k++) {
         n_max = std::max(n_max, (int)models[k]->layers.size());
-        tc = tc && models[k]->tc_eligible;
+        tc = tc && tc_eligible(models[k], ctx0->precision);
     }
     // decided on the input height with the deepest model: later steps only get taller
     const int nd = std::min((int)m->ctx.size(), height / (4 * n_max));

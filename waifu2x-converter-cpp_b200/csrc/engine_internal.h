@@ -69,6 +69,7 @@ struct DevModel {                       // device-resident copy of one model
     std::vector<std::vector<float>> b_host;   // the same on the host (the tensor-core kernels take them as kernel parameters)
     std::vector<DevBuf<uint16_t>> pack; // per layer tensor-core operand image (empty if not eligible)
     std::vector<DevBuf<uint8_t>> pack8; // same for the "f8" flavour (fp16 main product + e4m3 corrections)
+    std::vector<DevBuf<uint16_t>> pack_bf16;   // same for bf16x3: uploaded when the context first converts in that precision
     std::vector<float> out_scale;       // 1 / (wscale * ACT_SCALE)
     std::vector<float> last_w_t;        // HOST: last layer's weights transposed to [9][Cin] (fused last layer, passed as kernel parameters)
     int band_sessions = 0;              // live w2x_band sessions that launch with these copies (w2x_ctx_forget_model refuses while > 0)
@@ -203,6 +204,13 @@ void note_kernel(w2x_ctx *ctx, int layer, const char *name);
 int ensure_tc(w2x_ctx *ctx);
 int check_ctx(w2x_ctx *ctx);
 int pick_engine(w2x_ctx *ctx, const w2x_model *m);
+// Whether the tensor-core engine can run the model in the precision: its shape, and inner weights the precision's operand images
+// hold (finite and below 65520 for the fp16 images, finite for bf16x3).
+inline bool tc_eligible(const w2x_model *m, int precision) {
+    return precision == W2X_PRECISION_BF16X3 ? m->tc_eligible_bf16 : m->tc_eligible;
+}
+// The bf16x3 operand images of every tensor-core layer on the context's device (once per model and context).
+int upload_pack_bf16(w2x_ctx *ctx, const w2x_model *m, DevModel *dm);
 void emit_reference_progress(w2x_ctx *ctx, int w, int h, int n_layers, bool split);   // the reference's stdout lines of one convertWithModels call
 // The lines of one plane of w x h through w2x_convert_plane (host) / w2x_convert_plane_device: a step of w2x_convert_chain*
 void emit_plane_progress(w2x_ctx *ctx, const w2x_model *m, int w, int h, int block_splitting, bool host);

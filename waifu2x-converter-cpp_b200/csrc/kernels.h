@@ -5,6 +5,8 @@
 #include <cuda_runtime.h>
 #include <cstdint>
 
+#include "w2x_b200.h"
+
 namespace w2x {
 
 // The padded input frame of a conversion, pw x ph pixels, read by the first layer (tc::launch_first) or materialised by launch_pad:
@@ -98,7 +100,19 @@ cudaError_t launch_tta_mean(const TtaPlane *tab, int n_planes, int n_tiles, cuda
 namespace tc {
 constexpr int REGION = 16;          // a tile-set covers REGION x REGION output pixels (two 8x16 M-tiles)
 constexpr int HALO = REGION + 2;    // staged input footprint per side
-constexpr float ACT_SCALE = 16.0f;  // activations are stored as fp16 hi/lo of (value * ACT_SCALE)
+constexpr float ACT_SCALE = 16.0f;  // activations are stored as hi/lo records of (value * ACT_SCALE)
+
+// The record format of the activation frames between layers (RECORD frames, see launch_tc_layer): 128 bytes per pixel per
+// 32-channel block, 4 bytes per element, in every format.
+enum class Rec : int {
+    F16 = 0,    // {hi fp16 x32 | lo fp16 x32}                 W2X_PRECISION_F16X3, W2X_PRECISION_F16
+    F8 = 1,     // {xh fp16 x32 | xh8 e4m3 x32 | xl8 e4m3 x32}  W2X_PRECISION_F16_F8X2
+    BF16 = 2,   // {hi bf16 x32 | lo bf16 x32}                 W2X_PRECISION_BF16X3
+};
+// The one place a precision (W2X_PRECISION_*) decides the record format.
+inline Rec rec_format(int precision) {
+    return precision == W2X_PRECISION_F16_F8X2 ? Rec::F8 : precision == W2X_PRECISION_BF16X3 ? Rec::BF16 : Rec::F16;
+}
 
 // Activation frame between layers: 4 bytes per element (RECORD frame, see launch_tc_layer).
 inline size_t act_bytes(int C, int Wp, int Hp) { return (size_t)Hp * Wp * C * 4; }
@@ -112,18 +126,18 @@ cudaError_t init_kernels();
 // whose padding is folded into the loads (FrameSource::padded() reads an already padded region).  -> RECORD frame.
 // `wgt` ([C][9]) and `bias` ((float)bias) are HOST pointers: they travel as kernel parameters.
 cudaError_t launch_first(const FrameSource &src, int pw, int ph, const float *wgt /*[C][9]*/, const float *bias, int cout, __half *out,
-                         cudaStream_t s, int f8 = 0, int out_y0 = 0, int out_rows = -1);
+                         cudaStream_t s, Rec rec, int out_y0 = 0, int out_rows = -1);
 // Tensor-core (wgmma) layer: in/out NHWC frames (pw x ph); the tensor maps are built inside.
 // `bias` is a HOST pointer to the layer's (float)bias values (they travel as kernel parameters).
-// mode = W2X_PRECISION_*: F16X3 (0) and F16 (2): "f16x3" frames [hi][lo], wpack = TcPack::bytes (F16 reads only its wh
-// halves);  F16_F8X2 (1): frames [xh][xh8][xl8], wpack = TcPack::bytes8.
+// mode = W2X_PRECISION_*, records rec_format(mode): F16X3 (0) and F16 (2): Rec::F16 frames, wpack = TcPack::bytes (F16 reads
+// only its wh halves);  F16_F8X2 (1): Rec::F8 frames, wpack = TcPack::bytes8;  BF16X3 (4): Rec::BF16 frames,
+// wpack = TcPack::bytes_bf16.
 cudaError_t launch_tc_layer(const __half *in, const void *wpack, const float *bias, __half *out,
                             int cin, int cout, int pw, int ph, float out_scale, int mode, int num_sms,
                             cudaStream_t s, unsigned long long *prof = nullptr, const float *last_w = nullptr,
                             float *partial = nullptr, int out_y0 = 0, int out_rows = -1);
 // Frames: every activation between layers is a RECORD frame [Hp][Wp][C/32][128 B] -- one 128-byte record per pixel per
-// 32-channel block = {xh fp16 x32 | xh8 e4m3 x32 | xl8 e4m3 x32} (f8) or {hi fp16 x32 | lo fp16 x32} (f16x3): 4 bytes per
-// element, one TMA box row per record (SWIZZLE_128B).
+// 32-channel block in the format Rec: 4 bytes per element, one TMA box row per record (SWIZZLE_128B).
 // out_y0 / out_rows (both launchers): only frame rows [out_y0, out_y0 + out_rows) are stored (-1 = the whole frame); a
 // row-band session keeps its halo rows out of the window because its neighbours write them.
 // Fused last layer: launch_tc_layer(..., last_w = HOST pointer to [9][cout] fp32 tap-major, partial = [ph][pw][12] fp32) makes the
@@ -155,14 +169,14 @@ cudaError_t launch_gather_planes(const float *partial, int fw, const PlaneRect *
                                  cudaStream_t s);
 constexpr int PROF_WORDS = 16;      // per-CTA profile record (see tc_config.cuh PROF_*)
 constexpr int PROF_MAX_CTAS = 256;
-// Last layer (Cout = 1): NHWC hi/lo frame -> fp32 plane, interior only: out(y,x) for
+// Last layer (Cout = 1): RECORD frame -> fp32 plane, interior only: out(y,x) for
 // y in [crop, ph-crop), x in [crop, pw-crop) is written to dst[(y-crop)*stride + (x-crop)].
 cudaError_t launch_last(const __half *in, int cin, int pw, int ph, const float *wgt /*[C][9]*/, float bias,
-                        int crop, float *dst, long dst_stride_floats, cudaStream_t s, int f8 = 0);
-// planar fp32 [C][h][w] -> NHWC hi/lo frame (h+2) x (w+2), replicate ring of 1 (for w2x_filter_layer)
-cudaError_t launch_planar_to_nhwc(const float *in, int C, int w, int h, __half *out, cudaStream_t s, int f8 = 0);
-// NHWC hi/lo frame (h+2) x (w+2) -> planar fp32 [C][h][w] (interior)
-cudaError_t launch_nhwc_to_planar(const __half *in, int C, int w, int h, float *out, cudaStream_t s, int f8 = 0);
+                        int crop, float *dst, long dst_stride_floats, cudaStream_t s, Rec rec);
+// planar fp32 [C][h][w] -> RECORD frame (h+2) x (w+2), replicate ring of 1 (for w2x_filter_layer)
+cudaError_t launch_planar_to_nhwc(const float *in, int C, int w, int h, __half *out, cudaStream_t s, Rec rec);
+// RECORD frame (h+2) x (w+2) -> planar fp32 [C][h][w] (interior)
+cudaError_t launch_nhwc_to_planar(const __half *in, int C, int w, int h, float *out, cudaStream_t s, Rec rec);
 
 }  // namespace tc
 

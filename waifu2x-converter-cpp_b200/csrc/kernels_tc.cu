@@ -13,6 +13,8 @@
 //              operands (K = 32 per instruction, twice the rate) -- the default, 2.0 instead of 3.0 passes
 //   f16        xh*wh alone, by the f16x3 kernels on the f16x3 frames and weights: 1.0 pass, not
 //              fp32-faithful (8-bit outputs within 1 LSB); chosen by the caller, never by default
+//   bf16x3     f16x3's three products on bf16 hi/lo records and weights (conv3x3_bf16x3_kernel, Rec::BF16): fp32's
+//              exponent range, so no activation or weight scale saturates or underflows; chosen by the caller
 //
 // Data layout in HBM: every activation is an NHWC "frame" of 4 bytes per element holding value*ACT_SCALE,
 // [hi fp16][lo fp16] or [xh fp16][xh8 e4m3][xl8 e4m3] planes of [Hp][Wp][C]; all layers of one pass share
@@ -69,13 +71,20 @@ static cudaError_t set_attr1() {
     return cudaFuncSetAttribute(tc_conv3x3_kernel<CIN, COUT, FUSE, F8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                 Cfg<CIN, COUT, FUSE, F8>::SMEM_BYTES);
 }
+template <int CIN, int COUT, bool FUSE>
+static cudaError_t set_attr_bf16() {   // Rec::BF16 keeps the f16x3 shared-memory map (Cfg with F8 = false)
+    return cudaFuncSetAttribute(conv3x3_bf16x3_kernel<CIN, COUT, FUSE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                Cfg<CIN, COUT, FUSE, false>::SMEM_BYTES);
+}
 template <int CIN, int COUT>
 static cudaError_t set_attr() {
     cudaError_t e;
     if ((e = set_attr1<CIN, COUT, false, false>()) != cudaSuccess) return e;
     if ((e = set_attr1<CIN, COUT, true, false>()) != cudaSuccess) return e;
     if ((e = set_attr1<CIN, COUT, false, true>()) != cudaSuccess) return e;
-    return set_attr1<CIN, COUT, true, true>();
+    if ((e = set_attr1<CIN, COUT, true, true>()) != cudaSuccess) return e;
+    if ((e = set_attr_bf16<CIN, COUT, false>()) != cudaSuccess) return e;
+    return set_attr_bf16<CIN, COUT, true>();
 }
 
 #define W2X_TC_SHAPES(X) \
@@ -104,10 +113,17 @@ static cudaError_t launch_k(const CUtensorMap *tmap, const CUtensorMap *omap, co
     return cudaGetLastError();
 }
 
+template <int CIN, int COUT, bool FUSE>
+static cudaError_t launch_k_bf16(const CUtensorMap *tmap, const CUtensorMap *omap, const TcParams &p, int grid, cudaStream_t s) {
+    conv3x3_bf16x3_kernel<CIN, COUT, FUSE><<<grid, NUM_THREADS, Cfg<CIN, COUT, FUSE, false>::SMEM_BYTES, s>>>(*tmap, *omap, p);
+    return cudaGetLastError();
+}
+
 template <int CIN, int COUT>
-static cudaError_t launch_one(const CUtensorMap *tmap, const CUtensorMap *omap, const TcParams &p, int num_sms, bool f8, cudaStream_t s) {
+static cudaError_t launch_one(const CUtensorMap *tmap, const CUtensorMap *omap, const TcParams &p, int num_sms, Rec rec, cudaStream_t s) {
     int grid = p.n_tilesets < num_sms ? p.n_tilesets : num_sms;
-    if (f8) return p.partial ? launch_k<CIN, COUT, true, true>(tmap, omap, p, grid, s) : launch_k<CIN, COUT, false, true>(tmap, omap, p, grid, s);
+    if (rec == Rec::BF16) return p.partial ? launch_k_bf16<CIN, COUT, true>(tmap, omap, p, grid, s) : launch_k_bf16<CIN, COUT, false>(tmap, omap, p, grid, s);
+    if (rec == Rec::F8) return p.partial ? launch_k<CIN, COUT, true, true>(tmap, omap, p, grid, s) : launch_k<CIN, COUT, false, true>(tmap, omap, p, grid, s);
     return p.partial ? launch_k<CIN, COUT, true, false>(tmap, omap, p, grid, s) : launch_k<CIN, COUT, false, false>(tmap, omap, p, grid, s);
 }
 
@@ -132,6 +148,7 @@ cudaError_t launch_tc_layer(const __half *in, const void *wpack, const float *bi
     p.n_tilesets = p.tiles_x * ((out_rows + REGION - 1) / REGION);   // tile-sets tile the store window (TMA store coordinates stay non-negative)
     p.out_scale = out_scale * ACT_SCALE;
     p.xh_only = mode == W2X_PRECISION_F16 ? 1 : 0;
+    const Rec rec = rec_format(mode);
     p.prof = prof;
     p.partial = partial;
     if (partial) {
@@ -143,14 +160,14 @@ cudaError_t launch_tc_layer(const __half *in, const void *wpack, const float *bi
     if (partial) omap = tmap_in;
     else if (make_rec_map(&omap, out, cout, pw, ph, 8, 16, out_y0, out_rows)) return cudaErrorInvalidValue;
 #define X(ci, co) \
-    if (cin == ci && cout == co) return launch_one<ci, co>(&tmap_in, &omap, p, num_sms, mode == W2X_PRECISION_F16_F8X2, s);
+    if (cin == ci && cout == co) return launch_one<ci, co>(&tmap_in, &omap, p, num_sms, rec, s);
     W2X_TC_SHAPES(X)
 #undef X
     return cudaErrorInvalidValue;
 }
 
 template <int COUT>
-static cudaError_t launch_first_c(const FrameSource &src, int pw, int ph, const float *wgt, const float *bias, __half *out, cudaStream_t s, int f8,
+static cudaError_t launch_first_c(const FrameSource &src, int pw, int ph, const float *wgt, const float *bias, __half *out, cudaStream_t s, Rec rec,
                                   int out_y0, int out_rows) {
     static_assert(FIRST_TILE_BYTES + 1024 <= 48 * 1024, "the first layer's staging tile stays under the default dynamic shared memory limit");
     FirstParams<COUT> prm;                                    // HOST pointers -> kernel parameters; ACT_SCALE folded in (exact: a power of two)
@@ -162,37 +179,42 @@ static cudaError_t launch_first_c(const FrameSource &src, int pw, int ph, const 
     dim3 grid((pw + 31) / 32, (out_rows + 7) / 8);   // blocks tile the store window
     if (grid.y > 65535) return cudaErrorInvalidConfiguration;
     if (make_rec_map(&omap, out, COUT, pw, ph, 32, 8, out_y0, out_rows)) return cudaErrorInvalidValue;
+#define W2X_FIRST(R, UP2X) first_layer_kernel<COUT, R, UP2X><<<grid, 256, FIRST_TILE_BYTES + 1024, s>>>(src, pw, ph, out_y0, omap, prm)
     if (src.up2x) {
-        if (f8) first_layer_kernel<COUT, true, true><<<grid, 256, FIRST_TILE_BYTES + 1024, s>>>(src, pw, ph, out_y0, omap, prm);
-        else first_layer_kernel<COUT, false, true><<<grid, 256, FIRST_TILE_BYTES + 1024, s>>>(src, pw, ph, out_y0, omap, prm);
+        if (rec == Rec::F8) W2X_FIRST(Rec::F8, true);
+        else if (rec == Rec::BF16) W2X_FIRST(Rec::BF16, true);
+        else W2X_FIRST(Rec::F16, true);
     } else {
-        if (f8) first_layer_kernel<COUT, true, false><<<grid, 256, FIRST_TILE_BYTES + 1024, s>>>(src, pw, ph, out_y0, omap, prm);
-        else first_layer_kernel<COUT, false, false><<<grid, 256, FIRST_TILE_BYTES + 1024, s>>>(src, pw, ph, out_y0, omap, prm);
+        if (rec == Rec::F8) W2X_FIRST(Rec::F8, false);
+        else if (rec == Rec::BF16) W2X_FIRST(Rec::BF16, false);
+        else W2X_FIRST(Rec::F16, false);
     }
+#undef W2X_FIRST
     return cudaGetLastError();
 }
 
-cudaError_t launch_first(const FrameSource &src, int pw, int ph, const float *wgt, const float *bias, int cout, __half *out, cudaStream_t s, int f8,
+cudaError_t launch_first(const FrameSource &src, int pw, int ph, const float *wgt, const float *bias, int cout, __half *out, cudaStream_t s, Rec rec,
                          int out_y0, int out_rows) {
     if (out_rows < 0) { out_y0 = 0; out_rows = ph; }
     switch (cout) {
-        case 32: return launch_first_c<32>(src, pw, ph, wgt, bias, out, s, f8, out_y0, out_rows);
-        case 64: return launch_first_c<64>(src, pw, ph, wgt, bias, out, s, f8, out_y0, out_rows);
-        case 128: return launch_first_c<128>(src, pw, ph, wgt, bias, out, s, f8, out_y0, out_rows);
+        case 32: return launch_first_c<32>(src, pw, ph, wgt, bias, out, s, rec, out_y0, out_rows);
+        case 64: return launch_first_c<64>(src, pw, ph, wgt, bias, out, s, rec, out_y0, out_rows);
+        case 128: return launch_first_c<128>(src, pw, ph, wgt, bias, out, s, rec, out_y0, out_rows);
         default: return cudaErrorInvalidValue;
     }
 }
 
 cudaError_t launch_last(const __half *in, int cin, int pw, int ph, const float *wgt, float bias, int crop, float *dst,
-                        long dst_stride_floats, cudaStream_t s, int f8) {
+                        long dst_stride_floats, cudaStream_t s, Rec rec) {
     const int ow = pw - 2 * crop, oh = ph - 2 * crop;
     if (ow < 1 || oh < 1 || crop < 1) return cudaErrorInvalidValue;
     dim3 grid((ow + 31) / 32, (oh + 7) / 8);
     if (grid.y > 65535) return cudaErrorInvalidConfiguration;
 #define W2X_LAST(C)                                                                                              \
     case C:                                                                                                          \
-        if (f8) last_layer_kernel<C, true><<<grid, 256, 0, s>>>(in, pw, ph, wgt, bias, crop, dst, dst_stride_floats);    \
-        else last_layer_kernel<C, false><<<grid, 256, 0, s>>>(in, pw, ph, wgt, bias, crop, dst, dst_stride_floats);      \
+        if (rec == Rec::F8) last_layer_kernel<C, Rec::F8><<<grid, 256, 0, s>>>(in, pw, ph, wgt, bias, crop, dst, dst_stride_floats);        \
+        else if (rec == Rec::BF16) last_layer_kernel<C, Rec::BF16><<<grid, 256, 0, s>>>(in, pw, ph, wgt, bias, crop, dst, dst_stride_floats); \
+        else last_layer_kernel<C, Rec::F16><<<grid, 256, 0, s>>>(in, pw, ph, wgt, bias, crop, dst, dst_stride_floats);           \
         break;
     switch (cin) {
         W2X_LAST(32) W2X_LAST(64) W2X_LAST(128)
@@ -229,15 +251,17 @@ cudaError_t launch_gather_planes(const float *partial, int fw, const PlaneRect *
     return cudaGetLastError();
 }
 
-cudaError_t launch_planar_to_nhwc(const float *in, int C, int w, int h, __half *out, cudaStream_t s, int f8) {
+cudaError_t launch_planar_to_nhwc(const float *in, int C, int w, int h, __half *out, cudaStream_t s, Rec rec) {
     long total = (long)(w + 2) * (h + 2) * C;
-    planar_to_nhwc_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(in, C, w, h, out, f8);
+    if (rec == Rec::BF16) planar_to_nhwc_bf16_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(in, C, w, h, out);
+    else planar_to_nhwc_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(in, C, w, h, out, rec == Rec::F8 ? 1 : 0);
     return cudaGetLastError();
 }
 
-cudaError_t launch_nhwc_to_planar(const __half *in, int C, int w, int h, float *out, cudaStream_t s, int f8) {
+cudaError_t launch_nhwc_to_planar(const __half *in, int C, int w, int h, float *out, cudaStream_t s, Rec rec) {
     long total = (long)w * h * C;
-    nhwc_to_planar_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(in, C, w, h, out, f8);
+    if (rec == Rec::BF16) nhwc_bf16_to_planar_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(in, C, w, h, out);
+    else nhwc_to_planar_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(in, C, w, h, out, rec == Rec::F8 ? 1 : 0);
     return cudaGetLastError();
 }
 

@@ -62,6 +62,23 @@ uint16_t f32_to_f16_rn(float f) {
     return (uint16_t)(sign | h);
 }
 
+uint16_t f32_to_bf16_rn(float f) {
+    uint32_t x;
+    std::memcpy(&x, &f, 4);
+    if ((x & 0x7fffffffu) > 0x7f800000u) return (uint16_t)((x >> 16) | 0x40u);   // NaN stays NaN
+    if ((x & 0x7fffffffu) == 0x7f800000u) return (uint16_t)(x >> 16);             // +-inf
+    x += 0x7fffu + ((x >> 16) & 1u);                                               // ties to even; may carry into the exponent
+    if ((x & 0x7fffffffu) >= 0x7f800000u) x = (x & 0x80000000u) | 0x7f7f0000u;     // satfinite: a finite value stays finite
+    return (uint16_t)(x >> 16);
+}
+
+float bf16_to_f32(uint16_t h) {
+    const uint32_t x = (uint32_t)h << 16;
+    float f;
+    std::memcpy(&f, &x, 4);
+    return f;
+}
+
 float f16_to_f32(uint16_t h) {
     uint32_t sign = (uint32_t)(h & 0x8000u) << 16;
     uint32_t e = (h >> 10) & 0x1f, m = h & 0x3ffu;
@@ -389,6 +406,26 @@ static void pack_tc_layer(const Layer &L, TcPack &P) {
             }
 }
 
+// The bf16x3 operand image of the same layer (see TcPack::bytes_bf16): the f16x3 layout and swizzle, bf16 halves at wscale 1.
+// bf16 has fp32's exponent range, so no power-of-two lift is needed and every finite weight packs.
+static void pack_tc_layer_bf16(const Layer &L, TcPack &P) {
+    const int kc = 32, n_chunk = L.n_in / kc, row_bytes = kc * 2;
+    const size_t block_elems = (size_t)L.n_out * kc;
+    P.bytes_bf16.assign((size_t)n_chunk * 9 * 2 * block_elems, 0);
+    for (int c = 0; c < n_chunk; c++)
+        for (int t = 0; t < 9; t++) {
+            uint16_t *hi = P.bytes_bf16.data() + ((size_t)c * 9 + t) * 2 * block_elems, *lo = hi + block_elems;
+            for (int n = 0; n < L.n_out; n++)
+                for (int k = 0; k < kc; k++) {
+                    const float w = L.w[((size_t)n * L.n_in + c * kc + k) * 9 + t];
+                    const uint16_t h = f32_to_bf16_rn(w);
+                    const size_t off = swizzled_offset((size_t)n * row_bytes + 2 * (size_t)k, row_bytes) / 2;
+                    hi[off] = h;
+                    lo[off] = f32_to_bf16_rn(w - bf16_to_f32(h));                  // exact difference
+                }
+        }
+}
+
 // The "f8" operand image of the same layer (see TcPack::bytes8).
 static inline size_t swizzle32(size_t logical) { return logical ^ (((logical >> 7) & 1) << 4); }
 
@@ -460,6 +497,12 @@ static bool tc_packable(const Layer &L) {
         if (!(std::fabs(v) < 65520.f)) return false;
     return true;
 }
+// ... and the bf16x3 image: every finite weight.
+static bool tc_packable_bf16(const Layer &L) {
+    for (float v : L.w)
+        if (!std::isfinite(v)) return false;
+    return true;
+}
 
 int finalize_model(w2x_model *m) {
     if (m->layers.empty()) return fail(W2X_ERR_MODEL, "Error : model has no layers");
@@ -472,19 +515,28 @@ int finalize_model(w2x_model *m) {
                         i, L.n_in, m->layers[i - 1].n_out);
     }
     // tensor-core eligibility: 1 -> C1 -> ... -> Cn -> 1 with every inner width in {32, 64, 128} and every inner layer packable
+    // (fp16 images: finite weights below 65520; bf16x3: finite weights)
     auto okc = [](int c) { return c == 32 || c == 64 || c == 128; };
     size_t n = m->layers.size();
-    bool ok = n >= 3 && m->layers.front().n_in == 1 && m->layers.back().n_out == 1 &&
-              okc(m->layers.front().n_out) && okc(m->layers.back().n_in);
-    for (size_t i = 1; ok && i + 1 < n; i++) ok = okc(m->layers[i].n_in) && okc(m->layers[i].n_out) && tc_packable(m->layers[i]);
+    const bool shape = n >= 3 && m->layers.front().n_in == 1 && m->layers.back().n_out == 1 &&
+                       okc(m->layers.front().n_out) && okc(m->layers.back().n_in);
+    bool ok = shape, ok_bf16 = shape;
+    for (size_t i = 1; i + 1 < n; i++) {
+        const bool c = okc(m->layers[i].n_in) && okc(m->layers[i].n_out);
+        ok = ok && c && tc_packable(m->layers[i]);
+        ok_bf16 = ok_bf16 && c && tc_packable_bf16(m->layers[i]);
+    }
     m->tc_eligible = ok;
+    m->tc_eligible_bf16 = ok_bf16;
     m->tc.assign(n, TcPack());
     for (size_t i = 0; i < n; i++) {
         const Layer &L = m->layers[i];
-        if (okc(L.n_in) && okc(L.n_out) && tc_packable(L)) {
+        if (!okc(L.n_in) || !okc(L.n_out)) continue;
+        if (tc_packable(L)) {
             pack_tc_layer(L, m->tc[i]);
             pack_tc_layer_f8(L, m->tc[i]);
         }
+        if (tc_packable_bf16(L)) pack_tc_layer_bf16(L, m->tc[i]);
     }
     m->uid = g_uid.fetch_add(1);
     return W2X_OK;
@@ -585,6 +637,16 @@ W2X_API int w2x_debug_tc_strip(const w2x_model *model, int layer, int f8, const 
     const std::vector<uint8_t> &v = f8 ? P.strip8 : P.strip;
     if (data) *data = v.data();
     if (n_bytes) *n_bytes = v.size();
+    return W2X_OK;
+}
+
+// The bf16x3 operand image of one layer (TcPack::bytes_bf16: bf16 bit patterns in the f16x3 layout, wscale 1); empty for layers
+// outside the tensor-core shapes or with a non-finite weight.
+W2X_API int w2x_debug_tc_pack_bf16(const w2x_model *model, int layer, const uint16_t **data, size_t *n_elems) {
+    if (!model || layer < 0 || layer >= (int)model->tc.size())
+        return w2x::fail(W2X_ERR_ARG, "w2x_debug_tc_pack_bf16: bad model or layer index");
+    if (data) *data = model->tc[(size_t)layer].bytes_bf16.data();
+    if (n_elems) *n_elems = model->tc[(size_t)layer].bytes_bf16.size();
     return W2X_OK;
 }
 

@@ -17,6 +17,7 @@
 // F8 = false with TcParams::xh_only ("f16", W2X_PRECISION_F16): xh*wh alone (1.0 pass-equivalent, not fp32-faithful) on the
 //             same f16x3 records and weight image, of which only the wh half of each stage is loaded.  A runtime flag, not
 //             a template parameter: the f16x3 kernels run it, choosing the loop once per tile-set.
+// Rec::BF16 ("bf16x3", W2X_PRECISION_BF16X3): f16x3 with bf16 hi/lo records and weights, Cfg<..., F8 = false>'s layout.
 constexpr int F8_A = 10, F8_C = 1;   // xl8 = e4m3((x16 - xh) * 2^F8_A), xh8 = e4m3(xh * 2^-F8_C); must match w2x_internal.h
 
 template <int CIN, int COUT, bool FUSE = false, bool F8 = false>

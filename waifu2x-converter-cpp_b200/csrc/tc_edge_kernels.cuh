@@ -28,8 +28,8 @@ __device__ __forceinline__ float2 f32x2_fma(float2 a, float2 b, float2 c) { retu
 __device__ __forceinline__ float2 f32x2_mul(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 __device__ __forceinline__ float2 f32x2_add(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 
-// UP2X = src.up2x.
-template <int COUT, bool F8, bool UP2X>
+// UP2X = src.up2x.  R = the record format it writes.
+template <int COUT, Rec R, bool UP2X>
 __global__ void __launch_bounds__(256, 4)
 first_layer_kernel(const FrameSource src, int pw, int ph, int out_y0, const __grid_constant__ CUtensorMap tmap_out,
                    const __grid_constant__ FirstParams<COUT> prm) {
@@ -49,6 +49,7 @@ first_layer_kernel(const FrameSource src, int pw, int ph, int out_y0, const __gr
             const int rx = frame_src<UP2X>(fx, src.pad_x, src.w, src.cols_left, src.cols_right);
             v[ky * 3 + kx] = __ldg(src.in + (long)ry * src.stride_floats + rx);
         }
+    constexpr bool F8 = R == Rec::F8;
     const uint32_t r = (uint32_t)threadIdx.x;                            // pixel index inside the block = row of the staged image
     const uint32_t sw128 = r & 7u;
 #pragma unroll 1
@@ -70,6 +71,12 @@ first_layer_kernel(const FrameSource src, int pw, int ph, int out_y0, const __gr
                 const float2 rr = f32x2_add(t, prm.b[pr]);               // (0 + t) + (float)bias
                 const float2 sc = f32x2_mul(rr, make_float2(0.1f, 0.1f));
                 const float a0 = fmaxf(rr.x, sc.x), a1 = fmaxf(rr.y, sc.y);     // leaky-ReLU 0.1, already x ACT_SCALE
+                if constexpr (R == Rec::BF16) {                          // hi = bf16(a), lo = bf16(a - hi), the difference exact
+                    hi[i] = f32x2_to_bf16x2_sat(a0, a1);
+                    const float2 hb = bf16x2_to_f32x2(hi[i]);
+                    lo[i] = f32x2_to_bf16x2_sat(a0 - hb.x, a1 - hb.y);
+                    continue;
+                }
                 __half2 h = f32x2_to_f16x2_sat(a0, a1);
                 float2 hf = __half22float2(h);
                 hi[i] = *reinterpret_cast<uint32_t *>(&h);
@@ -86,7 +93,7 @@ first_layer_kernel(const FrameSource src, int pw, int ph, int out_y0, const __gr
                     lo[i] = *reinterpret_cast<uint32_t *>(&l);
                 }
             }
-            // record row of 128 B: units 0..3 fp16, then [xh8 16+16 B | xl8 16+16 B] or the lo half
+            // record row of 128 B: units 0..3 fp16 (bf16), then [xh8 16+16 B | xl8 16+16 B] or the lo half
             sts128(tile + r * 128u + (((uint32_t)c8 ^ sw128) << 4), make_uint4(hi[0], hi[1], hi[2], hi[3]));
             if constexpr (F8) {
                 const uint32_t half = ((uint32_t)c8 & 1u) * 8u;
@@ -110,10 +117,11 @@ first_layer_kernel(const FrameSource src, int pw, int ph, int out_y0, const __gr
 
 // Last layer: nOutputPlanes = 1.  fp32 arithmetic in the reference's association: per input plane a
 // 9-tap sum, planes added in ascending order, then bias and leaky-ReLU.  One thread per pixel.
-template <int CIN, bool F8>
+template <int CIN, Rec R>
 __global__ void __launch_bounds__(256)
 last_layer_kernel(const __half *__restrict__ in, int pw, int ph, const float *__restrict__ wgt, float bias, int crop,
                   float *__restrict__ dst, long dst_stride) {
+    constexpr bool F8 = R == Rec::F8;
     __shared__ float s_w[CIN * 9];
     for (int i = threadIdx.x; i < CIN * 9; i += blockDim.x) s_w[i] = wgt[i];
     __syncthreads();
@@ -143,13 +151,20 @@ last_layer_kernel(const __half *__restrict__ in, int pw, int ph, const float *__
                 const __nv_fp8x2_storage_t *l8 = reinterpret_cast<const __nv_fp8x2_storage_t *>(&ul8);
 #pragma unroll
                 for (int i = 0; i < 4; i++) {
-                    float2 hf = __half22float2(h2[i]), lf;
-                    if constexpr (F8) {
+                    float2 hf, lf;
+                    if constexpr (R == Rec::BF16) {                   // the same record positions, bf16 pairs
+                        hf = bf16x2_to_f32x2(reinterpret_cast<const uint32_t *>(&uh)[i]);
+                        lf = bf16x2_to_f32x2(reinterpret_cast<const uint32_t *>(&ul)[i]);
+                    } else if constexpr (F8) {
+                        hf = __half22float2(h2[i]);
                         __half2_raw r = __nv_cvt_fp8x2_to_halfraw2(l8[i], __NV_E4M3);
                         lf = __half22float2(*reinterpret_cast<__half2 *>(&r));
                         lf.x *= 1.0f / (float)(1 << F8_A);
                         lf.y *= 1.0f / (float)(1 << F8_A);
-                    } else lf = __half22float2(l2[i]);
+                    } else {
+                        hf = __half22float2(h2[i]);
+                        lf = __half22float2(l2[i]);
+                    }
                     float a0 = (hf.x + lf.x) * inv, a1 = (hf.y + lf.y) * inv;
                     const int tap = ky * 3 + kx;
                     t[2 * i] = fmaf(s_w[(c8 * 8 + 2 * i) * 9 + tap], a0, t[2 * i]);
@@ -284,4 +299,34 @@ __global__ void nhwc_to_planar_kernel(const __half *__restrict__ in, int C, int 
         lo = __half2float(*reinterpret_cast<__half *>(&hr)) * (1.0f / (float)(1 << F8_A));
     } else lo = __half2float(reinterpret_cast<const __half *>(recp + 64)[k]);
     out[idx] = (__half2float(reinterpret_cast<const __half *>(recp)[k]) + lo) * (1.0f / ACT_SCALE);
+}
+
+// The two converters above for Rec::BF16 records {hi bf16 x32 | lo bf16 x32}: hi = bf16(16 v), lo = bf16(16 v - hi).
+__global__ void planar_to_nhwc_bf16_kernel(const float *__restrict__ in, int C, int w, int h, __half *__restrict__ out) {
+    const int pw = w + 2, ph = h + 2;
+    long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    long total = (long)pw * ph * C;
+    if (idx >= total) return;
+    int c = (int)(idx % C);
+    long pix = idx / C;
+    int x = (int)(pix % pw), y = (int)(pix / pw);
+    int sx = min(max(x - 1, 0), w - 1), sy = min(max(y - 1, 0), h - 1);
+    const float a = in[((long)c * h + sy) * w + sx] * ACT_SCALE;
+    const uint32_t hi = f32x2_to_bf16x2_sat(a, 0.f) & 0xffffu;
+    uint16_t *recp = reinterpret_cast<uint16_t *>(reinterpret_cast<uint8_t *>(out) + (pix * (C / 32) + c / 32) * 128);
+    recp[c % 32] = (uint16_t)hi;
+    recp[32 + c % 32] = (uint16_t)f32x2_to_bf16x2_sat(a - bf16x2_to_f32x2(hi).x, 0.f);
+}
+
+__global__ void nhwc_bf16_to_planar_kernel(const __half *__restrict__ in, int C, int w, int h, float *__restrict__ out) {
+    const int pw = w + 2;
+    long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    long total = (long)w * h * C;
+    if (idx >= total) return;
+    int x = (int)(idx % w);
+    long r = idx / w;
+    int y = (int)(r % h), c = (int)(r / h);
+    const uint16_t *recp = reinterpret_cast<const uint16_t *>(reinterpret_cast<const uint8_t *>(in) + ((((long)(y + 1) * pw + (x + 1)) * (C / 32)) + c / 32) * 128);
+    const float hi = bf16x2_to_f32x2(recp[c % 32]).x, lo = bf16x2_to_f32x2(recp[32 + c % 32]).x;
+    out[idx] = (hi + lo) * (1.0f / ACT_SCALE);
 }

@@ -1,4 +1,4 @@
-// tc_kernel.cuh -- tc_conv3x3_kernel: the layer kernel (warp roles, pipelines, epilogue)
+// tc_kernel.cuh -- tc_conv3x3_kernel, conv3x3_bf16x3_kernel: the layer kernel (warp roles, pipelines, epilogue)
 // Part of the tensor-core engine's single translation unit: included by kernels_tc.cu inside namespace w2x::tc, in this order:
 //   tc_ptx.cuh, tc_wgmma.cuh, tc_config.cuh, tc_kernel.cuh, tc_edge_kernels.cuh
 // (pure code organisation: the generated SASS is the same as with one file).
@@ -11,9 +11,18 @@ __device__ __forceinline__ float activate(float acc, float scale, float bias) {
 
 // The record of activated channels cc, cc + 1 (cc even, within the 32-channel block) of one pixel, written into the staging
 // row at rowaddr (swizzle phase sw = row & 7) in the TMA SWIZZLE_128B pattern: fp16 at byte 2 cc, then xh8 at 64 + cc and
-// xl8 at 96 + cc (F8) or lo fp16 at 64 + 2 cc.
-template <bool F8>
+// xl8 at 96 + cc (Rec::F8) or lo fp16 at 64 + 2 cc (Rec::F16); Rec::BF16: hi = bf16(v) at 2 cc, lo = bf16(v - hi) at 64 + 2 cc.
+template <Rec R>
 __device__ __forceinline__ void store_record_pair(uint32_t rowaddr, uint32_t sw, uint32_t cc, float v0, float v1) {
+    constexpr bool F8 = R == Rec::F8;
+    if constexpr (R == Rec::BF16) {
+        const uint32_t hh = f32x2_to_bf16x2_sat(v0, v1);
+        const float2 hf = bf16x2_to_f32x2(hh);
+        const uint32_t lo = f32x2_to_bf16x2_sat(v0 - hf.x, v1 - hf.y);                  // v - hi: exact in fp32
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(rowaddr + (((cc >> 3) ^ sw) << 4) + 2u * (cc & 7u)), "r"(hh) : "memory");
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(rowaddr + (((4u + (cc >> 3)) ^ sw) << 4) + 2u * (cc & 7u)), "r"(lo) : "memory");
+        return;
+    }
     const __half2 hh = f32x2_to_f16x2_sat(v0, v1);
     const float2 hf = __half22float2(hh);
     asm volatile("st.shared.b32 [%0], %1;" ::"r"(rowaddr + (((cc >> 3) ^ sw) << 4) + 2u * (cc & 7u)), "r"(*reinterpret_cast<const uint32_t *>(&hh)) : "memory");
@@ -34,7 +43,7 @@ __device__ __forceinline__ void store_record_pair(uint32_t rowaddr, uint32_t sw,
 // leaky-ReLU -> records of each 32-channel block written into the warpgroup's staging tile in the TMA SWIZZLE_128B pattern
 // (staging row = pixel = y * 8 + x, conflict-free: the eight rows a warp writes at once fall into eight different 16-byte
 // units) and sent as ONE 8x16-pixel TMA store box; the frame edge is clipped by the TMA unit.
-template <int COUT, bool F8>
+template <int COUT, Rec R>
 __device__ __forceinline__ void epilogue_store(const TcParams &p, const float *bias, const CUtensorMap *tmap_out, const float (&acc)[2][COUT / 2],
                                                uint32_t stg, int wg, int wq, int lane, int gx0, int gy0) {
     const int q = lane & 3, r_lo = wq * 16 + (lane >> 2);
@@ -55,7 +64,7 @@ __device__ __forceinline__ void epilogue_store(const TcParams &p, const float *b
                     const int jj = cb * 4 + j, ch = 8 * jj + 2 * q;
                     const float v0 = activate(acc[h][4 * jj + 2 * e], p.out_scale, bias[ch]);
                     const float v1 = activate(acc[h][4 * jj + 2 * e + 1], p.out_scale, bias[ch + 1]);
-                    store_record_pair<F8>(rowaddr, sw, (uint32_t)(8 * j + 2 * q), v0, v1);
+                    store_record_pair<R>(rowaddr, sw, (uint32_t)(8 * j + 2 * q), v0, v1);
                 }
             }
         }
@@ -73,7 +82,7 @@ __device__ __forceinline__ void epilogue_store(const TcParams &p, const float *b
 // swap one value each, so the even lane holds channels ch, ch + 1 of pixel x = 2q and the odd lane those of x = 2q + 1:
 // the same channel pairs, expressions and stores as epilogue_store.  Warps 0, 1 hold block 0 and warps 2, 3 block 1, each
 // written into its own staging tile; warp 0 sends both boxes.
-template <bool F8>
+template <Rec R>
 __device__ __forceinline__ void epilogue_store_swapped(const TcParams &p, const float *bias, const CUtensorMap *tmap_out, const float (&acc)[64],
                                                        uint32_t stg, int wg, int wq, int lane, int gx0, int gy0) {
     const int q = lane & 3, r = lane >> 2, odd = r & 1;
@@ -95,7 +104,7 @@ __device__ __forceinline__ void epilogue_store_swapped(const TcParams &p, const 
             const float v0 = activate(odd ? other : a0, p.out_scale, b0);
             const float v1 = activate(odd ? a1 : other, p.out_scale, b1);
             const uint32_t row = 8u * (uint32_t)j + x;
-            store_record_pair<F8>(blk + row * 128u, x, cc, v0, v1);
+            store_record_pair<R>(blk + row * 128u, x, cc, v0, v1);
         }
     }
     fence_proxy_async();
@@ -182,6 +191,14 @@ __device__ __forceinline__ void epilogue_fuse(const TcParams &p, const float *bi
 constexpr uint32_t PRODUCER_REGS = 40, CONSUMER_REGS = 232;
 static_assert(128 * PRODUCER_REGS + 256 * CONSUMER_REGS == NUM_THREADS * 168, "register hand-off must balance");
 
+// The 16-bit product of a hi/lo record format: bf16 wgmmas on Rec::BF16 records and weights, f16 ones otherwise.  The two
+// formats share the record layout, the weight image layout and the descriptors; only the element type differs.
+template <int N, Rec R>
+__device__ __forceinline__ void mma16(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t scale_d) {
+    if constexpr (R == Rec::BF16) Wgmma<N>::bf16(d, a, b, scale_d);
+    else Wgmma<N>::f16(d, a, b, scale_d);
+}
+
 // The consumer warpgroup of a Cout = 64 layer (Cfg::SWAP): D[channel][pixel], A = the stage's 64 weight rows (the packed
 // image as it is: fp16 rows of 64 B, SWIZZLE_64B; e4m3 rows of 32 B, SWIZZLE_32B), B = the M-tile's 128 pixels (N = 128;
 // the record box with the same descriptor the m64 halves use, eight pixels per halo row).  Per (tap, chunk) one m64n128
@@ -193,9 +210,10 @@ static_assert(128 * PRODUCER_REGS + 256 * CONSUMER_REGS == NUM_THREADS * 168, "r
 //   F_0 X_0 | X_1 [wait: F_0, X_0 done; acc += corr[0]] F_1 | X_2 [wait; acc += corr[1]] F_2 | ... F_8 [wait all]: the
 //   next tap's corrections run while the adds do, and per element the order stays f16 product of tap t, correction of
 //   tap t, f16 product of tap t + 1.  Taps unrolled, the chunk ends with an empty pipe (see below).
-template <int CIN, bool F8>
+template <int CIN, Rec R>
 __device__ __forceinline__ void consume_swapped(const TcParams &p, const CUtensorMap *tmap_out, uint32_t a_base, uint32_t b_base, uint32_t stg,
                                                 uint32_t bar_base, const float *prm, int wg, int wq, int lane, unsigned long long *prof) {
+    constexpr bool F8 = R == Rec::F8;
     using C = Cfg<CIN, 64, false, F8>;
     auto a_full = [&](uint32_t i) { return bar_base + 8u * i; };
     auto a_empty = [&](uint32_t i) { return bar_base + 8u * (2u + i); };
@@ -289,13 +307,13 @@ __device__ __forceinline__ void consume_swapped(const TcParams &p, const CUtenso
                         const uint32_t first = (c | t) != 0 ? 1u : 0u;
                         acc_fence(acc);
                         wgmma_fence();
-                        Wgmma<128>::f16(acc, make_desc(W_HI, w), make_desc(X_HI, x), first);              // wh * xh
-                        Wgmma<128>::f16(acc, make_desc(W_HI, w + 32u), make_desc(X_HI, x + 32u), 1u);
+                        mma16<128, R>(acc, make_desc(W_HI, w), make_desc(X_HI, x), first);              // wh * xh
+                        mma16<128, R>(acc, make_desc(W_HI, w + 32u), make_desc(X_HI, x + 32u), 1u);
                         if constexpr (!XH_ONLY) {
-                            Wgmma<128>::f16(acc, make_desc(W_HI, w), make_desc(X_HI, x + 64u), 1u);       // wh * xl
-                            Wgmma<128>::f16(acc, make_desc(W_HI, w + 32u), make_desc(X_HI, x + 96u), 1u);
-                            Wgmma<128>::f16(acc, make_desc(W_HI, wl), make_desc(X_HI, x), 1u);             // wl * xh
-                            Wgmma<128>::f16(acc, make_desc(W_HI, wl + 32u), make_desc(X_HI, x + 32u), 1u);
+                            mma16<128, R>(acc, make_desc(W_HI, w), make_desc(X_HI, x + 64u), 1u);       // wh * xl
+                            mma16<128, R>(acc, make_desc(W_HI, w + 32u), make_desc(X_HI, x + 96u), 1u);
+                            mma16<128, R>(acc, make_desc(W_HI, wl), make_desc(X_HI, x), 1u);             // wl * xh
+                            mma16<128, R>(acc, make_desc(W_HI, wl + 32u), make_desc(X_HI, x + 32u), 1u);
                         }
                         wgmma_commit();
                         wgmma_wait<1>();                             // the previous group is done: its stage / slot may be refilled
@@ -315,10 +333,10 @@ __device__ __forceinline__ void consume_swapped(const TcParams &p, const CUtenso
                     if (pend_a >= 0) mbar_arrive(a_empty((uint32_t)pend_a));
                 }
             };
-            if (p.xh_only) chunks(std::true_type{});
+            if (R == Rec::F16 && p.xh_only) chunks(std::true_type{});
             else chunks(std::false_type{});
         }
-        epilogue_store_swapped<F8>(p, prm, tmap_out, acc, stg, wg, wq, lane, tx * REGION + 8 * wg, ty * REGION);
+        epilogue_store_swapped<R>(p, prm, tmap_out, acc, stg, wg, wq, lane, tx * REGION + 8 * wg, ty * REGION);
     }
     if (wq == 0) bulk_wait_all();    // this warpgroup's TMA stores are complete before the CTA may exit
     if (prof_on && wg == 0 && wq == 0 && lane == 0) {
@@ -329,9 +347,10 @@ __device__ __forceinline__ void consume_swapped(const TcParams &p, const CUtenso
     }
 }
 
-template <int CIN, int COUT, bool FUSE, bool F8>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-tc_conv3x3_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ TcParams p) {
+// The kernel body, for every record format; tc_conv3x3_kernel and conv3x3_bf16x3_kernel below are its entry points.
+template <int CIN, int COUT, bool FUSE, Rec R>
+__device__ __forceinline__ void conv3x3_body(const CUtensorMap &tmap_in, const CUtensorMap &tmap_out, const TcParams &p) {
+    constexpr bool F8 = R == Rec::F8;
     using C = Cfg<CIN, COUT, FUSE, F8>;
     extern __shared__ uint8_t smem_raw[];
     // 1024-byte alignment: the SWIZZLE_128B pattern repeats every 1024 B
@@ -396,7 +415,7 @@ tc_conv3x3_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_cons
             uint32_t stage = 0, phase = 0;
             unsigned long long w_b = 0;
             const uint8_t *src = reinterpret_cast<const uint8_t *>(p.wpack);
-            const uint32_t b_bytes = !F8 && p.xh_only ? (uint32_t)C::B_BLOCK : (uint32_t)C::B_STAGE;   // xh_only: the wh half of each stage
+            const uint32_t b_bytes = R == Rec::F16 && p.xh_only ? (uint32_t)C::B_BLOCK : (uint32_t)C::B_STAGE;   // xh_only: the wh half of each stage
             for (int ts = blockIdx.x; ts < p.n_tilesets; ts += gridDim.x) {
                 if (C::RESIDENT && ts != (int)blockIdx.x) break;           // resident weights: one pass fills every stage for good
                 for (int blk = 0; blk < C::STAGES_PER_TILESET; blk++) {
@@ -410,7 +429,7 @@ tc_conv3x3_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_cons
         }
     } else if constexpr (C::SWAP) {
         setmaxnreg_inc<CONSUMER_REGS>();
-        consume_swapped<CIN, F8>(p, &tmap_out, a_base, b_base, stg_base + (uint32_t)((warp - 4) >> 2) * C::STG_WG, bar_base, prm, (warp - 4) >> 2,
+        consume_swapped<CIN, R>(p, &tmap_out, a_base, b_base, stg_base + (uint32_t)((warp - 4) >> 2) * C::STG_WG, bar_base, prm, (warp - 4) >> 2,
                                  warp & 3, lane, prof);
     } else {
         setmaxnreg_inc<CONSUMER_REGS>();
@@ -525,13 +544,13 @@ tc_conv3x3_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_cons
 #pragma unroll
                             for (int h = 0; h < 2; h++) {
                                 const uint32_t ah = a0 + (uint32_t)h * HALF + tap;
-                                Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah), make_desc(B_HI, b), first);                   // xh * wh
-                                Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah + 32u), make_desc(B_HI, b + 32u), 1u);
+                                mma16<COUT, R>(acc[h], make_desc(A_HI, ah), make_desc(B_HI, b), first);                   // xh * wh
+                                mma16<COUT, R>(acc[h], make_desc(A_HI, ah + 32u), make_desc(B_HI, b + 32u), 1u);
                                 if constexpr (!XH_ONLY) {
-                                    Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah + 64u), make_desc(B_HI, b), 1u);            // xl * wh
-                                    Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah + 96u), make_desc(B_HI, b + 32u), 1u);
-                                    Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah), make_desc(B_HI, b + COUT * 64u), 1u);     // xh * wl
-                                    Wgmma<COUT>::f16(acc[h], make_desc(A_HI, ah + 32u), make_desc(B_HI, b + COUT * 64u + 32u), 1u);
+                                    mma16<COUT, R>(acc[h], make_desc(A_HI, ah + 64u), make_desc(B_HI, b), 1u);            // xl * wh
+                                    mma16<COUT, R>(acc[h], make_desc(A_HI, ah + 96u), make_desc(B_HI, b + 32u), 1u);
+                                    mma16<COUT, R>(acc[h], make_desc(A_HI, ah), make_desc(B_HI, b + COUT * 64u), 1u);     // xh * wl
+                                    mma16<COUT, R>(acc[h], make_desc(A_HI, ah + 32u), make_desc(B_HI, b + COUT * 64u + 32u), 1u);
                                 }
                             }
                             wgmma_commit();
@@ -545,7 +564,7 @@ tc_conv3x3_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_cons
                         }
                     }
                 };
-                if (p.xh_only) chunks(std::true_type{});
+                if (R == Rec::F16 && p.xh_only) chunks(std::true_type{});
                 else chunks(std::false_type{});
                 wgmma_wait<0>();
                 acc_fence(acc[0]);
@@ -555,7 +574,7 @@ tc_conv3x3_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_cons
             if constexpr (FUSE)
                 epilogue_fuse<COUT>(p, prm, prm + COUT, acc, wq, lane, tx * REGION + 8 * wg, p.out_y0 + ty * REGION);
             else
-                epilogue_store<COUT, F8>(p, prm, &tmap_out, acc, stg_base + (uint32_t)wg * C::STG_WG, wg, wq, lane, tx * REGION + 8 * wg, ty * REGION);
+                epilogue_store<COUT, R>(p, prm, &tmap_out, acc, stg_base + (uint32_t)wg * C::STG_WG, wg, wq, lane, tx * REGION + 8 * wg, ty * REGION);
         }
         if constexpr (!FUSE) {
             if (wq == 0) bulk_wait_all();    // this warpgroup's TMA stores are complete before the CTA may exit
@@ -567,4 +586,18 @@ tc_conv3x3_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_cons
             prof[PROF_TILESETS] += n;
         }
     }
+}
+
+// The fp16 record formats: F8 = false Rec::F16 (f16x3, and f16 through TcParams::xh_only), F8 = true Rec::F8.
+template <int CIN, int COUT, bool FUSE, bool F8>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+tc_conv3x3_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ TcParams p) {
+    conv3x3_body<CIN, COUT, FUSE, F8 ? Rec::F8 : Rec::F16>(tmap_in, tmap_out, p);
+}
+
+// bf16x3 (Rec::BF16): the f16x3 kernel with bf16 records, weights and wgmmas (TcParams::xh_only is ignored).
+template <int CIN, int COUT, bool FUSE>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+conv3x3_bf16x3_kernel(const __grid_constant__ CUtensorMap tmap_in, const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ TcParams p) {
+    conv3x3_body<CIN, COUT, FUSE, Rec::BF16>(tmap_in, tmap_out, p);
 }

@@ -9,7 +9,7 @@
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 // fp32 -> fp16, round to nearest even, saturating: a value that would round to +-inf becomes +-65504 (NaN stays NaN), every
-// other value converts to the bits __float2half_rn gives.  The record encodings use these, so an activation beyond the fp16
+// other value converts to the bits __float2half_rn gives.  The fp16 record encodings use these, so an activation beyond the fp16
 // range leaves a finite record (hi = +-65504, lo = v - hi saturated the same way) instead of hi = inf, lo = -inf.
 __device__ __forceinline__ __half2 f32x2_to_f16x2_sat(float a, float b) {     // low half a, high half b (= __floats2half2_rn)
     uint32_t r;
@@ -21,6 +21,16 @@ __device__ __forceinline__ __half f32_to_f16_sat(float a) {
     asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(r) : "f"(a));
     return *reinterpret_cast<__half *>(&r);
 }
+// fp32 -> bf16 pair (low half a, high half b), round to nearest even, saturating the same way: a value that would round to
+// +-inf (|v| >= 0x1.ffp127) becomes the largest bf16, +-0x1.fep127; NaN stays NaN.  bf16 has fp32's exponent range, so only
+// values within half a bf16 ulp of the top of the fp32 range saturate.
+__device__ __forceinline__ uint32_t f32x2_to_bf16x2_sat(float a, float b) {
+    uint32_t r;
+    asm("cvt.rn.satfinite.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(b), "f"(a));
+    return r;
+}
+// The two values of a bf16 pair (low half first): exact, a bf16 is the high half of an fp32.
+__device__ __forceinline__ float2 bf16x2_to_f32x2(uint32_t p) { return make_float2(__uint_as_float(p << 16), __uint_as_float(p & 0xffff0000u)); }
 
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));

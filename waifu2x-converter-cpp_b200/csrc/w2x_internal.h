@@ -34,6 +34,9 @@ struct TcPack {
     //   [wh fp16: n_out rows x 64 B, SWIZZLE_64B][wh8 = e4m3(wh * 2^-F8_A): n_out rows x 32 B, SWIZZLE_32B]
     //   [wl8 = e4m3((w*wscale - wh) * 2^F8_C): n_out rows x 32 B, SWIZZLE_32B]
     std::vector<uint8_t> bytes8;
+    // bf16x3 flavour (W2X_PRECISION_BF16X3): bytes' layout and swizzle with bf16 bit patterns at wscale 1,
+    // hi = bf16(w), lo = bf16(w - hi).  Packed for every finite layer of a tensor-core shape, fp16-packable or not.
+    std::vector<uint16_t> bytes_bf16;
     // Row-strip design images, built only on request by w2x_debug_tc_strip (Cin, Cout <= 64 only, else empty): [chunk][kx] stages with ky-major rows, see model.cpp
     // pack_tc_layer_strip.  strip = f16x3 flavour [wh | wl], strip8 = f8 flavour [wh | wh8 | wl8].
     std::vector<uint8_t> strip, strip8;
@@ -48,7 +51,8 @@ constexpr int F8_A = 10, F8_C = 1;
 struct w2x_model {
     std::vector<w2x::Layer> layers;
     std::vector<w2x::TcPack> tc;   // per layer; empty pack when the layer is not tensor-core-eligible
-    bool tc_eligible = false;      // 1->32 ... ->1 chain with every inner layer in {32,64,128}
+    bool tc_eligible = false;      // 1->32 ... ->1 chain with every inner layer in {32,64,128}, inner weights finite and below 65520
+    bool tc_eligible_bf16 = false; // the same chain with finite inner weights (W2X_PRECISION_BF16X3)
     uint64_t uid = 0;              // identity for per-context device caches
 };
 
@@ -58,6 +62,8 @@ int parse_model_json(const char *path, w2x_model **out);
 int finalize_model(w2x_model *m);   // validation + tensor-core packing
 uint16_t f32_to_f16_rn(float f);    // round-to-nearest-even, subnormals kept
 float f16_to_f32(uint16_t h);
+uint16_t f32_to_bf16_rn(float f);   // round-to-nearest-even, saturating (cvt.rn.satfinite.bf16x2.f32): finite stays finite
+float bf16_to_f32(uint16_t h);
 uint8_t f32_to_e4m3_rn(float f);    // OCP e4m3 (max 448, no inf), round-to-nearest-even, saturating (cvt.rn.satfinite.e4m3x2.f32)
 
 // The most rows a frame (a padded plane, band or packed frame that one layer pass covers) may have: the first layer, the
